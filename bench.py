@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 tracking-correlator hot path (BASELINE.json metric
+"""bench.py -- headline benchmark of the tracking-correlator hot path on one H100 (BASELINE.json metric
 "Msamples/s through N-channel E/P/L correlator"), workload = BASELINE configs[1] (SURVEY 8d "C2"):
 GPS L1 C/A, 32 channels, 25 Msps synthetic IQ, 3 taps (E/P/L), 1 s of signal per step
 (1000 epochs of 25000 samples per channel => 8e8 channel-samples per step).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
 
 One JSON line on stdout (rank 0).  See DESIGN.md "Measurement" for every field.
 """
@@ -43,7 +43,7 @@ def config_dict(n_gpus):
                         "open-loop per-epoch NCO parameters",
             "channels_per_gpu": N_CH, "fs_sps": FS, "epoch_samples": EPOCH, "epochs_per_step": N_EPOCHS, "taps": TAPS,
             "channel_samples_per_step_per_gpu": N_CH * EPOCH * N_EPOCHS,
-            "l2_policy": "IQ band (200 MB) exceeds L2 (126 MB); streamed once per step, shared by the 32 channels",
+            "l2_policy": "IQ band (200 MB) exceeds L2 (50 MB); streamed once per step, shared by the 32 channels",
             "sharding": (f"ONE receiver, ONE band, {N_CH} x {n_gpus} channels: every rank correlates its own {N_CH} channels on the same IQ "
                          "stream; end to end the band crosses PCIe once (rank 0) and fans out to the peers by one NCCL broadcast over "
                          "NVLink per step (SURVEY 8e); no other data-path collective") if n_gpus > 1 else "single GPU"}
@@ -97,7 +97,7 @@ def synth_iq_device(torch, codes, svs, n, seed, device):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -147,43 +147,15 @@ class ClockSampler:
                 "samples": len(sm), "reasons": sorted(reasons)}
 
 
-def measured_peak_gbs():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    try:
-        with open(p) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+# H100 SXM data-sheet HBM3 bandwidth: the denominator of the roofline fractions, not a measured rate
+HBM_PEAK_GBS = 3350.0
 
 
-def ncu_traffic_bytes():
-    p = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    try:
-        with open(p) as f:
-            return json.load(f).get("trk_correlate_kernel_bytes_per_launch")
-    except Exception:
-        return None
-
-
-def ncu_acq_traffic_bytes():
-    """DRAM bytes of one acq_corr_kernel launch (C4 sweep) from the committed ncu capture."""
-    p = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    try:
-        with open(p) as f:
-            d = json.load(f).get("acq_corr_kernel<512>", {})
-            return int(d.get("dram__bytes_read.sum", 0)) + int(d.get("dram__bytes_write.sum", 0))
-    except Exception:
-        return None
-
-
-def ncu_limiter():
-    """What ncu says bounds the dominant kernel (committed summary of the --set full capture)."""
-    p = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    try:
-        with open(p) as f:
-            return json.load(f).get("limiter")
-    except Exception:
-        return None
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: each named array as out_dir/<name>.npy (float32), for output-by-output comparison of two builds."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 _AFFINITY_BEFORE_BINDING = None
@@ -206,7 +178,7 @@ class whole_host:
 
 def bind_to_gpu_numa(torch, local_rank):
     """Bind this rank (and with it the first-touch placement of its pinned buffers) to the NUMA node its GPU hangs off.
-    Round 1: eight unbound ranks pushing 54 GB/s each halved the 8-GPU end-to-end efficiency."""
+    Unbound ranks pushing samples over PCIe from a remote NUMA node lower the multi-GPU end-to-end rate."""
     bus = None
     try:
         if bus is None:
@@ -480,7 +452,7 @@ def bench_acq(torch, capi, eng, dev, steps, warmup, with_cpu, dist=None, rank=0,
         tdt = torch.tensor([dt], dtype=torch.float64, device=dev)
         dist.all_reduce(tdt, op=dist.ReduceOp.MAX)
         dt = float(tdt.item())
-    peak, peak_src = measured_peak_gbs()
+    peak, peak_src = HBM_PEAK_GBS, "H100 SXM data sheet"
     out = {"metric": "acquisitions/s over Doppler grid", "unit": "acquisitions/s",
            "config": {"workload": f"C4: GPS L1 C/A PCPS, {ACQ_PRNS} PRNs x {bins} Doppler bins x N={ACQ_N} (25 Msps, 1 ms), CFAR statistic, "
                                   "forward FFTs shared by all PRNs"},
@@ -491,7 +463,7 @@ def bench_acq(torch, capi, eng, dev, steps, warmup, with_cpu, dist=None, rank=0,
                    "path": "b200_acq_search_submit / _wait alternating over two acquisition objects"},
            "gpu_launches_per_sweep": launches / steps, "cuda_graph": graph is not None,
            "roofline": {"bound": "hbm", "kernel": "acq_corr_kernel", "achieved": abytes / (ms * 1e-3) / 1e9, "peak": peak,
-                        "unit": "GB/s", "frac": abytes / (ms * 1e-3) / 1e9 / peak, "traffic": ncu_acq_traffic_bytes(),
+                        "unit": "GB/s", "frac": abytes / (ms * 1e-3) / 1e9 / peak,
                         "algorithmic_bytes_per_sweep": abytes, "algorithmic_gflop_per_sweep": aflops / 1e9,
                         "achieved_tflops": aflops / (ms * 1e-3) / 1e12, "peak_source": peak_src,
                         "note": "16N bytes per (PRN,bin) row (SURVEY 8d); operands are L2-resident, the kernel is "
@@ -627,9 +599,8 @@ def cpu_baseline(budget_s=12.0, sweep=False, threads=None):
             t0 = time.perf_counter()
             oracle.port.multicorrelator_batch(1, threads, np.tile(iq, max(1, n // EPOCH + 1)), 0, code, SHIFTS, params, n)
             return time.perf_counter() - t0
-    # Hyper-threaded hosts: on the 2 x 32-core box of this pool 128 pinned threads deliver 3.6 Gsamples/s and 64 deliver 13.7
-    # (AVX units and L2 shared by sibling threads; round 1's 2 919 vs 15 675 Msamples/s on two boxes was this).  The arm
-    # uses the thread count that is FASTEST among {nproc, nproc/2, nproc/4} and says which.
+    # Hyper-threaded hosts: sibling threads share AVX units and L2, so all hardware threads can deliver far less than half of
+    # them.  The arm uses the thread count that is FASTEST among {nproc, nproc/2, nproc/4} and says which.
     best = None
     probe = 2000   # epochs per thread: >= 0.15 s per probe, long enough for sibling-thread contention to show
     for T in (sorted({cores, max(1, cores // 2), max(1, cores // 4)}, reverse=True) if threads is None else [threads]):
@@ -752,7 +723,9 @@ def run_reference_arm(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=200, help="timed steps of the headline leg (the value and --dump-outputs); "
+                    "the acquisition leg runs max(5, min(steps, 50)) sweeps, the sustained leg at least 2.2 s of steps and the "
+                    "other configs max(5, min(steps, 20))")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -760,7 +733,11 @@ def main():
     ap.add_argument("--no-acq", action="store_true")
     ap.add_argument("--no-loop", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the sustained leg, the other BASELINE configs and the coalescer leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the E/P/L taps of the last timed step "
+                                                          "(items x taps x [re, im], float32) to DIR/taps.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the GPU path's taps; the reference arm has no such step")
     if args.warmup < 3 and args.impl == "b200":
         args.warmup = 3
     if args.impl == "reference":
@@ -833,6 +810,8 @@ def main():
         ev[k + 1].record()
     barrier()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"taps": out_dev.cpu().numpy()})
     total_ms = ev[0].elapsed_time(ev[-1])
     launches = eng.launch_count() - l0
     # cross-check with the library's own CUDA-event timer on the engine stream (one extra step)
@@ -1055,7 +1034,7 @@ def main():
         except Exception as ex:
             closed = {"error": repr(ex)}
 
-    # ---- sustained leg: the same step back to back for >= 2 s (the 20-step timed region above is 17 ms) -------------
+    # ---- sustained leg: the same step back to back for >= 2 s (a 20-step timed region above lasts about 21 ms) ------
     sustained = None
     if not args.no_extra:
         n_sus = int(max(args.steps, 2.2 / max(ms_per_step * 1e-3, 1e-6)))
@@ -1107,11 +1086,10 @@ def main():
 
     # ---- roofline of the dominant kernel -------------------------------------------------------------------------
     # `achieved` follows the contract: ALGORITHMIC bytes (8 B per channel-sample, SURVEY 8d) per launch / mean launch time of the
-    # timed region.  On C2 the 32 channels share one IQ stream, so those bytes do not cross HBM 32 times (`traffic` = what
-    # ncu saw) and frac can exceed 1: it is NOT the kernel's distance from a limit.  Two companions say what is:
-    #   hbm_true   the same arithmetic with every (channel, epoch) reading its own samples: 8 B per channel-sample really from HBM;
-    #   fp32_issue what ncu names as the limiter of the C2 launch (instruction issue / FMA pipe), from profiles/.
-    peak, peak_src = measured_peak_gbs()
+    # timed region.  On C2 the 32 channels share one IQ stream, so those bytes do not cross HBM 32 times and frac can exceed 1:
+    # it is NOT the kernel's distance from a limit.  `hbm_true` is: the same arithmetic with every (channel, epoch) reading its
+    # own samples, 8 B per channel-sample really from HBM.
+    peak, peak_src = HBM_PEAK_GBS, "H100 SXM data sheet"
     launch_ms = float(np.mean(per_launch_ms))
     achieved = ch_samples_step * ALGO_BYTES_PER_CHANNEL_SAMPLE / (launch_ms * 1e-3) / 1e9
     hbm_true = None
@@ -1122,13 +1100,12 @@ def main():
                     "kernel": "trk_correlate_kernel<3> (per-item)",
                     "note": "band = channels x samples: no sharing between channels, DRAM traffic == algorithmic bytes (+ items/taps)"}
     roofline = {"bound": "hbm", "kernel": "trk_shared_kernel<3>", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": ncu_traffic_bytes(),
+                "frac": achieved / peak,
                 "algorithmic_bytes_per_launch": ch_samples_step * ALGO_BYTES_PER_CHANNEL_SAMPLE,
-                "launch_ms": launch_ms, "peak_source": peak_src, "limiter": ncu_limiter(), "hbm_true": hbm_true,
-                "note": "achieved/frac = algorithmic bytes (8 B per channel-sample, SURVEY 8d) over the launch time, as the contract defines "
-                        "them; the 32 channels of C2 share one IQ stream, so real DRAM traffic is `traffic` (the 200 MB stream once) and "
-                        "frac > 1 is possible - see `hbm_true` for the fraction with distinct samples per channel-epoch and `limiter` for "
-                        "what ncu names as the bound of the C2 launch (FP32 instruction issue / FMA pipe)"}
+                "launch_ms": launch_ms, "peak_source": peak_src, "hbm_true": hbm_true,
+                "note": "achieved/frac = algorithmic bytes (8 B per channel-sample, SURVEY 8d) over the launch time; the 32 channels "
+                        "of C2 share one IQ stream, so real DRAM traffic is the 200 MB stream once and frac > 1 is possible - see "
+                        "`hbm_true` for the fraction with distinct samples per channel-epoch"}
     cb = None
     if not args.no_cpu_baseline and world == 1:
         with whole_host():

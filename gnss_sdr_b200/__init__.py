@@ -1,4 +1,4 @@
-"""gnss_sdr_b200 -- B200 (sm_100a) implementation of gnss-sdr's tracking-correlator and PCPS
+"""gnss_sdr_b200 -- H100 (sm_90a) implementation of gnss-sdr's tracking-correlator and PCPS
 acquisition hot paths behind a C ABI (include/b200gnss.h, libb200gnss.so).
 
 This package is only the thin Python face of that library (ctypes) used by tests and bench.py;

@@ -1,4 +1,4 @@
-"""Build libb200gnss.so in-tree with nvcc for sm_100a (no JIT cache, no torch extension).
+"""Build libb200gnss.so in-tree with nvcc for sm_90a (H100) (no JIT cache, no torch extension).
 
     python -m gnss_sdr_b200.build [--force] [--verbose]
 """
@@ -14,7 +14,7 @@ LIB = os.path.join(HERE, "libb200gnss.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-Wall",
     "--expt-relaxed-constexpr",

@@ -1,4 +1,4 @@
-// In-shared-memory mixed-radix complex FFT for sm_100a (no cuFFT).
+// In-shared-memory mixed-radix complex FFT for sm_90a (no cuFFT).
 //
 // Sizes are whatever the receiver's sampling rate dictates (N = fs * T: 4000, 8000, 16000,
 // 25000 = 2^3*5^5 ...), so radices 2,3,4,5,7,8 are supported and the planner factors N into them.
@@ -334,7 +334,7 @@ __device__ __forceinline__ void fft_stage(float2* __restrict__ s, int n, int M, 
     // Butterfly i works on block b, offset j (pos0 = b M + j, elements pos0 + q m).  Consecutive threads normally take
     // consecutive j: conflict-free while m >= 16.  In the late forward / early inverse stages m is small (5 for the
     // M = 125 stage of 25 000 = 8 . 25 . 25 . 5) and consecutive threads would hop to the next block every m lanes, which
-    // put 2-3 lanes on the same bank (ncu, round 1: 2.7-way conflicts on 27 % of the shared wavefronts).  There the block
+    // put 2-3 lanes on the same bank.  There the block
     // length M is odd (the planner runs the even radices first), so 16 consecutive BLOCKS at the same offset j hit 16
     // different bank pairs (M b mod 16 is a permutation): threads walk over b first.
     const bool by_block = (m < 16) && (M & 1) && (m > 1);

@@ -1,4 +1,4 @@
-// PCPS acquisition grid search for sm_100a.  Reference: src/algorithms/acquisition/
+// PCPS acquisition grid search for sm_90a.  Reference: src/algorithms/acquisition/
 // gnuradio_blocks/pcps_acquisition.cc (doppler_grid :522-560, statistics :409-519,
 // set_local_code :218-251, wipe-off grid :275-291).
 //

@@ -1,4 +1,4 @@
-// Shared host/device declarations for libb200gnss.so (sm_100a only).
+// Shared host/device declarations for libb200gnss.so (sm_90a only).
 #pragma once
 
 #include "../../include/b200gnss.h"

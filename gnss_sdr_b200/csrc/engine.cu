@@ -146,9 +146,9 @@ extern "C"
             }
         cudaDeviceProp prop{};
         B200_CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-        if (prop.major != 10)
+        if (prop.major != 9 || prop.minor != 0)
             {
-                set_error("device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+                set_error("device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
                 return B200_ERR_NODEV;
             }
         B200_ENTER_DEVICE(device);
@@ -841,7 +841,7 @@ extern "C"
                 // The work items travel on the COPY stream, queued behind the sample pushes made so far, and the compute
                 // stream waits on an event.  Issued on the compute stream instead, this small host->device copy sits in
                 // the copy engine's queue until the previous batch's kernel has finished and holds up every sample
-                // push queued behind it (measured: 41.7 instead of 54.6 GB/s of sustained host->device traffic).
+                // push queued behind it, which lowers the sustained host->device rate.
                 B200_CUDA_TRY(cudaMemcpyAsync(sl->items_dev, sl->items_pin, sizeof(b200_trk_item) * n_items, cudaMemcpyHostToDevice, e->copy_stream));
                 B200_CUDA_TRY(cudaEventRecord(sl->items_ready, e->copy_stream));
                 B200_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl->items_ready, 0));

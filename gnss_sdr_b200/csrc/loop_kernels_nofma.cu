@@ -18,8 +18,7 @@
 #include <cstdlib>
 #include "loop.cuh"
 // A persistent CTA has the SM to itself (8-16 warps): its tile loop may want more loads in flight than the batch kernel's, which
-// shares the SM with three other CTAs.  B200_LOOP_TILE_UNROLL sets it for this translation unit only (tools/loop_ab.sh);
-// measured with 32 loops: 4 (default) 9.2 us per epoch, 8 9.1, 12 10.7 - no reason to differ.
+// shares the SM with three other CTAs.  B200_LOOP_TILE_UNROLL sets it for this translation unit only (tools/loop_ab.sh).
 #ifdef B200_LOOP_TILE_UNROLL
 #define TRK_TILE_UNROLL_3 B200_LOOP_TILE_UNROLL
 #endif
@@ -482,10 +481,9 @@ __global__ void trk_loop_cycle_kernel(LoopDev* loops, int n_loops, int mode, Loo
 // kLoopThreads threads with the batch kernel's per-item templates, slices = 1).  Loops are independent, so there is no
 // grid-wide dependency and no launch per epoch; a CTA ends when its loop has run max_epochs cycles, loses lock, or
 // finds its next vector_length samples not resident (stall).
-// Each channel is a latency chain (epoch k+1's NCO commands need epoch k's taps); the CTA width is a build parameter.
-// Measured on B200 (tools/loop_ab.sh, 32 / 256 loops): 256 threads 10.9 / 19.1 us per epoch, 512 threads 10.5 / 26.3,
-// 1024 threads 12.9 / 30.9 - the serial double-precision loop update of thread 0, not the correlation, sets the epoch
-// time, and wider CTAs cost residency when many loops run.
+// Each channel is a latency chain (epoch k+1's NCO commands need epoch k's taps); the CTA width is a build parameter.  The
+// serial double-precision loop update, not the correlation, dominates the epoch time, and wider CTAs cost residency when
+// many loops run.
 #ifndef B200_LOOP_THREADS
 #define B200_LOOP_THREADS 256
 #endif
@@ -493,7 +491,7 @@ __global__ void trk_loop_cycle_kernel(LoopDev* loops, int n_loops, int mode, Loo
 #define B200_LOOP_SERIAL_UPDATE 0
 #endif
 constexpr int kLoopThreadsMany = B200_LOOP_THREADS;   // CTA width when loops outnumber the SMs (two CTAs per SM)
-constexpr int kLoopThreadsFew = 512;                  // one loop per SM at most: wider CTAs shorten the correlation (8.7 vs 9.3 us per epoch)
+constexpr int kLoopThreadsFew = 512;                  // one loop per SM at most: wider CTAs shorten the correlation
 
 template <int kLoopThreads>
 __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / kLoopThreads : 1) trk_loop_persistent_kernel(LoopDev* loops, int n_loops, int max_epochs, LoopAvail avail,
@@ -693,7 +691,8 @@ int launch_loop_persistent(LoopDev* loops, int n_loops, int max_epochs, const Lo
     if (tbl_cap > cap_limit) tbl_cap = cap_limit;
     tbl_cap = (tbl_cap + 3) & ~3;
     // width: each loop is a latency chain, so with no more loops than SMs a wide CTA is the faster one; beyond that two narrow
-    // CTAs per SM overlap each other's serial sections (256 loops: 17.5 us per epoch at 256 threads, 22.8 at 512).
+    // CTAs per SM overlap each other's serial sections.  On an H100 (400 W), us per epoch: 32 loops 10.1-10.5 at 512 threads,
+    // 11.2 at 256; 256 loops 29.5-30.0 at 256 threads, 33.6-34.0 at 512.
     // B200_LOOP_WIDTH = 256 | 512 forces one (A/B runs).
     int sms = 0, dev = 0;
     B200_CUDA_TRY(cudaGetDevice(&dev));

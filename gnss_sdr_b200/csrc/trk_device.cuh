@@ -82,42 +82,16 @@ __device__ __forceinline__ float2 ldg_stream8(const float2* p)
 }
 
 
-// ---- packed f32x2 arithmetic (Blackwell FADD2/FMUL2/FFMA2), explicit .rn/.rm in PTX so that
-// ptxas can never contract a separately rounded mul+add of the chip-index arithmetic into an FMA.
-typedef unsigned long long f2x;  // two packed floats: .x in the low word, .y in the high word
-__device__ __forceinline__ f2x pk(float lo, float hi)
+// ---- lane-wise float2 arithmetic on sample pairs (.x = sample n, .y = sample n+1).  Hopper has no
+// packed FP32 instructions, so each is two scalar operations with an explicit rounding mode: ptxas
+// never contracts a separately rounded mul+add of the chip-index arithmetic into an FMA.
+__device__ __forceinline__ float2 add2_rn(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2_rd(float2 a, float2 b) { return make_float2(__fadd_rd(a.x, b.x), __fadd_rd(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2_rn(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c)
 {
-    f2x r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
-__device__ __forceinline__ void unpk(f2x v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ void unpk_u(f2x v, unsigned int& lo, unsigned int& hi) { asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(v)); }
-__device__ __forceinline__ f2x mul2_rn(f2x a, f2x b)
-{
-    f2x r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ f2x add2_rn(f2x a, f2x b)
-{
-    f2x r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ f2x add2_rm(f2x a, f2x b)
-{
-    f2x r;
-    asm("add.rm.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ f2x fma2_rn(f2x a, f2x b, f2x c)
-{
-    f2x r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ f2x neg2(f2x a) { return a ^ 0x8000000080000000ULL; }
 __device__ __forceinline__ float lds_f32(unsigned int addr)
 {
     float v;

@@ -1,17 +1,18 @@
 // Per-item correlation of the multi-tap tracking correlator (device templates shared by the batch kernel in
 // trk_kernels.cu and the persistent free-running kernel in loop_kernels_nofma.cu).  See trk_kernels.cu for the
 // mapping to the reference's volk_gnsssdr kernels.  Every floating-point contraction in here is written
-// explicitly (fmaf / __fmul_rn / __fadd_rn / packed intrinsics), so the arithmetic does not depend on the
+// explicitly (fmaf / __fmul_rn / __fadd_rn and the float2 helpers of trk_device.cuh), so the arithmetic does not depend on the
 // translation unit's --fmad setting; tests/test_loop_gpu.py checks the two instantiations bit for bit.
 #pragma once
 
 #include "common.cuh"
 #include "trk_device.cuh"
 
-// tiles of the packed main loop unrolled per thread (one 16-byte load each): memory-level parallelism vs registers.  Measured
-// on B200 (tools/ab_item.sh): with five taps (C3, Galileo E1) 4.66 ms at 4, 3.92 at 8, 3.89 at 16 (= a whole re-seed group:
-// the kernel is waiting on L2, more loads in flight is what it wants); with three taps (distinct-IQ C2) 0.612 ms at 4, 0.633 at
-// 8, 0.908 at 2; the one-tap data correlator of a tracked pilot (C3 + pilot) 6.50 ms at 4, 6.18 at 8, 6.14 at 16.
+// tiles of the main loop unrolled per thread (one 16-byte load each): memory-level parallelism vs registers.  With five taps
+// (C3, Galileo E1) and one tap (the data correlator of a tracked pilot) the kernel waits on L2, so 16 = a whole re-seed group
+// of loads in flight; three taps (C2) take 4.  tools/ab_item.sh compares builds with other values.  On an H100 (400 W), ms per
+// step, default vs 8: five taps C3 5.52 vs 5.94; three taps C2 distinct-IQ 1.165 vs 1.178; one tap C3 + pilot 8.93-8.98 vs
+// 8.84 (within the spread of repeated runs of one build).
 #ifndef TRK_TILE_UNROLL_3
 #define TRK_TILE_UNROLL_3 4
 #endif
@@ -131,14 +132,11 @@ __device__ __forceinline__ void correlate_range(const ItemCtx& cx, const float (
 }
 
 
-// ---- main tiles, FAST path: packed arithmetic on sample pairs, no modulo, no F2I -------------------
-// Lane .x of every packed value belongs to sample n0, lane .y to sample n0+1 (one LDG.128).
+// ---- main tiles, FAST path: arithmetic on sample pairs, no modulo, no F2I -----------------------------
+// Lane .x of every float2 value belongs to sample n0, lane .y to sample n0+1 (one LDG.128).
 // floor() uses the 1.5*2^23 trick: fl_rm(aux + 12582912.f) has floor(aux) in its low mantissa bits
 // (exact for |aux| < 2^22, guaranteed by the caller's range check), so the table address is one LEA:
 //   addr = (bits << 2) + tbl_off,  tbl_off = smem(table) - 4*(tbl_base + 0x4B400000)  (mod 2^32).
-// NOTE: ptxas 12.9 contracts mul.rn.f32x2 + add.rn.f32x2 into FFMA2 even with explicit rounding
-// modifiers and --fmad=false, which would change chip indices; the products step*n therefore use
-// the scalar __fmul_rn (never contracted) and only the additions are packed.
 template <int TAPS, bool WRAPS, int THREADS = kTrkThreads>
 __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const float (&shifts)[TAPS], unsigned int tbl_off,
     int tile_begin, int tile_end, int head, float2 (&acc)[TAPS])
@@ -197,17 +195,17 @@ __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const fl
 #pragma unroll
                     for (int t = 0; t < TAPS; t++)
                         {
-                            const float2 tt = __fadd2_rd(__fadd2_rn(m2, aux2[t]), magic2);
+                            const float2 tt = add2_rd(add2_rn(m2, aux2[t]), magic2);
                             const float ca = lds_f32((__float_as_uint(tt.x) << 2) + tbl_off);
                             const float cb = lds_f32((__float_as_uint(tt.y) << 2) + tbl_off);
                             const float2 c2 = make_float2(ca, cb);
-                            are[t] = __ffma2_rn(wr2, c2, are[t]);
-                            aim[t] = __ffma2_rn(wi2, c2, aim[t]);
+                            are[t] = fma2_rn(wr2, c2, are[t]);
+                            aim[t] = fma2_rn(wi2, c2, aim[t]);
                         }
                     // z *= D
-                    const float2 t1 = __fmul2_rn(zi, Di2);
-                    const float2 nzr = __ffma2_rn(zr, Dr2, make_float2(-t1.x, -t1.y));
-                    zi = __ffma2_rn(zr, Di2, __fmul2_rn(zi, Dr2));
+                    const float2 t1 = mul2_rn(zi, Di2);
+                    const float2 nzr = fma2_rn(zr, Dr2, make_float2(-t1.x, -t1.y));
+                    zi = fma2_rn(zr, Di2, mul2_rn(zi, Dr2));
                     zr = nzr;
                     nfa += static_cast<float>(kTile);
                     nfb += static_cast<float>(kTile);
@@ -215,9 +213,9 @@ __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const fl
                     ptr += kTile;
                 }
             // group seed advances by G (few steps per epoch: error stays ~1e-7 per step)
-            const float2 t2 = __fmul2_rn(zi2, Gi2);
-            const float2 ngr = __ffma2_rn(zr2, Gr2, make_float2(-t2.x, -t2.y));
-            zi2 = __ffma2_rn(zr2, Gi2, __fmul2_rn(zi2, Gr2));
+            const float2 t2 = mul2_rn(zi2, Gi2);
+            const float2 ngr = fma2_rn(zr2, Gr2, make_float2(-t2.x, -t2.y));
+            zi2 = fma2_rn(zr2, Gi2, mul2_rn(zi2, Gr2));
             zr2 = ngr;
         }
 #pragma unroll

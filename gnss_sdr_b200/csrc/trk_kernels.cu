@@ -1,4 +1,4 @@
-// Multi-tap tracking correlator for sm_100a.
+// Multi-tap tracking correlator for sm_90a.
 //
 // One CTA per (work item, slice).  A work item is one (channel, epoch): N complex samples of the
 // band store, one code table, up to 8 taps.  The kernel fuses what the reference does in three
@@ -71,8 +71,10 @@ __device__ __forceinline__ void run_item(const b200_trk_item& it, const ChanDesc
 
 // TAPS_T > 0: every channel in the launch has exactly TAPS_T taps (specialised registers).
 // TAPS_T == 0: taps read per item.
-// No minimum-blocks hint by default: ptxas then settles on 64 registers = 4 CTAs per SM, which measures best by far
-// (tools/ab_item.sh, C3: 3.89 ms; TRK_MIN_BLOCKS=2 -> 128 registers 4.11 ms, =3 -> 80 registers 7.37 ms).
+// No minimum-blocks hint by default.  sm_90a, no spills: <3> 64 registers (4 CTAs per SM), <1> 60, <5> 80 (3 CTAs), <0> 128.
+// TRK_MIN_BLOCKS builds the alternatives for tools/ab_item.sh.  On an H100 (400 W), ms per step: TRK_MIN_BLOCKS=4 (everything
+// at 64 registers; <0> spills 3.3 KB) C3 5.43-5.46 vs 5.52-5.53, but C3 + pilot 9.12-9.14 vs 8.93-8.98 and the C5 share
+// 2.73-2.80 vs 2.60-2.64; TRK_MIN_BLOCKS=3 slower on all four legs.  The default stays.
 #ifdef TRK_MIN_BLOCKS
 #define TRK_LAUNCH_BOUNDS __launch_bounds__(kTrkThreads, TRK_MIN_BLOCKS)
 #else

@@ -1,8 +1,8 @@
-// Tracking correlator, "shared window" kernel for sm_100a.
+// Tracking correlator, "shared window" kernel for sm_90a.
 //
 // Why: the per-item kernel (trk_kernels.cu) re-reads every IQ sample from L2 once per channel.  With
 // 32 channels on one band that is 6.4 GB through the L2->SM crossbar per second of signal, and the
-// crossbar (~6.7 TB/s measured, profiles/roofline_traffic.json) becomes the bound.  Channels that are
+// crossbar becomes the bound.  Channels that are
 // in lock on the same band correlate the SAME samples, so here one CTA serves a GROUP of up to 8 work
 // items (one consumer warp each) from one copy of the samples:
 //
@@ -10,8 +10,8 @@
 //                   4-stage shared-memory ring, completion signalled on mbarriers (expect_tx bytes);
 //   8 consumer warps each owns one (channel, epoch) item of the group: waits for the tile, reads its
 //                   samples with conflict-free LDS.128, rotates, looks its three (five, ...) chips up
-//                   in a warp-private shared-memory code table, accumulates E/P/L in packed f32x2
-//                   registers, releases the tile.
+//                   in a warp-private shared-memory code table, accumulates E/P/L in per-sample-pair
+//                   float2 registers, releases the tile.
 //
 // The arithmetic per sample is exactly that of trk_kernels.cu (same chip-index float sequence, same
 // 64-bit fixed-point carrier phase), so results follow the same contract.  Items of a group need
@@ -28,8 +28,12 @@ constexpr int kShTile = 512;     // samples per tile (4 KB)
 #ifndef SH_STAGES
 #define SH_STAGES 4
 #endif
+// Minimum resident CTAs per SM (__launch_bounds__).  sm_90a, 288 threads: 3 caps the kernel at 72 registers and spills
+// (<3>: 166 B stores / 248 B loads), 2 gives 96 registers (<3>: 8 B / 8 B), 1 no spills at 127-152.  On an H100 (400 W), ms
+// per C2 step: 2 -> 0.969-0.970, 3 -> 1.051-1.058, 1 -> 1.189-1.191, 4 -> 1.179; distinct-IQ through this kernel 1.237 at 2,
+// 1.393 at 3.
 #ifndef SH_MINB
-#define SH_MINB 3
+#define SH_MINB 2
 #endif
 constexpr int kShStages = SH_STAGES;
 // SH_STRESS (test builds only, tests/test_ring_stress_gpu.py): pseudo-random delays in the producer and in every consumer
@@ -187,16 +191,16 @@ __device__ __forceinline__ void warp_tile(const Loader& load, float vlo, float v
 #pragma unroll
             for (int t = 0; t < TAPS; t++)
                 {
-                    const float2 tt = __fadd2_rd(__fadd2_rn(m2, aux2[t]), magic2);
+                    const float2 tt = add2_rd(add2_rn(m2, aux2[t]), magic2);
                     const float ca = lds_f32((__float_as_uint(tt.x) << 2) + tbl_off);
                     const float cb = lds_f32((__float_as_uint(tt.y) << 2) + tbl_off);
                     const float2 c2 = make_float2(ca, cb);
-                    are[t] = __ffma2_rn(wr2, c2, are[t]);
-                    aim[t] = __ffma2_rn(wi2, c2, aim[t]);
+                    are[t] = fma2_rn(wr2, c2, are[t]);
+                    aim[t] = fma2_rn(wi2, c2, aim[t]);
                 }
-            const float2 t1 = __fmul2_rn(zi, Di2);
-            const float2 nzr = __ffma2_rn(zr, Dr2, make_float2(-t1.x, -t1.y));
-            zi = __ffma2_rn(zr, Di2, __fmul2_rn(zi, Dr2));
+            const float2 t1 = mul2_rn(zi, Di2);
+            const float2 nzr = fma2_rn(zr, Dr2, make_float2(-t1.x, -t1.y));
+            zi = fma2_rn(zr, Di2, mul2_rn(zi, Dr2));
             zr = nzr;
             fa += 64.0f;
             fb += 64.0f;
@@ -466,9 +470,9 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
             {
                 // re-seed: the group seed advances by G = exp(j DT 64*kShReseed) and replaces the
                 // running phasor (bounds the drift of the 64 recurrence steps in between)
-                const float2 t2 = __fmul2_rn(zi2, Gi2);
-                const float2 ngr = __ffma2_rn(zr2, Gr2, make_float2(-t2.x, -t2.y));
-                zi2 = __ffma2_rn(zr2, Gi2, __fmul2_rn(zi2, Gr2));
+                const float2 t2 = mul2_rn(zi2, Gi2);
+                const float2 ngr = fma2_rn(zr2, Gr2, make_float2(-t2.x, -t2.y));
+                zi2 = fma2_rn(zr2, Gi2, mul2_rn(zi2, Gr2));
                 zr2 = ngr;
                 zr = zr2;
                 zi = zi2;
@@ -593,9 +597,9 @@ int launch_trk_shared(const b200_trk_item* items, int n_items, const ChanDesc* c
     return B200_OK;
 }
 
-// Longest code table for which every epoch takes the whole-table mode (measured faster than the per-item
-// kernel: 0.85 vs 0.92 ms on C2).  Longer tables (E1 8184, L5 10230) work through the sliding window but
-// measure slower than the per-item kernel (C3: 5.4 vs 4.7 ms), so the engine only picks them when forced.
+// Longest code table for which every epoch takes the whole-table mode (faster than the per-item kernel on C2).
+// Longer tables (E1 8184, L5 10230) work through the sliding window but are slower than the per-item kernel
+// (C3), so the engine only picks them when forced.
 int trk_shared_max_code_len() { return kShTblCap - 64; }
 
 }  // namespace b200

@@ -315,7 +315,7 @@ bool Trk_Coalescer::wait(int id, std::complex<float>* out)
     if (s == nullptr) return false;
     // spin briefly (the GPU round trip of a batch is tens of microseconds), then sleep on the slot's state word - but only
     // while the block threads leave cores free: with more waiters than half the hardware threads, spinning waiters push the
-    // tick thread off its core (measured with 256 threads on 128: batch round trip 340 us instead of 50)
+    // tick thread off its core and the batch round trip grows several-fold
     static const int hw = static_cast<int>(std::thread::hardware_concurrency());
     const int spin_limit = (d_n_active.load(std::memory_order_relaxed) * 2 <= hw) ? 2000 : 0;
     int st;

@@ -1,5 +1,5 @@
 /*
- * b200gnss.h -- C ABI of libb200gnss.so: the B200 (sm_100a) implementation of gnss-sdr's two
+ * b200gnss.h -- C ABI of libb200gnss.so: the H100 (sm_90a) implementation of gnss-sdr's two
  * data-parallel hot paths, the multi-tap tracking correlator and the PCPS acquisition grid
  * search.  Plain pointers and sizes only; no C++/torch types cross this boundary.
  *
@@ -37,7 +37,7 @@ extern "C"
 #define B200_ERR_NOMEM (-3)  /* host or device allocation failed */
 #define B200_ERR_STATE (-4)  /* call sequence error (e.g. correlate before set_local_code) */
 #define B200_ERR_RANGE (-5)  /* size outside what the engine was created for */
-#define B200_ERR_NODEV (-6)  /* no usable sm_100 device */
+#define B200_ERR_NODEV (-6)  /* no usable sm_90 device */
 
 #define B200_MAX_TAPS 8
 

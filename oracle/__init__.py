@@ -35,6 +35,7 @@ def build(verbose: bool = False) -> None:
     # the reference's blocks compiled where they lie + the build check of integration/src (needs libb200gnss.so, which
     # gnss_sdr_b200.build produces first); both are skipped, keeping prebuilt libraries, where /root/reference is absent
     subprocess.check_call(["make", "-C", _HERE, "blocks"], stdout=out)
+    subprocess.check_call(["make", "-C", _HERE, "patchcheck"], stdout=out)
 
 
 def _fp(a: np.ndarray):

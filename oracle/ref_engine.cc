@@ -107,7 +107,7 @@ extern "C"
     }
 
     /* pin != 0: thread t is bound to the t-th CPU of the process's affinity mask (round robin), so that the figure does
-     * not depend on where the scheduler happens to put 128 threads (round 1: 2 919 vs 15 675 Msamples/s on two boxes). */
+     * not depend on where the scheduler happens to put the threads. */
     double ref_mc_bench_pinned(int threads, int n, int taps, int code_len, int iters, int n_epochs_buf, int high_dyn, int pin)
     {
         std::vector<RefMc*> pool(threads);

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -21,5 +21,5 @@ def oracle():
 @pytest.fixture(scope="session")
 def ref(oracle):
     if oracle.ref is None:
-        pytest.skip("oracle/_ref/liboracle_ref.so not built (no /root/reference here)")
+        pytest.skip("oracle/_ref/liboracle_ref.so not built (no reference sources here)")
     return oracle.ref

@@ -13,6 +13,7 @@ fixtures hold only parameters and the reference's outputs:
                        discriminator / lock-detector code (oracle/ref_loop.cc) for seeded correlator outputs
   acq_ref_golden.npz   volk_gnsssdr_s32f_sincos_32fc a_avx2 wipe-off rows (bit patterns) for a few
                        Doppler bins, and volk_gnsssdr_32f_index_max_32u results
+  port_vs_ref_sha256.json  SHA-256 of the reference kernels' outputs in tests/test_oracle_port_vs_ref.py, per test
 """
 import os
 import sys
@@ -109,6 +110,10 @@ def main():
         lp[f"{name}/records"] = np.frombuffer(np.array(recs, ol.DUMP_RECORD_DTYPE).tobytes(), np.uint8)
         lp[f"{name}/items"] = np.array(items, np.uint64)
     np.savez_compressed(os.path.join(HERE, "loop_ref_golden.npz"), **lp)
+    # SHA-256 of the reference kernels' outputs behind tests/test_oracle_port_vs_ref.py
+    import subprocess
+    subprocess.check_call([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", os.path.join(ROOT, "tests", "test_oracle_port_vs_ref.py")],
+                          env=dict(os.environ, PORT_VS_REF_DIGESTS=os.path.join(HERE, "port_vs_ref_sha256.json")), cwd=ROOT)
     print("wrote", os.listdir(HERE))
 
 

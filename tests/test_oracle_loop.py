@@ -14,7 +14,7 @@ import loop_harness as lh
 def reflib():
     lib = ol.ref_lib()
     if lib is None:
-        pytest.skip("oracle/_ref/liboracle_ref_loop.so not built (no /root/reference here)")
+        pytest.skip("oracle/_ref/liboracle_ref_loop.so not built (no reference sources here)")
     return lib
 
 
