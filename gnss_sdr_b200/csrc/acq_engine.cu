@@ -7,6 +7,7 @@
 
 #include <cmath>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -25,37 +26,36 @@ using namespace b200;
 
 struct b200_acq
 {
+    CudaStream stream;  // own, or the engine's; declared first, so released after the buffers used on it
     b200_engine* e{nullptr};
     b200_acq_conf c{};
     FftPlan plan{};
-    cudaStream_t stream{nullptr};
-    bool own_stream{false};
     int doppler_center{0};
     int doppler_bias{0};
-    float2* tw{nullptr};
-    float2* wipe{nullptr};     // bins x n
-    float2* X{nullptr};        // bins x n   forward spectra (digit-reversed)
-    float2* codes{nullptr};    // slots x n  conj(FFT(code)) (digit-reversed)
-    float2* in_dev{nullptr};   // consumed
-    short* raw_dev{nullptr};   // 2 x consumed int16 (cshort input, converted on the device)
-    float2* code_stage{nullptr};
-    float* grid{nullptr};      // slots x bins x ne (optional)
-    float2* wipe2{nullptr};    // step-two wipe-offs (bins2 x n)
-    float2* Z{nullptr};        // two-level FFT only: rows x fft_size inverse-transformed blocks
-    AcqRowStat* partial{nullptr};
+    DevBuf<float2> tw;
+    DevBuf<float2> wipe;        // bins x n
+    DevBuf<float2> X;           // bins x n   forward spectra (digit-reversed)
+    DevBuf<float2> codes;       // slots x n  conj(FFT(code)) (digit-reversed)
+    DevBuf<float2> in_dev;      // consumed
+    DevBuf<short> raw_dev;      // 2 x consumed int16 (cshort input, converted on the device)
+    DevBuf<float2> code_stage;
+    DevBuf<float> grid;         // slots x bins x ne (optional)
+    DevBuf<float2> wipe2;       // step-two wipe-offs (bins2 x n)
+    DevBuf<float2> Z;           // two-level FFT only: rows x fft_size inverse-transformed blocks
+    DevBuf<AcqRowStat> partial;
     float center2{0.f}, step2{0.f};
     uint32_t bins2{0};
-    AcqRowStat* rowstat{nullptr};
-    int* slot_list{nullptr};
-    void* best{nullptr};
-    float* second_peak{nullptr};
-    b200_acq_result* results_dev{nullptr};
-    b200_acq_result* results_pin{nullptr};
-    int* slot_pin{nullptr};
+    DevBuf<AcqRowStat> rowstat;
+    DevBuf<int> slot_list;
+    DevBuf<unsigned char> best;  // 8 bytes per slot
+    DevBuf<float> second_peak;
+    DevBuf<b200_acq_result> results_dev;
+    PinBuf<b200_acq_result> results_pin;
+    PinBuf<int> slot_pin;
     std::vector<char> slot_set;
     // asynchronous search (b200_acq_search_submit / _wait): one sweep in flight per object
-    float2* in_pin{nullptr};
-    cudaEvent_t done{nullptr};
+    PinBuf<float2> in_pin;
+    CudaEvent done;
     uint32_t pending_slots{0};
     bool pending{false};
     std::vector<int> slots_on_device;  // slot list last uploaded (sweeps usually repeat it)
@@ -65,21 +65,26 @@ struct b200_acq
     {
         int M{0};
         FftPlan plM{};
-        float2* twM{nullptr};
-        float2* chirp{nullptr};        // w[k] = exp(+j pi k^2 / N), k < N
-        float2* chirp_conj_M{nullptr}; // conj(w[k]) / M
-        float2* chirp_M{nullptr};      // w[k] / M
-        float2* chirp_conj{nullptr};   // conj(w[k])
-        float2* filt{nullptr};         // 2 x M: FFT_M(h), FFT_M(conj h), h = w extended symmetrically
-        float2* mult{nullptr};         // bins x N: wipe-off . conj(w)
-        float2* A{nullptr};            // bins x M spectra of the padded, chirped rows
-        float2* Zw{nullptr};           // bins x M inverse workspace
-        float2* Xs{nullptr};           // bins x N: DFT_N(signal . wipe-off)
-        float2* CW{nullptr};           // slots x N: conj(DFT_N(code)) . w / M
-        int* slot_ids{nullptr};        // device {0, 1}
-        AcqRowStat* partial{nullptr};
+        DevBuf<float2> twM;
+        DevBuf<float2> chirp;         // w[k] = exp(+j pi k^2 / N), k < N
+        DevBuf<float2> chirp_conj_M;  // conj(w[k]) / M
+        DevBuf<float2> chirp_M;       // w[k] / M
+        DevBuf<float2> chirp_conj;    // conj(w[k])
+        DevBuf<float2> filt;          // 2 x M: FFT_M(h), FFT_M(conj h), h = w extended symmetrically
+        DevBuf<float2> mult;          // bins x N: wipe-off . conj(w)
+        DevBuf<float2> A;             // bins x M spectra of the padded, chirped rows
+        DevBuf<float2> Zw;            // bins x M inverse workspace
+        DevBuf<float2> Xs;            // bins x N: DFT_N(signal . wipe-off)
+        DevBuf<float2> CW;            // slots x N: conj(DFT_N(code)) . w / M
+        DevBuf<int> slot_ids;         // device {0, 1}
+        DevBuf<AcqRowStat> partial;
     };
-    Bluestein* bl{nullptr};
+    std::unique_ptr<Bluestein> bl;
+
+    ~b200_acq()
+    {
+        if (stream) cudaStreamSynchronize(stream);
+    }
 };
 
 namespace
@@ -124,7 +129,7 @@ int search_impl(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32
             B200_CUDA_TRY(cudaStreamSynchronize(st));
             for (uint32_t i = 0; i < n_slots; i++) a->slot_pin[i] = static_cast<int>(slots[i]);
             B200_CUDA_TRY(cudaMemcpyAsync(a->slot_list, a->slot_pin, sizeof(int) * n_slots, cudaMemcpyHostToDevice, st));
-            a->slots_on_device.assign(a->slot_pin, a->slot_pin + n_slots);
+            a->slots_on_device.assign(a->slot_pin.get(), a->slot_pin.get() + n_slots);
         }
     const int n = static_cast<int>(c.fft_size);
     if (step_two && (a->bins2 == 0 || !a->wipe2 || n_slots != 1))
@@ -182,7 +187,7 @@ int bluestein_size(int n, FftPlan* pl)
 int bluestein_refresh_mult(b200_acq* a)
 {
     // mult[d][i] = wipe[d][i] * conj(w[i]): the wipe-off grid keeps the reference's float32 sincos values, the chirp is extra
-    b200_acq::Bluestein* b = a->bl;
+    b200_acq::Bluestein* b = a->bl.get();
     const int n = static_cast<int>(a->c.fft_size);
     return acq_launch_rows_times_vector(a->wipe, n, b->chirp_conj, n, 0, b->mult, n, static_cast<int>(a->c.num_doppler_bins), a->stream);
 }
@@ -202,9 +207,9 @@ int bluestein_setup_queue(b200_acq* a, std::vector<float2> (&host)[6])
 {
     const b200_acq_conf& c = a->c;
     const int n = static_cast<int>(c.fft_size);
-    auto* b = new (std::nothrow) b200_acq::Bluestein();
-    if (!b) return B200_ERR_NOMEM;
-    a->bl = b;
+    a->bl.reset(new (std::nothrow) b200_acq::Bluestein());
+    if (!a->bl) return B200_ERR_NOMEM;
+    b200_acq::Bluestein* b = a->bl.get();
     b->M = bluestein_size(n, &b->plM);
     if (b->M == 0)
         {
@@ -212,19 +217,19 @@ int bluestein_setup_queue(b200_acq* a, std::vector<float2> (&host)[6])
             return B200_ERR_RANGE;
         }
     const size_t M = static_cast<size_t>(b->M), bins = c.num_doppler_bins, slots = c.n_code_slots;
-    B200_CUDA_TRY(cudaMalloc(&b->twM, sizeof(float2) * M));
-    B200_CUDA_TRY(cudaMalloc(&b->chirp, sizeof(float2) * n));
-    B200_CUDA_TRY(cudaMalloc(&b->chirp_conj, sizeof(float2) * n));
-    B200_CUDA_TRY(cudaMalloc(&b->chirp_conj_M, sizeof(float2) * n));
-    B200_CUDA_TRY(cudaMalloc(&b->chirp_M, sizeof(float2) * n));
-    B200_CUDA_TRY(cudaMalloc(&b->filt, sizeof(float2) * 2 * M));
-    B200_CUDA_TRY(cudaMalloc(&b->mult, sizeof(float2) * bins * n));
-    B200_CUDA_TRY(cudaMalloc(&b->A, sizeof(float2) * bins * M));
-    B200_CUDA_TRY(cudaMalloc(&b->Zw, sizeof(float2) * bins * M));
-    B200_CUDA_TRY(cudaMalloc(&b->Xs, sizeof(float2) * bins * n));
-    B200_CUDA_TRY(cudaMalloc(&b->CW, sizeof(float2) * slots * n));
-    B200_CUDA_TRY(cudaMalloc(&b->slot_ids, sizeof(int) * 2));
-    B200_CUDA_TRY(cudaMalloc(&b->partial, sizeof(AcqRowStat) * bins * acq_final_chunks(b->plM)));
+    B200_CUDA_TRY(b->twM.alloc(M));
+    B200_CUDA_TRY(b->chirp.alloc(n));
+    B200_CUDA_TRY(b->chirp_conj.alloc(n));
+    B200_CUDA_TRY(b->chirp_conj_M.alloc(n));
+    B200_CUDA_TRY(b->chirp_M.alloc(n));
+    B200_CUDA_TRY(b->filt.alloc(2 * M));
+    B200_CUDA_TRY(b->mult.alloc(bins * n));
+    B200_CUDA_TRY(b->A.alloc(bins * M));
+    B200_CUDA_TRY(b->Zw.alloc(bins * M));
+    B200_CUDA_TRY(b->Xs.alloc(bins * n));
+    B200_CUDA_TRY(b->CW.alloc(slots * n));
+    B200_CUDA_TRY(b->slot_ids.alloc(2));
+    B200_CUDA_TRY(b->partial.alloc(bins * acq_final_chunks(b->plM)));
     // every copy below goes through a->stream: a synchronous cudaMemcpy from pageable memory may return before its DMA has
     // landed and is ordered only against the legacy default stream, which a->stream (non-blocking) does not wait for - the
     // filter kernels launched right after it read a half-written chirp (found on sizes with M > 32768)
@@ -272,31 +277,10 @@ int bluestein_setup_queue(b200_acq* a, std::vector<float2> (&host)[6])
     return rc;
 }
 
-void bluestein_free(b200_acq* a)
-{
-    b200_acq::Bluestein* b = a->bl;
-    if (!b) return;
-    cudaFree(b->twM);
-    cudaFree(b->chirp);
-    cudaFree(b->chirp_conj);
-    cudaFree(b->chirp_conj_M);
-    cudaFree(b->chirp_M);
-    cudaFree(b->filt);
-    cudaFree(b->mult);
-    cudaFree(b->A);
-    cudaFree(b->Zw);
-    cudaFree(b->Xs);
-    cudaFree(b->CW);
-    cudaFree(b->slot_ids);
-    cudaFree(b->partial);
-    delete b;
-    a->bl = nullptr;
-}
-
 // rows x N: out[r] = DFT_N(in[r * in_stride .. ] . mult[r * mult_stride ..])   (forward chirp-z, natural order)
 int bluestein_forward_rows(b200_acq* a, const float2* in, size_t in_stride, const float2* mult, size_t mult_stride, int rows, float2* out)
 {
-    b200_acq::Bluestein* b = a->bl;
+    b200_acq::Bluestein* b = a->bl.get();
     const int n = static_cast<int>(a->c.fft_size);
     int rc = acq_launch_fwd_rows(in, in_stride, n, mult, mult_stride, b->A, rows, b->plM, b->twM, a->stream);
     if (rc) return rc;
@@ -305,7 +289,7 @@ int bluestein_forward_rows(b200_acq* a, const float2* in, size_t in_stride, cons
 
 int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev)
 {
-    b200_acq::Bluestein* b = a->bl;
+    b200_acq::Bluestein* b = a->bl.get();
     const b200_acq_conf& c = a->c;
     const int n = static_cast<int>(c.fft_size);
     const int bins = static_cast<int>(c.num_doppler_bins);
@@ -376,52 +360,44 @@ extern "C"
                     }
             }
         B200_ENTER_DEVICE(e->device);
-        b200_acq* a = new (std::nothrow) b200_acq();
+        std::unique_ptr<b200_acq> a(new (std::nothrow) b200_acq());
         if (!a) return B200_ERR_NOMEM;
         a->e = e;
-        // every early return of the body below destroys the half-built object
-        rc = [&]() -> int {
         a->c = c;
         a->plan = pl;
         a->slot_set.assign(c.n_code_slots, 0);
         const size_t n = c.fft_size, bins = c.num_doppler_bins, slots = c.n_code_slots, ne = c.effective_fft_size;
-        if (e->own_stream)
-            {
-                // one private stream per acquisition object: blocks of different channels overlap
-                B200_CUDA_TRY(cudaStreamCreateWithFlags(&a->stream, cudaStreamNonBlocking));
-                a->own_stream = true;
-            }
+        if (e->stream.owned())
+            B200_CUDA_TRY(a->stream.create(cudaStreamNonBlocking));  // one private stream per acquisition object: blocks of different channels overlap
         else
-            {
-                a->stream = e->stream;  // caller-owned stream (e.g. for event timing on that stream)
-            }
-        B200_CUDA_TRY(cudaMalloc(&a->tw, sizeof(float2) * n));
-        B200_CUDA_TRY(cudaMalloc(&a->wipe, sizeof(float2) * n * bins));
-        B200_CUDA_TRY(cudaMalloc(&a->X, sizeof(float2) * n * bins));
-        B200_CUDA_TRY(cudaMalloc(&a->codes, sizeof(float2) * n * slots));
-        B200_CUDA_TRY(cudaMalloc(&a->in_dev, sizeof(float2) * n));
-        B200_CUDA_TRY(cudaMalloc(&a->code_stage, sizeof(float2) * n));
-        B200_CUDA_TRY(cudaMalloc(&a->rowstat, sizeof(AcqRowStat) * bins * slots));
-        B200_CUDA_TRY(cudaMalloc(&a->slot_list, sizeof(int) * slots));
-        B200_CUDA_TRY(cudaMalloc(&a->best, 8 * slots));
-        B200_CUDA_TRY(cudaMalloc(&a->second_peak, sizeof(float) * slots));
-        B200_CUDA_TRY(cudaMalloc(&a->results_dev, sizeof(b200_acq_result) * slots));
-        B200_CUDA_TRY(cudaMallocHost(&a->results_pin, sizeof(b200_acq_result) * slots));
-        B200_CUDA_TRY(cudaMallocHost(&a->slot_pin, sizeof(int) * slots));
+            a->stream.borrow(e->stream);  // caller-owned stream (e.g. for event timing on that stream)
+        B200_CUDA_TRY(a->tw.alloc(n));
+        B200_CUDA_TRY(a->wipe.alloc(n * bins));
+        B200_CUDA_TRY(a->X.alloc(n * bins));
+        B200_CUDA_TRY(a->codes.alloc(n * slots));
+        B200_CUDA_TRY(a->in_dev.alloc(n));
+        B200_CUDA_TRY(a->code_stage.alloc(n));
+        B200_CUDA_TRY(a->rowstat.alloc(bins * slots));
+        B200_CUDA_TRY(a->slot_list.alloc(slots));
+        B200_CUDA_TRY(a->best.alloc(8 * slots));
+        B200_CUDA_TRY(a->second_peak.alloc(slots));
+        B200_CUDA_TRY(a->results_dev.alloc(slots));
+        B200_CUDA_TRY(a->results_pin.alloc(slots));
+        B200_CUDA_TRY(a->slot_pin.alloc(slots));
         if (pl.n1 > 1)
             {
                 const size_t rows = bins * slots;
-                cudaError_t zerr = cudaMalloc(&a->Z, sizeof(float2) * n * rows);
+                cudaError_t zerr = a->Z.alloc(n * rows);
                 if (zerr != cudaSuccess)
                     {
                         set_error("two-level FFT workspace (%zu bytes): %s", sizeof(float2) * n * rows, cudaGetErrorString(zerr));
                         return B200_ERR_NOMEM;
                     }
-                B200_CUDA_TRY(cudaMalloc(&a->partial, sizeof(AcqRowStat) * rows * acq_final_chunks(pl)));
+                B200_CUDA_TRY(a->partial.alloc(rows * acq_final_chunks(pl)));
             }
         if (c.max_dwells > 1 || c.keep_grid)
             {
-                cudaError_t err = cudaMalloc(&a->grid, sizeof(float) * ne * bins * slots);
+                cudaError_t err = a->grid.alloc(ne * bins * slots);
                 if (err != cudaSuccess)
                     {
                         set_error("magnitude grid (%zu bytes): %s", sizeof(float) * ne * bins * slots, cudaGetErrorString(err));
@@ -429,31 +405,24 @@ extern "C"
                     }
                 B200_CUDA_TRY(cudaMemsetAsync(a->grid, 0, sizeof(float) * ne * bins * slots, a->stream));
             }
-        int r2 = B200_OK;
         if (use_bluestein)
             {
-                r2 = acq_launch_wipeoff(a->wipe, static_cast<int>(n), static_cast<int>(bins), c.doppler_max, 0, c.doppler_step, 0, c.fs_in, 0, 0.f, 0.f, a->stream);
-                if (r2) return r2;
-                r2 = bluestein_setup(a);
-                if (r2) return r2;
-                r2 = bluestein_refresh_mult(a);
-                if (r2) return r2;
-                B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-                return B200_OK;
+                rc = acq_launch_wipeoff(a->wipe, static_cast<int>(n), static_cast<int>(bins), c.doppler_max, 0, c.doppler_step, 0, c.fs_in, 0, 0.f, 0.f, a->stream);
+                if (rc) return rc;
+                rc = bluestein_setup(a.get());
+                if (rc) return rc;
+                rc = bluestein_refresh_mult(a.get());
+                if (rc) return rc;
             }
-        r2 = acq_launch_twiddles(a->tw, a->plan, a->stream);
-        if (r2) return r2;
-        r2 = acq_launch_wipeoff(a->wipe, static_cast<int>(n), static_cast<int>(bins), c.doppler_max, 0, c.doppler_step, 0, c.fs_in, 0, 0.f, 0.f, a->stream);
-        if (r2) return r2;
-        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-        return B200_OK;
-        }();
-        if (rc != B200_OK)
+        else
             {
-                b200_acq_destroy(a);
-                return rc;
+                rc = acq_launch_twiddles(a->tw, a->plan, a->stream);
+                if (rc) return rc;
+                rc = acq_launch_wipeoff(a->wipe, static_cast<int>(n), static_cast<int>(bins), c.doppler_max, 0, c.doppler_step, 0, c.fs_in, 0, 0.f, 0.f, a->stream);
+                if (rc) return rc;
             }
-        *out = a;
+        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
+        *out = a.release();
         return B200_OK;
     }
 
@@ -468,7 +437,7 @@ extern "C"
         if (a->bl)
             {
                 // CW = conj(DFT_N(code)) . w / M  (volk_32fc_conjugate_32fc of set_local_code :250, then the inverse chirp-z pre-multiplier)
-                b200_acq::Bluestein* b = a->bl;
+                b200_acq::Bluestein* b = a->bl.get();
                 const int n = static_cast<int>(c.fft_size);
                 int rcb = bluestein_forward_rows(a, a->code_stage, 0, b->chirp_conj, 0, 1, b->Xs);
                 if (rcb) return rcb;
@@ -514,8 +483,8 @@ extern "C"
                 return B200_ERR_STATE;
             }
         B200_ENTER_DEVICE(a->e->device);
-        if (!a->in_pin) B200_CUDA_TRY(cudaMallocHost(&a->in_pin, sizeof(float2) * a->c.fft_size));
-        if (!a->done) B200_CUDA_TRY(cudaEventCreateWithFlags(&a->done, cudaEventDisableTiming));
+        if (!a->in_pin) B200_CUDA_TRY(a->in_pin.alloc(a->c.fft_size));
+        if (!a->done) B200_CUDA_TRY(a->done.create(cudaEventDisableTiming));
         // the caller's buffer is free as soon as this returns: stage it in pinned memory so that the copy is truly asynchronous
         std::memcpy(a->in_pin, in_host, sizeof(float2) * a->c.consumed_samples);
         B200_CUDA_TRY(cudaMemcpyAsync(a->in_dev, a->in_pin, sizeof(float2) * a->c.consumed_samples, cudaMemcpyHostToDevice, a->stream));
@@ -558,8 +527,8 @@ extern "C"
     static int upload_i16(b200_acq* a, const int16_t* in_host_iq)
     {
         const size_t n = a->c.consumed_samples;
-        if (!a->in_pin) B200_CUDA_TRY(cudaMallocHost(&a->in_pin, sizeof(float2) * a->c.fft_size));
-        if (!a->raw_dev) B200_CUDA_TRY(cudaMalloc(&a->raw_dev, sizeof(short) * 2 * a->c.fft_size));
+        if (!a->in_pin) B200_CUDA_TRY(a->in_pin.alloc(a->c.fft_size));
+        if (!a->raw_dev) B200_CUDA_TRY(a->raw_dev.alloc(2 * a->c.fft_size));
         std::memcpy(a->in_pin, in_host_iq, sizeof(int16_t) * 2 * n);
         B200_CUDA_TRY(cudaMemcpyAsync(a->raw_dev, a->in_pin, sizeof(int16_t) * 2 * n, cudaMemcpyHostToDevice, a->stream));
         const int rc = launch_convert_i16(a->raw_dev, a->in_dev, ~0ULL, 0ULL, n, a->stream);
@@ -618,8 +587,7 @@ extern "C"
         if (!a->wipe2 || a->bins2 < num_doppler_bins_step2)
             {
                 B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-                if (a->wipe2) B200_CUDA_TRY(cudaFree(a->wipe2));
-                B200_CUDA_TRY(cudaMalloc(&a->wipe2, sizeof(float2) * a->c.fft_size * num_doppler_bins_step2));
+                B200_CUDA_TRY(a->wipe2.alloc(a->c.fft_size * num_doppler_bins_step2));
             }
         a->bins2 = num_doppler_bins_step2;
         a->center2 = doppler_center_step_two;
@@ -726,29 +694,6 @@ extern "C"
     {
         if (!a) return B200_ERR_ARG;
         cudaSetDevice(a->e->device);
-        if (a->stream) cudaStreamSynchronize(a->stream);
-        bluestein_free(a);
-        cudaFree(a->tw);
-        cudaFree(a->wipe);
-        cudaFree(a->wipe2);
-        cudaFree(a->Z);
-        cudaFree(a->partial);
-        cudaFree(a->X);
-        cudaFree(a->codes);
-        if (a->in_pin) cudaFreeHost(a->in_pin);
-        if (a->done) cudaEventDestroy(a->done);
-        cudaFree(a->in_dev);
-        cudaFree(a->raw_dev);
-        cudaFree(a->code_stage);
-        cudaFree(a->grid);
-        cudaFree(a->rowstat);
-        cudaFree(a->slot_list);
-        cudaFree(a->best);
-        cudaFree(a->second_peak);
-        cudaFree(a->results_dev);
-        if (a->results_pin) cudaFreeHost(a->results_pin);
-        if (a->slot_pin) cudaFreeHost(a->slot_pin);
-        if (a->stream && a->own_stream) cudaStreamDestroy(a->stream);
         delete a;
         return B200_OK;
     }

@@ -13,7 +13,9 @@
 #include "acq_fft.cuh"
 #include "engine.cuh"
 
+#include <memory>
 #include <new>
+#include <vector>
 
 namespace b200
 {
@@ -43,7 +45,7 @@ __global__ void acq_fine_modulate_kernel(const float2* __restrict__ code, int n1
 
 // frequency index of the value stored at position g of a forward spectrum (see FftPlan: two-level block order,
 // permuted storage of single-level plans, digit reversal of the in-shared-memory stages)
-__device__ int storage_to_freq(const FftPlan& pl, int g)
+__host__ __device__ int storage_to_freq(const FftPlan& pl, int g)
 {
     int blk = 0, p = g;
     if (pl.n1 > 1)
@@ -131,19 +133,20 @@ __global__ void __launch_bounds__(1024) acq_fine_argmax_kernel(const float2* __r
 
 struct b200_acq_fine
 {
+    CudaStream stream;  // own, or the engine's; declared first, so released after the buffers used on it
     b200_engine* e{nullptr};
-    cudaStream_t stream{nullptr};
-    bool own_stream{false};
     int n1ms{0};
     int m{0};
     FftPlan plan{};
-    float2* tw{nullptr};
-    float2* code_dev{nullptr};  // n1ms
-    float2* rows{nullptr};      // 8 x m modulated code replicas
-    float2* in_dev{nullptr};    // m
-    float2* X{nullptr};         // 8 x m
-    FineBest* best_dev{nullptr};
-    FineBest* best_pin{nullptr};
+    DevBuf<float2> tw;
+    DevBuf<float2> code_dev;  // n1ms
+    DevBuf<float2> rows;      // 8 x m modulated code replicas
+    DevBuf<float2> in_dev;    // m
+    DevBuf<float2> X;         // 8 x m
+    DevBuf<FineBest> best_dev;
+    PinBuf<FineBest> best_pin;
+
+    ~b200_acq_fine() { cudaStreamSynchronize(stream); }
 };
 
 extern "C"
@@ -152,15 +155,6 @@ extern "C"
     {
         if (!f) return B200_ERR_ARG;
         cudaSetDevice(f->e->device);
-        cudaStreamSynchronize(f->stream);
-        if (f->tw) cudaFree(f->tw);
-        if (f->code_dev) cudaFree(f->code_dev);
-        if (f->rows) cudaFree(f->rows);
-        if (f->in_dev) cudaFree(f->in_dev);
-        if (f->X) cudaFree(f->X);
-        if (f->best_dev) cudaFree(f->best_dev);
-        if (f->best_pin) cudaFreeHost(f->best_pin);
-        if (f->own_stream) cudaStreamDestroy(f->stream);
         delete f;
         return B200_OK;
     }
@@ -177,49 +171,33 @@ extern "C"
                 return B200_ERR_RANGE;
             }
         B200_ENTER_DEVICE(e->device);
-        b200_acq_fine* f = new (std::nothrow) b200_acq_fine();
+        std::unique_ptr<b200_acq_fine> f(new (std::nothrow) b200_acq_fine());
         if (!f) return B200_ERR_NOMEM;
         f->e = e;
         f->n1ms = static_cast<int>(fft_size);
         f->m = static_cast<int>(m);
         f->plan = pl;
-#define B200_FINE_TRY(expr)                                                                              \
-    do                                                                                                   \
-        {                                                                                                \
-            const cudaError_t _e = (expr);                                                               \
-            if (_e != cudaSuccess)                                                                       \
-                {                                                                                        \
-                    set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e));     \
-                    b200_acq_fine_destroy(f);                                                            \
-                    return _e == cudaErrorMemoryAllocation ? B200_ERR_NOMEM : B200_ERR_CUDA;             \
-                }                                                                                        \
-        }                                                                                                \
-    while (0)
-        if (e->own_stream)
-            {
-                B200_FINE_TRY(cudaStreamCreateWithFlags(&f->stream, cudaStreamNonBlocking));
-                f->own_stream = true;
-            }
+        cudaError_t err = cudaSuccess;
+        if (e->stream.owned())
+            err = f->stream.create(cudaStreamNonBlocking);
         else
+            f->stream.borrow(e->stream);
+        if (err == cudaSuccess) err = f->tw.alloc(m);
+        if (err == cudaSuccess) err = f->code_dev.alloc(fft_size);
+        if (err == cudaSuccess) err = f->rows.alloc(m * kZeroPadding);
+        if (err == cudaSuccess) err = f->in_dev.alloc(m);
+        if (err == cudaSuccess) err = f->X.alloc(m * kZeroPadding);
+        if (err == cudaSuccess) err = f->best_dev.alloc(1);
+        if (err == cudaSuccess) err = f->best_pin.alloc(1);
+        if (err != cudaSuccess)
             {
-                f->stream = e->stream;
+                set_error("fine Doppler buffers: %s", cudaGetErrorString(err));
+                return err == cudaErrorMemoryAllocation ? B200_ERR_NOMEM : B200_ERR_CUDA;
             }
-        B200_FINE_TRY(cudaMalloc(&f->tw, sizeof(float2) * m));
-        B200_FINE_TRY(cudaMalloc(&f->code_dev, sizeof(float2) * fft_size));
-        B200_FINE_TRY(cudaMalloc(&f->rows, sizeof(float2) * m * kZeroPadding));
-        B200_FINE_TRY(cudaMalloc(&f->in_dev, sizeof(float2) * m));
-        B200_FINE_TRY(cudaMalloc(&f->X, sizeof(float2) * m * kZeroPadding));
-        B200_FINE_TRY(cudaMalloc(&f->best_dev, sizeof(FineBest)));
-        B200_FINE_TRY(cudaMallocHost(&f->best_pin, sizeof(FineBest)));
-#undef B200_FINE_TRY
-        int rc = acq_launch_twiddles(f->tw, f->plan, f->stream);
-        if (rc)
-            {
-                b200_acq_fine_destroy(f);
-                return rc;
-            }
+        const int rc = acq_launch_twiddles(f->tw, f->plan, f->stream);
+        if (rc) return rc;
         B200_CUDA_TRY(cudaStreamSynchronize(f->stream));
-        *out = f;
+        *out = f.release();
         return B200_OK;
     }
 
@@ -260,30 +238,7 @@ extern "C"
         for (int s = 0; s < kZeroPadding; s++)
             for (int g = 0; g < f->m; g++)
                 {
-                    // host copy of storage_to_freq
-                    int blk = 0, p = g;
-                    if (pl.n1 > 1)
-                        {
-                            blk = g / pl.n;
-                            p = g - blk * pl.n;
-                        }
-                    else if (pl.perm_r > 1)
-                        {
-                            const int q = p / pl.perm_nb;
-                            const int b = p - q * pl.perm_nb;
-                            p = b * pl.perm_r + q;
-                        }
-                    int M = pl.n, mult = 1, r = 0;
-                    for (int st = 0; st < pl.n_stages; st++)
-                        {
-                            const int mm = M / pl.radix[st];
-                            const int q = p / mm;
-                            p -= q * mm;
-                            r += q * mult;
-                            mult *= pl.radix[st];
-                            M = mm;
-                        }
-                    const int freq = (pl.n1 > 1) ? blk + pl.n1 * r : r;
+                    const int freq = storage_to_freq(pl, g);
                     const float2 v = x[static_cast<size_t>(s) * f->m + g];
                     mag_host[static_cast<size_t>(kZeroPadding) * freq + s] = v.x * v.x + v.y * v.y;
                 }

@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <vector>
@@ -47,12 +48,7 @@ int upload_tables(b200_engine* e)
         }
     B200_CUDA_TRY(cudaMemcpyAsync(e->bands_dev, bd, sizeof(bd), cudaMemcpyHostToDevice, e->stream));
     const int n = static_cast<int>(e->chans.size());
-    if (n > e->chans_dev_cap)
-        {
-            if (e->chans_dev) B200_CUDA_TRY(cudaFree(e->chans_dev));
-            e->chans_dev_cap = n + 64;
-            B200_CUDA_TRY(cudaMalloc(&e->chans_dev, sizeof(ChanDesc) * e->chans_dev_cap));
-        }
+    B200_CUDA_TRY(e->chans_dev.grow(n, n + 64));
     e->max_code_len = 0;
     e->taps_uniform = -1;
     e->taps_mask = 0u;
@@ -85,20 +81,22 @@ int ensure_partials(b200_engine* e, int n_items, int slices)
 {
     if (slices <= 1) return B200_OK;
     const size_t need = trk_partial_elems(n_items, slices);
-    if (need > e->partial_cap)
+    B200_CUDA_TRY(e->partial.grow(need, need + need / 4));
+    if (!e->counters.fits(n_items))
         {
-            if (e->partial) B200_CUDA_TRY(cudaFree(e->partial));
-            e->partial_cap = need + need / 4;
-            B200_CUDA_TRY(cudaMalloc(&e->partial, sizeof(float2) * e->partial_cap));
-        }
-    if (n_items > e->counters_cap)
-        {
-            if (e->counters) B200_CUDA_TRY(cudaFree(e->counters));
-            e->counters_cap = n_items + n_items / 4 + 16;
-            B200_CUDA_TRY(cudaMalloc(&e->counters, sizeof(unsigned int) * e->counters_cap));
-            B200_CUDA_TRY(cudaMemsetAsync(e->counters, 0, sizeof(unsigned int) * e->counters_cap, e->stream));
+            B200_CUDA_TRY(e->counters.alloc(n_items + n_items / 4 + 16));
+            B200_CUDA_TRY(cudaMemsetAsync(e->counters, 0, sizeof(unsigned int) * e->counters.capacity(), e->stream));
         }
     return B200_OK;
+}
+
+// few items: split epochs into slices so the whole chip works on them
+int batch_slices(int n_items)
+{
+    int slices = 1;
+    if (n_items < 592) slices = (592 + n_items - 1) / n_items;
+    if (slices > 64) slices = 64;
+    return slices;
 }
 
 unsigned long long next_pow2(unsigned long long v)
@@ -152,32 +150,19 @@ extern "C"
                 return B200_ERR_NODEV;
             }
         B200_ENTER_DEVICE(device);
-        b200_engine* e = new (std::nothrow) b200_engine();
+        std::unique_ptr<b200_engine> e(new (std::nothrow) b200_engine());
         if (!e) return B200_ERR_NOMEM;
         e->device = device;
-        const int rc = [&]() -> int {
-            if (stream)
-                {
-                    e->stream = static_cast<cudaStream_t>(stream);
-                }
-            else
-                {
-                    B200_CUDA_TRY(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-                    e->own_stream = true;
-                }
-            B200_CUDA_TRY(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-            B200_CUDA_TRY(cudaEventCreateWithFlags(&e->copy_done, cudaEventDisableTiming));
-            B200_CUDA_TRY(cudaEventCreate(&e->t0));
-            B200_CUDA_TRY(cudaEventCreate(&e->t1));
-            B200_CUDA_TRY(cudaMalloc(&e->bands_dev, sizeof(BandDesc) * kMaxBands));
-            return B200_OK;
-        }();
-        if (rc != B200_OK)
-            {
-                b200_engine_destroy(e);  // tolerates a half-built engine
-                return rc;
-            }
-        *out = e;
+        if (stream)
+            e->stream.borrow(static_cast<cudaStream_t>(stream));
+        else
+            B200_CUDA_TRY(e->stream.create(cudaStreamNonBlocking));
+        B200_CUDA_TRY(e->copy_stream.create(cudaStreamNonBlocking));
+        B200_CUDA_TRY(e->copy_done.create(cudaEventDisableTiming));
+        B200_CUDA_TRY(e->t0.create(cudaEventDefault));
+        B200_CUDA_TRY(e->t1.create(cudaEventDefault));
+        B200_CUDA_TRY(e->bands_dev.alloc(kMaxBands));
+        *out = e.release();
         return B200_OK;
     }
 
@@ -185,42 +170,6 @@ extern "C"
     {
         if (!e) return B200_ERR_ARG;
         cudaSetDevice(e->device);
-        if (e->stream) cudaStreamSynchronize(e->stream);
-        if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
-        for (auto& b : e->bands)
-            {
-                if (b.dev) cudaFree(b.dev);
-                for (int k = 0; k < 2; k++)
-                    {
-                        if (b.raw_stage[k]) cudaFree(b.raw_stage[k]);
-                        if (b.raw_free[k]) cudaEventDestroy(b.raw_free[k]);
-                    }
-            }
-        for (auto& c : e->chans)
-            if (c.code_dev) cudaFree(c.code_dev);
-        if (e->bands_dev) cudaFree(e->bands_dev);
-        if (e->chans_dev) cudaFree(e->chans_dev);
-        if (e->items_dev) cudaFree(e->items_dev);
-        if (e->items_pin) cudaFreeHost(e->items_pin);
-        if (e->out_dev) cudaFree(e->out_dev);
-        if (e->out_pin) cudaFreeHost(e->out_pin);
-        if (e->partial) cudaFree(e->partial);
-        if (e->counters) cudaFree(e->counters);
-        loops_free(e);
-        for (auto& sl : e->slots)
-            {
-                if (sl.items_dev) cudaFree(sl.items_dev);
-                if (sl.items_pin) cudaFreeHost(sl.items_pin);
-                if (sl.out_dev) cudaFree(sl.out_dev);
-                if (sl.out_pin) cudaFreeHost(sl.out_pin);
-                if (sl.done) cudaEventDestroy(sl.done);
-                if (sl.items_ready) cudaEventDestroy(sl.items_ready);
-            }
-        if (e->copy_done) cudaEventDestroy(e->copy_done);
-        if (e->t0) cudaEventDestroy(e->t0);
-        if (e->t1) cudaEventDestroy(e->t1);
-        if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-        if (e->own_stream && e->stream) cudaStreamDestroy(e->stream);
         delete e;
         return B200_OK;
     }
@@ -266,14 +215,13 @@ extern "C"
         if (b.dev)
             {
                 B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
-                B200_CUDA_TRY(cudaFree(b.dev));
-                b.dev = nullptr;
+                B200_CUDA_TRY(b.dev.reset());
             }
         const unsigned long long cap = next_pow2(capacity_samples);
-        cudaError_t err = cudaMalloc(&b.dev, cap * sizeof(float2));
+        cudaError_t err = b.dev.alloc(cap);
         if (err != cudaSuccess)
             {
-                set_error("band %d: cudaMalloc(%llu samples): %s", band, cap, cudaGetErrorString(err));
+                set_error("band %d: device allocation of %llu samples: %s", band, cap, cudaGetErrorString(err));
                 return B200_ERR_NOMEM;
             }
         b.base = b.dev;
@@ -293,11 +241,7 @@ extern "C"
         if (!e || band < 0 || band >= kMaxBands || (!host && n)) return B200_ERR_ARG;
         std::lock_guard<std::mutex> lk(e->mu);
         Band& b = e->bands[band];
-        if (!b.in_use || b.attached || !b.dev)
-            {
-                set_error("band %d is not an owned ring (call b200_iq_create)", band);
-                return B200_ERR_STATE;
-            }
+        if (const int rc = b.check_owned_ring(band)) return rc;
         if (n > b.capacity)
             {
                 set_error("push of %llu samples exceeds ring capacity %llu", (unsigned long long)n, b.capacity);
@@ -324,11 +268,7 @@ extern "C"
         if (!e || band < 0 || band >= kMaxBands || (!host && n)) return B200_ERR_ARG;
         std::lock_guard<std::mutex> lk(e->mu);
         Band& b = e->bands[band];
-        if (!b.in_use || b.attached || !b.dev)
-            {
-                set_error("band %d is not an owned ring (call b200_iq_create)", band);
-                return B200_ERR_STATE;
-            }
+        if (const int rc = b.check_owned_ring(band)) return rc;
         if (n > b.capacity)
             {
                 set_error("push of %llu samples exceeds ring capacity %llu", (unsigned long long)n, b.capacity);
@@ -339,14 +279,12 @@ extern "C"
         const unsigned long long bytes = n * 2ULL * static_cast<unsigned long long>(bytes_per_component);
         const int k = b.raw_next;
         b.raw_next ^= 1;
-        if (!b.raw_free[k]) B200_CUDA_TRY(cudaEventCreateWithFlags(&b.raw_free[k], cudaEventDisableTiming));
-        if (bytes > b.raw_cap[k])
+        if (!b.raw_free[k]) B200_CUDA_TRY(b.raw_free[k].create(cudaEventDisableTiming));
+        if (!b.raw_stage[k].fits(bytes))
             {
                 B200_CUDA_TRY(cudaStreamSynchronize(e->copy_stream));
                 B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
-                if (b.raw_stage[k]) B200_CUDA_TRY(cudaFree(b.raw_stage[k]));
-                b.raw_cap[k] = bytes + bytes / 4 + 256;
-                B200_CUDA_TRY(cudaMalloc(&b.raw_stage[k], b.raw_cap[k]));
+                B200_CUDA_TRY(b.raw_stage[k].alloc(bytes + bytes / 4 + 256));
                 B200_CUDA_TRY(cudaEventRecord(b.raw_free[k], e->stream));
             }
         if (n)
@@ -359,8 +297,8 @@ extern "C"
                 B200_CUDA_TRY(cudaEventRecord(e->copy_done, e->copy_stream));
                 B200_CUDA_TRY(cudaStreamWaitEvent(e->stream, e->copy_done, 0));
                 int rc = (bytes_per_component == 2)
-                             ? launch_convert_i16(static_cast<const short*>(b.raw_stage[k]), b.dev, b.mask, b.write_index, n, e->stream)
-                             : launch_convert_i8(static_cast<const signed char*>(b.raw_stage[k]), b.dev, b.mask, b.write_index, n, e->stream);
+                             ? launch_convert_i16(reinterpret_cast<const short*>(b.raw_stage[k].get()), b.dev, b.mask, b.write_index, n, e->stream)
+                             : launch_convert_i8(reinterpret_cast<const signed char*>(b.raw_stage[k].get()), b.dev, b.mask, b.write_index, n, e->stream);
                 if (rc) return rc;
                 e->launches++;
                 B200_CUDA_TRY(cudaEventRecord(b.raw_free[k], e->stream));
@@ -380,14 +318,9 @@ extern "C"
         {
             std::lock_guard<std::mutex> lk(e->mu);
             Band& b = e->bands[band];
-            if (!b.in_use || b.attached || !b.dev)
-                {
-                    set_error("band %d is not an owned ring (call b200_iq_create)", band);
-                    return B200_ERR_STATE;
-                }
+            if (const int rc = b.check_owned_ring(band)) return rc;
             // what the ring holds right now
-            const unsigned long long oldest = b.write_index > b.capacity ? b.write_index - b.capacity : 0ULL;
-            const unsigned long long lo = b.valid_from > oldest ? b.valid_from : oldest;
+            const unsigned long long lo = std::max(b.valid_from, b.oldest());
             if (abs_index >= lo && abs_index + n <= b.write_index) return B200_OK;  // every sample of this block is already in the band
             if (abs_index > b.write_index || abs_index < lo)
                 {
@@ -421,8 +354,7 @@ extern "C"
         std::lock_guard<std::mutex> lk(e->mu);
         const Band& b = e->bands[band];
         if (!b.in_use) return B200_ERR_STATE;
-        const unsigned long long oldest = (!b.attached && b.write_index > b.capacity) ? b.write_index - b.capacity : b.first_index;
-        if (valid_from) *valid_from = b.valid_from > oldest ? b.valid_from : oldest;
+        if (valid_from) *valid_from = std::max(b.valid_from, b.oldest());
         if (write_index) *write_index = b.write_index;
         return B200_OK;
     }
@@ -458,11 +390,7 @@ extern "C"
         {
             std::lock_guard<std::mutex> lk(e->mu);
             const Band& b = e->bands[band];
-            if (!b.in_use || b.attached || !b.dev)
-                {
-                    set_error("band %d is not an owned ring (call b200_iq_create)", band);
-                    return B200_ERR_STATE;
-                }
+            if (const int rc = b.check_owned_ring(band)) return rc;
             capacity = b.capacity;
         }
         if (chunk_samples == 0) chunk_samples = 1ULL << 20;
@@ -483,13 +411,12 @@ extern "C"
                 return B200_ERR_RANGE;
             }
         // two pinned staging buffers: the disk read of block k+1 overlaps the host->device copy of block k
-        void* stage[2] = {nullptr, nullptr};
-        cudaEvent_t freed[2] = {nullptr, nullptr};
+        PinBuf<unsigned char> stage[2];
+        CudaEvent freed[2];
         int rc = B200_OK;
         for (int k = 0; k < 2 && rc == B200_OK; k++)
             {
-                if (cudaMallocHost(&stage[k], chunk_samples * sample_bytes) != cudaSuccess ||
-                    cudaEventCreateWithFlags(&freed[k], cudaEventDisableTiming) != cudaSuccess)
+                if (stage[k].alloc(chunk_samples * sample_bytes) != cudaSuccess || freed[k].create(cudaEventDisableTiming) != cudaSuccess)
                     {
                         set_error("iq_push_file: pinned staging allocation failed");
                         rc = B200_ERR_NOMEM;
@@ -510,11 +437,11 @@ extern "C"
                 if (got == 0) break;
                 uint64_t first = 0;
                 if (bytes_per_component == 4)
-                    rc = b200_iq_push(e, band, static_cast<const b200_cf32*>(stage[k]), got, &first);
+                    rc = b200_iq_push(e, band, reinterpret_cast<const b200_cf32*>(stage[k].get()), got, &first);
                 else if (bytes_per_component == 2)
-                    rc = b200_iq_push_i16(e, band, static_cast<const int16_t*>(stage[k]), got, &first);
+                    rc = b200_iq_push_i16(e, band, reinterpret_cast<const int16_t*>(stage[k].get()), got, &first);
                 else
-                    rc = b200_iq_push_i8(e, band, static_cast<const int8_t*>(stage[k]), got, &first);
+                    rc = b200_iq_push_i8(e, band, reinterpret_cast<const int8_t*>(stage[k].get()), got, &first);
                 if (rc != B200_OK) break;
                 if (cudaEventRecord(freed[k], e->copy_stream) != cudaSuccess) rc = B200_ERR_CUDA;
                 if (!have_first)
@@ -526,12 +453,7 @@ extern "C"
                 if (got < want) break;  // end of file
             }
         std::fclose(f);
-        cudaStreamSynchronize(e->copy_stream);
-        for (int k = 0; k < 2; k++)
-            {
-                if (stage[k]) cudaFreeHost(stage[k]);
-                if (freed[k]) cudaEventDestroy(freed[k]);
-            }
+        cudaStreamSynchronize(e->copy_stream);  // before the staging buffers are released
         if (samples_pushed) *samples_pushed = total;
         return rc;
     }
@@ -550,8 +472,7 @@ extern "C"
             {
                 B200_ENTER_DEVICE(e->device);
                 B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
-                B200_CUDA_TRY(cudaFree(b.dev));
-                b.dev = nullptr;
+                B200_CUDA_TRY(b.dev.reset());
             }
         b.base = reinterpret_cast<const float2*>(dev);
         b.capacity = n_samples;
@@ -613,7 +534,7 @@ extern "C"
         c.desc.code_len = 0;
         c.desc.high_dyn = 0;
         for (float& s : c.desc.shifts) s = 0.f;
-        e->chans.push_back(c);
+        e->chans.push_back(std::move(c));
         *channel_id = static_cast<int>(e->chans.size()) - 1;
         e->tables_dirty = true;
         return B200_OK;
@@ -627,12 +548,13 @@ extern "C"
         B200_ENTER_DEVICE(e->device);
         Channel& c = e->chans[channel_id];
         // a new table may be read by launches already queued: allocate fresh if it must grow
-        if (code_length_chips > c.code_cap)
+        if (!c.code_dev.fits(code_length_chips))
             {
                 B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
-                if (c.code_dev) B200_CUDA_TRY(cudaFree(c.code_dev));
-                c.code_cap = code_length_chips;
-                B200_CUDA_TRY(cudaMalloc(&c.code_dev, sizeof(float) * c.code_cap));
+                // the old table is released here: until the new one is in place the channel has none
+                c.desc.code = nullptr;
+                e->tables_dirty = true;
+                B200_CUDA_TRY(c.code_dev.alloc(code_length_chips));
             }
         B200_CUDA_TRY(cudaMemcpyAsync(c.code_dev, local_code_in, sizeof(float) * code_length_chips, cudaMemcpyHostToDevice, e->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(e->stream));  // caller's buffer may go away
@@ -742,11 +664,10 @@ extern "C"
                 if (b.in_use && !b.attached && items_host[i].n > 0)
                     {
                         const unsigned long long s0 = items_host[i].sample_index, s1 = s0 + static_cast<unsigned long long>(items_host[i].n);
-                        const unsigned long long oldest = b.write_index > b.capacity ? b.write_index - b.capacity : 0ULL;
-                        if (s0 < b.valid_from || s0 < oldest || s1 > b.write_index)
+                        const unsigned long long lo = std::max(b.valid_from, b.oldest());
+                        if (s0 < lo || s1 > b.write_index)
                             {
-                                set_error("item %d: samples [%llu, %llu) are outside the band's window [%llu, %llu)", i, s0, s1,
-                                    b.valid_from > oldest ? b.valid_from : oldest, b.write_index);
+                                set_error("item %d: samples [%llu, %llu) are outside the band's window [%llu, %llu)", i, s0, s1, lo, b.write_index);
                                 return B200_ERR_RANGE;
                             }
                     }
@@ -774,33 +695,13 @@ extern "C"
             }
         } guard{sl};
         sl->busy = true;
-        if (!sl->done) B200_CUDA_TRY(cudaEventCreateWithFlags(&sl->done, cudaEventDisableTiming));
-        if (!sl->items_ready) B200_CUDA_TRY(cudaEventCreateWithFlags(&sl->items_ready, cudaEventDisableTiming));
-        if (n_items > sl->items_cap)
-            {
-                if (sl->items_dev) B200_CUDA_TRY(cudaFree(sl->items_dev));
-                sl->items_dev = nullptr;
-                if (sl->items_pin) B200_CUDA_TRY(cudaFreeHost(sl->items_pin));
-                sl->items_pin = nullptr;
-                sl->items_cap = 0;
-                const int cap = n_items + n_items / 2 + 64;
-                B200_CUDA_TRY(cudaMalloc(&sl->items_dev, sizeof(b200_trk_item) * cap));
-                B200_CUDA_TRY(cudaMallocHost(&sl->items_pin, sizeof(b200_trk_item) * cap));
-                sl->items_cap = cap;
-            }
+        if (!sl->done) B200_CUDA_TRY(sl->done.create(cudaEventDisableTiming));
+        if (!sl->items_ready) B200_CUDA_TRY(sl->items_ready.create(cudaEventDisableTiming));
+        B200_CUDA_TRY(sl->items_dev.grow(n_items, n_items + n_items / 2 + 64));
+        B200_CUDA_TRY(sl->items_pin.grow(n_items, n_items + n_items / 2 + 64));
         const int out_elems = n_items * out_stride;
-        if (out_elems > sl->out_cap)
-            {
-                if (sl->out_dev) B200_CUDA_TRY(cudaFree(sl->out_dev));
-                sl->out_dev = nullptr;
-                if (sl->out_pin) B200_CUDA_TRY(cudaFreeHost(sl->out_pin));
-                sl->out_pin = nullptr;
-                sl->out_cap = 0;
-                const int cap = out_elems + out_elems / 2 + 64;
-                B200_CUDA_TRY(cudaMalloc(&sl->out_dev, sizeof(float2) * cap));
-                B200_CUDA_TRY(cudaMallocHost(&sl->out_pin, sizeof(float2) * cap));
-                sl->out_cap = cap;
-            }
+        B200_CUDA_TRY(sl->out_dev.grow(out_elems, out_elems + out_elems / 2 + 64));
+        B200_CUDA_TRY(sl->out_pin.grow(out_elems, out_elems + out_elems / 2 + 64));
         sl->n_items = n_items;
         sl->out_stride = out_stride;
         // The shared-window kernel serves items 8g..8g+7 from one copy of the samples, so items
@@ -821,10 +722,7 @@ extern "C"
                     [&](int a, int b) { return items_host[a].sample_index < items_host[b].sample_index; });
                 for (int i = 0; i < n_items; i++) sl->items_pin[i] = items_host[sl->perm[i]];
             }
-        // few items: split epochs into slices so the whole chip works on them
-        int slices = 1;
-        if (n_items < 592) slices = (592 + n_items - 1) / n_items;
-        if (slices > 64) slices = 64;
+        const int slices = batch_slices(n_items);
         // Latency path (a handful of channels waiting for their taps, e.g. the block threads behind the coalescer): the
         // kernel reads the work items straight from the pinned host buffer and writes the taps straight into pinned host
         // memory (unified addressing: cudaMallocHost memory is device-accessible at the same address), so the submission
@@ -832,7 +730,7 @@ extern "C"
         sl->zero_copy = n_items <= 1024;
         if (sl->zero_copy)
             {
-                const int rc = batch_dev_impl(e, sl->items_pin, n_items, reinterpret_cast<b200_cf32*>(sl->out_pin), out_stride, slices);
+                const int rc = batch_dev_impl(e, sl->items_pin, n_items, reinterpret_cast<b200_cf32*>(sl->out_pin.get()), out_stride, slices);
                 if (rc) return rc;
                 B200_CUDA_TRY(cudaEventRecord(sl->done, e->stream));
             }
@@ -861,7 +759,7 @@ extern "C"
                         sum_hull += hi - lo;
                     }
                 const int layout_hint = (sum_n > 2 * sum_hull) ? 1 : 0;
-                const int rc = batch_dev_impl(e, sl->items_dev, n_items, reinterpret_cast<b200_cf32*>(sl->out_dev), out_stride, slices, layout_hint);
+                const int rc = batch_dev_impl(e, sl->items_dev, n_items, reinterpret_cast<b200_cf32*>(sl->out_dev.get()), out_stride, slices, layout_hint);
                 if (rc) return rc;
                 B200_CUDA_TRY(cudaMemcpyAsync(sl->out_pin, sl->out_dev, sizeof(float2) * n_items * out_stride, cudaMemcpyDeviceToHost, e->stream));
                 B200_CUDA_TRY(cudaEventRecord(sl->done, e->stream));
@@ -917,14 +815,13 @@ extern "C"
 // ---- single correlator object (Cpu_Multicorrelator_Real_Codes shape) ----------------------------
 struct b200_trk
 {
+    CudaStream stream;  // declared first, so released after the buffers used on it
     b200_engine* e{nullptr};
     int max_len{0};
     int taps{0};
     int high_dyn{0};
-    cudaStream_t stream{nullptr};
-    float2* sig_dev{nullptr};
-    float* code_dev{nullptr};
-    int code_cap{0};
+    DevBuf<float2> sig_dev;
+    DevBuf<float> code_dev;
     // host-mapped control block: the kernel reads the item and descriptors and writes the taps
     // straight into pinned host memory (no D2H memcpy on the latency path)
     struct Ctl
@@ -934,20 +831,25 @@ struct b200_trk
         BandDesc band;
         float2 out[B200_MAX_TAPS];
     };
-    Ctl* ctl{nullptr};
-    float2* partial{nullptr};
-    unsigned int* counter{nullptr};
+    PinBuf<Ctl> ctl;
+    DevBuf<float2> partial;
+    DevBuf<unsigned int> counter;
     int slices_cap{0};
     bool have_code{false};
     // legacy variants (trk_variants.cu): complex local code / 16-bit samples and code
-    float2* cplx_code_dev{nullptr};
+    DevBuf<float2> cplx_code_dev;
     int cplx_code_len{0};
-    short* code16_dev{nullptr};
+    DevBuf<short> code16_dev;
     int code16_len{0};
-    short* sig16_dev{nullptr};
-    short* out16_dev{nullptr};
-    float2* out_cplx_dev{nullptr};
+    DevBuf<short> sig16_dev;
+    DevBuf<short> out16_dev;
+    DevBuf<float2> out_cplx_dev;
     float var_shifts[B200_MAX_TAPS] = {0};
+
+    ~b200_trk()
+    {
+        if (stream) cudaStreamSynchronize(stream);
+    }
 };
 
 extern "C"
@@ -961,28 +863,20 @@ extern "C"
                 return B200_ERR_RANGE;
             }
         B200_ENTER_DEVICE(e->device);
-        b200_trk* t = new (std::nothrow) b200_trk();
+        std::unique_ptr<b200_trk> t(new (std::nothrow) b200_trk());
         if (!t) return B200_ERR_NOMEM;
         t->e = e;
         t->max_len = max_signal_length_samples;
         t->taps = n_correlators;
-        const int rc = [&]() -> int {
-            B200_CUDA_TRY(cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking));
-            B200_CUDA_TRY(cudaMalloc(&t->sig_dev, sizeof(float2) * (static_cast<size_t>(t->max_len) + 2)));
-            B200_CUDA_TRY(cudaHostAlloc(&t->ctl, sizeof(b200_trk::Ctl), cudaHostAllocMapped));
-            std::memset(t->ctl, 0, sizeof(b200_trk::Ctl));
-            t->slices_cap = 64;
-            B200_CUDA_TRY(cudaMalloc(&t->partial, sizeof(float2) * trk_partial_elems(1, t->slices_cap)));
-            B200_CUDA_TRY(cudaMalloc(&t->counter, sizeof(unsigned int)));
-            B200_CUDA_TRY(cudaMemsetAsync(t->counter, 0, sizeof(unsigned int), t->stream));
-            return B200_OK;
-        }();
-        if (rc != B200_OK)
-            {
-                b200_trk_destroy(t);  // tolerates a half-built correlator
-                return rc;
-            }
-        *out = t;
+        B200_CUDA_TRY(t->stream.create(cudaStreamNonBlocking));
+        B200_CUDA_TRY(t->sig_dev.alloc(static_cast<size_t>(t->max_len) + 2));
+        B200_CUDA_TRY(t->ctl.alloc(1, cudaHostAllocMapped));
+        std::memset(t->ctl, 0, sizeof(b200_trk::Ctl));
+        t->slices_cap = 64;
+        B200_CUDA_TRY(t->partial.alloc(trk_partial_elems(1, t->slices_cap)));
+        B200_CUDA_TRY(t->counter.alloc(1));
+        B200_CUDA_TRY(cudaMemsetAsync(t->counter, 0, sizeof(unsigned int), t->stream));
+        *out = t.release();
         return B200_OK;
     }
 
@@ -998,11 +892,10 @@ extern "C"
         if (!t || !local_code_in || !shifts_chips || code_length_chips < 1) return B200_ERR_ARG;
         B200_ENTER_DEVICE(t->e->device);
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
-        if (code_length_chips > t->code_cap)
+        if (!t->code_dev.fits(code_length_chips))
             {
-                if (t->code_dev) B200_CUDA_TRY(cudaFree(t->code_dev));
-                t->code_cap = code_length_chips;
-                B200_CUDA_TRY(cudaMalloc(&t->code_dev, sizeof(float) * t->code_cap));
+                t->have_code = false;  // the old table is released here
+                B200_CUDA_TRY(t->code_dev.alloc(code_length_chips));
             }
         B200_CUDA_TRY(cudaMemcpyAsync(t->code_dev, local_code_in, sizeof(float) * code_length_chips, cudaMemcpyHostToDevice, t->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
@@ -1084,13 +977,9 @@ extern "C"
         if (!t || !local_code_in || !shifts_chips || code_length_chips < 1) return B200_ERR_ARG;
         B200_ENTER_DEVICE(t->e->device);
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
-        if (code_length_chips > t->cplx_code_len)
-            {
-                if (t->cplx_code_dev) B200_CUDA_TRY(cudaFree(t->cplx_code_dev));
-                t->cplx_code_dev = nullptr;
-                B200_CUDA_TRY(cudaMalloc(&t->cplx_code_dev, sizeof(float2) * code_length_chips));
-            }
-        if (!t->out_cplx_dev) B200_CUDA_TRY(cudaMalloc(&t->out_cplx_dev, sizeof(float2) * B200_MAX_TAPS));
+        // the code table last: b200_trk_correlate_cplx takes a code table to mean that the output buffer exists
+        if (!t->out_cplx_dev) B200_CUDA_TRY(t->out_cplx_dev.alloc(B200_MAX_TAPS));
+        if (code_length_chips > t->cplx_code_len) B200_CUDA_TRY(t->cplx_code_dev.alloc(code_length_chips));
         t->cplx_code_len = code_length_chips;
         B200_CUDA_TRY(cudaMemcpyAsync(t->cplx_code_dev, local_code_in, sizeof(float2) * code_length_chips, cudaMemcpyHostToDevice, t->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
@@ -1133,14 +1022,10 @@ extern "C"
         if (!t || !local_code_iq || !shifts_chips || code_length_chips < 1) return B200_ERR_ARG;
         B200_ENTER_DEVICE(t->e->device);
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
-        if (code_length_chips > t->code16_len)
-            {
-                if (t->code16_dev) B200_CUDA_TRY(cudaFree(t->code16_dev));
-                t->code16_dev = nullptr;
-                B200_CUDA_TRY(cudaMalloc(&t->code16_dev, sizeof(short) * 2 * code_length_chips));
-            }
-        if (!t->sig16_dev) B200_CUDA_TRY(cudaMalloc(&t->sig16_dev, sizeof(short) * 2 * (static_cast<size_t>(t->max_len) + 2)));
-        if (!t->out16_dev) B200_CUDA_TRY(cudaMalloc(&t->out16_dev, sizeof(short) * 2 * B200_MAX_TAPS));
+        // the code table last: b200_trk_correlate_16sc takes a code table to mean that all three buffers exist
+        if (!t->sig16_dev) B200_CUDA_TRY(t->sig16_dev.alloc(2 * (static_cast<size_t>(t->max_len) + 2)));
+        if (!t->out16_dev) B200_CUDA_TRY(t->out16_dev.alloc(2 * B200_MAX_TAPS));
+        if (code_length_chips > t->code16_len) B200_CUDA_TRY(t->code16_dev.alloc(2 * code_length_chips));
         t->code16_len = code_length_chips;
         B200_CUDA_TRY(cudaMemcpyAsync(t->code16_dev, local_code_iq, sizeof(short) * 2 * code_length_chips, cudaMemcpyHostToDevice, t->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
@@ -1181,18 +1066,6 @@ extern "C"
     {
         if (!t) return B200_ERR_ARG;
         cudaSetDevice(t->e->device);
-        if (t->stream) cudaStreamSynchronize(t->stream);
-        if (t->sig_dev) cudaFree(t->sig_dev);
-        if (t->code_dev) cudaFree(t->code_dev);
-        if (t->ctl) cudaFreeHost(t->ctl);
-        if (t->partial) cudaFree(t->partial);
-        if (t->counter) cudaFree(t->counter);
-        if (t->cplx_code_dev) cudaFree(t->cplx_code_dev);
-        if (t->code16_dev) cudaFree(t->code16_dev);
-        if (t->sig16_dev) cudaFree(t->sig16_dev);
-        if (t->out16_dev) cudaFree(t->out16_dev);
-        if (t->out_cplx_dev) cudaFree(t->out_cplx_dev);
-        if (t->stream) cudaStreamDestroy(t->stream);
         delete t;
         return B200_OK;
     }

@@ -2,6 +2,7 @@
 #pragma once
 
 #include "common.cuh"
+#include "cuda_owned.cuh"
 #include "loop.cuh"
 
 #include <mutex>
@@ -13,7 +14,7 @@ constexpr int kMaxBands = 16;
 
 struct Band
 {
-    float2* dev{nullptr};      // owned ring (nullptr when attached)
+    DevBuf<float2> dev;        // owned ring (empty when attached)
     const float2* base{nullptr};
     unsigned long long mask{0};
     unsigned long long first_index{0};
@@ -24,67 +25,63 @@ struct Band
     bool in_use{false};
     // device staging for integer sample pushes: two buffers, so that the next raw copy runs while the previous
     // block is being converted on the compute stream
-    void* raw_stage[2]{nullptr, nullptr};
-    unsigned long long raw_cap[2]{0, 0};  // bytes
-    cudaEvent_t raw_free[2]{nullptr, nullptr};  // conversion that read the buffer has finished
+    DevBuf<unsigned char> raw_stage[2];
+    CudaEvent raw_free[2];  // conversion that read the buffer has finished
     int raw_next{0};
+
+    // B200_OK, or B200_ERR_STATE with the error text when this is not a ring made by b200_iq_create
+    int check_owned_ring(int band) const
+    {
+        if (in_use && !attached && dev) return B200_OK;
+        set_error("band %d is not an owned ring (call b200_iq_create)", band);
+        return B200_ERR_STATE;
+    }
+    // oldest absolute index still held: an owned ring (first_index 0) keeps the last `capacity` samples pushed
+    unsigned long long oldest() const { return (!attached && write_index > capacity) ? write_index - capacity : first_index; }
 };
 
 struct Channel
 {
-    float* code_dev{nullptr};
-    int code_cap{0};
+    DevBuf<float> code_dev;
     ChanDesc desc{};
 };
 }  // namespace b200
 
 struct b200_engine
 {
+    // declared first, so released last: every buffer and event below was used on these streams
+    b200::CudaStream stream;  // the caller's (borrowed) or the engine's own
+    b200::CudaStream copy_stream;
     int device{0};
-    cudaStream_t stream{nullptr};
-    bool own_stream{false};
-    cudaStream_t copy_stream{nullptr};
-    cudaEvent_t copy_done{nullptr};
-    cudaEvent_t t0{nullptr}, t1{nullptr};
+    b200::CudaEvent copy_done;
+    b200::CudaEvent t0, t1;
     std::mutex mu;
     std::mutex push_mu[b200::kMaxBands];  // serialises competing producers of one band (b200_iq_push_at)
     b200::Band bands[b200::kMaxBands];
     std::vector<b200::Channel> chans;
     // device mirrors
-    b200::BandDesc* bands_dev{nullptr};
-    b200::ChanDesc* chans_dev{nullptr};
-    int chans_dev_cap{0};
+    b200::DevBuf<b200::BandDesc> bands_dev;
+    b200::DevBuf<b200::ChanDesc> chans_dev;
     bool tables_dirty{true};
     int max_code_len{0};
     int taps_uniform{-1};
     unsigned int taps_mask{0};   // bit t set: some channel with a code table has t taps (mixed batches run one launch per tap count)
     bool any_high_dyn{false};
     int shared_mode{-1};   // -1 auto, 0 never, 1 always-when-legal (env B200_TRK_SHARED)
-    // batch staging
-    b200_trk_item* items_dev{nullptr};
-    b200_trk_item* items_pin{nullptr};
-    float2* out_dev{nullptr};
-    float2* out_pin{nullptr};
-    int batch_cap{0};
-    int out_cap{0};
-    float2* partial{nullptr};
-    unsigned int* counters{nullptr};
-    size_t partial_cap{0};
-    int counters_cap{0};
+    b200::DevBuf<float2> partial;
+    b200::DevBuf<unsigned int> counters;
     uint64_t launches{0};
     // asynchronous batches (b200_trk_submit / b200_trk_wait)
     struct Slot
     {
-        b200_trk_item* items_pin{nullptr};
-        b200_trk_item* items_dev{nullptr};
-        float2* out_dev{nullptr};
-        float2* out_pin{nullptr};
-        int items_cap{0};
-        int out_cap{0};
+        b200::PinBuf<b200_trk_item> items_pin;
+        b200::DevBuf<b200_trk_item> items_dev;
+        b200::DevBuf<float2> out_dev;
+        b200::PinBuf<float2> out_pin;
         int n_items{0};
         int out_stride{0};
-        cudaEvent_t done{nullptr};
-        cudaEvent_t items_ready{nullptr};  // work items have arrived (copy stream)
+        b200::CudaEvent done;
+        b200::CudaEvent items_ready;  // work items have arrived (copy stream)
         bool busy{false};
         bool zero_copy{false};  // items read from / taps written to the pinned host buffers directly (small batches)
         uint64_t ticket{0};
@@ -95,14 +92,18 @@ struct b200_engine
     uint64_t next_ticket{1};
     // free-running DLL/PLL loops (loop_engine.cu)
     std::vector<b200::LoopDev> loops;  // host mirror: configuration and start-of-tracking state
-    b200::LoopDev* loops_dev{nullptr};
-    int loops_dev_cap{0};
-    b200_trk_item* loop_items_dev{nullptr};
-    float2* loop_taps_dev{nullptr};
-    int* loop_nrec_dev{nullptr};
-    unsigned int* loop_rec_dev{nullptr};
-    size_t loop_rec_cap{0};  // 32-bit words
+    b200::DevBuf<b200::LoopDev> loops_dev;
+    b200::DevBuf<b200_trk_item> loop_items_dev;
+    b200::DevBuf<float2> loop_taps_dev;
+    b200::DevBuf<int> loop_nrec_dev;
+    b200::DevBuf<unsigned int> loop_rec_dev;
     int loop_mode{-1};       // 0 persistent kernel (default), 1 one launch pair per epoch with slices = 1, 2 same with automatic slices
+
+    ~b200_engine()
+    {
+        if (stream) cudaStreamSynchronize(stream);
+        if (copy_stream) cudaStreamSynchronize(copy_stream);
+    }
 };
 
 namespace b200
@@ -110,6 +111,5 @@ namespace b200
 // engine.cu
 int upload_tables(b200_engine* e);
 int ensure_partials(b200_engine* e, int n_items, int slices);
-void loops_free(b200_engine* e);  // loop_engine.cu
+int batch_slices(int n_items);
 }  // namespace b200
-

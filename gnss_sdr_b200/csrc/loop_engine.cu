@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <utility>
 #include <vector>
 
 using namespace b200;
@@ -110,37 +111,29 @@ void smoother_init(LoopSmoother& s, float alpha, float min_value, float offset, 
 int ensure_loop_buffers(b200_engine* e, int rec_capacity)
 {
     const int n = static_cast<int>(e->loops.size());
-    if (n > e->loops_dev_cap)
+    if (!e->loops_dev.fits(n))
         {
+            // the loop states are kept; loops_dev is replaced last, so after a failure its capacity still asks for all four
             const int cap = n + 32;
-            LoopDev* nd = nullptr;
-            B200_CUDA_TRY(cudaMalloc(&nd, sizeof(LoopDev) * cap));
+            DevBuf<LoopDev> nd;
+            B200_CUDA_TRY(nd.alloc(cap));
             B200_CUDA_TRY(cudaMemsetAsync(nd, 0, sizeof(LoopDev) * cap, e->stream));
-            if (e->loops_dev && e->loops_dev_cap > 0)
-                B200_CUDA_TRY(cudaMemcpyAsync(nd, e->loops_dev, sizeof(LoopDev) * e->loops_dev_cap, cudaMemcpyDeviceToDevice, e->stream));
+            if (e->loops_dev)
+                B200_CUDA_TRY(cudaMemcpyAsync(nd, e->loops_dev, sizeof(LoopDev) * e->loops_dev.capacity(), cudaMemcpyDeviceToDevice, e->stream));
             B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
-            if (e->loops_dev) B200_CUDA_TRY(cudaFree(e->loops_dev));
-            if (e->loop_items_dev) B200_CUDA_TRY(cudaFree(e->loop_items_dev));
-            if (e->loop_taps_dev) B200_CUDA_TRY(cudaFree(e->loop_taps_dev));
-            if (e->loop_nrec_dev) B200_CUDA_TRY(cudaFree(e->loop_nrec_dev));
-            e->loops_dev = nd;
-            e->loops_dev_cap = cap;
-            B200_CUDA_TRY(cudaMalloc(&e->loop_items_dev, sizeof(b200_trk_item) * cap));
-            B200_CUDA_TRY(cudaMalloc(&e->loop_taps_dev, sizeof(float2) * kLoopTapStride * cap));
-            B200_CUDA_TRY(cudaMalloc(&e->loop_nrec_dev, sizeof(int) * cap));
+            B200_CUDA_TRY(e->loop_items_dev.alloc(cap));
+            B200_CUDA_TRY(e->loop_taps_dev.alloc(kLoopTapStride * cap));
+            B200_CUDA_TRY(e->loop_nrec_dev.alloc(cap));
             B200_CUDA_TRY(cudaMemsetAsync(e->loop_items_dev, 0, sizeof(b200_trk_item) * cap, e->stream));
             B200_CUDA_TRY(cudaMemsetAsync(e->loop_taps_dev, 0, sizeof(float2) * kLoopTapStride * cap, e->stream));
+            e->loops_dev = std::move(nd);
         }
     const size_t words = static_cast<size_t>(n) * static_cast<size_t>(rec_capacity > 0 ? rec_capacity : 1) * kLoopRecordWords;
-    if (words > e->loop_rec_cap)
-        {
-            if (e->loop_rec_dev) B200_CUDA_TRY(cudaFree(e->loop_rec_dev));
-            e->loop_rec_cap = words + words / 4;
-            B200_CUDA_TRY(cudaMalloc(&e->loop_rec_dev, sizeof(unsigned int) * e->loop_rec_cap));
-        }
+    B200_CUDA_TRY(e->loop_rec_dev.grow(words, words + words / 4));
     return B200_OK;
 }
 
+// what the bands hold right now; unlike the push and submit checks, the window ignores valid_from
 LoopAvail snapshot_avail(const b200_engine* e)
 {
     LoopAvail a{};
@@ -148,26 +141,10 @@ LoopAvail snapshot_avail(const b200_engine* e)
         {
             const Band& b = e->bands[i];
             if (!b.in_use) continue;
-            if (b.attached)
-                {
-                    a.lo[i] = b.first_index;
-                    a.hi[i] = b.first_index + b.capacity;
-                }
-            else
-                {
-                    a.hi[i] = b.write_index;
-                    a.lo[i] = (b.write_index - b.first_index > b.capacity) ? b.write_index - b.capacity : b.first_index;
-                }
+            a.lo[i] = b.oldest();
+            a.hi[i] = b.attached ? b.first_index + b.capacity : b.write_index;
         }
     return a;
-}
-
-int batch_slices(int n_items)
-{
-    int slices = 1;
-    if (n_items < 592) slices = (592 + n_items - 1) / n_items;
-    if (slices > 64) slices = 64;
-    return slices;
 }
 
 int correlate_loop_items(b200_engine* e, int n, int slices)
@@ -178,18 +155,6 @@ int correlate_loop_items(b200_engine* e, int n, int slices)
     return rc;
 }
 }  // namespace
-
-namespace b200
-{
-void loops_free(b200_engine* e)
-{
-    if (e->loops_dev) cudaFree(e->loops_dev);
-    if (e->loop_items_dev) cudaFree(e->loop_items_dev);
-    if (e->loop_taps_dev) cudaFree(e->loop_taps_dev);
-    if (e->loop_nrec_dev) cudaFree(e->loop_nrec_dev);
-    if (e->loop_rec_dev) cudaFree(e->loop_rec_dev);
-}
-}  // namespace b200
 
 extern "C"
 {
