@@ -72,6 +72,7 @@ struct b200_acq
         DevBuf<float2> chirp_conj;    // conj(w[k])
         DevBuf<float2> filt;          // 2 x M: FFT_M(h), FFT_M(conj h), h = w extended symmetrically
         DevBuf<float2> mult;          // bins x N: wipe-off . conj(w)
+        DevBuf<float2> mult2;         // bins2 x N: step-two wipe-off . conj(w)
         DevBuf<float2> A;             // bins x M spectra of the padded, chirped rows
         DevBuf<float2> Zw;            // bins x M inverse workspace
         DevBuf<float2> Xs;            // bins x N: DFT_N(signal . wipe-off)
@@ -89,7 +90,8 @@ struct b200_acq
 
 namespace
 {
-int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev);
+int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev,
+    int step_two, float prev_input_power);
 
 int search_impl(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
     b200_acq_result* results_dev, int step_two = 0, float prev_input_power = 0.f)
@@ -113,12 +115,12 @@ int search_impl(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32
         }
     if (a->bl)
         {
-            if (step_two)
+            if (step_two && (a->bins2 == 0 || !a->bl->mult2 || n_slots != 1))
                 {
-                    set_error("two-step acquisition is not available for chirp-z transform sizes");
+                    set_error("step two needs b200_acq_set_step_two first and exactly one slot");
                     return B200_ERR_STATE;
                 }
-            return bluestein_search(a, in_dev, slots, n_slots, dwell_counter, results_dev);
+            return bluestein_search(a, in_dev, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power);
         }
     cudaStream_t st = a->stream;
     bool same = a->slots_on_device.size() == n_slots;
@@ -277,24 +279,30 @@ int bluestein_setup_queue(b200_acq* a, std::vector<float2> (&host)[6])
     return rc;
 }
 
-// rows x N: out[r] = DFT_N(in[r * in_stride .. ] . mult[r * mult_stride ..])   (forward chirp-z, natural order)
-int bluestein_forward_rows(b200_acq* a, const float2* in, size_t in_stride, const float2* mult, size_t mult_stride, int rows, float2* out)
+// rows x N: out[r] = DFT_N(in[r * in_stride .. ] . mult[r * mult_stride ..])   (forward chirp-z, natural order); inputs past
+// `consumed` count as zeros (acquisition_core zero-pads the consumed samples to fft_size, :657-664)
+int bluestein_forward_rows(b200_acq* a, const float2* in, size_t in_stride, int consumed, const float2* mult, size_t mult_stride, int rows,
+    float2* out)
 {
     b200_acq::Bluestein* b = a->bl.get();
     const int n = static_cast<int>(a->c.fft_size);
-    int rc = acq_launch_fwd_rows(in, in_stride, n, mult, mult_stride, b->A, rows, b->plM, b->twM, a->stream);
+    int rc = acq_launch_fwd_rows(in, in_stride, consumed, mult, mult_stride, b->A, rows, b->plM, b->twM, a->stream);
     if (rc) return rc;
     return acq_launch_inverse_store_rows(b->A, b->filt, b->slot_ids, rows, b->plM, b->twM, b->Zw, b->chirp_conj_M, n, out, n, a->stream);
 }
 
-int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev)
+int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev,
+    int step_two, float prev_input_power)
 {
     b200_acq::Bluestein* b = a->bl.get();
     const b200_acq_conf& c = a->c;
     const int n = static_cast<int>(c.fft_size);
-    const int bins = static_cast<int>(c.num_doppler_bins);
-    // X_d = DFT_N(x . wipe_d) for every Doppler bin, once per sweep
-    int rc = bluestein_forward_rows(a, in_dev, 0, b->mult, n, bins, b->Xs);
+    const int bins = step_two ? static_cast<int>(a->bins2) : static_cast<int>(c.num_doppler_bins);
+    const float2* mult = step_two ? b->mult2 : b->mult;
+    const int ne = static_cast<int>(c.effective_fft_size);
+    const int off = c.bit_transition_flag ? ne : 0;
+    // X_d = DFT_N(x . wipe_d) for every Doppler bin, once per sweep (x: the consumed samples, zero-padded to N)
+    int rc = bluestein_forward_rows(a, in_dev, 0, static_cast<int>(c.consumed_samples), mult, n, bins, b->Xs);
     if (rc) return rc;
     uint64_t launched = 4;
     for (uint32_t i = 0; i < n_slots; i++)
@@ -302,15 +310,16 @@ int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, u
             // rows of this PRN: y = IDFT_N(X_d . C) = w . IFFT_M(FFT_M(pad(X_d . C . w)) . FFT_M(conj h)) / M ; |w| = 1
             rc = acq_launch_fwd_rows(b->Xs, n, n, b->CW + static_cast<size_t>(slots[i]) * n, 0, b->A, bins, b->plM, b->twM, a->stream);
             if (rc) return rc;
-            // the correlation kernel addresses the grid by code-slot id, and the "code" here is filter slot 1
-            float* grid = a->grid ? a->grid + (static_cast<ptrdiff_t>(slots[i]) - 1) * static_cast<ptrdiff_t>(bins) * n : nullptr;
-            rc = acq_launch_corr(b->A, b->filt, b->slot_ids + 1, 1, bins, b->plM, b->twM, 0, n, a->rowstat + static_cast<size_t>(i) * bins, grid,
+            // the correlation kernel addresses the grid by code-slot id, and the "code" here is filter slot 1; the grid rows are
+            // [off, off + ne) of y, so slot s lands where the mixed-radix search puts it: (s * bins + bin) * ne
+            float* grid = a->grid ? a->grid + (static_cast<ptrdiff_t>(slots[i]) - 1) * static_cast<ptrdiff_t>(bins) * ne : nullptr;
+            rc = acq_launch_corr(b->A, b->filt, b->slot_ids + 1, 1, bins, b->plM, b->twM, off, ne, a->rowstat + static_cast<size_t>(i) * bins, grid,
                 dwell_counter > 1 ? 1 : 0, 0, nullptr, 0, nullptr, b->Zw, b->partial, a->stream);
             if (rc) return rc;
             launched += 5;
         }
-    rc = acq_launch_stats(a->rowstat, static_cast<int>(n_slots), bins, n, c.doppler_max, a->doppler_center, c.doppler_step, dwell_counter, c.use_cfar,
-        a->best, results_dev, 0, 0.f, 0.f, 0.f, a->stream);
+    rc = acq_launch_stats(a->rowstat, static_cast<int>(n_slots), bins, ne, c.doppler_max, a->doppler_center, c.doppler_step, dwell_counter, c.use_cfar,
+        a->best, results_dev, step_two, a->center2, a->step2, prev_input_power, a->stream);
     if (rc) return rc;
     {
         std::lock_guard<std::mutex> lk(a->e->mu);
@@ -340,10 +349,9 @@ extern "C"
         if (rc)
             {
                 // sizes with prime factors > 7 (16 368 = 16.368 Msps x 1 ms, a standard front-end rate): chirp-z through M-point
-                // transforms; plain layout and the CFAR statistic only
+                // transforms, every code layout; the CFAR statistic only, and N <= 5 x 27 648 (M <= 10 x 27 648, two-level plan)
                 FftPlan probe{};
-                if (c.code_layout == 0 && !c.bit_transition_flag && c.effective_fft_size == c.fft_size && c.consumed_samples == c.fft_size &&
-                    c.use_cfar && bluestein_size(static_cast<int>(c.fft_size), &probe) != 0)
+                if (c.use_cfar && bluestein_size(static_cast<int>(c.fft_size), &probe) != 0)
                     {
                         use_bluestein = true;
                         pl = FftPlan{};
@@ -354,7 +362,7 @@ extern "C"
                 else
                     {
                         set_error("fft_size %u unsupported: prime factors must be 2,3,5,7 and fft_size <= 10 x %d (sizes with larger prime "
-                                  "factors are supported up to %d points for the plain layout with the CFAR statistic)",
+                                  "factors need use_cfar = 1 and fft_size <= %d)",
                             c.fft_size, kAcqMaxSmemPoints, 5 * kAcqMaxSmemPoints);
                         return rc;
                     }
@@ -433,13 +441,17 @@ extern "C"
         B200_ENTER_DEVICE(a->e->device);
         const b200_acq_conf& c = a->c;
         const size_t need = (c.code_layout == 1) ? c.fft_size / 2 : c.consumed_samples;
-        B200_CUDA_TRY(cudaMemcpyAsync(a->code_stage, code_host, sizeof(float2) * need, cudaMemcpyHostToDevice, a->stream));
         if (a->bl)
             {
-                // CW = conj(DFT_N(code)) . w / M  (volk_32fc_conjugate_32fc of set_local_code :250, then the inverse chirp-z pre-multiplier)
+                // the code staged in an N-point buffer where set_local_code places it (:230-246): layout 0 at the front, layout 1 in
+                // the second half, layout 2 at the end, zeros elsewhere
                 b200_acq::Bluestein* b = a->bl.get();
                 const int n = static_cast<int>(c.fft_size);
-                int rcb = bluestein_forward_rows(a, a->code_stage, 0, b->chirp_conj, 0, 1, b->Xs);
+                const size_t place = (c.code_layout == 1) ? c.fft_size / 2 : (c.code_layout == 2) ? c.fft_size - c.consumed_samples : 0;
+                if (need < c.fft_size) B200_CUDA_TRY(cudaMemsetAsync(a->code_stage, 0, sizeof(float2) * c.fft_size, a->stream));
+                B200_CUDA_TRY(cudaMemcpyAsync(a->code_stage + place, code_host, sizeof(float2) * need, cudaMemcpyHostToDevice, a->stream));
+                // CW = conj(DFT_N(code)) . w / M  (volk_32fc_conjugate_32fc of set_local_code :250, then the inverse chirp-z pre-multiplier)
+                int rcb = bluestein_forward_rows(a, a->code_stage, 0, n, b->chirp_conj, 0, 1, b->Xs);
                 if (rcb) return rcb;
                 rcb = acq_launch_rows_times_vector(b->Xs, n, b->chirp_M, n, 1, b->CW + static_cast<size_t>(slot) * n, n, 1, a->stream);
                 if (rcb) return rcb;
@@ -447,6 +459,7 @@ extern "C"
                 a->slot_set[slot] = 1;
                 return B200_OK;
             }
+        B200_CUDA_TRY(cudaMemcpyAsync(a->code_stage, code_host, sizeof(float2) * need, cudaMemcpyHostToDevice, a->stream));
         int rc = acq_launch_code_fft(a->code_stage, static_cast<int>(c.consumed_samples), static_cast<int>(c.code_layout),
             a->codes + static_cast<size_t>(slot) * c.fft_size, a->plan, a->tw, a->stream);
         if (rc) return rc;
@@ -589,12 +602,24 @@ extern "C"
                 B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
                 B200_CUDA_TRY(a->wipe2.alloc(a->c.fft_size * num_doppler_bins_step2));
             }
+        if (a->bl && !a->bl->mult2.fits(a->c.fft_size * num_doppler_bins_step2))
+            {
+                B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
+                B200_CUDA_TRY(a->bl->mult2.alloc(a->c.fft_size * num_doppler_bins_step2));
+            }
         a->bins2 = num_doppler_bins_step2;
         a->center2 = doppler_center_step_two;
         a->step2 = doppler_step2;
         int rc = acq_launch_wipeoff(a->wipe2, static_cast<int>(a->c.fft_size), static_cast<int>(a->bins2), 0, 0, 0, a->doppler_bias, a->c.fs_in, 1,
             doppler_center_step_two, doppler_step2, a->stream);
         if (rc) return rc;
+        if (a->bl)
+            {
+                // chirped step-two rows, as bluestein_refresh_mult builds the step-one rows
+                const int n = static_cast<int>(a->c.fft_size);
+                rc = acq_launch_rows_times_vector(a->wipe2, n, a->bl->chirp_conj, n, 0, a->bl->mult2, n, static_cast<int>(a->bins2), a->stream);
+                if (rc) return rc;
+            }
         B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
         return B200_OK;
     }
@@ -647,7 +672,7 @@ extern "C"
         B200_ENTER_DEVICE(a->e->device);
         const size_t n = a->c.fft_size;
         B200_CUDA_TRY(cudaMemcpyAsync(a->code_stage, in_host, sizeof(float2) * n, cudaMemcpyHostToDevice, a->stream));
-        const int rc = bluestein_forward_rows(a, a->code_stage, 0, a->bl->chirp_conj, 0, 1, a->bl->Xs);
+        const int rc = bluestein_forward_rows(a, a->code_stage, 0, static_cast<int>(n), a->bl->chirp_conj, 0, 1, a->bl->Xs);
         if (rc) return rc;
         B200_CUDA_TRY(cudaMemcpyAsync(out_host, a->bl->Xs, sizeof(float2) * n, cudaMemcpyDeviceToHost, a->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(a->stream));

@@ -357,9 +357,10 @@ extern "C"
 
     /* pcps_acquisition::pcps_acquisition(conf)  (:100-193): plan, buffers, wipe-off grid for center 0.
      * fft_size: prime factors 2, 3, 5, 7 up to 10 x 27 648 points run on the mixed-radix plans (in shared memory up to 27 648,
-     * two-level beyond).  Any other size up to 5 x 27 648 (16 368 points = 16.368 Msps x 1 ms, ...) runs through chirp-z
-     * (Bluestein) on the same kernels, for code_layout 0 with use_cfar = 1 (dwells, keep_grid, assisted Doppler centre
-     * included); everything else is B200_ERR_RANGE with the reason in b200_last_error(). */
+     * two-level beyond).  Any other size (16 368 points = 16.368 Msps x 1 ms, ...) runs through chirp-z (Bluestein) on the
+     * same kernels, with every code layout, bit_transition_flag, consumed_samples < fft_size, dwells, keep_grid, the assisted
+     * Doppler centre and two-step acquisition.  Two limits remain there: use_cfar = 1 is required, and fft_size <= 5 x 27 648.
+     * Everything else is B200_ERR_RANGE with the reason in b200_last_error(). */
     int b200_acq_create(b200_engine* e, const b200_acq_conf* conf, b200_acq** out);
     /* set_local_code(code)  (:218-251): code_host holds consumed_samples (layout 0/2) or fft_size/2
      * (layout 1) complex samples; stores conj(FFT(padded code)) in slot `slot`. */
