@@ -7,14 +7,16 @@
 // items (one consumer warp each) from one copy of the samples:
 //
 //   producer warp   cp.async.bulk (TMA bulk copy, UBLKCP) of 512-sample tiles of the band store into a
-//                   4-stage shared-memory ring, completion signalled on mbarriers (expect_tx bytes);
+//                   4-stage shared-memory ring (8 padded runs per tile), completion signalled on mbarriers
+//                   (expect_tx bytes);
 //   8 consumer warps each owns one (channel, epoch) item of the group: waits for the tile, reads its
-//                   samples with conflict-free LDS.128, rotates, looks its three (five, ...) chips up
-//                   in a warp-private shared-memory code table, accumulates E/P/L in per-sample-pair
-//                   float2 registers, releases the tile.
+//                   samples with conflict-free LDS.128, correlates them against a warp-private shared-memory
+//                   code table, releases the tile.  warp_tile looks every tap's chip up per sample;
+//                   warp_tile_chunks (C/A-like steps) splits 16-sample chunks at their one exact chip
+//                   boundary per tap and multiplies two chip values into chunk sums.
 //
-// The arithmetic per sample is exactly that of trk_kernels.cu (same chip-index float sequence, same
-// 64-bit fixed-point carrier phase), so results follow the same contract.  Items of a group need
+// Both use the chip-index float sequence and the 64-bit fixed-point carrier phase of trk_kernels.cu, so
+// indices are bit-exact and results follow the same contract.  Items of a group need
 // not start at the same sample: the tile range is the hull of the group and a warp only works on
 // tiles that intersect its own epoch (masked at the ends).  Group membership is the caller's item
 // ORDER (items 8g .. 8g+7); the host API sorts by start sample, bench.py's epoch-major order already
@@ -31,7 +33,7 @@ constexpr int kShTile = 512;     // samples per tile (4 KB)
 // Minimum resident CTAs per SM (__launch_bounds__).  sm_90a, 288 threads: 3 caps the kernel at 72 registers and spills
 // (<3>: 166 B stores / 248 B loads), 2 gives 96 registers (<3>: 8 B / 8 B), 1 no spills at 127-152.  On an H100 (400 W), ms
 // per C2 step: 2 -> 0.969-0.970, 3 -> 1.051-1.058, 1 -> 1.189-1.191, 4 -> 1.179; distinct-IQ through this kernel 1.237 at 2,
-// 1.393 at 3.
+// 1.393 at 3.  With the chunk path's scratch a CTA takes about 92 KB of shared memory, so three no longer fit on an SM.
 #ifndef SH_MINB
 #define SH_MINB 2
 #endif
@@ -56,13 +58,24 @@ constexpr int kShTblCap = 1152;  // floats of warp-private code storage: whole-e
 constexpr int kShWin = 256;      // ... else two 256-entry windows (double-buffered, refilled per tile with cp.async)
 constexpr int kShThreads = (kShK + 1) * 32;
 constexpr int kShReseed = 64;    // 64-sample steps between exact phasor re-seeds (4096 samples)
+// Tiles sit in shared memory as 8 runs of 64 samples (4 chunks of 16), each run followed by 16 bytes of padding: 528-byte
+// run stride, one bulk copy per run.  On the chunk path lane l owns chunk 4 (l % 8) + l / 8, so the 8 lanes of a quarter
+// warp read 8 different runs, whose starts fall on 8 distinct 16-byte bank groups: LDS.128 without conflicts.
+constexpr int kShChunk = 16;
+constexpr int kShRun = 4 * kShChunk;          // samples per bulk copy
+constexpr int kShRunStride = kShRun + 2;      // float2 per run slot
+constexpr int kShTileSlot = kShTile / kShRun * kShRunStride;
+constexpr int kShChunkStride = kShChunk + 2;  // float2 per lane in the prefix scratch (144 B: conflict-free STS.128)
+__device__ __forceinline__ int lane_chunk(int lane) { return 4 * (lane & 7) + (lane >> 3); }
 
 namespace
 {
 struct __align__(128) ShSmem
 {
-    float2 tiles[kShStages][kShTile];
+    float2 tiles[kShStages][kShTileSlot];
     float tbl[kShK][kShTblCap];
+    float2 prefix[kShK][32 * kShChunkStride];  // chunk path: each lane's running sums of its rotated chunk
+    float2 rot[kShK][kShChunk];                // chunk path: D^j, j = 0..15, D = the item's per-sample phasor
     unsigned long long full[kShStages];
     unsigned long long empty[kShStages];
     unsigned long long item_start[kShK];  // offset of the item's first sample in the band (band-relative)
@@ -110,13 +123,13 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
 
 // Correct-for-anything fallback for one warp: direct global loads, exact phasor per sample, integer
 // modulo lookup in the global code table.  Used when an item cannot take the table path.
+// T0, DT: the item's carrier phase and phase step in 64-bit turns.
 template <int TAPS>
-__device__ void warp_correlate_general(const b200_trk_item& it, const ChanDesc& ch, const BandDesc& bd, float2 (&acc)[TAPS])
+__device__ void warp_correlate_general(const b200_trk_item& it, const ChanDesc& ch, const BandDesc& bd, unsigned long long T0,
+    unsigned long long DT, float2 (&acc)[TAPS])
 {
     const int lane = threadIdx.x & 31;
     const unsigned long long s0 = it.sample_index - bd.first_index;
-    const unsigned long long T0 = turns_from_rad(-static_cast<double>(it.rem_carrier_phase_rad));
-    const unsigned long long DT = turns_from_rad(-static_cast<double>(it.phase_step_rad));
     const int body = (it.n / 8) * 8;
     for (int n = lane; n < it.n; n += 32)
         {
@@ -145,8 +158,8 @@ __device__ void warp_correlate_general(const b200_trk_item& it, const ChanDesc& 
 // where a warp gets the tile's samples from: the CTA's shared ring (normal case) ...
 struct SmemTileLoader
 {
-    const float4* p;  // tile + lane
-    __device__ __forceinline__ float4 operator()(int k) const { return p[32 * k]; }
+    const float4* p;  // tile + lane: sample pair lane + 32 k is pair `lane` of run k
+    __device__ __forceinline__ float4 operator()(int k) const { return p[(kShRunStride / 2) * k]; }
 };
 // ... or straight from the band store, when the group's items cannot share a window (different bands,
 // epochs far apart): same arithmetic, the samples just come through L2 per item as in trk_kernels.cu.
@@ -204,6 +217,63 @@ __device__ __forceinline__ void warp_tile(const Loader& load, float vlo, float v
             zr = nzr;
             fa += 64.0f;
             fb += 64.0f;
+        }
+}
+
+// Chunk path: one tile for one warp, lane l owns the 16 contiguous samples of chunk lane_chunk(l) of the tile, n0f is
+// the epoch index of the first of them.  The lane rotates its chunk in the chunk frame, u_j = x_j D^j, and stores the
+// running sums R_j = u_0 + ... + u_j.  Every tap's chip index rises at most once inside a chunk (the step test at the
+// item set-up), so with i0 the index of the first sample and m the number of samples that keep it, the tap gets
+//     z0 (c[i0] R_{m-1} + c[i0+1] (S - R_{m-1})),   S = R_15,   z0 = the phasor of the chunk's first sample.
+// m comes from a 4-step binary search on the exact index formula floor(fl(fl(step n) + aux)), which is non-decreasing
+// in n for step > 0: no sample's index is estimated.  MASKED as in warp_tile.  Accumulates into acc_re / acc_im.
+template <int TAPS, bool MASKED>
+__device__ __forceinline__ void warp_tile_chunks(const float4* x4, float4* pre4, const float4* rot4, float n0f, float vlo, float vhi,
+    float step, const float2 (&aux2)[TAPS], unsigned int tbl_off, float2 z0, float2 (&acc_re)[TAPS], float2 (&acc_im)[TAPS])
+{
+    const float magic = 12582912.0f;
+    float2 r = make_float2(0.f, 0.f);
+#pragma unroll
+    for (int k = 0; k < kShChunk / 2; k++)
+        {
+            float4 v = x4[k];
+            const float4 d = rot4[k];  // D^(2k), D^(2k+1)
+            if (MASKED)
+                {
+                    const float na = n0f + static_cast<float>(2 * k), nb = na + 1.0f;
+                    if (na < vlo || na > vhi) v.x = v.y = 0.f;
+                    if (nb < vlo || nb > vhi) v.z = v.w = 0.f;
+                }
+            r.x += fmaf(v.x, d.x, -v.y * d.y);
+            r.y += fmaf(v.x, d.y, v.y * d.x);
+            const float2 ra = r;
+            r.x += fmaf(v.z, d.z, -v.w * d.w);
+            r.y += fmaf(v.z, d.w, v.w * d.z);
+            pre4[k] = make_float4(ra.x, ra.y, r.x, r.y);
+        }
+    const float2* pre = reinterpret_cast<const float2*>(pre4);
+    const float lo = MASKED ? fminf(fmaxf(n0f, vlo), vhi) : n0f;
+#pragma unroll
+    for (int t = 0; t < TAPS; t++)
+        {
+            const float a = aux2[t].x;
+            const float t0 = __fadd_rd(__fadd_rn(__fmul_rn(step, lo), a), magic);
+            float q = n0f;  // last sample of the chunk known to keep index i0
+#pragma unroll
+            for (int s = 8; s > 0; s >>= 1)
+                {
+                    const float cand = q + static_cast<float>(s);
+                    const float ce = MASKED ? fminf(fmaxf(cand, vlo), vhi) : cand;
+                    const float tc = __fadd_rd(__fadd_rn(__fmul_rn(step, ce), a), magic);
+                    q = (tc == t0) ? cand : q;
+                }
+            const float2 P = pre[__float2int_rz(q - n0f)];
+            const unsigned int addr = (__float_as_uint(t0) << 2) + tbl_off;
+            const float c0 = lds_f32(addr), c1 = lds_f32(addr + 4u);
+            const float dc = c0 - c1;
+            const float vr = fmaf(dc, P.x, c1 * r.x), vi = fmaf(dc, P.y, c1 * r.y);
+            acc_re[t].x = fmaf(z0.x, vr, fmaf(-z0.y, vi, acc_re[t].x));
+            acc_im[t].x = fmaf(z0.x, vi, fmaf(z0.y, vr, acc_im[t].x));
         }
 }
 
@@ -273,7 +343,7 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
     if (!consumer)
         {
             // ---- producer warp: stream the hull through the ring ---------------------------------------
-            if (lane == 0 && n_tiles > 0)
+            if (n_tiles > 0)
                 {
                     BandDesc pb;
                     {
@@ -283,6 +353,8 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                     }
                     const bool ring = (pb.mask != ~0ULL);
                     const unsigned long long cap = ring ? pb.mask + 1ULL : pb.limit;
+                    // lane r < 8 copies samples [64r, 64r + 64) of every tile into run slot r (padded layout)
+                    const unsigned int c0 = static_cast<unsigned int>(lane) * kShRun;
                     for (int t = 0; t < n_tiles; t++)
                         {
                             const int s = t % kShStages;
@@ -292,27 +364,28 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                             stress_delay(static_cast<unsigned int>(t) * 31u + blockIdx.x * 7u + 3u);
 #endif
                             unsigned long long src = hull_start + static_cast<unsigned long long>(t) * kShTile;
-                            unsigned int n1 = kShTile, n2 = 0;
+                            unsigned int valid = kShTile;
                             if (ring)
+                                src &= pb.mask;
+                            else if (src >= cap)
+                                valid = 0;  // linear band: never read past its end (the clipped samples are outside every item)
+                            else if (src + kShTile > cap)
+                                valid = static_cast<unsigned int>(cap - src) & ~1u;
+                            if (lane == 0) mbar_arrive_expect_tx(&sm.full[s], valid * 8u);
+                            __syncwarp();
+                            float2* dst = &sm.tiles[s][lane * kShRunStride];
+                            if (lane < kShTile / kShRun && ring)
                                 {
-                                    src &= pb.mask;
-                                    if (src + kShTile > cap)
-                                        {
-                                            n1 = static_cast<unsigned int>(cap - src);
-                                            n2 = kShTile - n1;
-                                        }
+                                    // a run that straddles the end of the ring is split in two copies
+                                    const unsigned long long p = (src + c0) & pb.mask;
+                                    const unsigned int n1 = static_cast<unsigned int>(min(static_cast<unsigned long long>(kShRun), cap - p));
+                                    bulk_g2s(dst, pb.base + p, n1 * 8u, &sm.full[s]);
+                                    if (n1 < kShRun) bulk_g2s(dst + n1, pb.base, (kShRun - n1) * 8u, &sm.full[s]);
                                 }
-                            else
+                            else if (lane < kShTile / kShRun && valid > c0)
                                 {
-                                    // linear band: never read past its end (the clipped samples are outside every item)
-                                    if (src >= cap)
-                                        n1 = 0;
-                                    else if (src + kShTile > cap)
-                                        n1 = static_cast<unsigned int>(cap - src) & ~1u;
+                                    bulk_g2s(dst, pb.base + src + c0, min(valid - c0, static_cast<unsigned int>(kShRun)) * 8u, &sm.full[s]);
                                 }
-                            mbar_arrive_expect_tx(&sm.full[s], (n1 + n2) * 8u);
-                            if (n1) bulk_g2s(&sm.tiles[s][0], pb.base + src, n1 * 8u, &sm.full[s]);
-                            if (n2) bulk_g2s(&sm.tiles[s][n1], pb.base, n2 * 8u, &sm.full[s]);
                         }
                 }
             return;
@@ -323,7 +396,8 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
 #pragma unroll
     for (int t = 0; t < TAPS; t++) acc[t] = make_float2(0.f, 0.f);
 
-    bool table_path = false, whole_table = false;
+    bool table_path = false, whole_table = false, chunked = false;
+    float2 z0 = make_float2(0.f, 0.f), E = z0;  // chunk path: phasor of the lane's chunk start, its advance per tile
     unsigned long long my_hull = 0;
     int body = 0, a_i = 0, t_first = 0, t_last = 0;
     float step = 0.f;
@@ -371,6 +445,14 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                                 ehi = max(ehi, max(i0, i1));
                             }
                         whole_table = (static_cast<long long>(ehi) - elo + 3) <= kShTblCap;
+                        // Chunk path: the index a(n) = fl(fl(step n) + aux) of every tap may rise at most once over the
+                        // 16 samples of a chunk.  Both roundings err by at most half an ulp of a value of magnitude
+                        // <= M = step (body - 1) + max(|elo|, |ehi|) + 1, so a(n + 15) - a(n) <= 15 step + 2 ulp(M)
+                        // <= 15 step + M 2^-22; below 1, floor(a) rises at most once.  Only a shared window is laid
+                        // out in per-lane chunks, so items that stream their own tiles keep warp_tile.
+                        const double M = static_cast<double>(step) * nl + static_cast<double>(max(abs(elo), abs(ehi))) + 1.0;
+                        chunked = whole_table && sm.share && step > 0.f &&
+                                  static_cast<double>(kShChunk - 1) * static_cast<double>(step) + M * 0x1p-22 < 1.0;
                         if (whole_table)
                             {
                                 const int wb = elo - 1;
@@ -408,6 +490,13 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                     zi2 = make_float2(za.y, zb.y);
                     zr = zr2;
                     zi = zi2;
+                    if (chunked)
+                        {
+                            if (lane < kShChunk) sm.rot[warp][lane] = phasor_from_turns(DT * static_cast<unsigned long long>(lane));
+                            __syncwarp();
+                            E = phasor_from_turns(DT * static_cast<unsigned long long>(kShTile));
+                            z0 = phasor_from_turns(T0 + DT * static_cast<unsigned long long>(static_cast<long long>(t_first) * kShTile + kShChunk * lane_chunk(lane) - a_i));
+                        }
                 }
         }
 
@@ -481,35 +570,70 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
         __syncwarp();
     };
 
-    for (int t = 0; t < n_tiles; t++)
-        {
-            const int s = t % kShStages;
-            const unsigned int par = static_cast<unsigned int>((t / kShStages) & 1);
-            // Every consumer waits for every tile, also the ones it skips: a warp that ran ahead could
-            // otherwise arrive twice on empty[s] within one phase and let the producer overwrite a slot
-            // that a slower warp is still reading.
-            mbar_wait(&sm.full[s], par);
+    // Walks the group's tiles through the ring, calling work(t, slot) on the tiles of this warp's epoch.  Every consumer
+    // waits for every tile, also the ones it skips: a warp that ran ahead could otherwise arrive twice on empty[s] within
+    // one phase and let the producer overwrite a slot that a slower warp is still reading.
+    auto for_each_ring_tile = [&](const auto& work) {
+        for (int t = 0; t < n_tiles; t++)
+            {
+                const int s = t % kShStages;
+                const unsigned int par = static_cast<unsigned int>((t / kShStages) & 1);
+                mbar_wait(&sm.full[s], par);
 #if SH_STRESS
-            stress_delay(static_cast<unsigned int>(t) * 17u + static_cast<unsigned int>(warp) * 101u + blockIdx.x * 13u);
+                stress_delay(static_cast<unsigned int>(t) * 17u + static_cast<unsigned int>(warp) * 101u + blockIdx.x * 13u);
 #endif
-            if (table_path && t >= t_first && t < t_last)
-                {
+                if (t >= t_first && t < t_last) work(t, s);
+#if SH_STRESS
+                stress_delay(static_cast<unsigned int>(t) * 29u + static_cast<unsigned int>(warp) * 53u + blockIdx.x * 5u + 1u);
+                __syncwarp();
+#endif
+                if (lane == 0) mbar_arrive(&sm.empty[s]);
+            }
+    };
+    // The two paths walk the ring in separate loops, so that none of warp_tile's lane state is live on the chunk path.
+    if (chunked)
+        {
+            for_each_ring_tile([&](int t, int s) {
+                const int n_tile0 = t * kShTile - a_i;
+                const float n0f = static_cast<float>(n_tile0 + kShChunk * lane_chunk(lane));
+                const float vlo = static_cast<float>(max(n_tile0, 0)), vhi = static_cast<float>(min(n_tile0 + kShTile, body) - 1);
+                const float4* x4 = reinterpret_cast<const float4*>(&sm.tiles[s][(lane & 7) * kShRunStride + (lane >> 3) * kShChunk]);
+                float4* pre4 = reinterpret_cast<float4*>(&sm.prefix[warp][lane * kShChunkStride]);
+                const float4* rot4 = reinterpret_cast<const float4*>(&sm.rot[warp][0]);
+                if (n_tile0 >= 0 && n_tile0 + kShTile <= body)
+                    warp_tile_chunks<TAPS, false>(x4, pre4, rot4, n0f, vlo, vhi, step, aux2, tbl_off, z0, are, aim);
+                else
+                    warp_tile_chunks<TAPS, true>(x4, pre4, rot4, n0f, vlo, vhi, step, aux2, tbl_off, z0, are, aim);
+                if ((t - t_first + 1) % (kShReseed / 8) == 0)
+                    {
+                        // exact re-seed from the 64-bit phase of the lane's next chunk start, every 4096 samples
+                        const long long n_next = static_cast<long long>(t + 1) * kShTile + kShChunk * lane_chunk(lane) - a_i;
+                        z0 = phasor_from_turns(T0 + DT * static_cast<unsigned long long>(n_next));
+                    }
+                else
+                    {
+                        z0 = cmulf(z0, E);
+                    }
+                __syncwarp();
+            });
+        }
+    else
+        {
+            if (table_path)
+                for_each_ring_tile([&](int t, int s) {
                     const SmemTileLoader ld{reinterpret_cast<const float4*>(&sm.tiles[s][0]) + lane};
                     process_tile(t, ld);
-                }
-#if SH_STRESS
-            stress_delay(static_cast<unsigned int>(t) * 29u + static_cast<unsigned int>(warp) * 53u + blockIdx.x * 5u + 1u);
-            __syncwarp();
-#endif
-            if (lane == 0) mbar_arrive(&sm.empty[s]);
-        }
-    if (!sm.share && table_path)
-        {
-            // no shared window for this group: stream this item's own tiles from the band store
-            for (int t = t_first; t < t_last; t++)
+                });
+            else
+                for_each_ring_tile([](int, int) {});
+            if (!sm.share && table_path)
                 {
-                    const GlobalTileLoader ld{bd.base, bd.mask, my_hull + static_cast<unsigned long long>(t) * kShTile + 2ULL * lane, bd.limit};
-                    process_tile(t, ld);
+                    // no shared window for this group: stream this item's own tiles from the band store
+                    for (int t = t_first; t < t_last; t++)
+                        {
+                            const GlobalTileLoader ld{bd.base, bd.mask, my_hull + static_cast<unsigned long long>(t) * kShTile + 2ULL * lane, bd.limit};
+                            process_tile(t, ld);
+                        }
                 }
         }
     if (have_item && it.n > 0)
@@ -543,7 +667,7 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                 }
             else
                 {
-                    warp_correlate_general<TAPS>(it, *ch, bd, acc);
+                    warp_correlate_general<TAPS>(it, *ch, bd, T0, DT, acc);
                 }
 #pragma unroll
             for (int t = 0; t < TAPS; t++)
