@@ -133,7 +133,8 @@ int ensure_loop_buffers(b200_engine* e, int rec_capacity)
     return B200_OK;
 }
 
-// what the bands hold right now; unlike the push and submit checks, the window ignores valid_from
+// what the bands hold right now: [valid_from, write_index) of an owned ring, as b200_iq_window, b200_iq_push_at and
+// b200_trk_submit see it (ring slots below valid_from still hold the stream from before a gap, restart or forget)
 LoopAvail snapshot_avail(const b200_engine* e)
 {
     LoopAvail a{};
@@ -141,7 +142,7 @@ LoopAvail snapshot_avail(const b200_engine* e)
         {
             const Band& b = e->bands[i];
             if (!b.in_use) continue;
-            a.lo[i] = b.oldest();
+            a.lo[i] = b.attached ? b.first_index : std::max(b.valid_from, b.oldest());
             a.hi[i] = b.attached ? b.first_index + b.capacity : b.write_index;
         }
     return a;

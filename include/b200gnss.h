@@ -299,7 +299,9 @@ extern "C"
     int b200_trk_loop_start(b200_engine* e, int loop_id, double acq_delay_samples, double acq_doppler_hz,
         uint64_t acq_samplestamp_samples, uint64_t nitems_read);
     /* Run up to max_epochs cycles of every started loop: per epoch one correlator launch over all loops
-     * and one loop-update launch; a loop whose next vector_length samples are not in its band yet stalls.
+     * and one loop-update launch; a loop whose next vector_length samples are not all inside its band's
+     * [valid_from, write_index) (the window b200_iq_window reports) stalls: samples not pushed yet, overwritten,
+     * or left behind by a gap, a restart or b200_iq_forget are never correlated.
      * records_host: n_loops x max_epochs records (loop-major); n_records_host[loop] = cycles logged.
      * Either output may be NULL. */
     int b200_trk_loop_run(b200_engine* e, int max_epochs, b200_trk_dump_record* records_host, int* n_records_host);

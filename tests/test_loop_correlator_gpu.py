@@ -1,0 +1,553 @@
+"""The correlator inside the free-running DLL/PLL loops (b200_trk_loop_run), epoch by epoch against exact references.
+
+In the tracking state b200_trk_loop_peek_items is a pure function of the loop state, and loop_run(1) correlates exactly
+that item and logs one record carrying the P tap's bits (prompt_I, prompt_Q) and hypotf of every tap (abs_*).  So
+peek -> run(1) -> compare checks every epoch a loop actually produced, in each way the loops can run:
+
+  * mode 0, the persistent CTA per loop, at both widths (B200_LOOP_WIDTH = 256 | 512; the launcher reads it per launch);
+  * mode 1, the batch correlator with one slice per item and a loop-update launch per epoch;
+  * mode 2, the same with each epoch split over several CTAs (batch_slices).
+
+Integer samples with a zero imaginary part and loops at 0 Hz keep every tap an exactly representable integer (the PLL
+error is exactly 0, so the carrier stays at phase 0 with step 0): those runs must EQUAL the integer oracle built from the
+reference's chip indices.  Float data with a rotating carrier stays within the batch-kernel contract (DESIGN a2),
+1e-5 |P| of the float64 truth.  One launch of N epochs must equal N launches of one epoch byte for byte (in mode 0 only
+the chip-table window cache differs), and the persistent kernel's split loop update must equal the sequential update
+(b200_trk_loop_step_taps) byte for byte.  Finally the loops stall outside [valid_from, write_index), the window
+b200_iq_window reports: after a gap, a restart or b200_iq_forget they never correlate what the ring held before."""
+import numpy as np
+import pytest
+
+from oracle import loop as ol
+
+pytestmark = pytest.mark.gpu
+
+FS = 4e6
+CA_RATE = 1.023e6
+TRUTH_RTOL = 1e-5
+# (mode, B200_LOOP_WIDTH)
+MODES = {"persistent256": (0, "256"), "persistent512": (0, "512"), "per_epoch": (1, None), "sliced": (2, None)}
+PERSISTENT = ["persistent256", "persistent512"]
+
+
+@pytest.fixture(scope="module")
+def capi():
+    import gnss_sdr_b200.capi as c
+    return c
+
+
+def set_mode(monkeypatch, e, name):
+    mode, width = MODES[name]
+    if width is None:
+        monkeypatch.delenv("B200_LOOP_WIDTH", raising=False)
+    else:
+        monkeypatch.setenv("B200_LOOP_WIDTH", width)
+    e.loop_set_mode(mode)
+
+
+def conf_to_capi(capi, c):
+    out = capi.TrkLoopConf()
+    for name, _ in ol.LoopConf._fields_:
+        setattr(out, name, getattr(c, name))
+    return out
+
+
+def shifts_of(conf):
+    spc, els = conf.code_samples_per_chip, conf.early_late_space_chips
+    if conf.veml:
+        return [-0.5 * spc, -els * spc, 0.0, els * spc, 0.5 * spc]
+    return [-els * spc, 0.0, els * spc]
+
+
+def int_signal(rng, table, n, amp, code_phase, rate, noise=2):
+    """round(amp * code(t - tau)) + uniform integer noise in [-noise, noise]: real integers (int64[n])"""
+    t = np.arange(n, dtype=np.float64)
+    idx = np.floor(code_phase + t * rate).astype(np.int64) % len(table)
+    return np.rint(amp * table[idx]).astype(np.int64) + rng.integers(-noise, noise + 1, n)
+
+
+class Stream:
+    """The samples of one band: host copy x (int64 or complex64) starting at absolute index x0."""
+
+    def __init__(self, x, x0):
+        self.x, self.x0 = x, x0
+
+    def seg(self, s, n):
+        a = int(s) - self.x0
+        assert 0 <= a and a + n <= len(self.x), (s, n, self.x0, len(self.x))
+        return self.x[a:a + n]
+
+
+class LoopSpec:
+    """One loop: band, code table, configuration, start (acq delay, acq Doppler, acq stamp, nitems_read) and the
+    stream its band carries (for the reference)."""
+
+    def __init__(self, band, table, conf, start, stream):
+        self.band, self.table, self.conf, self.start, self.stream = band, np.asarray(table, np.float32), conf, start, stream
+        self.shifts = shifts_of(conf)
+        self.taps = len(self.shifts)
+
+
+def make_engine(capi, specs, capacities):
+    e = capi.Engine()
+    for band, cap in capacities.items():
+        e.iq_create(band, cap)
+    ids = []
+    for sp in specs:
+        ch = e.channel_create(sp.band, sp.taps)
+        e.channel_set_code(ch, sp.table, sp.shifts)
+        ids.append(e.loop_create(ch, conf_to_capi(capi, sp.conf)))
+    return e, ids
+
+
+def start_all(e, ids, specs):
+    for lid, sp in zip(ids, specs):
+        e.loop_start(lid, *sp.start)
+
+
+def int_taps(sp, item):
+    """exact integer taps of one peeked item on integer data"""
+    n = int(item["n"])
+    _, idx = ol_port().resampler(1, sp.table, float(item["rem_code_phase_chips"]), float(item["code_phase_step_chips"]), sp.shifts, n,
+                                 return_idx=True)
+    x = sp.stream.seg(item["sample_index"], n)
+    return (x[None, :] * sp.table.astype(np.int64)[idx]).sum(axis=1)
+
+
+def f64_taps(sp, item):
+    n = int(item["n"])
+    return ol_port().multicorrelator_f64(1, sp.stream.seg(item["sample_index"], n), sp.table, sp.shifts, float(item["rem_carrier_phase_rad"]),
+                                         float(item["phase_step_rad"]), float(item["rem_code_phase_chips"]),
+                                         float(item["code_phase_step_chips"]), n)
+
+
+def ol_port():
+    import oracle
+    return oracle.port
+
+
+def rec_mags(sp, r):
+    return np.array([r["abs_VE"], r["abs_E"], r["abs_P"], r["abs_L"], r["abs_VL"]] if sp.taps == 5 else [r["abs_E"], r["abs_P"], r["abs_L"]],
+                    np.float64)
+
+
+def check_int_epoch(sp, item, r, what):
+    assert item["rem_carrier_phase_rad"] == 0.0 and item["phase_step_rad"] == 0.0 and item["phase_rate_step_rad"] == 0.0, (what, item)
+    want = int_taps(sp, item)
+    p = sp.taps // 2
+    assert r["prompt_I"] == want[p] and r["prompt_Q"] == 0.0, (what, r["prompt_I"], r["prompt_Q"], want)
+    assert np.array_equal(rec_mags(sp, r), np.abs(want).astype(np.float64)), (what, rec_mags(sp, r), want)
+    if sp.taps == 3:
+        assert r["abs_VE"] == 0.0 and r["abs_VL"] == 0.0, what
+
+
+def check_float_epoch(sp, item, r, what):
+    truth = f64_taps(sp, item)
+    p = sp.taps // 2
+    scale = TRUTH_RTOL * abs(truth[p])
+    assert abs(complex(float(r["prompt_I"]), float(r["prompt_Q"])) - truth[p]) <= scale, (what, r["prompt_I"], r["prompt_Q"], truth[p])
+    err = np.abs(rec_mags(sp, r) - np.abs(truth))
+    assert np.all(err <= scale), (what, err / abs(truth[p]))
+
+
+def run_per_epoch(e, ids, n_ep, feed=None):
+    """peek -> run(1), n_ep times.  feed(items) pushes what the peeked items need first.
+    -> per loop: (items, records) of the epochs that logged a record"""
+    items_out = [[] for _ in ids]
+    recs_out = [[] for _ in ids]
+    for _ in range(n_ep):
+        items = e.loop_peek_items()
+        if feed is not None:
+            feed(items)
+        rec, cnt = e.loop_run(1)
+        for i in range(len(ids)):
+            if cnt[i]:
+                items_out[i].append(items[i])
+                recs_out[i].append(rec[i, 0])
+    return [(np.array(a, items.dtype), np.array(b, rec.dtype)) for a, b in zip(items_out, recs_out)]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# configurations with integer data
+
+RING_BASE = (1 << 32) - 50_000          # absolute indices cross 2^32 inside the run
+RING_CAP = 1 << 15
+
+
+def gps_int_case(rng, n_ep, base=0, delay=1234, amp=3.0, code_ppm=0.0, conf_kw=None, prn=1, extra=8000):
+    code = ol_port().gps_ca_code(prn)
+    rate = CA_RATE * (1 + code_ppm * 1e-6) / FS
+    x = int_signal(rng, code, 4000 * n_ep + delay + extra, amp, (-delay * rate) % 1023, rate)
+    conf = ol.default_conf(fs_in=FS, prn=prn, **(conf_kw or {}))
+    return LoopSpec(0, code, conf, (delay + 0.3, 0.0, base, base), Stream(x, base))
+
+
+def galileo_int_case(rng, n_ep, band=0, base=0):
+    primary = (2 * rng.integers(0, 2, 4092) - 1).astype(np.int32)
+    table = ol_port().sinboc11(primary)
+    L = len(table)
+    rate = CA_RATE * 2.0 / FS                                          # table entries per sample
+    cp = 2711.0
+    delay = ((L - cp) % L) / rate
+    x = int_signal(rng, table, 16000 * (n_ep + 4), 4.0, cp, rate)
+    conf = ol.default_conf(fs_in=FS, prn=1, code_length_chips=4092, code_period=0.004, vector_length=16000, code_samples_per_chip=2,
+                           veml=1, early_late_space_chips=0.15)
+    return LoopSpec(band, table, conf, (delay + 0.2, 0.0, base, base), Stream(x, base))
+
+
+def veml_int_case(rng, n_ep):
+    code = np.repeat(ol_port().gps_ca_code(7), 2)
+    delay = 2222
+    rate = 2 * CA_RATE / FS
+    x = int_signal(rng, code, 4000 * (n_ep + 2), 3.0, (-delay * rate) % len(code), rate)
+    conf = ol.default_conf(fs_in=FS, prn=7, veml=1, code_samples_per_chip=2, early_late_space_chips=0.15, cn0_samples=10)
+    return LoopSpec(0, code, conf, (delay - 0.4, 0.0, 0, 0), Stream(x, 0))
+
+
+def int_configs(n_ep):
+    """name -> (specs, band capacities, ring-fed?)"""
+    rng = np.random.default_rng(2024)
+    ring = gps_int_case(rng, n_ep, base=RING_BASE, amp=1.0)
+    two_a = gps_int_case(rng, n_ep, delay=3001, prn=9)
+    two_b = galileo_int_case(rng, n_ep, band=1, base=5_000_000)
+    return {
+        "gps_ring": ([ring], {0: RING_CAP}, True),
+        "veml_2spc": ([veml_int_case(rng, n_ep)], None, False),
+        "galileo_like": ([galileo_int_case(rng, n_ep)], None, False),
+        "two_bands": ([two_a, two_b], None, False),
+    }
+
+
+class RingFeeder:
+    """Pushes a band's stream into a small ring block by block, never ahead of what the ring can hold behind the loop."""
+
+    def __init__(self, e, band, stream, block=8192):
+        self.e, self.band, self.s, self.block = e, band, stream, block
+        self.pos = 0
+        e.iq_push_at(band, stream.x0, stream.x[:0].astype(np.complex64))
+
+    def push_block(self):
+        blk = self.s.x[self.pos:self.pos + self.block]
+        if len(blk):
+            self.e.iq_push_at(self.band, self.s.x0 + self.pos, blk.astype(np.complex64))
+            self.pos += len(blk)
+        return len(blk)
+
+    def until(self, end):
+        while self.s.x0 + self.pos < end and self.push_block():
+            pass
+
+
+def push_all(e, specs):
+    seen = set()
+    for sp in specs:
+        if sp.band not in seen:
+            seen.add(sp.band)
+            e.iq_push_at(sp.band, sp.stream.x0, sp.stream.x.astype(np.complex64))
+
+
+def capacities_for(specs, caps):
+    if caps is not None:
+        return caps
+    return {sp.band: len(sp.stream.x) + 16 for sp in specs}
+
+
+def run_config(capi, monkeypatch, specs, caps, ring, mode, n_ep):
+    """-> per-epoch results (run_per_epoch), records of the multi-epoch twin, final status of both"""
+    caps = capacities_for(specs, caps)
+    e, ids = make_engine(capi, specs, caps)
+    set_mode(monkeypatch, e, mode)
+    if ring:
+        assert len(specs) == 1
+        feeder = RingFeeder(e, 0, specs[0].stream)
+        start_all(e, ids, specs)
+        per = run_per_epoch(e, ids, n_ep, feed=lambda items: feeder.until(int(items[0]["sample_index"]) + int(items[0]["n"])))
+    else:
+        push_all(e, specs)
+        start_all(e, ids, specs)
+        per = run_per_epoch(e, ids, n_ep)
+    st = [e.loop_status(l) for l in ids]
+    e.close()
+
+    # the twin: the same loops in launches of many epochs
+    e, ids = make_engine(capi, specs, caps)
+    set_mode(monkeypatch, e, mode)
+    if ring:
+        feeder = RingFeeder(e, 0, specs[0].stream)
+        start_all(e, ids, specs)
+        got = [[] for _ in ids]
+        while sum(len(g) for g in got) < n_ep:
+            if not feeder.push_block():
+                break
+            rec, cnt = e.loop_run(16)
+            got[0].append(rec[0, :cnt[0]])
+        multi = [np.concatenate(g)[:n_ep] for g in got]
+    else:
+        push_all(e, specs)
+        start_all(e, ids, specs)
+        rec, cnt = e.loop_run(n_ep)
+        multi = [rec[i, :cnt[i]] for i in range(len(ids))]
+    st2 = [e.loop_status(l) for l in ids]
+    e.close()
+    return per, multi, st, st2
+
+
+N_EP = 300
+
+
+@pytest.mark.parametrize("mode", list(MODES))
+@pytest.mark.parametrize("config", ["gps_ring", "veml_2spc", "galileo_like", "two_bands"])
+def test_integer_epochs_equal_the_integer_oracle(capi, monkeypatch, config, mode):
+    """(a) every epoch's taps equal the integer oracle exactly, and (c) one launch of many epochs gives the same records,
+    byte for byte, as one launch per epoch."""
+    specs, caps, ring = int_configs(N_EP)[config]
+    per, multi, st, st2 = run_config(capi, monkeypatch, specs, caps, ring, mode, N_EP)
+    for i, sp in enumerate(specs):
+        items, recs = per[i]
+        assert len(recs) == N_EP, (config, i, len(recs))
+        for k in range(len(recs)):
+            check_int_epoch(sp, items[k], recs[k], (config, mode, i, k))
+        # the DLL moves the code phase every epoch, and the code step now and then
+        assert len(np.unique(items["rem_code_phase_chips"])) > len(items) // 2
+        assert len(np.unique(items["code_phase_step_chips"])) > 1
+        if config == "gps_ring":
+            d = np.diff(items["sample_index"].astype(np.int64))
+            assert set(np.unique(d)) == {3999, 4000, 4001}, np.unique(d, return_counts=True)
+            assert items["sample_index"][0] < (1 << 32) < items["sample_index"][-1]
+            assert int(items["sample_index"][-1]) - RING_BASE > 20 * RING_CAP
+        assert len(multi[i]) == N_EP and multi[i].tobytes() == recs.tobytes(), (config, mode, i)
+    if not ring:
+        for a, b in zip(st, st2):
+            assert (a.state, a.sample_counter, a.epochs) == (b.state, b.sample_counter, b.epochs)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# float data, rotating carrier
+
+def float_configs(n_ep):
+    from gnss_synth import make_iq
+    port = ol_port()
+    out = {}
+    for name, prn, doppler, delay, veml in (("gps_3taps", 4, 1234.0, 1777, 0), ("veml_5taps", 12, -2710.0, 909, 1)):
+        code = port.gps_ca_code(prn)
+        spc = 2 if veml else 1
+        table = np.repeat(code, spc)
+        n = 4000 * (n_ep + 2) + delay
+        iq = make_iq({prn: table}, FS, n, [dict(prn=prn, doppler=doppler, code_phase_chips=(-delay * spc * CA_RATE / FS) % len(table),
+                                                cn0=60.0, phase0=0.7)], seed=prn, chips_per_table_chip=spc)
+        kw = dict(veml=1, code_samples_per_chip=2, early_late_space_chips=0.15) if veml else {}
+        conf = ol.default_conf(fs_in=FS, prn=prn, pull_in_time_s=1, **kw)
+        out[name] = LoopSpec(0, table, conf, (delay + 0.2, doppler - 6.0, 0, 0), Stream(iq, 0))
+    return out
+
+
+@pytest.mark.parametrize("mode", list(MODES))
+@pytest.mark.parametrize("config", ["gps_3taps", "veml_5taps"])
+def test_float_epochs_within_the_float64_truth(capi, monkeypatch, config, mode):
+    """(b) complex samples with a real Doppler: every epoch's P and |tap| within 1e-5 |P| of the float64 correlation of the
+    peeked item, and (c) one launch of many epochs equals one launch per epoch byte for byte."""
+    sp = float_configs(N_EP)[config]
+    per, multi, st, st2 = run_config(capi, monkeypatch, [sp], None, False, mode, N_EP)
+    items, recs = per[0]
+    assert len(recs) == N_EP
+    assert np.all(items["phase_step_rad"] != 0.0)
+    for k in range(N_EP):
+        check_float_epoch(sp, items[k], recs[k], (config, mode, k))
+    assert abs(np.mean(recs["carrier_doppler_hz"][-100:]) - (1234.0 if config == "gps_3taps" else -2710.0)) < 2.0
+    assert len(multi[0]) == N_EP and multi[0].tobytes() == recs.tobytes(), (config, mode)
+    assert (st[0].sample_counter, st[0].epochs) == (st2[0].sample_counter, st2[0].epochs)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the persistent kernel's split loop update against the sequential one
+
+def lock_loss_case(rng):
+    """integer data; cn0_min above the signal's C/N0 (about 70 dB-Hz), no pull-in time and the acquisition stamp a
+    second before the first sample: the code-lock counter runs out after about 85 epochs"""
+    base = 4_000_000
+    sp = gps_int_case(rng, 120, conf_kw=dict(pull_in_time_s=0, max_code_lock_fail=60, cn0_min=80), prn=17)
+    sp.start = (sp.start[0], 0.0, 0, base)
+    sp.stream = Stream(sp.stream.x, base)      # 4e6 samples are exactly 1000 code periods: same code phase
+    return sp
+
+
+def split_configs():
+    rng = np.random.default_rng(77)
+    return {
+        "gps_float_3taps": (float_configs(N_EP)["gps_3taps"], N_EP),
+        "veml_int_5taps": (veml_int_case(rng, N_EP), N_EP),
+        "gps_int_lock_loss": (lock_loss_case(rng), 120),
+    }
+
+
+def rebuilt_taps(sp, r):
+    """the taps of a record, exact for 3-tap loops and for integer data: P = (prompt_I, prompt_Q), the others (|tap|, 0)"""
+    p = complex(float(r["prompt_I"]), float(r["prompt_Q"]))
+    if sp.taps == 3:
+        return np.array([r["abs_E"], p, r["abs_L"]], np.complex64)
+    return np.array([r["abs_VE"], r["abs_E"], p, r["abs_L"], r["abs_VL"]], np.complex64)
+
+
+@pytest.mark.parametrize("mode", PERSISTENT)
+@pytest.mark.parametrize("config", ["gps_float_3taps", "veml_int_5taps", "gps_int_lock_loss"])
+def test_split_update_equals_the_sequential_update(capi, monkeypatch, config, mode):
+    """(d) The persistent kernel updates the loop on three warps at once and, on a lost-lock verdict, restores its backup
+    and replays the update.  Feeding its taps to b200_trk_loop_step_taps (the sequential update) on a twin started
+    identically must reproduce every peeked item and every record byte for byte; the lock-loss configuration also
+    takes the restore-and-replay branch."""
+    sp, n_ep = split_configs()[config]
+    caps = {0: len(sp.stream.x) + 16}
+    e, ids = make_engine(capi, [sp], caps)
+    set_mode(monkeypatch, e, mode)
+    push_all(e, [sp])
+    start_all(e, ids, [sp])
+    items, recs = run_per_epoch(e, ids, n_ep)[0]
+    st = e.loop_status(ids[0])
+    e.close()
+    lost = config == "gps_int_lock_loss"
+    if lost:
+        assert 40 < len(recs) < n_ep - 10 and st.state == 0 and st.loss_of_lock == 1, (len(recs), st.state, st.loss_of_lock)
+        for k in range(len(recs)):
+            check_int_epoch(sp, items[k], recs[k], (config, mode, k))
+    else:
+        assert len(recs) == n_ep and st.state == 2 and st.loss_of_lock == 0
+
+    t, tids = make_engine(capi, [sp], caps)
+    push_all(t, [sp])
+    start_all(t, tids, [sp])
+    for k in range(len(recs)):
+        it = t.loop_peek_items()
+        assert it[0].tobytes() == items[k].tobytes(), (config, mode, k)
+        r, logged = t.loop_step_taps(rebuilt_taps(sp, recs[k])[None, :])
+        assert logged[0] == 1 and r[0].tobytes() == recs[k].tobytes(), (config, mode, k)
+    if lost:
+        # the epoch that lost lock logged no record: its taps come from the integer oracle
+        it = t.loop_peek_items()
+        r, logged = t.loop_step_taps(int_taps(sp, it[0]).astype(np.complex64)[None, :])
+        assert logged[0] == 0
+    s2 = t.loop_status(tids[0])
+    t.close()
+    assert bytes(st) == bytes(s2), (config, mode)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the loops' sample window is [valid_from, write_index)
+
+DELAY = 1234
+
+
+def gps_stream(rng, prn, x0, n):
+    """integer GPS C/A samples from absolute index x0 whose code starts DELAY samples after x0 (and every 4000 after)"""
+    code = ol_port().gps_ca_code(prn)
+    rate = CA_RATE / FS
+    return code, Stream(int_signal(rng, code, n, 3.0, (-DELAY * rate) % 1023, rate), x0)
+
+
+def window_engine(capi, monkeypatch, mode, specs, caps):
+    e, ids = make_engine(capi, specs, caps)
+    set_mode(monkeypatch, e, mode)
+    return e, ids
+
+
+def other_band(rng, n_ep):
+    """a loop on band 1 that must run undisturbed through whatever happens on band 0"""
+    code, s = gps_stream(rng, 21, 0, 4000 * n_ep + 12000)
+    return LoopSpec(1, code, ol.default_conf(fs_in=FS, prn=21), (DELAY + 0.3, 0.0, 0, 0), s)
+
+
+def check_loop(sp, res, n, what):
+    items, recs = res
+    assert len(recs) == n, (what, len(recs), n)
+    for k in range(n):
+        check_int_epoch(sp, items[k], recs[k], (what, k))
+
+
+@pytest.mark.parametrize("mode", list(MODES))
+def test_loops_below_valid_from_stall_after_a_gap(capi, monkeypatch, mode):
+    """iq_push_at(0, A[:60000]) then iq_push_at(1_000_000, B[:30000]) into a 2^16 ring: ring slots below valid_from still
+    hold A.  A loop whose epochs lie below 1_000_000 must stall (no record, sample counter frozen after its first
+    prepare); a loop started at 1_000_000 tracks B exactly; a loop on another band is unaffected."""
+    rng = np.random.default_rng(5)
+    code, a = gps_stream(rng, 3, 0, 60_000)
+    _, b = gps_stream(rng, 3, 1_000_000, 30_000)
+    low = LoopSpec(0, code, ol.default_conf(fs_in=FS, prn=3), (DELAY + 0.3, 0.0, 990_000, 990_000), None)
+    high = LoopSpec(0, code, ol.default_conf(fs_in=FS, prn=3), (DELAY + 0.3, 0.0, 1_000_000, 1_000_000), b)
+    oth = other_band(rng, 12)
+    e, ids = window_engine(capi, monkeypatch, mode, [low, high, oth], {0: 1 << 16, 1: len(oth.stream.x) + 16})
+    e.iq_push_at(0, 0, a.x.astype(np.complex64))
+    e.iq_push_at(0, 1_000_000, b.x.astype(np.complex64))
+    push_all(e, [oth])
+    assert e.iq_window(0) == (1_000_000, 1_030_000)
+    start_all(e, ids, [low, high, oth])
+    e.loop_peek_items()
+    frozen = e.loop_status(ids[0]).sample_counter
+    assert 990_000 < frozen < 1_000_000
+    res = run_per_epoch(e, ids, 12)
+    s = e.loop_status(ids[0])
+    assert len(res[0][1]) == 0 and s.sample_counter == frozen and s.state == 2 and s.epochs == 0, (len(res[0][1]), s.sample_counter)
+    check_loop(high, res[1], 6, "after the gap")
+    check_loop(oth, res[2], 12, "other band")
+    e.close()
+
+
+@pytest.mark.parametrize("mode", list(MODES))
+def test_loops_stall_after_iq_forget(capi, monkeypatch, mode):
+    """After b200_iq_forget every sample in the band is history: both of its loops stall, although the ring still holds
+    those samples and more arrive behind them; the loop on the other band keeps running."""
+    rng = np.random.default_rng(6)
+    code, s = gps_stream(rng, 8, 0, 100_000)
+    l0 = LoopSpec(0, code, ol.default_conf(fs_in=FS, prn=8), (DELAY + 0.3, 0.0, 0, 0), s)
+    l1 = LoopSpec(0, code, ol.default_conf(fs_in=FS, prn=8, early_late_space_chips=0.25), (DELAY - 0.2, 0.0, 0, 0), s)
+    oth = other_band(rng, 10)
+    e, ids = window_engine(capi, monkeypatch, mode, [l0, l1, oth], {0: 1 << 17, 1: len(oth.stream.x) + 16})
+    e.iq_push_at(0, 0, s.x[:60_000].astype(np.complex64))
+    push_all(e, [oth])
+    start_all(e, ids, [l0, l1, oth])
+    before = run_per_epoch(e, ids, 5)
+    check_loop(l0, before[0], 5, "before forget")
+    check_loop(l1, before[1], 5, "before forget")
+    e.iq_forget(0)
+    e.iq_push_at(0, 60_000, s.x[60_000:].astype(np.complex64))     # contiguous: valid_from stays at 60_000
+    assert e.iq_window(0) == (60_000, 100_000)
+    counters = [e.loop_status(l).sample_counter for l in ids[:2]]
+    after = run_per_epoch(e, ids, 5)
+    assert len(after[0][1]) == 0 and len(after[1][1]) == 0
+    assert [e.loop_status(l).sample_counter for l in ids[:2]] == counters
+    check_loop(oth, (np.concatenate([before[2][0], after[2][0]]), np.concatenate([before[2][1], after[2][1]])), 10, "other band")
+    e.close()
+
+
+@pytest.mark.parametrize("mode", list(MODES))
+def test_loops_follow_a_restarted_stream(capi, monkeypatch, mode):
+    """A stream at 1_000_000 into a 2^16 ring, then a restart iq_push_at at the older index 500_000.  The loop on the old
+    stream stalls, a loop started at 500_000 runs on the new samples exactly, and one started at 480_000 (below the new
+    valid_from, yet inside what the ring's slots span) stalls instead of correlating the old stream."""
+    rng = np.random.default_rng(7)
+    code, s1 = gps_stream(rng, 30, 1_000_000, 60_000)
+    _, s2 = gps_stream(rng, 30, 500_000, 40_000)
+    conf = ol.default_conf(fs_in=FS, prn=30)
+    old = LoopSpec(0, code, conf, (DELAY + 0.3, 0.0, 1_000_000, 1_000_000), s1)
+    new = LoopSpec(0, code, conf, (DELAY + 0.3, 0.0, 500_000, 500_000), s2)
+    below = LoopSpec(0, code, conf, (DELAY + 0.3, 0.0, 480_000, 480_000), None)
+    oth = other_band(rng, 12)
+    specs = [old, new, below, oth]
+    e, ids = window_engine(capi, monkeypatch, mode, specs, {0: 1 << 16, 1: len(oth.stream.x) + 16})
+    e.iq_push_at(0, 1_000_000, s1.x.astype(np.complex64))
+    push_all(e, [oth])
+    e.loop_start(ids[0], *old.start)
+    e.loop_start(ids[3], *oth.start)
+    first = run_per_epoch(e, ids, 4)
+    check_loop(old, first[0], 4, "old stream")
+    e.iq_push_at(0, 500_000, s2.x.astype(np.complex64))
+    assert e.iq_window(0) == (500_000, 540_000)
+    e.loop_start(ids[1], *new.start)
+    e.loop_start(ids[2], *below.start)
+    e.loop_peek_items()
+    frozen = [e.loop_status(ids[i]).sample_counter for i in (0, 2)]
+    assert 480_000 < frozen[1] < 500_000
+    second = run_per_epoch(e, ids, 8)
+    assert len(second[0][1]) == 0 and len(second[2][1]) == 0
+    assert [e.loop_status(ids[i]).sample_counter for i in (0, 2)] == frozen
+    check_loop(new, second[1], 8, "new stream")
+    check_loop(oth, (np.concatenate([first[3][0], second[3][0]]), np.concatenate([first[3][1], second[3][1]])), 12, "other band")
+    e.close()
