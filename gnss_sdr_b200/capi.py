@@ -119,7 +119,6 @@ _SIGS.update({
     "b200_acq_search_dev": ([_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp], C.c_int),
     "b200_acq_read_grid": ([_vp, C.c_uint32, _vp], C.c_int),
     "b200_acq_selftest_dft": ([_vp, _vp, _vp], C.c_int),
-    "b200_acq_selftest_read": ([_vp, C.c_int, _vp], C.c_int),
     "b200_acq_read_wipeoffs": ([_vp, _vp], C.c_int),
     "b200_acq_destroy": ([_vp], C.c_int),
 })
@@ -549,12 +548,6 @@ class PcpsAcquisition:
         assert x.size == self.conf.fft_size
         out = np.empty(x.size, np.complex64)
         _chk(lib.b200_acq_selftest_dft(self.h, x.ctypes.data, out.ctypes.data), "b200_acq_selftest_dft")
-        return out
-
-    def selftest_read(self, what: int) -> np.ndarray:
-        rows = self.conf.num_doppler_bins if what == 0 else self.conf.n_code_slots
-        out = np.empty((rows, self.conf.fft_size), np.complex64)
-        _chk(lib.b200_acq_selftest_read(self.h, what, out.ctypes.data), "b200_acq_selftest_read")
         return out
 
     def read_grid(self, slot: int) -> np.ndarray:

@@ -11,17 +11,6 @@
 #include <new>
 #include <vector>
 
-namespace b200
-{
-struct AcqRowStat
-{
-    float max;
-    unsigned int argmax;
-    float sum;
-    float pad;
-};
-}  // namespace b200
-
 using namespace b200;
 
 struct b200_acq
@@ -47,7 +36,7 @@ struct b200_acq
     uint32_t bins2{0};
     DevBuf<AcqRowStat> rowstat;
     DevBuf<int> slot_list;
-    DevBuf<unsigned char> best;  // 8 bytes per slot
+    DevBuf<AcqBest> best;
     DevBuf<float> second_peak;
     DevBuf<b200_acq_result> results_dev;
     PinBuf<b200_acq_result> results_pin;
@@ -91,7 +80,41 @@ struct b200_acq
 namespace
 {
 int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev,
-    int step_two, float prev_input_power);
+    int step_two, float prev_input_power, uint64_t& launched);
+
+int mixed_radix_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
+    b200_acq_result* results_dev, int step_two, float prev_input_power, uint64_t& launched)
+{
+    const b200_acq_conf& c = a->c;
+    cudaStream_t st = a->stream;
+    bool same = a->slots_on_device.size() == n_slots;
+    for (uint32_t i = 0; same && i < n_slots; i++) same = a->slots_on_device[i] == static_cast<int>(slots[i]);
+    if (!same)
+        {
+            // slot_pin is read by the asynchronous copy: wait for a previous upload's reader before rewriting it
+            B200_CUDA_TRY(cudaStreamSynchronize(st));
+            for (uint32_t i = 0; i < n_slots; i++) a->slot_pin[i] = static_cast<int>(slots[i]);
+            B200_CUDA_TRY(cudaMemcpyAsync(a->slot_list, a->slot_pin, sizeof(int) * n_slots, cudaMemcpyHostToDevice, st));
+            a->slots_on_device.assign(a->slot_pin.get(), a->slot_pin.get() + n_slots);
+        }
+    const int bins = step_two ? static_cast<int>(a->bins2) : static_cast<int>(c.num_doppler_bins);
+    const float2* wipe = step_two ? a->wipe2 : a->wipe;
+    const int ne = static_cast<int>(c.effective_fft_size);
+    const int off = c.bit_transition_flag ? ne : 0;
+    int rc = acq_launch_fwd(in_dev, static_cast<int>(c.consumed_samples), wipe, a->X, bins, a->plan, a->tw, launched, st);
+    if (rc) return rc;
+    rc = acq_launch_row_stats(a->X, a->codes, a->slot_list, static_cast<int>(n_slots), bins, a->plan, a->tw, off, ne, a->grid,
+        dwell_counter > 1 ? 1 : 0, a->rowstat, a->Z, a->partial, launched, st);
+    if (rc) return rc;
+    rc = acq_launch_stats(a->rowstat, static_cast<int>(n_slots), bins, ne, c.doppler_max, a->doppler_center, c.doppler_step,
+        dwell_counter, c.use_cfar, a->best, results_dev, step_two, a->center2, a->step2, prev_input_power, launched, st);
+    if (rc) return rc;
+    if (c.use_cfar) return B200_OK;
+    rc = acq_launch_second_peak(a->X, a->codes, a->slot_list, static_cast<int>(n_slots), bins, a->plan, a->tw, off, ne, a->grid, a->best,
+        static_cast<int>(c.samples_per_chip), a->second_peak, a->Z, a->partial, launched, st);
+    if (rc) return rc;
+    return acq_launch_finish_second_peak(a->second_peak, static_cast<int>(n_slots), results_dev, launched, st);
+}
 
 int search_impl(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
     b200_acq_result* results_dev, int step_two = 0, float prev_input_power = 0.f)
@@ -113,59 +136,18 @@ int search_impl(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32
                     return B200_ERR_STATE;
                 }
         }
-    if (a->bl)
-        {
-            if (step_two && (a->bins2 == 0 || !a->bl->mult2 || n_slots != 1))
-                {
-                    set_error("step two needs b200_acq_set_step_two first and exactly one slot");
-                    return B200_ERR_STATE;
-                }
-            return bluestein_search(a, in_dev, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power);
-        }
-    cudaStream_t st = a->stream;
-    bool same = a->slots_on_device.size() == n_slots;
-    for (uint32_t i = 0; same && i < n_slots; i++) same = a->slots_on_device[i] == static_cast<int>(slots[i]);
-    if (!same)
-        {
-            // slot_pin is read by the asynchronous copy: wait for a previous upload's reader before rewriting it
-            B200_CUDA_TRY(cudaStreamSynchronize(st));
-            for (uint32_t i = 0; i < n_slots; i++) a->slot_pin[i] = static_cast<int>(slots[i]);
-            B200_CUDA_TRY(cudaMemcpyAsync(a->slot_list, a->slot_pin, sizeof(int) * n_slots, cudaMemcpyHostToDevice, st));
-            a->slots_on_device.assign(a->slot_pin.get(), a->slot_pin.get() + n_slots);
-        }
-    const int n = static_cast<int>(c.fft_size);
-    if (step_two && (a->bins2 == 0 || !a->wipe2 || n_slots != 1))
+    const float2* rows2 = a->bl ? a->bl->mult2.get() : a->wipe2.get();  // the step-two rows b200_acq_set_step_two built
+    if (step_two && (a->bins2 == 0 || !rows2 || n_slots != 1))
         {
             set_error("step two needs b200_acq_set_step_two first and exactly one slot");
             return B200_ERR_STATE;
         }
-    const int bins = step_two ? static_cast<int>(a->bins2) : static_cast<int>(c.num_doppler_bins);
-    const float2* wipe = step_two ? a->wipe2 : a->wipe;
-    const int ne = static_cast<int>(c.effective_fft_size);
-    const int off = c.bit_transition_flag ? ne : 0;
-    int rc = acq_launch_fwd(in_dev, static_cast<int>(c.consumed_samples), wipe, a->X, bins, a->plan, a->tw, st);
+    uint64_t launched = 0;
+    const int rc = a->bl ? bluestein_search(a, in_dev, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power, launched)
+                         : mixed_radix_search(a, in_dev, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power, launched);
     if (rc) return rc;
-    rc = acq_launch_corr(a->X, a->codes, a->slot_list, static_cast<int>(n_slots), bins, a->plan, a->tw, off, ne, a->rowstat, a->grid,
-        dwell_counter > 1 ? 1 : 0, 0, nullptr, 0, nullptr, a->Z, a->partial, st);
-    if (rc) return rc;
-    rc = acq_launch_stats(a->rowstat, static_cast<int>(n_slots), bins, ne, c.doppler_max, a->doppler_center, c.doppler_step,
-        dwell_counter, c.use_cfar, a->best, results_dev, step_two, a->center2, a->step2, prev_input_power, st);
-    if (rc) return rc;
-    uint64_t launched = 3;
-    if (!c.use_cfar)
-        {
-            rc = acq_launch_corr(a->X, a->codes, a->slot_list, static_cast<int>(n_slots), bins, a->plan, a->tw, off, ne, a->rowstat,
-                a->grid, 0, 1, a->best, static_cast<int>(c.samples_per_chip), a->second_peak, a->Z, a->partial, st);
-            if (rc) return rc;
-            rc = acq_launch_finish_second_peak(a->second_peak, static_cast<int>(n_slots), results_dev, st);
-            if (rc) return rc;
-            launched += 2;
-        }
-    {
-        std::lock_guard<std::mutex> lk(a->e->mu);
-        a->e->launches += launched;
-    }
-    (void)n;
+    std::lock_guard<std::mutex> lk(a->e->mu);
+    a->e->launches += launched;
     return B200_OK;
 }
 }  // namespace
@@ -282,17 +264,18 @@ int bluestein_setup_queue(b200_acq* a, std::vector<float2> (&host)[6])
 // rows x N: out[r] = DFT_N(in[r * in_stride .. ] . mult[r * mult_stride ..])   (forward chirp-z, natural order); inputs past
 // `consumed` count as zeros (acquisition_core zero-pads the consumed samples to fft_size, :657-664)
 int bluestein_forward_rows(b200_acq* a, const float2* in, size_t in_stride, int consumed, const float2* mult, size_t mult_stride, int rows,
-    float2* out)
+    float2* out, uint64_t& launched)
 {
     b200_acq::Bluestein* b = a->bl.get();
     const int n = static_cast<int>(a->c.fft_size);
-    int rc = acq_launch_fwd_rows(in, in_stride, consumed, mult, mult_stride, b->A, rows, b->plM, b->twM, a->stream);
+    int rc = acq_launch_fwd_rows(in, in_stride, consumed, mult, mult_stride, b->A, rows, b->plM, b->twM, launched, a->stream);
     if (rc) return rc;
-    return acq_launch_inverse_store_rows(b->A, b->filt, b->slot_ids, rows, b->plM, b->twM, b->Zw, b->chirp_conj_M, n, out, n, a->stream);
+    return acq_launch_inverse_store_rows(b->A, b->filt, b->slot_ids, rows, b->plM, b->twM, b->Zw, b->chirp_conj_M, n, out, n, launched,
+        a->stream);
 }
 
 int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev,
-    int step_two, float prev_input_power)
+    int step_two, float prev_input_power, uint64_t& launched)
 {
     b200_acq::Bluestein* b = a->bl.get();
     const b200_acq_conf& c = a->c;
@@ -302,30 +285,22 @@ int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, u
     const int ne = static_cast<int>(c.effective_fft_size);
     const int off = c.bit_transition_flag ? ne : 0;
     // X_d = DFT_N(x . wipe_d) for every Doppler bin, once per sweep (x: the consumed samples, zero-padded to N)
-    int rc = bluestein_forward_rows(a, in_dev, 0, static_cast<int>(c.consumed_samples), mult, n, bins, b->Xs);
+    int rc = bluestein_forward_rows(a, in_dev, 0, static_cast<int>(c.consumed_samples), mult, n, bins, b->Xs, launched);
     if (rc) return rc;
-    uint64_t launched = 4;
     for (uint32_t i = 0; i < n_slots; i++)
         {
             // rows of this PRN: y = IDFT_N(X_d . C) = w . IFFT_M(FFT_M(pad(X_d . C . w)) . FFT_M(conj h)) / M ; |w| = 1
-            rc = acq_launch_fwd_rows(b->Xs, n, n, b->CW + static_cast<size_t>(slots[i]) * n, 0, b->A, bins, b->plM, b->twM, a->stream);
+            rc = acq_launch_fwd_rows(b->Xs, n, n, b->CW + static_cast<size_t>(slots[i]) * n, 0, b->A, bins, b->plM, b->twM, launched, a->stream);
             if (rc) return rc;
             // the correlation kernel addresses the grid by code-slot id, and the "code" here is filter slot 1; the grid rows are
             // [off, off + ne) of y, so slot s lands where the mixed-radix search puts it: (s * bins + bin) * ne
             float* grid = a->grid ? a->grid + (static_cast<ptrdiff_t>(slots[i]) - 1) * static_cast<ptrdiff_t>(bins) * ne : nullptr;
-            rc = acq_launch_corr(b->A, b->filt, b->slot_ids + 1, 1, bins, b->plM, b->twM, off, ne, a->rowstat + static_cast<size_t>(i) * bins, grid,
-                dwell_counter > 1 ? 1 : 0, 0, nullptr, 0, nullptr, b->Zw, b->partial, a->stream);
+            rc = acq_launch_row_stats(b->A, b->filt, b->slot_ids + 1, 1, bins, b->plM, b->twM, off, ne, grid, dwell_counter > 1 ? 1 : 0,
+                a->rowstat + static_cast<size_t>(i) * bins, b->Zw, b->partial, launched, a->stream);
             if (rc) return rc;
-            launched += 5;
         }
-    rc = acq_launch_stats(a->rowstat, static_cast<int>(n_slots), bins, ne, c.doppler_max, a->doppler_center, c.doppler_step, dwell_counter, c.use_cfar,
-        a->best, results_dev, step_two, a->center2, a->step2, prev_input_power, a->stream);
-    if (rc) return rc;
-    {
-        std::lock_guard<std::mutex> lk(a->e->mu);
-        a->e->launches += launched + 1;
-    }
-    return B200_OK;
+    return acq_launch_stats(a->rowstat, static_cast<int>(n_slots), bins, ne, c.doppler_max, a->doppler_center, c.doppler_step, dwell_counter,
+        c.use_cfar, a->best, results_dev, step_two, a->center2, a->step2, prev_input_power, launched, a->stream);
 }
 }  // namespace
 
@@ -387,7 +362,7 @@ extern "C"
         B200_CUDA_TRY(a->code_stage.alloc(n));
         B200_CUDA_TRY(a->rowstat.alloc(bins * slots));
         B200_CUDA_TRY(a->slot_list.alloc(slots));
-        B200_CUDA_TRY(a->best.alloc(8 * slots));
+        B200_CUDA_TRY(a->best.alloc(slots));
         B200_CUDA_TRY(a->second_peak.alloc(slots));
         B200_CUDA_TRY(a->results_dev.alloc(slots));
         B200_CUDA_TRY(a->results_pin.alloc(slots));
@@ -443,15 +418,15 @@ extern "C"
         const size_t need = (c.code_layout == 1) ? c.fft_size / 2 : c.consumed_samples;
         if (a->bl)
             {
-                // the code staged in an N-point buffer where set_local_code places it (:230-246): layout 0 at the front, layout 1 in
-                // the second half, layout 2 at the end, zeros elsewhere
+                // the code staged in an N-point buffer where set_local_code places it (acq_code_offset), zeros elsewhere
                 b200_acq::Bluestein* b = a->bl.get();
                 const int n = static_cast<int>(c.fft_size);
-                const size_t place = (c.code_layout == 1) ? c.fft_size / 2 : (c.code_layout == 2) ? c.fft_size - c.consumed_samples : 0;
+                const int place = acq_code_offset(static_cast<int>(c.code_layout), n, static_cast<int>(c.consumed_samples));
                 if (need < c.fft_size) B200_CUDA_TRY(cudaMemsetAsync(a->code_stage, 0, sizeof(float2) * c.fft_size, a->stream));
                 B200_CUDA_TRY(cudaMemcpyAsync(a->code_stage + place, code_host, sizeof(float2) * need, cudaMemcpyHostToDevice, a->stream));
                 // CW = conj(DFT_N(code)) . w / M  (volk_32fc_conjugate_32fc of set_local_code :250, then the inverse chirp-z pre-multiplier)
-                int rcb = bluestein_forward_rows(a, a->code_stage, 0, n, b->chirp_conj, 0, 1, b->Xs);
+                uint64_t setup_launches = 0;  // set-up, not counted
+                int rcb = bluestein_forward_rows(a, a->code_stage, 0, n, b->chirp_conj, 0, 1, b->Xs, setup_launches);
                 if (rcb) return rcb;
                 rcb = acq_launch_rows_times_vector(b->Xs, n, b->chirp_M, n, 1, b->CW + static_cast<size_t>(slot) * n, n, 1, a->stream);
                 if (rcb) return rcb;
@@ -553,6 +528,18 @@ extern "C"
         return rc;
     }
 
+    // search the samples in a->in_dev, then bring the n_slots result records back to the host
+    static int search_to_host(b200_acq* a, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, int step_two, float prev_input_power,
+        b200_acq_result* results_host)
+    {
+        const int rc = search_impl(a, a->in_dev, slots, n_slots, dwell_counter, a->results_dev, step_two, prev_input_power);
+        if (rc) return rc;
+        B200_CUDA_TRY(cudaMemcpyAsync(a->results_pin, a->results_dev, sizeof(b200_acq_result) * n_slots, cudaMemcpyDeviceToHost, a->stream));
+        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
+        std::memcpy(results_host, a->results_pin, sizeof(b200_acq_result) * n_slots);
+        return B200_OK;
+    }
+
     int b200_acq_search_i16(b200_acq* a, const int16_t* in_host_iq, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
         b200_acq_result* results_host)
     {
@@ -563,14 +550,9 @@ extern "C"
                 return B200_ERR_STATE;
             }
         B200_ENTER_DEVICE(a->e->device);
-        int rc = upload_i16(a, in_host_iq);
+        const int rc = upload_i16(a, in_host_iq);
         if (rc) return rc;
-        rc = search_impl(a, a->in_dev, slots, n_slots, dwell_counter, a->results_dev);
-        if (rc) return rc;
-        B200_CUDA_TRY(cudaMemcpyAsync(a->results_pin, a->results_dev, sizeof(b200_acq_result) * n_slots, cudaMemcpyDeviceToHost, a->stream));
-        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-        std::memcpy(results_host, a->results_pin, sizeof(b200_acq_result) * n_slots);
-        return B200_OK;
+        return search_to_host(a, slots, n_slots, dwell_counter, 0, 0.f, results_host);
     }
 
     int b200_acq_search_step_two_i16(b200_acq* a, const int16_t* in_host_iq, uint32_t slot, uint32_t dwell_counter, float prev_input_power,
@@ -578,14 +560,9 @@ extern "C"
     {
         if (!a || !in_host_iq || !result_host) return B200_ERR_ARG;
         B200_ENTER_DEVICE(a->e->device);
-        int rc = upload_i16(a, in_host_iq);
+        const int rc = upload_i16(a, in_host_iq);
         if (rc) return rc;
-        rc = search_impl(a, a->in_dev, &slot, 1, dwell_counter, a->results_dev, 1, prev_input_power);
-        if (rc) return rc;
-        B200_CUDA_TRY(cudaMemcpyAsync(a->results_pin, a->results_dev, sizeof(b200_acq_result), cudaMemcpyDeviceToHost, a->stream));
-        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-        *result_host = a->results_pin[0];
-        return B200_OK;
+        return search_to_host(a, &slot, 1, dwell_counter, 1, prev_input_power, result_host);
     }
 
     int b200_acq_set_step_two(b200_acq* a, float doppler_center_step_two, float doppler_step2, uint32_t num_doppler_bins_step2)
@@ -630,12 +607,7 @@ extern "C"
         if (!a || !in_host || !result_host) return B200_ERR_ARG;
         B200_ENTER_DEVICE(a->e->device);
         B200_CUDA_TRY(cudaMemcpyAsync(a->in_dev, in_host, sizeof(float2) * a->c.consumed_samples, cudaMemcpyHostToDevice, a->stream));
-        int rc = search_impl(a, a->in_dev, &slot, 1, dwell_counter, a->results_dev, 1, prev_input_power);
-        if (rc) return rc;
-        B200_CUDA_TRY(cudaMemcpyAsync(a->results_pin, a->results_dev, sizeof(b200_acq_result), cudaMemcpyDeviceToHost, a->stream));
-        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-        *result_host = a->results_pin[0];
-        return B200_OK;
+        return search_to_host(a, &slot, 1, dwell_counter, 1, prev_input_power, result_host);
     }
 
     int b200_acq_search_dev(b200_acq* a, const b200_cf32* in_dev, const uint32_t* slots_host, uint32_t n_slots,
@@ -652,13 +624,12 @@ extern "C"
         b200_acq_peak* peak_dev)
     {
         if (!a || !results_dev || !prn_of_result_dev || !peak_dev) return B200_ERR_ARG;
-        const int rc = acq_launch_sweep_best(results_dev, prn_of_result_dev, static_cast<int>(n_results), peak_dev, a->stream);
-        if (rc == B200_OK)
-            {
-                std::lock_guard<std::mutex> lk(a->e->mu);
-                a->e->launches++;
-            }
-        return rc;
+        uint64_t launched = 0;
+        const int rc = acq_launch_sweep_best(results_dev, prn_of_result_dev, static_cast<int>(n_results), peak_dev, launched, a->stream);
+        if (rc) return rc;
+        std::lock_guard<std::mutex> lk(a->e->mu);
+        a->e->launches += launched;
+        return B200_OK;
     }
 
     int b200_acq_selftest_dft(b200_acq* a, const b200_cf32* in_host, b200_cf32* out_host)
@@ -672,21 +643,10 @@ extern "C"
         B200_ENTER_DEVICE(a->e->device);
         const size_t n = a->c.fft_size;
         B200_CUDA_TRY(cudaMemcpyAsync(a->code_stage, in_host, sizeof(float2) * n, cudaMemcpyHostToDevice, a->stream));
-        const int rc = bluestein_forward_rows(a, a->code_stage, 0, static_cast<int>(n), a->bl->chirp_conj, 0, 1, a->bl->Xs);
+        uint64_t selftest_launches = 0;  // a self-test, not a search: not counted
+        const int rc = bluestein_forward_rows(a, a->code_stage, 0, static_cast<int>(n), a->bl->chirp_conj, 0, 1, a->bl->Xs, selftest_launches);
         if (rc) return rc;
         B200_CUDA_TRY(cudaMemcpyAsync(out_host, a->bl->Xs, sizeof(float2) * n, cudaMemcpyDeviceToHost, a->stream));
-        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-        return B200_OK;
-    }
-
-    int b200_acq_selftest_read(b200_acq* a, int what, b200_cf32* out_host)
-    {
-        if (!a || !out_host || what < 0 || what > 1) return B200_ERR_ARG;
-        if (!a->bl) return B200_ERR_STATE;
-        B200_ENTER_DEVICE(a->e->device);
-        const size_t n = a->c.fft_size;
-        const size_t rows = what == 0 ? a->c.num_doppler_bins : a->c.n_code_slots;
-        B200_CUDA_TRY(cudaMemcpyAsync(out_host, what == 0 ? a->bl->Xs : a->bl->CW, sizeof(float2) * n * rows, cudaMemcpyDeviceToHost, a->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
         return B200_OK;
     }

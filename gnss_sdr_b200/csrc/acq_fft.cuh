@@ -54,6 +54,11 @@ __device__ __forceinline__ float2 cmul(float2 a, float2 b)
 {
     return make_float2(fmaf(a.x, b.x, -a.y * b.y), fmaf(a.x, b.y, a.y * b.x));
 }
+// volk_32fc_x2_multiply_32fc: every product and sum rounded on its own, in the reference's order
+__device__ __forceinline__ float2 cmul_rn(float2 a, float2 b)
+{
+    return make_float2(__fsub_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)), __fadd_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x)));
+}
 __device__ __forceinline__ float2 cmul_conj(float2 a, float2 b)  // a * conj(b)
 {
     return make_float2(fmaf(a.x, b.x, a.y * b.y), fmaf(a.y, b.x, -a.x * b.y));
@@ -466,12 +471,7 @@ __device__ __forceinline__ void fft_first_inv_stage_from_global(const float2* __
                     b[q] = __ldg(c + q * nb + i);
                 }
 #pragma unroll
-            for (int q = 0; q < R; q++)
-                {
-                    const float re = __fsub_rn(__fmul_rn(a[q].x, b[q].x), __fmul_rn(a[q].y, b[q].y));
-                    const float im = __fadd_rn(__fmul_rn(a[q].x, b[q].y), __fmul_rn(a[q].y, b[q].x));
-                    v[q] = make_float2(im, re);  // swap_ri: inverse = swap . forward . swap
-                }
+            for (int q = 0; q < R; q++) v[q] = swap_ri(cmul_rn(a[q], b[q]));  // inverse = swap . forward . swap
             Bfly<R>::fwd(v);
 #pragma unroll
             for (int q = 0; q < R; q++) s[i * R + q] = swap_ri(v[q]);

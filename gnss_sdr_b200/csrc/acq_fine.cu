@@ -17,10 +17,6 @@
 #include <new>
 #include <vector>
 
-namespace b200
-{
-struct AcqRowStat;
-}
 using namespace b200;
 
 namespace
@@ -78,10 +74,10 @@ struct FineBest
     unsigned int index;
 };
 
-__global__ void __launch_bounds__(1024) acq_fine_argmax_kernel(const float2* __restrict__ X, FftPlan pl, FineBest* __restrict__ out)
+constexpr int kArgmaxThreads = 1024;
+
+__global__ void __launch_bounds__(kArgmaxThreads) acq_fine_argmax_kernel(const float2* __restrict__ X, FftPlan pl, FineBest* __restrict__ out)
 {
-    __shared__ float red_v[32];
-    __shared__ unsigned int red_i[32];
     const int m = pl.n_total;
     float bv = -1.0f;
     unsigned int bi = 0xffffffffu;
@@ -100,31 +96,10 @@ __global__ void __launch_bounds__(1024) acq_fine_argmax_kernel(const float2* __r
                         }
                 }
         }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-        {
-            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-            const unsigned int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (ov > bv || (ov == bv && oi < bi))
-                {
-                    bv = ov;
-                    bi = oi;
-                }
-        }
-    if ((threadIdx.x & 31) == 0)
-        {
-            red_v[threadIdx.x >> 5] = bv;
-            red_i[threadIdx.x >> 5] = bi;
-        }
-    __syncthreads();
+    float no_sum = 0.0f;
+    acq_cta_first_max<kArgmaxThreads / 32>(bv, bi, no_sum);
     if (threadIdx.x == 0)
         {
-            for (int w = 1; w < static_cast<int>(blockDim.x >> 5); w++)
-                if (red_v[w] > bv || (red_v[w] == bv && red_i[w] < bi))
-                    {
-                        bv = red_v[w];
-                        bi = red_i[w];
-                    }
             out->peak = bv;
             out->index = bi;
         }
@@ -212,14 +187,16 @@ extern "C"
         const dim3 g((f->m + 255) / 256, kZeroPadding);
         acq_fine_modulate_kernel<<<g, 256, 0, f->stream>>>(f->code_dev, f->n1ms, f->m, f->rows);
         B200_CUDA_TRY(cudaGetLastError());
+        uint64_t launched = 1;  // acq_fine_modulate_kernel
         // volk_32fc_x2_multiply_32fc (:347) fused into the transform's load, then the 8 M-point FFTs
-        int rc = acq_launch_fwd(f->in_dev, f->m, f->rows, f->X, kZeroPadding, f->plan, f->tw, f->stream);
+        int rc = acq_launch_fwd(f->in_dev, f->m, f->rows, f->X, kZeroPadding, f->plan, f->tw, launched, f->stream);
         if (rc) return rc;
-        acq_fine_argmax_kernel<<<1, 1024, 0, f->stream>>>(f->X, f->plan, f->best_dev);
+        acq_fine_argmax_kernel<<<1, kArgmaxThreads, 0, f->stream>>>(f->X, f->plan, f->best_dev);
         B200_CUDA_TRY(cudaGetLastError());
+        launched += 1;
         B200_CUDA_TRY(cudaMemcpyAsync(f->best_pin, f->best_dev, sizeof(FineBest), cudaMemcpyDeviceToHost, f->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(f->stream));
-        f->e->launches += (f->plan.n1 > 1) ? 4 : 3;
+        f->e->launches += launched;  // (under e->mu, held for the whole estimate)
         *index_freq = f->best_pin->index;
         if (peak) *peak = f->best_pin->peak;
         return B200_OK;

@@ -25,14 +25,6 @@
 
 namespace b200
 {
-struct AcqRowStat
-{
-    float max;
-    unsigned int argmax;
-    float sum;
-    float pad;
-};
-
 namespace
 {
 // ---- wipe-off carrier, reference float32 semantics --------------------------------------------
@@ -134,34 +126,20 @@ __global__ void acq_wipeoff_kernel(float2* __restrict__ wipe, int n, int bins, i
 }
 
 // ---- set_local_code ------------------------------------------------------------------------------
-// layout 0: code[0..consumed) at the front (sampled_ms == ms_per_code)          (:238-241)
-// layout 1: bit_transition_flag: zeros in the first half, code[0..n/2) in the second (:230-235)
-// layout 2: zero-padded front: code[0..consumed) at [n-consumed, n)               (:243-246)
+// sample i of the n-point buffer that set_local_code fills from `code` (acq_code_offset)
+__device__ __forceinline__ float2 acq_code_sample(const float2* __restrict__ code, int i, int n, int consumed, int layout)
+{
+    const int off = acq_code_offset(layout, n, consumed);
+    const int end = (layout == 0) ? consumed : n;
+    return (i >= off && i < end) ? code[i - off] : make_float2(0.f, 0.f);
+}
+
 template <int THREADS>
 __global__ void __launch_bounds__(THREADS, 1) acq_code_fft_kernel(const float2* __restrict__ code, int consumed, int layout,
     float2* __restrict__ out, FftPlan pl, const float2* __restrict__ tw)
 {
     extern __shared__ __align__(16) float2 s[];
-    const int n = pl.n;
-    for (int i = threadIdx.x; i < n; i += blockDim.x)
-        {
-            float2 v = make_float2(0.f, 0.f);
-            if (layout == 0)
-                {
-                    if (i < consumed) v = code[i];
-                }
-            else if (layout == 1)
-                {
-                    const int off = n / 2;
-                    if (i >= off) v = code[i - off];
-                }
-            else
-                {
-                    const int off = n - consumed;
-                    if (i >= off) v = code[i - off];
-                }
-            s[i] = v;
-        }
+    for (int i = threadIdx.x; i < pl.n; i += blockDim.x) s[i] = acq_code_sample(code, i, pl.n, consumed, layout);
     // forward FFT, then volk_32fc_conjugate_32fc (:250) fused into the store
     fft_forward_to_global<true, THREADS == kAcqThreads25>(s, pl, tw, out);
 }
@@ -179,31 +157,63 @@ __global__ void __launch_bounds__(THREADS, 1) acq_fwd_kernel(const float2* __res
     for (int i = threadIdx.x; i < n; i += blockDim.x)
         {
             // acquisition_core zero-pads beyond consumed samples (:657-664); volk_32fc_x2_multiply_32fc (:531)
-            float2 v = make_float2(0.f, 0.f);
-            if (i < consumed)
-                {
-                    const float2 a = in[i];
-                    const float2 b = w[i];
-                    v.x = __fsub_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
-                    v.y = __fadd_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x));
-                }
-            s[i] = v;
+            s[i] = (i < consumed) ? cmul_rn(in[i], w[i]) : make_float2(0.f, 0.f);
         }
     fft_forward_to_global<false, THREADS == kAcqThreads25>(s, pl, tw, X + static_cast<size_t>(d) * n);
 }
 
 // ---- correlation rows ---------------------------------------------------------------------------------
+// Row r of a correlation launch.  best == nullptr: every (slot, bin) row, r = slot_pos * bins + bin.  Otherwise the
+// second-peak pass: r = slot_pos, its winning bin from best[r], and the window of +-samples_per_chip around the winning
+// index_time excluded (pcps_acquisition.cc:485-497).
+struct AcqRow
+{
+    int slot_pos, bin;
+    int ex1, ex2;  // excluded window [ex1, ex2) with wrap-around; ex1 < 0: none
+    __device__ __forceinline__ AcqRow(int r, int bins, const AcqBest* __restrict__ best, int samples_per_chip, int ne)
+    {
+        if (best == nullptr)
+            {
+                slot_pos = r / bins;
+                bin = r - slot_pos * bins;
+                ex1 = ex2 = -1;
+                return;
+            }
+        slot_pos = r;
+        bin = static_cast<int>(best[r].index_doppler);
+        ex1 = static_cast<int>(best[r].index_time) - samples_per_chip;
+        ex2 = static_cast<int>(best[r].index_time) + samples_per_chip;
+        if (ex1 < 0)
+            ex1 = ne + ex1;
+        else if (ex2 >= ne)
+            ex2 = ex2 - ne;
+    }
+    __device__ __forceinline__ bool in_window(int t) const { return (ex1 <= ex2) ? (t >= ex1 && t < ex2) : (t >= ex1 || t < ex2); }
+};
+
 struct RowSink
 {
     // natural-order outputs of the last inverse stage -> |y|^2 -> running statistics
     int off;        // first output index that counts (bit_transition: effective_fft_size, else 0)
     int ne;         // effective_fft_size
-    int ex1, ex2;   // excluded window [ex1, ex2) with wrap-around; ex1 < 0 disables
+    AcqRow row;
     float* grid;    // optional magnitude row (ne floats): store or accumulate
     int accumulate;
     float best;
     unsigned int best_t;
     float sum;
+    __device__ __forceinline__ RowSink(int off_, int ne_, const AcqRow& row_, float* grid_, int accumulate_)
+        : off(off_), ne(ne_), row(row_), grid(grid_), accumulate(accumulate_), best(-1.0f), best_t(0xffffffffu), sum(0.0f)
+    {
+    }
+    __device__ __forceinline__ void keep_first_max(float mag, int t)
+    {
+        if (mag > best || (mag == best && static_cast<unsigned int>(t) < best_t))
+            {
+                best = mag;
+                best_t = static_cast<unsigned int>(t);
+            }
+    }
     __device__ __forceinline__ void operator()(float2* /*p*/, int pos, float2 v)
     {
         const int t = pos - off;
@@ -215,99 +225,37 @@ struct RowSink
                 if (accumulate) mag = __fadd_rn(grid[t], mag);  // volk_32f_x2_add_32f (:552)
                 grid[t] = mag;
             }
-        if (ex1 >= 0)
-            {
-                const bool excluded = (ex1 <= ex2) ? (t >= ex1 && t < ex2) : (t >= ex1 || t < ex2);
-                if (excluded) mag = 0.0f;  // the reference zeroes the window before its second arg-max (:499-509)
-            }
+        // the reference zeroes the window before its second arg-max (:499-509)
+        if (row.ex1 >= 0 && row.in_window(t)) mag = 0.0f;
         sum += mag;
-        if (mag > best || (mag == best && static_cast<unsigned int>(t) < best_t))
-            {
-                best = mag;
-                best_t = static_cast<unsigned int>(t);
-            }
+        keep_first_max(mag, t);
     }
 };
 
-struct AcqBest
-{
-    unsigned int index_time;
-    unsigned int index_doppler;
-};
-
-// mode 0: grid = n_slots * bins rows; row r -> slot_list[r / bins], bin r % bins; writes rowstat.
-// mode 1: grid = n_slots; row = the winning (bin, index_time) in best[]; excluded window of
-//         +-samples_per_chip around the peak; writes second_peak[slot].
+// best == nullptr: one CTA per (slot, bin) row, writes rowstat.  Otherwise one CTA per slot over its winning row (AcqRow),
+// writes second_peak[slot_pos].
 template <int THREADS>
 __global__ void __launch_bounds__(THREADS, 1) acq_corr_kernel(const float2* __restrict__ X, const float2* __restrict__ codes,
     const int* __restrict__ slot_list, int bins, FftPlan pl, const float2* __restrict__ tw, int off, int ne,
-    AcqRowStat* __restrict__ rowstat, float* __restrict__ grid, int accumulate, int mode,
+    AcqRowStat* __restrict__ rowstat, float* __restrict__ grid, int accumulate,
     const AcqBest* __restrict__ best, int samples_per_chip, float* __restrict__ second_peak)
 {
     extern __shared__ __align__(16) float2 s[];
-    __shared__ float red_v[THREADS / 32];
-    __shared__ unsigned int red_i[THREADS / 32];
-    __shared__ float red_s[THREADS / 32];
     const int n = pl.n;
-    int slot_pos, bin;
-    RowSink sink;
-    sink.off = off;
-    sink.ne = ne;
-    sink.ex1 = -1;
-    sink.ex2 = -1;
-    sink.grid = nullptr;
-    sink.accumulate = accumulate;
-    if (mode == 0)
-        {
-            slot_pos = blockIdx.x / bins;
-            bin = blockIdx.x - slot_pos * bins;
-        }
-    else
-        {
-            slot_pos = blockIdx.x;
-            bin = static_cast<int>(best[slot_pos].index_doppler);
-            // pcps_acquisition.cc:485-497
-            int e1 = static_cast<int>(best[slot_pos].index_time) - samples_per_chip;
-            int e2 = static_cast<int>(best[slot_pos].index_time) + samples_per_chip;
-            if (e1 < 0)
-                e1 = ne + e1;
-            else if (e2 >= ne)
-                e2 = e2 - ne;
-            sink.ex1 = e1;
-            sink.ex2 = e2;
-        }
-    const int slot = slot_list[slot_pos];
-    if (grid != nullptr)
-        {
-            sink.grid = grid + (static_cast<size_t>(slot) * bins + bin) * ne;
-            if (mode == 1)
-                {
-                    // second-peak pass over an already accumulated grid row: read it, do not touch it
-                    sink.grid = nullptr;
-                }
-        }
-    sink.best = -1.0f;
-    sink.best_t = 0xffffffffu;
-    sink.sum = 0.0f;
+    const AcqRow row(blockIdx.x, bins, best, samples_per_chip, ne);
+    const int slot = slot_list[row.slot_pos];
+    float* g = (grid != nullptr) ? grid + (static_cast<size_t>(slot) * bins + row.bin) * ne : nullptr;
+    // the second-peak pass reads an already accumulated grid row and does not touch it
+    RowSink sink(off, ne, row, best ? nullptr : g, accumulate);
 
-    if (mode == 1 && grid != nullptr)
+    if (best != nullptr && g != nullptr)
         {
             // dwell-accumulated grids: statistics come from the stored row, not from a recomputation
-            const float* g = grid + (static_cast<size_t>(slot) * bins + bin) * ne;
-            for (int t = threadIdx.x; t < ne; t += blockDim.x)
-                {
-                    const bool excluded = (sink.ex1 <= sink.ex2) ? (t >= sink.ex1 && t < sink.ex2) : (t >= sink.ex1 || t < sink.ex2);
-                    const float mag = excluded ? 0.0f : g[t];
-                    if (mag > sink.best || (mag == sink.best && static_cast<unsigned int>(t) < sink.best_t))
-                        {
-                            sink.best = mag;
-                            sink.best_t = static_cast<unsigned int>(t);
-                        }
-                }
+            for (int t = threadIdx.x; t < ne; t += blockDim.x) sink.keep_first_max(row.in_window(t) ? 0.0f : g[t], t);
         }
     else
         {
-            const float2* x = X + static_cast<size_t>(bin) * n;
+            const float2* x = X + static_cast<size_t>(row.bin) * n;
             const float2* c = codes + static_cast<size_t>(slot) * n;
             if (pl.perm_r > 1)
                 {
@@ -317,65 +265,21 @@ __global__ void __launch_bounds__(THREADS, 1) acq_corr_kernel(const float2* __re
             else
                 {
 #pragma unroll 4
-            for (int i = threadIdx.x; i < n; i += blockDim.x)
-                {
-                    // volk_32fc_x2_multiply_32fc (:538)
-                    const float2 a = __ldg(x + i);
-                    const float2 b = __ldg(c + i);
-                    s[i] = make_float2(__fsub_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)), __fadd_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x)));
-                }
-            fft_inverse_smem(s, pl, tw, sink);
+                    for (int i = threadIdx.x; i < n; i += blockDim.x) s[i] = cmul_rn(__ldg(x + i), __ldg(c + i));  // (:538)
+                    fft_inverse_smem(s, pl, tw, sink);
                 }
         }
 
-    // CTA reduction with "first maximum" tie-break
     float bv = sink.best;
     unsigned int bi = sink.best_t;
     float sm = sink.sum;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-        {
-            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-            const unsigned int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            sm += __shfl_xor_sync(0xffffffffu, sm, o);
-            if (ov > bv || (ov == bv && oi < bi))
-                {
-                    bv = ov;
-                    bi = oi;
-                }
-        }
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (lane == 0)
-        {
-            red_v[warp] = bv;
-            red_i[warp] = bi;
-            red_s[warp] = sm;
-        }
-    __syncthreads();
+    acq_cta_first_max<THREADS / 32>(bv, bi, sm);
     if (threadIdx.x == 0)
         {
-            for (int w = 1; w < THREADS / 32; w++)
-                {
-                    if (red_v[w] > bv || (red_v[w] == bv && red_i[w] < bi))
-                        {
-                            bv = red_v[w];
-                            bi = red_i[w];
-                        }
-                    sm += red_s[w];
-                }
-            if (mode == 0)
-                {
-                    AcqRowStat r;
-                    r.max = bv;
-                    r.argmax = bi;
-                    r.sum = sm;
-                    r.pad = 0.f;
-                    rowstat[static_cast<size_t>(slot_pos) * bins + bin] = r;
-                }
+            if (best == nullptr)
+                rowstat[static_cast<size_t>(row.slot_pos) * bins + row.bin] = AcqRowStat{bv, bi, sm, 0.f};
             else
-                {
-                    second_peak[slot_pos] = bv;
-                }
+                second_peak[row.slot_pos] = bv;
         }
 }
 
@@ -387,34 +291,9 @@ __device__ __forceinline__ float2 acq_source(const float2* __restrict__ in, cons
     int layout, int n_total)
 {
     // wipe != nullptr: signal * wipe-off, zero-padded beyond consumed (acquisition_core :657-664, :531)
-    // wipe == nullptr: local code placed by `layout` (set_local_code :230-246)
-    float2 v = make_float2(0.f, 0.f);
-    if (wipe != nullptr)
-        {
-            if (i < consumed)
-                {
-                    const float2 a = in[i];
-                    const float2 b = wipe[i];
-                    v.x = __fsub_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
-                    v.y = __fadd_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x));
-                }
-            return v;
-        }
-    if (layout == 0)
-        {
-            if (i < consumed) v = in[i];
-        }
-    else if (layout == 1)
-        {
-            const int off = n_total / 2;
-            if (i >= off) v = in[i - off];
-        }
-    else
-        {
-            const int off = n_total - consumed;
-            if (i >= off) v = in[i - off];
-        }
-    return v;
+    // wipe == nullptr: local code placed by `layout`
+    if (wipe != nullptr) return (i < consumed) ? cmul_rn(in[i], wipe[i]) : make_float2(0.f, 0.f);
+    return acq_code_sample(in, i, n_total, consumed, layout);
 }
 
 // in_stride / wipe_stride: elements between the inputs / multiplier tables of consecutive rows (0 = one shared by all rows)
@@ -456,83 +335,31 @@ __global__ void __launch_bounds__(kAcqThreads, 1) acq_block_fft_kernel(float2* _
     for (int i = threadIdx.x; i < n; i += blockDim.x) blk[i] = conj_out ? make_float2(s[i].x, -s[i].y) : s[i];
 }
 
-// rows: mode 0 -> r = slot_pos * bins + bin ; mode 1 -> r = slot_pos (bin from best[])
+// block p of row r (AcqRow; the exclusion window is the final stage's)
 __global__ void __launch_bounds__(kAcqThreads, 1) acq_corr_block_kernel(const float2* __restrict__ X, const float2* __restrict__ codes,
-    const int* __restrict__ slot_list, int bins, FftPlan pl, const float2* __restrict__ tw, float2* __restrict__ Z, int mode,
+    const int* __restrict__ slot_list, int bins, FftPlan pl, const float2* __restrict__ tw, float2* __restrict__ Z,
     const AcqBest* __restrict__ best)
 {
     extern __shared__ __align__(16) float2 s[];
     const int n = pl.n;
     const int p = blockIdx.x;
     const int r = blockIdx.y;
-    int slot_pos, bin;
-    if (mode == 0)
-        {
-            slot_pos = r / bins;
-            bin = r - slot_pos * bins;
-        }
-    else
-        {
-            slot_pos = r;
-            bin = static_cast<int>(best[r].index_doppler);
-        }
-    const int slot = slot_list[slot_pos];
-    const float2* x = X + static_cast<size_t>(bin) * pl.n_total + static_cast<size_t>(p) * n;
+    const AcqRow row(r, bins, best, 0, 0);
+    const int slot = slot_list[row.slot_pos];
+    const float2* x = X + static_cast<size_t>(row.bin) * pl.n_total + static_cast<size_t>(p) * n;
     const float2* c = codes + static_cast<size_t>(slot) * pl.n_total + static_cast<size_t>(p) * n;
 #pragma unroll 4
-    for (int i = threadIdx.x; i < n; i += blockDim.x)
-        {
-            const float2 a = __ldg(x + i);
-            const float2 b = __ldg(c + i);
-            s[i] = make_float2(__fsub_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)), __fadd_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x)));
-        }
+    for (int i = threadIdx.x; i < n; i += blockDim.x) s[i] = cmul_rn(__ldg(x + i), __ldg(c + i));
     fft_inverse_smem_inplace(s, pl, tw);
     float2* z = Z + static_cast<size_t>(r) * pl.n_total + static_cast<size_t>(p) * n;
     for (int i = threadIdx.x; i < n; i += blockDim.x) z[i] = s[i];
 }
 
-// final radix-n1 DIT stage + |.|^2 + statistics; grid (chunks, rows); partial[r * chunks + chunk]
-template <int R>
-__global__ void __launch_bounds__(256) acq_global_final_stage(const float2* __restrict__ Z, FftPlan pl, const float2* __restrict__ tw,
-    const int* __restrict__ slot_list, int bins, int off, int ne, float* __restrict__ grid, int accumulate, int mode,
-    const AcqBest* __restrict__ best, int samples_per_chip, AcqRowStat* __restrict__ partial)
+// final radix-n1 DIT stage of row z over the CTAs of grid.x: natural-order output k goes to sink(nullptr, k, y[k])
+template <int R, class Sink>
+__device__ __forceinline__ void acq_global_final_dit(const float2* __restrict__ z, const FftPlan& pl, const float2* __restrict__ tw, Sink& sink)
 {
-    __shared__ float red_v[8];
-    __shared__ unsigned int red_i[8];
-    __shared__ float red_s[8];
-    const int r = blockIdx.y;
     const int n2 = pl.n;
-    int slot_pos, bin;
-    RowSink sink;
-    sink.off = off;
-    sink.ne = ne;
-    sink.ex1 = -1;
-    sink.ex2 = -1;
-    sink.grid = nullptr;
-    sink.accumulate = accumulate;
-    if (mode == 0)
-        {
-            slot_pos = r / bins;
-            bin = r - slot_pos * bins;
-        }
-    else
-        {
-            slot_pos = r;
-            bin = static_cast<int>(best[r].index_doppler);
-            int e1 = static_cast<int>(best[r].index_time) - samples_per_chip;
-            int e2 = static_cast<int>(best[r].index_time) + samples_per_chip;
-            if (e1 < 0)
-                e1 = ne + e1;
-            else if (e2 >= ne)
-                e2 = e2 - ne;
-            sink.ex1 = e1;
-            sink.ex2 = e2;
-        }
-    if (grid != nullptr && mode == 0) sink.grid = grid + (static_cast<size_t>(slot_list[slot_pos]) * bins + bin) * ne;
-    sink.best = -1.0f;
-    sink.best_t = 0xffffffffu;
-    sink.sum = 0.0f;
-    const float2* z = Z + static_cast<size_t>(r) * pl.n_total;
     for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n2; j += gridDim.x * blockDim.x)
         {
             float2 v[R];
@@ -552,83 +379,48 @@ __global__ void __launch_bounds__(256) acq_global_final_stage(const float2* __re
 #pragma unroll
             for (int q = 0; q < R; q++) sink(nullptr, j + q * n2, swap_ri(v[q]));
         }
+}
+
+// final radix-n1 DIT stage + |.|^2 + statistics; grid (chunks, rows); partial[r * chunks + chunk]
+template <int R>
+__global__ void __launch_bounds__(256) acq_global_final_stage(const float2* __restrict__ Z, FftPlan pl, const float2* __restrict__ tw,
+    const int* __restrict__ slot_list, int bins, int off, int ne, float* __restrict__ grid, int accumulate,
+    const AcqBest* __restrict__ best, int samples_per_chip, AcqRowStat* __restrict__ partial)
+{
+    const int r = blockIdx.y;
+    const AcqRow row(r, bins, best, samples_per_chip, ne);
+    float* g = (grid != nullptr && best == nullptr) ? grid + (static_cast<size_t>(slot_list[row.slot_pos]) * bins + row.bin) * ne : nullptr;
+    RowSink sink(off, ne, row, g, accumulate);
+    acq_global_final_dit<R>(Z + static_cast<size_t>(r) * pl.n_total, pl, tw, sink);
     float bv = sink.best;
     unsigned int bi = sink.best_t;
     float sm = sink.sum;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-        {
-            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-            const unsigned int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            sm += __shfl_xor_sync(0xffffffffu, sm, o);
-            if (ov > bv || (ov == bv && oi < bi))
-                {
-                    bv = ov;
-                    bi = oi;
-                }
-        }
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (lane == 0)
-        {
-            red_v[warp] = bv;
-            red_i[warp] = bi;
-            red_s[warp] = sm;
-        }
-    __syncthreads();
-    if (threadIdx.x == 0)
-        {
-            for (int w = 1; w < 8; w++)
-                {
-                    if (red_v[w] > bv || (red_v[w] == bv && red_i[w] < bi))
-                        {
-                            bv = red_v[w];
-                            bi = red_i[w];
-                        }
-                    sm += red_s[w];
-                }
-            AcqRowStat st;
-            st.max = bv;
-            st.argmax = bi;
-            st.sum = sm;
-            st.pad = 0.f;
-            partial[static_cast<size_t>(r) * gridDim.x + blockIdx.x] = st;
-        }
+    acq_cta_first_max<256 / 32>(bv, bi, sm);
+    if (threadIdx.x == 0) partial[static_cast<size_t>(r) * gridDim.x + blockIdx.x] = AcqRowStat{bv, bi, sm, 0.f};
 }
 
 // ---- Bluestein (chirp-z) support: sizes the mixed-radix planner cannot factor (prime factors > 7, e.g. 16 368) --------
-// Final radix-n1 DIT stage of a two-level inverse transform whose first n_out natural-order outputs are multiplied by
-// post[k] and STORED (complex) instead of being reduced to statistics: out[r][k] = y[k] * post[k], k < n_out.
+// The first n_out natural-order outputs of a final stage, multiplied by post[k] and STORED (complex) instead of being
+// reduced to statistics: out[k] = y[k] * post[k], k < n_out.
+struct PostMulStoreSink
+{
+    const float2* __restrict__ post;
+    int n_out;
+    float2* __restrict__ out;
+    __device__ __forceinline__ void operator()(float2* /*p*/, int k, float2 v) const
+    {
+        if (k < n_out) out[k] = cmul(v, __ldg(post + k));
+    }
+};
+
 template <int R>
 __global__ void __launch_bounds__(256) acq_global_final_store_stage(const float2* __restrict__ Z, FftPlan pl, const float2* __restrict__ tw,
     const float2* __restrict__ post, int n_out, float2* __restrict__ out, size_t out_stride)
 {
     const int r = blockIdx.y;
-    const int n2 = pl.n;
     const float2* z = Z + static_cast<size_t>(r) * pl.n_total;
-    float2* o = out + static_cast<size_t>(r) * out_stride;
-    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n2; j += gridDim.x * blockDim.x)
-        {
-            float2 v[R];
-#pragma unroll
-            for (int q = 0; q < R; q++) v[q] = z[q * n2 + j];
-            const float2 w1 = __ldg(tw + pl.tw_goff + j);
-            float2 wp = w1;
-#pragma unroll
-            for (int q = 1; q < R; q++)
-                {
-                    v[q] = cmul_conj(v[q], wp);
-                    if (q + 1 < R) wp = cmul(wp, w1);
-                }
-#pragma unroll
-            for (int q = 0; q < R; q++) v[q] = swap_ri(v[q]);
-            Bfly<R>::fwd(v);
-#pragma unroll
-            for (int q = 0; q < R; q++)
-                {
-                    const int k = j + q * n2;
-                    if (k < n_out) o[k] = cmul(swap_ri(v[q]), __ldg(post + k));
-                }
-        }
+    PostMulStoreSink sink{post, n_out, out + static_cast<size_t>(r) * out_stride};
+    acq_global_final_dit<R>(z, pl, tw, sink);
 }
 
 // out[r][i] = a[r][i] * b[i] (conj_a: conj(a[r][i]) * b[i]), i < n; rows r < rows
@@ -644,8 +436,9 @@ __global__ void acq_rows_times_vector_kernel(const float2* __restrict__ a, size_
         }
 }
 
+// writes rowstat[r], or only the maximum to second_peak[r] when second_peak != nullptr
 __global__ void acq_row_reduce_kernel(const AcqRowStat* __restrict__ partial, int chunks, int rows, AcqRowStat* __restrict__ rowstat,
-    float* __restrict__ second_peak, int mode)
+    float* __restrict__ second_peak)
 {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= rows) return;
@@ -660,7 +453,7 @@ __global__ void acq_row_reduce_kernel(const AcqRowStat* __restrict__ partial, in
                 }
             a.sum += b.sum;
         }
-    if (mode == 0)
+    if (second_peak == nullptr)
         rowstat[r] = a;
     else
         second_peak[r] = a.max;
@@ -839,6 +632,29 @@ int set_attrs()
 // ---- launchers (called from acq_engine.cu) --------------------------------------------------------------
 static int acq_plan_make_smem(int n, FftPlan* pl, bool allow25);
 
+// two-level plan: the first global radix n1 of `cand` that divides n_total and leaves blocks the in-shared-memory planner takes
+static int acq_plan_make_global(int n_total, const int (&cand)[7], FftPlan* pl)
+{
+    for (int n1 : cand)
+        {
+            if (n_total % n1) continue;
+            const int n2 = n_total / n1;
+            if (n2 > kAcqMaxSmemPoints) continue;
+            if (acq_plan_make_smem(n2, pl, false) != B200_OK) continue;
+            pl->n1 = n1;
+            pl->n_total = n_total;
+            int off = 0, M = n2;
+            for (int st = 0; st < pl->n_stages; st++)
+                {
+                    M /= pl->radix[st];
+                    off += M;
+                }
+            pl->tw_goff = off;  // after the per-stage tables; n2 entries follow
+            return B200_OK;
+        }
+    return B200_ERR_RANGE;
+}
+
 int acq_plan_make(int n_total, FftPlan* pl)
 {
     if (n_total < 2) return B200_ERR_RANGE;
@@ -860,26 +676,12 @@ int acq_plan_make(int n_total, FftPlan* pl)
             return rc;
         }
     // two-level: smallest supported radix n1 that brings the blocks into shared memory
-    const int cand[7] = {2, 3, 4, 5, 7, 8, 10};
-    for (int n1 : cand)
-        {
-            if (n_total % n1) continue;
-            const int n2 = n_total / n1;
-            if (n2 > kAcqMaxSmemPoints) continue;
-            if (acq_plan_make_smem(n2, pl, false) != B200_OK) continue;
-            pl->n1 = n1;
-            pl->n_total = n_total;
-            int off = 0, M = n2;
-            for (int st = 0; st < pl->n_stages; st++)
-                {
-                    M /= pl->radix[st];
-                    off += M;
-                }
-            pl->tw_goff = off;  // after the per-stage tables; n2 entries follow
-            return B200_OK;
-        }
-    return B200_ERR_RANGE;
+    return acq_plan_make_global(n_total, {2, 3, 4, 5, 7, 8, 10}, pl);
 }
+
+// two-level plan for EXACTLY m points with a global radix n1 >= 2 even when m would fit shared memory (the chirp-z path is
+// written on the through-global-memory kernels only); powers of two first
+int acq_plan_make_two_level(int m, FftPlan* pl) { return acq_plan_make_global(m, {2, 4, 8, 3, 5, 7, 10}, pl); }
 
 static int acq_plan_make_smem(int n, FftPlan* pl, bool allow25)
 {
@@ -975,6 +777,16 @@ static int dispatch_radix(int r, F&& f)
         }
 }
 
+// the single-CTA kernels at the plan's CTA width
+template <typename F>
+static void dispatch_threads(const FftPlan& pl, F&& f)
+{
+    if (pl.threads == kAcqThreads25)
+        f(std::integral_constant<int, kAcqThreads25>{});
+    else
+        f(std::integral_constant<int, kAcqThreads>{});
+}
+
 int acq_final_chunks(const FftPlan& pl) { return pl.n1 > 1 ? (pl.n + 1023) / 1024 : 0; }
 
 int acq_launch_code_fft(const float2* code, int consumed, int layout, float2* out, const FftPlan& pl, const float2* tw, cudaStream_t st)
@@ -983,10 +795,9 @@ int acq_launch_code_fft(const float2* code, int consumed, int layout, float2* ou
     if (rc) return rc;
     if (pl.n1 == 1)
         {
-            if (pl.threads == kAcqThreads25)
-                acq_code_fft_kernel<kAcqThreads25><<<1, kAcqThreads25, pl.n * sizeof(float2), st>>>(code, consumed, layout, out, pl, tw);
-            else
-                acq_code_fft_kernel<kAcqThreads><<<1, kAcqThreads, pl.n * sizeof(float2), st>>>(code, consumed, layout, out, pl, tw);
+            dispatch_threads(pl, [&](auto T) {
+                acq_code_fft_kernel<decltype(T)::value><<<1, decltype(T)::value, pl.n * sizeof(float2), st>>>(code, consumed, layout, out, pl, tw);
+            });
         }
     else
         {
@@ -999,16 +810,16 @@ int acq_launch_code_fft(const float2* code, int consumed, int layout, float2* ou
     return B200_OK;
 }
 
-int acq_launch_fwd(const float2* in, int consumed, const float2* wipe, float2* X, int bins, const FftPlan& pl, const float2* tw, cudaStream_t st)
+int acq_launch_fwd(const float2* in, int consumed, const float2* wipe, float2* X, int bins, const FftPlan& pl, const float2* tw,
+    uint64_t& launched, cudaStream_t st)
 {
     int rc = set_attrs();
     if (rc) return rc;
     if (pl.n1 == 1)
         {
-            if (pl.threads == kAcqThreads25)
-                acq_fwd_kernel<kAcqThreads25><<<bins, kAcqThreads25, pl.n * sizeof(float2), st>>>(in, consumed, wipe, X, pl, tw);
-            else
-                acq_fwd_kernel<kAcqThreads><<<bins, kAcqThreads, pl.n * sizeof(float2), st>>>(in, consumed, wipe, X, pl, tw);
+            dispatch_threads(pl, [&](auto T) {
+                acq_fwd_kernel<decltype(T)::value><<<bins, decltype(T)::value, pl.n * sizeof(float2), st>>>(in, consumed, wipe, X, pl, tw);
+            });
         }
     else
         {
@@ -1018,95 +829,91 @@ int acq_launch_fwd(const float2* in, int consumed, const float2* wipe, float2* X
             acq_block_fft_kernel<<<dim3(pl.n1, bins), kAcqThreads, pl.n * sizeof(float2), st>>>(X, pl, tw, 0);
         }
     B200_CUDA_TRY(cudaGetLastError());
+    launched += (pl.n1 == 1) ? 1 : 2;
     return B200_OK;
 }
 
-int acq_launch_corr(const float2* X, const float2* codes, const int* slot_list, int n_slots, int bins, const FftPlan& pl,
-    const float2* tw, int off, int ne, AcqRowStat* rowstat, float* grid, int accumulate, int mode, const void* best,
-    int samples_per_chip, float* second_peak, float2* Z, AcqRowStat* partial, cudaStream_t st)
+// best == nullptr: statistics of every (slot, bin) row into rowstat; otherwise the second-peak pass into second_peak
+static int launch_corr(const float2* X, const float2* codes, const int* slot_list, int n_slots, int bins, const FftPlan& pl,
+    const float2* tw, int off, int ne, float* grid, int accumulate, const AcqBest* best, int samples_per_chip, AcqRowStat* rowstat,
+    float* second_peak, float2* Z, AcqRowStat* partial, uint64_t& launched, cudaStream_t st)
 {
     int rc = set_attrs();
     if (rc) return rc;
-    const int rows = (mode == 0) ? n_slots * bins : n_slots;
-    if (pl.n1 == 1 || (mode == 1 && grid != nullptr))
+    const int rows = (best == nullptr) ? n_slots * bins : n_slots;
+    const bool one_kernel = pl.n1 == 1 || (best != nullptr && grid != nullptr);
+    if (one_kernel)
         {
             const size_t smem = (pl.n1 == 1) ? pl.n * sizeof(float2) : 16;
-            if (pl.threads == kAcqThreads25)
-                acq_corr_kernel<kAcqThreads25><<<rows, kAcqThreads25, smem, st>>>(X, codes, slot_list, bins, pl, tw, off, ne, rowstat, grid,
-                    accumulate, mode, static_cast<const AcqBest*>(best), samples_per_chip, second_peak);
-            else
-                acq_corr_kernel<kAcqThreads><<<rows, kAcqThreads, smem, st>>>(X, codes, slot_list, bins, pl, tw, off, ne, rowstat, grid,
-                    accumulate, mode, static_cast<const AcqBest*>(best), samples_per_chip, second_peak);
+            dispatch_threads(pl, [&](auto T) {
+                acq_corr_kernel<decltype(T)::value><<<rows, decltype(T)::value, smem, st>>>(X, codes, slot_list, bins, pl, tw, off, ne, rowstat,
+                    grid, accumulate, best, samples_per_chip, second_peak);
+            });
         }
     else
         {
-            acq_corr_block_kernel<<<dim3(pl.n1, rows), kAcqThreads, pl.n * sizeof(float2), st>>>(X, codes, slot_list, bins, pl, tw, Z, mode,
-                static_cast<const AcqBest*>(best));
+            acq_corr_block_kernel<<<dim3(pl.n1, rows), kAcqThreads, pl.n * sizeof(float2), st>>>(X, codes, slot_list, bins, pl, tw, Z, best);
             const int chunks = acq_final_chunks(pl);
             rc = dispatch_radix(pl.n1, [&](auto R) {
                 acq_global_final_stage<decltype(R)::value><<<dim3(chunks, rows), 256, 0, st>>>(Z, pl, tw, slot_list, bins, off, ne, grid, accumulate,
-                    mode, static_cast<const AcqBest*>(best), samples_per_chip, partial);
+                    best, samples_per_chip, partial);
             });
             if (rc) return rc;
-            acq_row_reduce_kernel<<<(rows + 127) / 128, 128, 0, st>>>(partial, chunks, rows, rowstat, second_peak, mode);
+            acq_row_reduce_kernel<<<(rows + 127) / 128, 128, 0, st>>>(partial, chunks, rows, rowstat, second_peak);
         }
     B200_CUDA_TRY(cudaGetLastError());
+    launched += one_kernel ? 1 : 3;
     return B200_OK;
+}
+
+int acq_launch_row_stats(const float2* X, const float2* codes, const int* slot_list, int n_slots, int bins, const FftPlan& pl,
+    const float2* tw, int off, int ne, float* grid, int accumulate, AcqRowStat* rowstat, float2* Z, AcqRowStat* partial,
+    uint64_t& launched, cudaStream_t st)
+{
+    return launch_corr(X, codes, slot_list, n_slots, bins, pl, tw, off, ne, grid, accumulate, nullptr, 0, rowstat, nullptr, Z, partial,
+        launched, st);
+}
+
+int acq_launch_second_peak(const float2* X, const float2* codes, const int* slot_list, int n_slots, int bins, const FftPlan& pl,
+    const float2* tw, int off, int ne, float* grid, const AcqBest* best, int samples_per_chip, float* second_peak, float2* Z,
+    AcqRowStat* partial, uint64_t& launched, cudaStream_t st)
+{
+    return launch_corr(X, codes, slot_list, n_slots, bins, pl, tw, off, ne, grid, 0, best, samples_per_chip, nullptr, second_peak, Z,
+        partial, launched, st);
 }
 
 int acq_launch_stats(const AcqRowStat* rowstat, int n_slots, int bins, int ne, int doppler_max, int doppler_center,
-    int doppler_step, unsigned int dwell_counter, int use_cfar, void* best, b200_acq_result* results, int step_two, float center2,
-    float step2, float prev_input_power, cudaStream_t st)
+    int doppler_step, unsigned int dwell_counter, int use_cfar, AcqBest* best, b200_acq_result* results, int step_two, float center2,
+    float step2, float prev_input_power, uint64_t& launched, cudaStream_t st)
 {
     acq_stats_kernel<<<n_slots, 32, 0, st>>>(rowstat, n_slots, bins, ne, doppler_max, doppler_center, doppler_step,
-        dwell_counter, use_cfar, static_cast<AcqBest*>(best), results, step_two, center2, step2, prev_input_power);
+        dwell_counter, use_cfar, best, results, step_two, center2, step2, prev_input_power);
     B200_CUDA_TRY(cudaGetLastError());
+    launched += 1;
     return B200_OK;
 }
 
-int acq_launch_finish_second_peak(const float* second_peak, int n_slots, b200_acq_result* results, cudaStream_t st)
+int acq_launch_finish_second_peak(const float* second_peak, int n_slots, b200_acq_result* results, uint64_t& launched, cudaStream_t st)
 {
     acq_finish_second_peak_kernel<<<(n_slots + 63) / 64, 64, 0, st>>>(second_peak, n_slots, results);
     B200_CUDA_TRY(cudaGetLastError());
+    launched += 1;
     return B200_OK;
 }
 
-int acq_launch_sweep_best(const b200_acq_result* results, const unsigned int* prn_of_result, int n, b200_acq_peak* out, cudaStream_t st)
+int acq_launch_sweep_best(const b200_acq_result* results, const unsigned int* prn_of_result, int n, b200_acq_peak* out, uint64_t& launched,
+    cudaStream_t st)
 {
     acq_sweep_best_kernel<<<1, 32, 0, st>>>(results, prn_of_result, n, out);
     B200_CUDA_TRY(cudaGetLastError());
+    launched += 1;
     return B200_OK;
 }
 
 // ---- Bluestein building blocks (acq_engine.cu composes them) --------------------------------------------------------
-// two-level plan for EXACTLY m points with a global radix n1 >= 2 even when m would fit shared memory (the chirp-z path is
-// written on the through-global-memory kernels only)
-int acq_plan_make_two_level(int m, FftPlan* pl)
-{
-    const int cand[7] = {2, 4, 8, 3, 5, 7, 10};
-    for (int n1 : cand)
-        {
-            if (m % n1) continue;
-            const int n2 = m / n1;
-            if (n2 > kAcqMaxSmemPoints || n2 < 2) continue;
-            if (acq_plan_make_smem(n2, pl, false) != B200_OK) continue;
-            pl->n1 = n1;
-            pl->n_total = m;
-            int off = 0, M = n2;
-            for (int st = 0; st < pl->n_stages; st++)
-                {
-                    M /= pl->radix[st];
-                    off += M;
-                }
-            pl->tw_goff = off;
-            return B200_OK;
-        }
-    return B200_ERR_RANGE;
-}
-
 // X[r] = FFT_M( pad( in[r * in_stride + i] * mult[r * mult_stride + i], i < consumed ) ), rows r < rows (two-level plan)
 int acq_launch_fwd_rows(const float2* in, size_t in_stride, int consumed, const float2* mult, size_t mult_stride, float2* X, int rows,
-    const FftPlan& pl, const float2* tw, cudaStream_t st)
+    const FftPlan& pl, const float2* tw, uint64_t& launched, cudaStream_t st)
 {
     int rc = set_attrs();
     if (rc) return rc;
@@ -1116,23 +923,25 @@ int acq_launch_fwd_rows(const float2* in, size_t in_stride, int consumed, const 
     if (rc) return rc;
     acq_block_fft_kernel<<<dim3(pl.n1, rows), kAcqThreads, pl.n * sizeof(float2), st>>>(X, pl, tw, 0);
     B200_CUDA_TRY(cudaGetLastError());
+    launched += 2;
     return B200_OK;
 }
 
 // out[r][k] = IFFT_M( X[r] . filt )[k] * post[k], k < n_out   (Z: rows x M workspace; one_slot_dev: device int == 0)
 int acq_launch_inverse_store_rows(const float2* X, const float2* filt, const int* one_slot_dev, int rows, const FftPlan& pl, const float2* tw,
-    float2* Z, const float2* post, int n_out, float2* out, size_t out_stride, cudaStream_t st)
+    float2* Z, const float2* post, int n_out, float2* out, size_t out_stride, uint64_t& launched, cudaStream_t st)
 {
     int rc = set_attrs();
     if (rc) return rc;
     if (pl.n1 < 2) return B200_ERR_ARG;
-    acq_corr_block_kernel<<<dim3(pl.n1, rows), kAcqThreads, pl.n * sizeof(float2), st>>>(X, filt, one_slot_dev, rows, pl, tw, Z, 0, nullptr);
+    acq_corr_block_kernel<<<dim3(pl.n1, rows), kAcqThreads, pl.n * sizeof(float2), st>>>(X, filt, one_slot_dev, rows, pl, tw, Z, nullptr);
     const int chunks = acq_final_chunks(pl);
     rc = dispatch_radix(pl.n1, [&](auto R) {
         acq_global_final_store_stage<decltype(R)::value><<<dim3(chunks, rows), 256, 0, st>>>(Z, pl, tw, post, n_out, out, out_stride);
     });
     if (rc) return rc;
     B200_CUDA_TRY(cudaGetLastError());
+    launched += 2;
     return B200_OK;
 }
 

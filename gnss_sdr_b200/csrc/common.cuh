@@ -113,27 +113,103 @@ int launch_convert_i8(const signed char* raw, float2* ring, unsigned long long m
 namespace b200
 {
 struct FftPlan;
-struct AcqRowStat;
+
+// (max, first arg-max, sum) of |y|^2 over one correlation row
+struct AcqRowStat
+{
+    float max;
+    unsigned int argmax;
+    float sum;
+    float pad;
+};
+
+// winning cell of one searched slot, as acq_stats_kernel found it
+struct AcqBest
+{
+    unsigned int index_time;
+    unsigned int index_doppler;
+};
+
+// set_local_code (pcps_acquisition.cc:230-246): where the local code starts in the n-point buffer.  Layout 0: code[0..consumed)
+// at the front (sampled_ms == ms_per_code); 1: bit_transition_flag, code[0..n/2) in the second half; 2: zero-padded front,
+// code[0..consumed) at [n - consumed, n).  Zeros elsewhere.
+__host__ __device__ inline int acq_code_offset(int layout, int n, int consumed)
+{
+    return (layout == 1) ? n / 2 : (layout == 2) ? n - consumed : 0;
+}
+
+// CTA "first maximum" of (value, index) plus the sum of the values: xor-shuffle 16 -> 1 in each warp, then thread 0 combines
+// warps 1..WARPS-1 in ascending order.  The result is valid in thread 0 only.
+template <int WARPS>
+__device__ __forceinline__ void acq_cta_first_max(float& bv, unsigned int& bi, float& sm)
+{
+    __shared__ float red_v[WARPS];
+    __shared__ unsigned int red_i[WARPS];
+    __shared__ float red_s[WARPS];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+        {
+            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+            const unsigned int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            sm += __shfl_xor_sync(0xffffffffu, sm, o);
+            if (ov > bv || (ov == bv && oi < bi))
+                {
+                    bv = ov;
+                    bi = oi;
+                }
+        }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0)
+        {
+            red_v[warp] = bv;
+            red_i[warp] = bi;
+            red_s[warp] = sm;
+        }
+    __syncthreads();
+    if (threadIdx.x == 0)
+        {
+            for (int w = 1; w < WARPS; w++)
+                {
+                    if (red_v[w] > bv || (red_v[w] == bv && red_i[w] < bi))
+                        {
+                            bv = red_v[w];
+                            bi = red_i[w];
+                        }
+                    sm += red_s[w];
+                }
+        }
+}
+
+// Acquisition launchers (acq_kernels.cu).  Those on the search path add the number of kernels they issued to `launched`.
 int acq_plan_make(int n, FftPlan* pl);
+int acq_plan_make_two_level(int m, FftPlan* pl);
+int acq_final_chunks(const FftPlan& pl);
 int acq_launch_twiddles(float2* tw, const FftPlan& pl, cudaStream_t st);
 int acq_launch_wipeoff(float2* wipe, int n, int bins, int doppler_max, int doppler_center, int doppler_step,
     int doppler_bias, long long fs_in, int step_two, float center2, float step2, cudaStream_t st);
 int acq_launch_code_fft(const float2* code, int consumed, int layout, float2* out, const FftPlan& pl, const float2* tw, cudaStream_t st);
-int acq_launch_fwd(const float2* in, int consumed, const float2* wipe, float2* X, int bins, const FftPlan& pl, const float2* tw, cudaStream_t st);
-int acq_launch_corr(const float2* X, const float2* codes, const int* slot_list, int n_slots, int bins, const FftPlan& pl,
-    const float2* tw, int off, int ne, AcqRowStat* rowstat, float* grid, int accumulate, int mode, const void* best,
-    int samples_per_chip, float* second_peak, float2* Z, AcqRowStat* partial, cudaStream_t st);
-int acq_final_chunks(const FftPlan& pl);
+int acq_launch_fwd(const float2* in, int consumed, const float2* wipe, float2* X, int bins, const FftPlan& pl, const float2* tw,
+    uint64_t& launched, cudaStream_t st);
+// rowstat[slot_pos * bins + bin] for every (slot, bin) row over [off, off + ne) of the correlation; grid != nullptr: each row's
+// |y|^2 is stored there (accumulate: added to what is there)
+int acq_launch_row_stats(const float2* X, const float2* codes, const int* slot_list, int n_slots, int bins, const FftPlan& pl,
+    const float2* tw, int off, int ne, float* grid, int accumulate, AcqRowStat* rowstat, float2* Z, AcqRowStat* partial,
+    uint64_t& launched, cudaStream_t st);
+// second_peak[slot_pos]: maximum of the winning row best[slot_pos] with +-samples_per_chip around its peak zeroed, read from the
+// grid when there is one, else recomputed
+int acq_launch_second_peak(const float2* X, const float2* codes, const int* slot_list, int n_slots, int bins, const FftPlan& pl,
+    const float2* tw, int off, int ne, float* grid, const AcqBest* best, int samples_per_chip, float* second_peak, float2* Z,
+    AcqRowStat* partial, uint64_t& launched, cudaStream_t st);
 int acq_launch_stats(const AcqRowStat* rowstat, int n_slots, int bins, int ne, int doppler_max, int doppler_center,
-    int doppler_step, unsigned int dwell_counter, int use_cfar, void* best, b200_acq_result* results, int step_two, float center2,
-    float step2, float prev_input_power, cudaStream_t st);
-int acq_launch_finish_second_peak(const float* second_peak, int n_slots, b200_acq_result* results, cudaStream_t st);
-int acq_plan_make_two_level(int m, FftPlan* pl);
+    int doppler_step, unsigned int dwell_counter, int use_cfar, AcqBest* best, b200_acq_result* results, int step_two, float center2,
+    float step2, float prev_input_power, uint64_t& launched, cudaStream_t st);
+int acq_launch_finish_second_peak(const float* second_peak, int n_slots, b200_acq_result* results, uint64_t& launched, cudaStream_t st);
 int acq_launch_fwd_rows(const float2* in, size_t in_stride, int consumed, const float2* mult, size_t mult_stride, float2* X, int rows,
-    const FftPlan& pl, const float2* tw, cudaStream_t st);
+    const FftPlan& pl, const float2* tw, uint64_t& launched, cudaStream_t st);
 int acq_launch_inverse_store_rows(const float2* X, const float2* filt, const int* one_slot_dev, int rows, const FftPlan& pl, const float2* tw,
-    float2* Z, const float2* post, int n_out, float2* out, size_t out_stride, cudaStream_t st);
+    float2* Z, const float2* post, int n_out, float2* out, size_t out_stride, uint64_t& launched, cudaStream_t st);
 int acq_launch_rows_times_vector(const float2* a, size_t a_stride, const float2* b, int n, int conj_a, float2* out, size_t out_stride, int rows,
     cudaStream_t st);
-int acq_launch_sweep_best(const b200_acq_result* results, const unsigned int* prn_of_result, int n, b200_acq_peak* out, cudaStream_t st);
+int acq_launch_sweep_best(const b200_acq_result* results, const unsigned int* prn_of_result, int n, b200_acq_peak* out, uint64_t& launched,
+    cudaStream_t st);
 }  // namespace b200

@@ -421,9 +421,6 @@ extern "C"
      * object computes its spectra (chirp-z objects only; B200_ERR_STATE otherwise).  No reference counterpart: the
      * reference calls gr::fft, whose outputs no reference test holds either. */
     int b200_acq_selftest_dft(b200_acq* a, const b200_cf32* in_host, b200_cf32* out_host);
-    /* what = 0: the Doppler-bin spectra of the last search (bins x fft_size); what = 1: the stored code spectra
-     * conj(DFT(code)) . chirp / M (n_code_slots x fft_size).  Chirp-z objects only. */
-    int b200_acq_selftest_read(b200_acq* a, int what, b200_cf32* out_host);
     /* the wipe-off grid (bins x fft_size complex), for parity tests against volk_gnsssdr_s32f_sincos_32fc */
     int b200_acq_read_wipeoffs(b200_acq* a, b200_cf32* wipe_host);
     int b200_acq_destroy(b200_acq* a);
