@@ -167,6 +167,8 @@ _SIGS.update({
     "b200_trk_loop_create": ([_vp, C.c_int, C.POINTER(TrkLoopConf), C.POINTER(C.c_int)], C.c_int),
     "b200_trk_loop_start": ([_vp, C.c_int, C.c_double, C.c_double, C.c_uint64, C.c_uint64], C.c_int),
     "b200_trk_loop_run": ([_vp, C.c_int, _vp, _vp], C.c_int),
+    "b200_trk_loop_run_prompts": ([_vp, C.c_int, _vp, _vp, _vp], C.c_int),
+    "b200_trk_loop_set_data_channel": ([_vp, C.c_int, C.c_int], C.c_int),
     "b200_trk_loop_peek_items": ([_vp, _vp], C.c_int),
     "b200_trk_loop_set_mode": ([_vp, C.c_int], C.c_int),
     "b200_trk_loop_step_taps": ([_vp, _vp, _vp, _vp], C.c_int),
@@ -368,6 +370,19 @@ class Engine:
         cnt = np.zeros(n, np.int32)
         _chk(lib.b200_trk_loop_run(self.h, max_epochs, rec.ctypes.data, cnt.ctypes.data), "b200_trk_loop_run")
         return rec, cnt
+
+    def loop_set_data_channel(self, loop_id: int, channel: int):
+        """correlate the 1-tap `channel` beside the loop's pilot; the records then carry its prompt"""
+        _chk(lib.b200_trk_loop_set_data_channel(self.h, loop_id, channel), "b200_trk_loop_set_data_channel")
+
+    def loop_run_prompts(self, max_epochs: int):
+        """-> (records[n_loops, max_epochs], n_records[n_loops], pilot prompts complex64[n_loops, max_epochs])"""
+        n = getattr(self, "_n_loops", 0)
+        rec = np.zeros((n, max_epochs), TRK_DUMP_RECORD_DTYPE)
+        cnt = np.zeros(n, np.int32)
+        prm = np.zeros((n, max_epochs), np.complex64)
+        _chk(lib.b200_trk_loop_run_prompts(self.h, max_epochs, rec.ctypes.data, cnt.ctypes.data, prm.ctypes.data), "b200_trk_loop_run_prompts")
+        return rec, cnt, prm
 
     def loop_set_mode(self, mode: int):
         _chk(lib.b200_trk_loop_set_mode(self.h, mode), "b200_trk_loop_set_mode")

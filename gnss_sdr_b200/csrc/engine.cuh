@@ -97,6 +97,10 @@ struct b200_engine
     b200::DevBuf<float2> loop_taps_dev;
     b200::DevBuf<int> loop_nrec_dev;
     b200::DevBuf<unsigned int> loop_rec_dev;
+    b200::DevBuf<float2> loop_prm_dev;          // pilot prompts beside the records (b200_trk_loop_run_prompts)
+    std::vector<b200::LoopData> loop_data;      // data channel of each loop (b200_trk_loop_set_data_channel)
+    int loop_n_data{0};                         // loops that have one
+    b200::DevBuf<b200::LoopData> loop_data_dev;
     int loop_mode{-1};       // 0 persistent kernel (default), 1 one launch pair per epoch with slices = 1, 2 same with automatic slices
 
     ~b200_engine()

@@ -57,14 +57,26 @@ struct LoopAvail
     unsigned long long hi[16];
 };
 
+// The data correlator of a loop that tracks a pilot (track_pilot: d_correlator_data_cpu, dll_pll_veml_tracking.cc:637-668):
+// a 1-tap channel correlated on the loop's items with the pilot's NCO values.
+struct LoopData
+{
+    int channel;  // data channel, -1: none
+    int item;     // row of its item and tap in the batch buffers (kLoopDataItems): n_loops + its rank among the data loops
+};
+
 constexpr int kLoopPrepare = 1;     // prepare an item for loops that have none pending
 constexpr int kLoopUpdate = 2;      // consume taps for loops with a pending item
 constexpr int kLoopCheckAvail = 4;  // stall loops whose next vector_length samples are not resident
+constexpr int kLoopDataItems = 8;   // prepare writes the data items to their rows, and the update takes the data tap from there
+                                    // (without it the data tap is slot `taps` of the loop's own row, as b200_trk_loop_step_taps passes it)
 
-// loop_kernels_nofma.cu
+// loop_kernels_nofma.cu.  data: per loop (may be nullptr: no data channels); prompts: n_loops x rec_capacity pilot prompts
+// beside the records (may be nullptr).
 int launch_loop_cycle(LoopDev* loops, int n_loops, int mode, const LoopAvail& avail, b200_trk_item* items, const float2* taps,
-    unsigned int* records, int rec_capacity, int* n_records, cudaStream_t st);
-// persistent free-running tracker: one CTA per loop, up to max_epochs cycles without leaving the SM
+    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, cudaStream_t st);
+// persistent free-running tracker: one CTA per loop, up to max_epochs cycles without leaving the SM; data == nullptr when no
+// loop of the launch has a data channel (one code table in shared memory instead of two)
 int launch_loop_persistent(LoopDev* loops, int n_loops, int max_epochs, const LoopAvail& avail, const ChanDesc* chans, const BandDesc* bands,
-    unsigned int* records, int rec_capacity, int* n_records, int max_code_len, cudaStream_t st);
+    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, int max_code_len, cudaStream_t st);
 }  // namespace b200

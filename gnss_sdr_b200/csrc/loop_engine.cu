@@ -113,7 +113,7 @@ int ensure_loop_buffers(b200_engine* e, int rec_capacity)
     const int n = static_cast<int>(e->loops.size());
     if (!e->loops_dev.fits(n))
         {
-            // the loop states are kept; loops_dev is replaced last, so after a failure its capacity still asks for all four
+            // the loop states are kept; loops_dev is replaced last, so after a failure its capacity still asks for all the others
             const int cap = n + 32;
             DevBuf<LoopDev> nd;
             B200_CUDA_TRY(nd.alloc(cap));
@@ -121,11 +121,13 @@ int ensure_loop_buffers(b200_engine* e, int rec_capacity)
             if (e->loops_dev)
                 B200_CUDA_TRY(cudaMemcpyAsync(nd, e->loops_dev, sizeof(LoopDev) * e->loops_dev.capacity(), cudaMemcpyDeviceToDevice, e->stream));
             B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
-            B200_CUDA_TRY(e->loop_items_dev.alloc(cap));
-            B200_CUDA_TRY(e->loop_taps_dev.alloc(kLoopTapStride * cap));
+            // items and taps: one row per loop, then one per data channel (modes 1 and 2)
+            B200_CUDA_TRY(e->loop_items_dev.alloc(2 * cap));
+            B200_CUDA_TRY(e->loop_taps_dev.alloc(kLoopTapStride * 2 * cap));
             B200_CUDA_TRY(e->loop_nrec_dev.alloc(cap));
-            B200_CUDA_TRY(cudaMemsetAsync(e->loop_items_dev, 0, sizeof(b200_trk_item) * cap, e->stream));
-            B200_CUDA_TRY(cudaMemsetAsync(e->loop_taps_dev, 0, sizeof(float2) * kLoopTapStride * cap, e->stream));
+            B200_CUDA_TRY(e->loop_data_dev.alloc(cap));
+            B200_CUDA_TRY(cudaMemsetAsync(e->loop_items_dev, 0, sizeof(b200_trk_item) * 2 * cap, e->stream));
+            B200_CUDA_TRY(cudaMemsetAsync(e->loop_taps_dev, 0, sizeof(float2) * kLoopTapStride * 2 * cap, e->stream));
             e->loops_dev = std::move(nd);
         }
     const size_t words = static_cast<size_t>(n) * static_cast<size_t>(rec_capacity > 0 ? rec_capacity : 1) * kLoopRecordWords;
@@ -147,6 +149,21 @@ LoopAvail snapshot_avail(const b200_engine* e)
         }
     return a;
 }
+
+// numbers the data items (rows n_loops, n_loops + 1, ... in loop order) and uploads the table
+int upload_loop_data(b200_engine* e)
+{
+    const int n = static_cast<int>(e->loops.size());
+    int row = n;
+    for (LoopData& d : e->loop_data) d.item = d.channel >= 0 ? row++ : 0;
+    e->loop_n_data = row - n;
+    B200_CUDA_TRY(cudaMemcpyAsync(e->loop_data_dev, e->loop_data.data(), sizeof(LoopData) * n, cudaMemcpyHostToDevice, e->stream));
+    B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    return B200_OK;
+}
+
+// the kernels' view: nullptr while no loop has a data channel
+const LoopData* loop_data_dev(const b200_engine* e) { return e->loop_n_data ? e->loop_data_dev.get() : nullptr; }
 
 int correlate_loop_items(b200_engine* e, int n, int slices)
 {
@@ -214,13 +231,49 @@ extern "C"
         L.cloop = 1;
         L.state = 0;
         e->loops.push_back(L);
+        e->loop_data.push_back(LoopData{-1, 0});
         *loop_id = static_cast<int>(e->loops.size()) - 1;
         B200_ENTER_DEVICE(e->device);
         int rc = ensure_loop_buffers(e, 1);
         if (rc) return rc;
         B200_CUDA_TRY(cudaMemcpyAsync(e->loops_dev + *loop_id, &e->loops[*loop_id], sizeof(LoopDev), cudaMemcpyHostToDevice, e->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
-        return B200_OK;
+        return upload_loop_data(e);
+    }
+
+    int b200_trk_loop_set_data_channel(b200_engine* e, int loop_id, int data_channel)
+    {
+        if (!e) return B200_ERR_ARG;
+        std::lock_guard<std::mutex> lk(e->mu);
+        if (loop_id < 0 || loop_id >= static_cast<int>(e->loops.size()))
+            {
+                set_error("loop_set_data_channel: no loop %d", loop_id);
+                return B200_ERR_ARG;
+            }
+        if (data_channel < 0 || data_channel >= static_cast<int>(e->chans.size()) || e->chans[data_channel].desc.code == nullptr)
+            {
+                set_error("loop_set_data_channel: channel %d has no code table", data_channel);
+                return B200_ERR_ARG;
+            }
+        const ChanDesc& d = e->chans[data_channel].desc;
+        if (d.taps != 1)
+            {
+                set_error("loop_set_data_channel: channel %d has %d correlators, the data channel needs 1", data_channel, d.taps);
+                return B200_ERR_ARG;
+            }
+        if (d.band != e->loops[loop_id].band)
+            {
+                set_error("loop_set_data_channel: channel %d is on band %d, loop %d on band %d", data_channel, d.band, loop_id, e->loops[loop_id].band);
+                return B200_ERR_ARG;
+            }
+        if (d.high_dyn)
+            {
+                set_error("loop_set_data_channel: high-dynamics channels are not supported by the device loop");
+                return B200_ERR_ARG;
+            }
+        e->loop_data[loop_id].channel = data_channel;
+        B200_ENTER_DEVICE(e->device);
+        return upload_loop_data(e);
     }
 
     int b200_trk_loop_start(b200_engine* e, int loop_id, double acq_delay_samples, double acq_doppler_hz, uint64_t acq_samplestamp_samples,
@@ -285,6 +338,12 @@ extern "C"
 
     int b200_trk_loop_run(b200_engine* e, int max_epochs, b200_trk_dump_record* records_host, int* n_records_host)
     {
+        return b200_trk_loop_run_prompts(e, max_epochs, records_host, n_records_host, nullptr);
+    }
+
+    int b200_trk_loop_run_prompts(b200_engine* e, int max_epochs, b200_trk_dump_record* records_host, int* n_records_host,
+        b200_cf32* pilot_prompts_host)
+    {
         if (!e || max_epochs < 0) return B200_ERR_ARG;
         std::lock_guard<std::mutex> lk(e->mu);
         const int n = static_cast<int>(e->loops.size());
@@ -294,6 +353,14 @@ extern "C"
         if (rc) return rc;
         rc = ensure_loop_buffers(e, max_epochs);
         if (rc) return rc;
+        float2* prompts = nullptr;
+        if (pilot_prompts_host)
+            {
+                const size_t elems = static_cast<size_t>(n) * static_cast<size_t>(max_epochs);
+                B200_CUDA_TRY(e->loop_prm_dev.grow(elems, elems + elems / 4));
+                prompts = e->loop_prm_dev;
+            }
+        const LoopData* data = loop_data_dev(e);
         if (e->loop_mode < 0)
             {
                 const char* env = std::getenv("B200_LOOP_MODE");
@@ -303,26 +370,30 @@ extern "C"
         B200_CUDA_TRY(cudaMemsetAsync(e->loop_nrec_dev, 0, sizeof(int) * n, e->stream));
         if (e->loop_mode == 0)
             {
-                rc = launch_loop_persistent(e->loops_dev, n, max_epochs, avail, e->chans_dev, e->bands_dev, e->loop_rec_dev, max_epochs,
-                    e->loop_nrec_dev, e->max_code_len, e->stream);
+                rc = launch_loop_persistent(e->loops_dev, n, max_epochs, avail, e->chans_dev, e->bands_dev, data, e->loop_rec_dev, max_epochs,
+                    e->loop_nrec_dev, prompts, e->max_code_len, e->stream);
                 if (rc) return rc;
                 e->launches++;
             }
         else
             {
+                // the data items follow the loops' items in the same correlator launch (the mixed-tap path), split like them:
+                // the slice count follows the loops alone, so a data channel leaves the pilot taps bit for bit as they were
+                const int n_items = n + e->loop_n_data;
                 const int slices = e->loop_mode == 1 ? 1 : batch_slices(n);
-                rc = ensure_partials(e, n, slices);
+                const int data_items = data ? kLoopDataItems : 0;
+                rc = ensure_partials(e, n_items, slices);
                 if (rc) return rc;
-                rc = launch_loop_cycle(e->loops_dev, n, kLoopPrepare | kLoopCheckAvail, avail, e->loop_items_dev, e->loop_taps_dev, nullptr, 0,
-                    nullptr, e->stream);
+                rc = launch_loop_cycle(e->loops_dev, n, kLoopPrepare | kLoopCheckAvail | data_items, avail, e->loop_items_dev, e->loop_taps_dev, data,
+                    nullptr, 0, nullptr, nullptr, e->stream);
                 if (rc) return rc;
                 e->launches++;
                 for (int k = 0; k < max_epochs; k++)
                     {
-                        rc = correlate_loop_items(e, n, slices);
+                        rc = correlate_loop_items(e, n_items, slices);
                         if (rc) return rc;
-                        rc = launch_loop_cycle(e->loops_dev, n, kLoopUpdate | kLoopPrepare | kLoopCheckAvail, avail, e->loop_items_dev,
-                            e->loop_taps_dev, e->loop_rec_dev, max_epochs, e->loop_nrec_dev, e->stream);
+                        rc = launch_loop_cycle(e->loops_dev, n, kLoopUpdate | kLoopPrepare | kLoopCheckAvail | data_items, avail, e->loop_items_dev,
+                            e->loop_taps_dev, data, e->loop_rec_dev, max_epochs, e->loop_nrec_dev, prompts, e->stream);
                         if (rc) return rc;
                         e->launches++;
                     }
@@ -332,6 +403,9 @@ extern "C"
         if (records_host)
             B200_CUDA_TRY(cudaMemcpyAsync(records_host, e->loop_rec_dev, sizeof(b200_trk_dump_record) * static_cast<size_t>(n) * max_epochs,
                 cudaMemcpyDeviceToHost, e->stream));
+        if (pilot_prompts_host)
+            B200_CUDA_TRY(cudaMemcpyAsync(pilot_prompts_host, prompts, sizeof(float2) * static_cast<size_t>(n) * max_epochs, cudaMemcpyDeviceToHost,
+                e->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
         if (n_records_host)
             for (int i = 0; i < n; i++) n_records_host[i] = nrec[i] < max_epochs ? nrec[i] : max_epochs;
@@ -356,7 +430,8 @@ extern "C"
         int rc = ensure_loop_buffers(e, 1);
         if (rc) return rc;
         const LoopAvail avail{};
-        rc = launch_loop_cycle(e->loops_dev, n, kLoopPrepare, avail, e->loop_items_dev, e->loop_taps_dev, nullptr, 0, nullptr, e->stream);
+        rc = launch_loop_cycle(e->loops_dev, n, kLoopPrepare, avail, e->loop_items_dev, e->loop_taps_dev, loop_data_dev(e), nullptr, 0, nullptr,
+            nullptr, e->stream);
         if (rc) return rc;
         e->launches++;
         B200_CUDA_TRY(cudaMemcpyAsync(items_host, e->loop_items_dev, sizeof(b200_trk_item) * n, cudaMemcpyDeviceToHost, e->stream));
@@ -375,11 +450,12 @@ extern "C"
         if (rc) return rc;
         const LoopAvail avail{};
         B200_CUDA_TRY(cudaMemsetAsync(e->loop_nrec_dev, 0, sizeof(int) * n, e->stream));
-        rc = launch_loop_cycle(e->loops_dev, n, kLoopPrepare, avail, e->loop_items_dev, e->loop_taps_dev, nullptr, 0, nullptr, e->stream);
+        const LoopData* data = loop_data_dev(e);
+        rc = launch_loop_cycle(e->loops_dev, n, kLoopPrepare, avail, e->loop_items_dev, e->loop_taps_dev, data, nullptr, 0, nullptr, nullptr, e->stream);
         if (rc) return rc;
         B200_CUDA_TRY(cudaMemcpyAsync(e->loop_taps_dev, taps_host, sizeof(float2) * kLoopTapStride * n, cudaMemcpyHostToDevice, e->stream));
-        rc = launch_loop_cycle(e->loops_dev, n, kLoopUpdate, avail, e->loop_items_dev, e->loop_taps_dev, e->loop_rec_dev, 1, e->loop_nrec_dev,
-            e->stream);
+        rc = launch_loop_cycle(e->loops_dev, n, kLoopUpdate, avail, e->loop_items_dev, e->loop_taps_dev, data, e->loop_rec_dev, 1, e->loop_nrec_dev,
+            nullptr, e->stream);
         if (rc) return rc;
         e->launches += 2;
         if (records_host)

@@ -394,15 +394,21 @@ __device__ __forceinline__ unsigned long long loop_record_stamp(const LoopDev& L
     return L.nitems_read + static_cast<unsigned long long>(static_cast<long long>(L.current_prn_length_samples));
 }
 
-// mags: the five magnitudes (computed here when nullptr); stamp: loop_record_stamp() taken BEFORE loop_consume()
-__device__ void loop_record_part(const LoopDev& L, const float2* t, const float* mags, unsigned long long stamp, unsigned int* rec)
+// mags: the five magnitudes (computed here when nullptr); stamp: loop_record_stamp() taken BEFORE loop_consume().
+// data: the data prompt of a loop with a data channel (d_correlator_data_cpu, :1245-1256), nullptr without one; log_data
+// writes it as prompt_I/prompt_Q (:1614-1617), every other field comes from the pilot taps.  pilot_out (may be nullptr):
+// receives the pilot prompt.
+__device__ void loop_record_part(const LoopDev& L, const float2* t, const float2* data, const float* mags, unsigned long long stamp,
+    unsigned int* rec, float2* pilot_out)
 {
     const b200_trk_loop_conf& c = L.c;
     float2 VE, E, P, Lt, VL;
     loop_taps(c, t, VE, E, P, Lt, VL);
     for (int q = 0; q < 5; q++) rec[q] = __float_as_uint(mags ? mags[q] : loop_record_magnitude(c, t, q));
-    rec[5] = __float_as_uint(P.x);
-    rec[6] = __float_as_uint(P.y);
+    const float2 Pr = data ? *data : P;
+    rec[5] = __float_as_uint(Pr.x);
+    rec[6] = __float_as_uint(Pr.y);
+    if (pilot_out) *pilot_out = P;
     rec[7] = static_cast<unsigned int>(stamp);
     rec[8] = static_cast<unsigned int>(stamp >> 32);
     rec[9] = __float_as_uint(static_cast<float>(L.acc_carrier_phase_rad));
@@ -432,7 +438,7 @@ __device__ __forceinline__ void loop_consume(LoopDev& L)
 }
 
 // Returns true when a record was logged.
-__device__ bool loop_update(LoopDev& L, const float2* t, unsigned int* rec)
+__device__ bool loop_update(LoopDev& L, const float2* t, const float2* data, unsigned int* rec, float2* pilot_out)
 {
     bool logged = false;
     if (!loop_lock_part(L, t))
@@ -442,7 +448,7 @@ __device__ bool loop_update(LoopDev& L, const float2* t, unsigned int* rec)
     else
         {
             loop_track_part(L, t);
-            if (rec) loop_record_part(L, t, nullptr, loop_record_stamp(L), rec);
+            if (rec) loop_record_part(L, t, data, nullptr, loop_record_stamp(L), rec, pilot_out);
             logged = true;
         }
     loop_consume(L);
@@ -450,19 +456,30 @@ __device__ bool loop_update(LoopDev& L, const float2* t, unsigned int* rec)
 }
 
 __global__ void trk_loop_cycle_kernel(LoopDev* loops, int n_loops, int mode, LoopAvail avail, b200_trk_item* items,
-    const float2* __restrict__ taps, unsigned int* records, int rec_capacity, int* n_records)
+    const float2* __restrict__ taps, const LoopData* __restrict__ data, unsigned int* records, int rec_capacity, int* n_records,
+    float2* prompts)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_loops) return;
     LoopDev& L = loops[i];
     const bool check = (mode & kLoopCheckAvail) != 0;
     const unsigned long long lo = avail.lo[L.band & 15], hi = avail.hi[L.band & 15];
+    const LoopData d = data ? data[i] : LoopData{-1, 0};
     if ((mode & kLoopUpdate) && L.pending)
         {
             unsigned int* rec = nullptr;
+            float2* prm = nullptr;
             const int k = n_records ? n_records[i] : 0;
-            if (records && k < rec_capacity) rec = records + (static_cast<size_t>(i) * rec_capacity + k) * kLoopRecordWords;
-            const bool logged = loop_update(L, taps + static_cast<size_t>(i) * kLoopTapStride, rec);
+            if (records && k < rec_capacity)
+                {
+                    rec = records + (static_cast<size_t>(i) * rec_capacity + k) * kLoopRecordWords;
+                    if (prompts) prm = prompts + static_cast<size_t>(i) * rec_capacity + k;
+                }
+            const float2* t = taps + static_cast<size_t>(i) * kLoopTapStride;
+            // the data tap: row d.item of the correlator output, or the slot after the pilot taps (b200_trk_loop_step_taps)
+            const float2* pd = nullptr;
+            if (d.channel >= 0) pd = (mode & kLoopDataItems) ? taps + static_cast<size_t>(d.item) * kLoopTapStride : t + L.taps;
+            const bool logged = loop_update(L, t, pd, rec, prm);
             if (logged && n_records) n_records[i] = k + 1;
             L.pending = 0;
         }
@@ -474,6 +491,11 @@ __global__ void trk_loop_cycle_kernel(LoopDev* loops, int n_loops, int mode, Loo
             b200_trk_item it;
             L.pending = loop_prepare(L, it, check, lo, hi) ? 1 : 0;
             items[i] = it;
+            if (d.channel >= 0 && (mode & kLoopDataItems))
+                {
+                    it.channel = d.channel;   // the same epoch against the data code (n == 0 when the loop stalls)
+                    items[d.item] = it;
+                }
         }
 }
 // Persistent free-running tracker: one CTA per loop runs epoch after epoch without leaving the SM - loop update of the
@@ -493,14 +515,29 @@ __global__ void trk_loop_cycle_kernel(LoopDev* loops, int n_loops, int mode, Loo
 constexpr int kLoopThreadsMany = B200_LOOP_THREADS;   // CTA width when loops outnumber the SMs (two CTAs per SM)
 constexpr int kLoopThreadsFew = 512;                  // one loop per SM at most: wider CTAs shorten the correlation
 
+// The data pass of a loop with a data channel: its own function, not inlined, so that the pilot's code in the persistent
+// kernel stays laid out as without it (inlined, the 1-tap correlation made every epoch of a loop without a data channel about
+// 1 us slower on an H100).
+template <int kLoopThreads>
+__device__ __noinline__ float2 loop_correlate_data(const b200_trk_item& it, const ChanDesc& ch, const BandDesc& bd, float* smem_tbl, int tbl_cap,
+    float2* smem_red, int* tbl_cache)
+{
+    float2 r[1];
+    process_item<1, true, kLoopThreads>(it, ch, bd, smem_tbl, tbl_cap, smem_red, 0, 1, r, tbl_cache);
+    return r[0];
+}
+
+// data: nullptr when no loop of the launch has a data channel; otherwise the data channel of every loop (-1: none), and the
+// dynamic shared memory holds a second code table of tbl_cap entries for it, right after the pilot's.
 template <int kLoopThreads>
 __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / kLoopThreads : 1) trk_loop_persistent_kernel(LoopDev* loops, int n_loops, int max_epochs, LoopAvail avail,
-    const ChanDesc* __restrict__ chans, const BandDesc* __restrict__ bands, unsigned int* records, int rec_capacity, int* n_records,
-    int tbl_cap)
+    const ChanDesc* __restrict__ chans, const BandDesc* __restrict__ bands, const LoopData* __restrict__ data, unsigned int* records,
+    int rec_capacity, int* n_records, float2* prompts, int tbl_cap)
 {
     extern __shared__ __align__(16) float smem[];
     float* smem_tbl = smem;
-    float2* smem_red = reinterpret_cast<float2*>(smem + tbl_cap);
+    float* smem_tbl_data = data ? smem + tbl_cap : nullptr;
+    float2* smem_red = reinterpret_cast<float2*>(smem + (data ? 2 * tbl_cap : tbl_cap));
     LoopDev* sL = reinterpret_cast<LoopDev*>(smem_red + (kLoopThreads / 32) * B200_MAX_TAPS);
     LoopDev* sBackup = sL + 1;   // the state before the current update (see the loop)
     __shared__ b200_trk_item s_item;
@@ -508,8 +545,12 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
     __shared__ float s_mags[5];
     __shared__ unsigned long long s_stamp;
     __shared__ unsigned int* s_rec;
+    __shared__ float2* s_prm;
     __shared__ int s_go;
-    __shared__ int s_tbl_cache[2];  // chip-index window held in smem_tbl (process_item<.., REUSE>)
+    __shared__ int s_tbl_cache[2];       // chip-index window held in smem_tbl (process_item<.., REUSE>)
+    __shared__ int s_tbl_cache_data[2];  // the same for the data table in smem_tbl_data: the two never evict each other
+    __shared__ int s_data_channel;       // -1: none
+    __shared__ float2 s_data_tap;        // data prompt of the last epoch (kept here, not in registers across the correlation)
 
     const int i = blockIdx.x;
     const int tid = threadIdx.x;
@@ -518,7 +559,11 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
         const unsigned int* src = reinterpret_cast<const unsigned int*>(loops + i);
         unsigned int* dst = reinterpret_cast<unsigned int*>(sL);
         for (int w = tid; w < static_cast<int>(sizeof(LoopDev) / 4); w += kLoopThreads) dst[w] = src[w];
-        if (tid == 0) s_tbl_cache[0] = s_tbl_cache[1] = 0;
+        if (tid == 0)
+            {
+                s_tbl_cache[0] = s_tbl_cache[1] = s_tbl_cache_data[0] = s_tbl_cache_data[1] = 0;
+                s_data_channel = data ? data[i].channel : -1;
+            }
     }
     __syncthreads();
     const ChanDesc& ch = chans[sL->channel];
@@ -570,6 +615,7 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                             loop_track_part(*sL, t);
                             s_stamp = loop_record_stamp(*sL);
                             s_rec = (records && k_rec < rec_capacity) ? records + (static_cast<size_t>(i) * rec_capacity + k_rec) * kLoopRecordWords : nullptr;
+                            s_prm = (s_rec && prompts) ? prompts + static_cast<size_t>(i) * rec_capacity + k_rec : nullptr;
                         }
                     else if (tid == 32)
                         {
@@ -588,7 +634,8 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                     PF_MARK(3)   // waiting for the lock part / magnitudes
                     // the dump record goes out from warp 1 while thread 0 consumes the epoch and prepares the next one: in the
                     // tracking state neither of those writes a member the record reads (the sample stamp was taken above)
-                    if (tid == 32 && s_lock_ok > 0 && s_rec != nullptr) loop_record_part(*sL, t, s_mags, s_stamp, s_rec);
+                    if (tid == 32 && s_lock_ok > 0 && s_rec != nullptr) loop_record_part(*sL, t, s_data_channel >= 0 ? &s_data_tap : nullptr, s_mags, s_stamp, s_rec,
+                                                                                          s_prm);
                 }
 #endif
             if (tid == 0)
@@ -596,10 +643,15 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                     if (have_taps)
                         {
                             unsigned int* rec = nullptr;
-                            if (records && k_rec < rec_capacity) rec = records + (static_cast<size_t>(i) * rec_capacity + k_rec) * kLoopRecordWords;
+                            float2* prm = nullptr;
+                            if (records && k_rec < rec_capacity)
+                                {
+                                    rec = records + (static_cast<size_t>(i) * rec_capacity + k_rec) * kLoopRecordWords;
+                                    if (prompts) prm = prompts + static_cast<size_t>(i) * rec_capacity + k_rec;
+                                }
                             if (s_lock_ok < 0)
                                 {
-                                    if (loop_update(*sL, t, rec)) k_rec++;
+                                    if (loop_update(*sL, t, s_data_channel >= 0 ? &s_data_tap : nullptr, rec, prm)) k_rec++;
                                 }
                             else if (s_lock_ok)
                                 {
@@ -611,7 +663,7 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                                     const unsigned int* src = reinterpret_cast<const unsigned int*>(sBackup);
                                     unsigned int* dst = reinterpret_cast<unsigned int*>(sL);
                                     for (int w = 0; w < static_cast<int>(sizeof(LoopDev) / 4); w++) dst[w] = src[w];
-                                    if (loop_update(*sL, t, rec)) k_rec++;
+                                    if (loop_update(*sL, t, s_data_channel >= 0 ? &s_data_tap : nullptr, rec, prm)) k_rec++;
                                 }
                         }
                     PF_MARK(4)   // record + consume
@@ -644,6 +696,13 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
 #pragma unroll
                     for (int q = 0; q < 5; q++) t[q] = r[q];
                 }
+            if (s_data_channel >= 0)
+                {
+                    // the same epoch against the data code: a second pass over the samples (the next iteration's barriers order
+                    // thread 0's store before any read)
+                    const float2 r = loop_correlate_data<kLoopThreads>(s_item, chans[s_data_channel], bd, smem_tbl_data, tbl_cap, smem_red, s_tbl_cache_data);
+                    if (tid == 0) s_data_tap = r;
+                }
             have_taps = true;
         }
 #ifdef B200_LOOP_PROFILE
@@ -666,9 +725,10 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
 
 template <int THREADS>
 static int launch_loop_persistent_width(LoopDev* loops, int n_loops, int max_epochs, const LoopAvail& avail, const ChanDesc* chans, const BandDesc* bands,
-    unsigned int* records, int rec_capacity, int* n_records, int tbl_cap, cudaStream_t st)
+    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, int tbl_cap, cudaStream_t st)
 {
-    const size_t smem_bytes = static_cast<size_t>(tbl_cap) * 4 + (THREADS / 32) * B200_MAX_TAPS * sizeof(float2) + 2 * sizeof(LoopDev);
+    const size_t tables = data ? 2 : 1;
+    const size_t smem_bytes = tables * tbl_cap * 4 + (THREADS / 32) * B200_MAX_TAPS * sizeof(float2) + 2 * sizeof(LoopDev);
     static DeviceOnce once;
     const int once_dev = once.begin();
     if (once_dev >= 0)
@@ -676,18 +736,18 @@ static int launch_loop_persistent_width(LoopDev* loops, int n_loops, int max_epo
             B200_CUDA_TRY(cudaFuncSetAttribute(trk_loop_persistent_kernel<THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
             once.done(once_dev);
         }
-    trk_loop_persistent_kernel<THREADS><<<n_loops, THREADS, smem_bytes, st>>>(loops, n_loops, max_epochs, avail, chans, bands, records, rec_capacity,
-        n_records, tbl_cap);
+    trk_loop_persistent_kernel<THREADS><<<n_loops, THREADS, smem_bytes, st>>>(loops, n_loops, max_epochs, avail, chans, bands, data, records,
+        rec_capacity, n_records, prompts, tbl_cap);
     B200_CUDA_TRY(cudaGetLastError());
     return B200_OK;
 }
 
 int launch_loop_persistent(LoopDev* loops, int n_loops, int max_epochs, const LoopAvail& avail, const ChanDesc* chans, const BandDesc* bands,
-    unsigned int* records, int rec_capacity, int* n_records, int max_code_len, cudaStream_t st)
+    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, int max_code_len, cudaStream_t st)
 {
     if (n_loops <= 0 || max_epochs <= 0) return B200_OK;
     int tbl_cap = max_code_len + kTrkTablePad;
-    const int cap_limit = (200 * 1024 - 4096) / 4;
+    const int cap_limit = (200 * 1024 - 4096) / (data ? 8 : 4);   // one or two tables
     if (tbl_cap > cap_limit) tbl_cap = cap_limit;
     tbl_cap = (tbl_cap + 3) & ~3;
     // width: each loop is a latency chain, so with no more loops than SMs a wide CTA is the faster one; beyond that two narrow
@@ -700,17 +760,19 @@ int launch_loop_persistent(LoopDev* loops, int n_loops, int max_epochs, const Lo
     bool wide = n_loops <= sms;
     if (const char* env = std::getenv("B200_LOOP_WIDTH")) wide = std::atoi(env) >= kLoopThreadsFew;
     if (wide && kLoopThreadsMany < kLoopThreadsFew)
-        return launch_loop_persistent_width<kLoopThreadsFew>(loops, n_loops, max_epochs, avail, chans, bands, records, rec_capacity, n_records, tbl_cap, st);
-    return launch_loop_persistent_width<kLoopThreadsMany>(loops, n_loops, max_epochs, avail, chans, bands, records, rec_capacity, n_records, tbl_cap, st);
+        return launch_loop_persistent_width<kLoopThreadsFew>(loops, n_loops, max_epochs, avail, chans, bands, data, records, rec_capacity, n_records,
+            prompts, tbl_cap, st);
+    return launch_loop_persistent_width<kLoopThreadsMany>(loops, n_loops, max_epochs, avail, chans, bands, data, records, rec_capacity, n_records,
+        prompts, tbl_cap, st);
 }
 
 int launch_loop_cycle(LoopDev* loops, int n_loops, int mode, const LoopAvail& avail, b200_trk_item* items, const float2* taps,
-    unsigned int* records, int rec_capacity, int* n_records, cudaStream_t st)
+    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, cudaStream_t st)
 {
     if (n_loops <= 0) return B200_OK;
     const int threads = 32;  // one loop per thread, spread over SMs: the per-loop chain is latency-bound
-    trk_loop_cycle_kernel<<<(n_loops + threads - 1) / threads, threads, 0, st>>>(loops, n_loops, mode, avail, items, taps, records,
-        rec_capacity, n_records);
+    trk_loop_cycle_kernel<<<(n_loops + threads - 1) / threads, threads, 0, st>>>(loops, n_loops, mode, avail, items, taps, data, records,
+        rec_capacity, n_records, prompts);
     B200_CUDA_TRY(cudaGetLastError());
     return B200_OK;
 }

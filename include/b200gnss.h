@@ -205,8 +205,12 @@ extern "C"
      * cn0_and_tracking_lock_status :1167-1224, run_dll_pll :1260-1347, update_tracking_vars :1409-1483,
      * log_data :1599-1694), evaluated on the device between correlator launches, so that epoch k+1's
      * NCO commands never visit the host.  Types follow the reference member by member (float where it
-     * is float, double where it is double).  Bit synchronisation, the secondary-code search, extended
-     * integration (states 3/4) and telemetry stay with the host, which reads the per-epoch records.
+     * is float, double where it is double).  A loop correlates its own channel (3 or 5 taps) and, when it
+     * tracks a pilot and has a data channel (b200_trk_loop_set_data_channel), also the data code at the
+     * prompt's shift with the same NCO values, as track_pilot does (:637-668, :1245-1256); both run on the
+     * device.  Bit synchronisation, the secondary-code search, extended integration (states 3/4) and
+     * telemetry stay with the host, which reads the per-epoch records (and, with a data channel, the pilot
+     * prompts of b200_trk_loop_run_prompts).
      * Field names are Dll_Pll_Conf's (src/algorithms/tracking/libs/dll_pll_conf.h:32-89) or the
      * block's own members (dll_pll_veml_tracking.h:128-222). */
     typedef struct b200_trk_loop_conf
@@ -298,23 +302,37 @@ extern "C"
      * first sample the tracking block would see next (state 1 then skips to the PRN start). */
     int b200_trk_loop_start(b200_engine* e, int loop_id, double acq_delay_samples, double acq_doppler_hz,
         uint64_t acq_samplestamp_samples, uint64_t nitems_read);
-    /* Run up to max_epochs cycles of every started loop: per epoch one correlator launch over all loops
-     * and one loop-update launch; a loop whose next vector_length samples are not all inside its band's
-     * [valid_from, write_index) (the window b200_iq_window reports) stalls: samples not pushed yet, overwritten,
-     * or left behind by a gap, a restart or b200_iq_forget are never correlated.
+    /* Attach a data channel to a loop that tracks a pilot (track_pilot = true, :637-668, :820-903): every epoch
+     * then also correlates data_channel - one correlator, at the pilot prompt's shift, on the loop's band, not
+     * high-dynamics; anything else is refused with B200_ERR_ARG - on the loop's item.  The records' prompt_I /
+     * prompt_Q become the data prompt, as log_data writes it (:1614-1617); every other field and the whole loop
+     * update keep using the pilot taps.  Accepted before b200_trk_loop_run or between runs; a second call
+     * replaces the data channel.  Set cloop as a pilot loop needs it (b200_trk_loop_conf). */
+    int b200_trk_loop_set_data_channel(b200_engine* e, int loop_id, int data_channel);
+    /* Run up to max_epochs cycles of every started loop: per epoch the correlation of each loop's channel (and of
+     * its data channel, if it has one) and the loop update, all on the device; a loop whose next vector_length
+     * samples are not all inside its band's [valid_from, write_index) (the window b200_iq_window reports) stalls:
+     * samples not pushed yet, overwritten, or left behind by a gap, a restart or b200_iq_forget are never correlated.
      * records_host: n_loops x max_epochs records (loop-major); n_records_host[loop] = cycles logged.
-     * Either output may be NULL. */
+     * Either output may be NULL.  Same as b200_trk_loop_run_prompts with pilot_prompts_host = NULL. */
     int b200_trk_loop_run(b200_engine* e, int max_epochs, b200_trk_dump_record* records_host, int* n_records_host);
+    /* b200_trk_loop_run plus the complex pilot prompt of every logged record: pilot_prompts_host (NULL: not
+     * returned) is n_loops x max_epochs, loop-major like the records.  With a data channel the record carries the
+     * data prompt, and these are what the host's bit synchronisation and secondary-code search read (:2031, :2079). */
+    int b200_trk_loop_run_prompts(b200_engine* e, int max_epochs, b200_trk_dump_record* records_host, int* n_records_host,
+        b200_cf32* pilot_prompts_host);
     /* How b200_trk_loop_run schedules the work: 0 (default) one persistent kernel, one CTA per loop, free-running
      * for max_epochs cycles with no launch per epoch; 1 a correlator launch + a loop-update launch per epoch with
      * one CTA per loop (same integers as mode 0, floats within an ulp of atanf/log10f: the correlator sums in a different order); 2 the same with each epoch split over several CTAs
      * (lowest latency for a handful of channels).  Env B200_LOOP_MODE sets the initial value. */
     int b200_trk_loop_set_mode(b200_engine* e, int mode);
     /* Prepare (if not already pending) and return the next work item of every loop: the seven scalars
-     * do_correlation_step would pass, for hosts that correlate elsewhere.  n == 0 marks a loop in standby. */
+     * do_correlation_step would pass, for hosts that correlate elsewhere.  n == 0 marks a loop in standby.
+     * One item per loop: a loop's data item is that item with the data channel's id. */
     int b200_trk_loop_peek_items(b200_engine* e, b200_trk_item* items_host);
     /* One cycle with caller-supplied correlator outputs (taps_host: n_loops x taps of the loop's channel,
-     * loop-major, stride = 8): the loop arithmetic alone, for hosts that correlate elsewhere and for tests. */
+     * loop-major, stride = 8; a loop with a data channel takes its data tap in the slot after the pilot taps,
+     * 3 after E,P,L or 5 after VE..VL): the loop arithmetic alone, for hosts that correlate elsewhere and for tests. */
     int b200_trk_loop_step_taps(b200_engine* e, const b200_cf32* taps_host, b200_trk_dump_record* records_host, int* logged_host);
     int b200_trk_loop_status_get(b200_engine* e, int loop_id, b200_trk_loop_status* out);
     /* Append records to a tracking dump file in the reference's format (d_dump_file, :1599-1694). */
