@@ -8,6 +8,7 @@
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
+#include <type_traits>
 
 namespace b200
 {
@@ -84,21 +85,41 @@ constexpr int kTrkThreads = 256;            // threads per CTA
 constexpr int kTrkTile = 2 * kTrkThreads;   // samples per CTA iteration (one LDG.128 per thread)
 constexpr int kTrkReseed = 16;              // tiles between exact phasor re-seeds
 constexpr int kTrkTablePad = 64;            // extra entries of the extended code table
+constexpr int kTrkSmemMax = 200 * 1024;     // dynamic shared memory the per-item and loop kernels opt in to
 
-// Launchers (trk_kernels.cu).  All pointers are device-accessible.
+// entries of each extended code table in a CTA's shared memory: the longest code + padding, limited so that `tables` of them
+// and reserved_bytes of other data fit, rounded up to 4
+inline int trk_table_cap(int max_code_len, int tables, int reserved_bytes)
+{
+    const int cap_limit = (kTrkSmemMax - reserved_bytes) / (4 * tables);
+    const int cap = max_code_len + kTrkTablePad;
+    return ((cap < cap_limit ? cap : cap_limit) + 3) & ~3;
+}
+
+// f(std::integral_constant<int, T>{}) for the T of Ts that equals taps; B200_ERR_ARG when there is none
+template <int... Ts, class F>
+int with_taps(int taps, const F& f)
+{
+    int rc = B200_ERR_ARG;
+    (void)((taps == Ts ? (rc = f(std::integral_constant<int, Ts>{}), true) : false) || ...);
+    return rc;
+}
+
+// Launchers (trk_kernels.cu).  All pointers are device-accessible.  Each adds the number of kernels it issued to `launched`.
+// taps_mask: bit t set when some channel with a code table has t taps (one launch per tap count; an empty mask is an error)
 int launch_trk_batch(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands,
     float2* out, int out_stride, int slices, float2* partial, unsigned int* counters,
-    int max_code_len, int taps_uniform, cudaStream_t stream, unsigned int taps_mask = 0u);
+    int max_code_len, unsigned int taps_mask, cudaStream_t stream, uint64_t& launched);
 size_t trk_partial_elems(int n_items, int slices);
-// shared-window kernel (trk_shared_kernel.cu): groups of 8 items share one copy of the samples
+// shared-window kernel (trk_shared_kernel.cu): groups of 8 items share one copy of the samples; every channel has `taps` taps
 int launch_trk_shared(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands, float2* out,
-    int out_stride, int taps_uniform, cudaStream_t stream);
+    int out_stride, int taps, cudaStream_t stream, uint64_t& launched);
 int trk_shared_max_code_len();
 // legacy correlator variants (trk_variants.cu): complex local code, 16-bit samples and code
 int launch_trk_cplx_code(const float2* x, const float2* code, int n, int L, int taps, const float* shifts, float rem_carr, float dphi, float rem_code,
-    float step, float2* out, cudaStream_t st);
+    float step, float2* out, cudaStream_t st, uint64_t& launched);
 int launch_trk_16sc(const short* x_iq, const short* code_iq, int n, int L, int taps, const float* shifts, float rem_carr, float dphi, float rem_code,
-    float step, short* out_iq, cudaStream_t st);
+    float step, short* out_iq, cudaStream_t st, uint64_t& launched);
 
 }  // namespace b200
 

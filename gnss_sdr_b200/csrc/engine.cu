@@ -50,7 +50,6 @@ int upload_tables(b200_engine* e)
     const int n = static_cast<int>(e->chans.size());
     B200_CUDA_TRY(e->chans_dev.grow(n, n + 64));
     e->max_code_len = 0;
-    e->taps_uniform = -1;
     e->taps_mask = 0u;
     e->any_high_dyn = false;
     if (n > 0)
@@ -63,16 +62,11 @@ int upload_tables(b200_engine* e)
                     if (cd[i].code == nullptr) continue;
                     if (cd[i].high_dyn) e->any_high_dyn = true;
                     e->taps_mask |= 1u << cd[i].taps;
-                    if (e->taps_uniform == -1)
-                        e->taps_uniform = cd[i].taps;
-                    else if (e->taps_uniform != cd[i].taps)
-                        e->taps_uniform = 0;
                 }
             // synchronous-safe: source is a temporary, so block until the copy has been staged
             B200_CUDA_TRY(cudaMemcpyAsync(e->chans_dev, cd.data(), sizeof(ChanDesc) * n, cudaMemcpyHostToDevice, e->stream));
             B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
         }
-    if (e->taps_uniform < 0) e->taps_uniform = 0;
     e->tables_dirty = false;
     return B200_OK;
 }
@@ -600,27 +594,21 @@ extern "C"
                 const char* env = std::getenv("B200_TRK_SHARED");
                 e->shared_mode = env ? std::atoi(env) : 2;  // 2 = automatic
             }
-        const bool shared_legal = (e->taps_uniform == 1 || e->taps_uniform == 3 || e->taps_uniform == 5) && !e->any_high_dyn && slices == 1;
+        // the shared-window kernel takes batches whose channels all have 1, 3 or 5 taps
+        const unsigned int mask = e->taps_mask;
+        const bool shared_legal = (mask == (1u << 1) || mask == (1u << 3) || mask == (1u << 5)) && !e->any_high_dyn && slices == 1;
         const bool use_shared = shared_legal && (e->shared_mode == 1 || (e->shared_mode == 2 && n_items >= 1024 && layout_hint != 0 &&
                                                                             e->max_code_len <= trk_shared_max_code_len()));
+        uint64_t launched = 0;
         if (use_shared)
             rc = launch_trk_shared(items_dev, n_items, e->chans_dev, e->bands_dev, reinterpret_cast<float2*>(out_dev), out_stride,
-                e->taps_uniform, e->stream);
+                __builtin_ctz(mask), e->stream, launched);
         else
             rc = launch_trk_batch(items_dev, n_items, e->chans_dev, e->bands_dev, reinterpret_cast<float2*>(out_dev), out_stride,
-                slices, e->partial, e->counters, e->max_code_len, e->taps_uniform, e->stream, e->taps_uniform == 0 ? e->taps_mask : 0u);
-        if (rc == B200_OK)
-            {
-                // a batch with several tap counts on the per-item path is one launch per specialised kernel (trk_kernels.cu)
-                int n_launch = 1;
-                if (!use_shared && e->taps_uniform == 0 && e->taps_mask != 0u)
-                    {
-                        const unsigned int special = e->taps_mask & ((1u << 1) | (1u << 3) | (1u << 5));
-                        n_launch = __builtin_popcount(special) + ((e->taps_mask & ~special) ? 1 : 0);
-                    }
-                e->launches += static_cast<uint64_t>(n_launch);
-            }
-        return rc;
+                slices, e->partial, e->counters, e->max_code_len, mask, e->stream, launched);
+        if (rc) return rc;
+        e->launches += launched;
+        return B200_OK;
     }
 
     int b200_trk_kernel_choice(b200_engine* e, int mode)
@@ -955,12 +943,13 @@ extern "C"
         int slices = (n + 4 * kTrkTile - 1) / (4 * kTrkTile);
         if (slices < 1) slices = 1;
         if (slices > t->slices_cap) slices = t->slices_cap;
+        uint64_t launched = 0;
         int rc = launch_trk_batch(&c->item, 1, &c->chan, &c->band, c->out, B200_MAX_TAPS, slices, t->partial, t->counter,
-            c->chan.code_len, t->taps == 1 || t->taps == 3 || t->taps == 5 ? t->taps : 0, t->stream);
+            c->chan.code_len, 1u << t->taps, t->stream, launched);
         if (rc) return rc;
         {
             std::lock_guard<std::mutex> lk(t->e->mu);
-            t->e->launches++;
+            t->e->launches += launched;
         }
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
         for (int k = 0; k < t->taps; k++)
@@ -1004,12 +993,13 @@ extern "C"
             }
         B200_ENTER_DEVICE(t->e->device);
         if (n > 0) B200_CUDA_TRY(cudaMemcpyAsync(t->sig_dev, sig_in_host, sizeof(float2) * n, cudaMemcpyHostToDevice, t->stream));
+        uint64_t launched = 0;
         const int rc = launch_trk_cplx_code(t->sig_dev, t->cplx_code_dev, n, t->cplx_code_len, t->taps, t->var_shifts, rem_carrier_phase_in_rad,
-            phase_step_rad, rem_code_phase_chips, code_phase_step_chips, t->out_cplx_dev, t->stream);
+            phase_step_rad, rem_code_phase_chips, code_phase_step_chips, t->out_cplx_dev, t->stream, launched);
         if (rc) return rc;
         {
             std::lock_guard<std::mutex> lk(t->e->mu);
-            t->e->launches++;
+            t->e->launches += launched;
         }
         B200_CUDA_TRY(cudaMemcpyAsync(corr_out_host, t->out_cplx_dev, sizeof(float2) * t->taps, cudaMemcpyDeviceToHost, t->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
@@ -1050,12 +1040,13 @@ extern "C"
             }
         B200_ENTER_DEVICE(t->e->device);
         if (n > 0) B200_CUDA_TRY(cudaMemcpyAsync(t->sig16_dev, sig_in_iq_host, sizeof(short) * 2 * n, cudaMemcpyHostToDevice, t->stream));
+        uint64_t launched = 0;
         const int rc = launch_trk_16sc(t->sig16_dev, t->code16_dev, n, t->code16_len, t->taps, t->var_shifts, rem_carrier_phase_in_rad, phase_step_rad,
-            rem_code_phase_chips, code_phase_step_chips, t->out16_dev, t->stream);
+            rem_code_phase_chips, code_phase_step_chips, t->out16_dev, t->stream, launched);
         if (rc) return rc;
         {
             std::lock_guard<std::mutex> lk(t->e->mu);
-            t->e->launches++;
+            t->e->launches += launched;
         }
         B200_CUDA_TRY(cudaMemcpyAsync(corr_out_iq_host, t->out16_dev, sizeof(short) * 2 * t->taps, cudaMemcpyDeviceToHost, t->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));

@@ -64,8 +64,7 @@ struct b200_engine
     b200::DevBuf<b200::ChanDesc> chans_dev;
     bool tables_dirty{true};
     int max_code_len{0};
-    int taps_uniform{-1};
-    unsigned int taps_mask{0};   // bit t set: some channel with a code table has t taps (mixed batches run one launch per tap count)
+    unsigned int taps_mask{0};   // bit t set: some channel with a code table has t taps (a batch runs one launch per tap count)
     bool any_high_dyn{false};
     int shared_mode{-1};   // -1 auto, 0 never, 1 always-when-legal (env B200_TRK_SHARED)
     b200::DevBuf<float2> partial;

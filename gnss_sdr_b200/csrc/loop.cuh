@@ -72,11 +72,12 @@ constexpr int kLoopDataItems = 8;   // prepare writes the data items to their ro
                                     // (without it the data tap is slot `taps` of the loop's own row, as b200_trk_loop_step_taps passes it)
 
 // loop_kernels_nofma.cu.  data: per loop (may be nullptr: no data channels); prompts: n_loops x rec_capacity pilot prompts
-// beside the records (may be nullptr).
+// beside the records (may be nullptr).  Both launchers add the number of kernels they issued to `launched`.
 int launch_loop_cycle(LoopDev* loops, int n_loops, int mode, const LoopAvail& avail, b200_trk_item* items, const float2* taps,
-    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, cudaStream_t st);
+    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, cudaStream_t st, uint64_t& launched);
 // persistent free-running tracker: one CTA per loop, up to max_epochs cycles without leaving the SM; data == nullptr when no
 // loop of the launch has a data channel (one code table in shared memory instead of two)
 int launch_loop_persistent(LoopDev* loops, int n_loops, int max_epochs, const LoopAvail& avail, const ChanDesc* chans, const BandDesc* bands,
-    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, int max_code_len, cudaStream_t st);
+    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, int max_code_len, cudaStream_t st,
+    uint64_t& launched);
 }  // namespace b200

@@ -165,12 +165,10 @@ int upload_loop_data(b200_engine* e)
 // the kernels' view: nullptr while no loop has a data channel
 const LoopData* loop_data_dev(const b200_engine* e) { return e->loop_n_data ? e->loop_data_dev.get() : nullptr; }
 
-int correlate_loop_items(b200_engine* e, int n, int slices)
+int correlate_loop_items(b200_engine* e, int n, int slices, uint64_t& launched)
 {
-    int rc = launch_trk_batch(e->loop_items_dev, n, e->chans_dev, e->bands_dev, e->loop_taps_dev, kLoopTapStride, slices, e->partial,
-        e->counters, e->max_code_len, e->taps_uniform, e->stream, e->taps_uniform == 0 ? e->taps_mask : 0u);
-    if (rc == B200_OK) e->launches++;
-    return rc;
+    return launch_trk_batch(e->loop_items_dev, n, e->chans_dev, e->bands_dev, e->loop_taps_dev, kLoopTapStride, slices, e->partial,
+        e->counters, e->max_code_len, e->taps_mask, e->stream, launched);
 }
 }  // namespace
 
@@ -368,12 +366,12 @@ extern "C"
             }
         const LoopAvail avail = snapshot_avail(e);
         B200_CUDA_TRY(cudaMemsetAsync(e->loop_nrec_dev, 0, sizeof(int) * n, e->stream));
+        uint64_t launched = 0;
         if (e->loop_mode == 0)
             {
                 rc = launch_loop_persistent(e->loops_dev, n, max_epochs, avail, e->chans_dev, e->bands_dev, data, e->loop_rec_dev, max_epochs,
-                    e->loop_nrec_dev, prompts, e->max_code_len, e->stream);
+                    e->loop_nrec_dev, prompts, e->max_code_len, e->stream, launched);
                 if (rc) return rc;
-                e->launches++;
             }
         else
             {
@@ -385,19 +383,18 @@ extern "C"
                 rc = ensure_partials(e, n_items, slices);
                 if (rc) return rc;
                 rc = launch_loop_cycle(e->loops_dev, n, kLoopPrepare | kLoopCheckAvail | data_items, avail, e->loop_items_dev, e->loop_taps_dev, data,
-                    nullptr, 0, nullptr, nullptr, e->stream);
+                    nullptr, 0, nullptr, nullptr, e->stream, launched);
                 if (rc) return rc;
-                e->launches++;
                 for (int k = 0; k < max_epochs; k++)
                     {
-                        rc = correlate_loop_items(e, n_items, slices);
+                        rc = correlate_loop_items(e, n_items, slices, launched);
                         if (rc) return rc;
                         rc = launch_loop_cycle(e->loops_dev, n, kLoopUpdate | kLoopPrepare | kLoopCheckAvail | data_items, avail, e->loop_items_dev,
-                            e->loop_taps_dev, data, e->loop_rec_dev, max_epochs, e->loop_nrec_dev, prompts, e->stream);
+                            e->loop_taps_dev, data, e->loop_rec_dev, max_epochs, e->loop_nrec_dev, prompts, e->stream, launched);
                         if (rc) return rc;
-                        e->launches++;
                     }
             }
+        e->launches += launched;
         std::vector<int> nrec(n);
         B200_CUDA_TRY(cudaMemcpyAsync(nrec.data(), e->loop_nrec_dev, sizeof(int) * n, cudaMemcpyDeviceToHost, e->stream));
         if (records_host)
@@ -430,10 +427,11 @@ extern "C"
         int rc = ensure_loop_buffers(e, 1);
         if (rc) return rc;
         const LoopAvail avail{};
+        uint64_t launched = 0;
         rc = launch_loop_cycle(e->loops_dev, n, kLoopPrepare, avail, e->loop_items_dev, e->loop_taps_dev, loop_data_dev(e), nullptr, 0, nullptr,
-            nullptr, e->stream);
+            nullptr, e->stream, launched);
         if (rc) return rc;
-        e->launches++;
+        e->launches += launched;
         B200_CUDA_TRY(cudaMemcpyAsync(items_host, e->loop_items_dev, sizeof(b200_trk_item) * n, cudaMemcpyDeviceToHost, e->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
         return B200_OK;
@@ -451,13 +449,15 @@ extern "C"
         const LoopAvail avail{};
         B200_CUDA_TRY(cudaMemsetAsync(e->loop_nrec_dev, 0, sizeof(int) * n, e->stream));
         const LoopData* data = loop_data_dev(e);
-        rc = launch_loop_cycle(e->loops_dev, n, kLoopPrepare, avail, e->loop_items_dev, e->loop_taps_dev, data, nullptr, 0, nullptr, nullptr, e->stream);
+        uint64_t launched = 0;
+        rc = launch_loop_cycle(e->loops_dev, n, kLoopPrepare, avail, e->loop_items_dev, e->loop_taps_dev, data, nullptr, 0, nullptr, nullptr, e->stream,
+            launched);
         if (rc) return rc;
         B200_CUDA_TRY(cudaMemcpyAsync(e->loop_taps_dev, taps_host, sizeof(float2) * kLoopTapStride * n, cudaMemcpyHostToDevice, e->stream));
         rc = launch_loop_cycle(e->loops_dev, n, kLoopUpdate, avail, e->loop_items_dev, e->loop_taps_dev, data, e->loop_rec_dev, 1, e->loop_nrec_dev,
-            nullptr, e->stream);
+            nullptr, e->stream, launched);
         if (rc) return rc;
-        e->launches += 2;
+        e->launches += launched;
         if (records_host)
             B200_CUDA_TRY(cudaMemcpyAsync(records_host, e->loop_rec_dev, sizeof(b200_trk_dump_record) * n, cudaMemcpyDeviceToHost, e->stream));
         if (logged_host) B200_CUDA_TRY(cudaMemcpyAsync(logged_host, e->loop_nrec_dev, sizeof(int) * n, cudaMemcpyDeviceToHost, e->stream));

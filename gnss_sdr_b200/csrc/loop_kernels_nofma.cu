@@ -455,6 +455,16 @@ __device__ bool loop_update(LoopDev& L, const float2* t, const float2* data, uns
     return logged;
 }
 
+// The record slot k of loop i (nullptr when records is nullptr or the loop's capacity is used up) and its pilot prompt (nullptr
+// also without prompts).
+__device__ __forceinline__ unsigned int* record_slot(unsigned int* records, float2* prompts, int rec_capacity, int i, int k, float2*& prompt)
+{
+    prompt = nullptr;
+    if (!records || k >= rec_capacity) return nullptr;
+    if (prompts) prompt = prompts + static_cast<size_t>(i) * rec_capacity + k;
+    return records + (static_cast<size_t>(i) * rec_capacity + k) * kLoopRecordWords;
+}
+
 __global__ void trk_loop_cycle_kernel(LoopDev* loops, int n_loops, int mode, LoopAvail avail, b200_trk_item* items,
     const float2* __restrict__ taps, const LoopData* __restrict__ data, unsigned int* records, int rec_capacity, int* n_records,
     float2* prompts)
@@ -467,14 +477,9 @@ __global__ void trk_loop_cycle_kernel(LoopDev* loops, int n_loops, int mode, Loo
     const LoopData d = data ? data[i] : LoopData{-1, 0};
     if ((mode & kLoopUpdate) && L.pending)
         {
-            unsigned int* rec = nullptr;
-            float2* prm = nullptr;
             const int k = n_records ? n_records[i] : 0;
-            if (records && k < rec_capacity)
-                {
-                    rec = records + (static_cast<size_t>(i) * rec_capacity + k) * kLoopRecordWords;
-                    if (prompts) prm = prompts + static_cast<size_t>(i) * rec_capacity + k;
-                }
+            float2* prm;
+            unsigned int* rec = record_slot(records, prompts, rec_capacity, i, k, prm);
             const float2* t = taps + static_cast<size_t>(i) * kLoopTapStride;
             // the data tap: row d.item of the correlator output, or the slot after the pilot taps (b200_trk_loop_step_taps)
             const float2* pd = nullptr;
@@ -527,6 +532,14 @@ __device__ __noinline__ float2 loop_correlate_data(const b200_trk_item& it, cons
     return r[0];
 }
 
+// the persistent kernel's copies of a LoopDev between global and shared memory, word by word over the CTA (tid, stride)
+__device__ __forceinline__ void copy_words(LoopDev* dst, const LoopDev* src, int tid, int stride)
+{
+    unsigned int* d = reinterpret_cast<unsigned int*>(dst);
+    const unsigned int* s = reinterpret_cast<const unsigned int*>(src);
+    for (int w = tid; w < static_cast<int>(sizeof(LoopDev) / 4); w += stride) d[w] = s[w];
+}
+
 // data: nullptr when no loop of the launch has a data channel; otherwise the data channel of every loop (-1: none), and the
 // dynamic shared memory holds a second code table of tbl_cap entries for it, right after the pilot's.
 template <int kLoopThreads>
@@ -555,16 +568,12 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
     const int i = blockIdx.x;
     const int tid = threadIdx.x;
     if (i >= n_loops) return;
-    {
-        const unsigned int* src = reinterpret_cast<const unsigned int*>(loops + i);
-        unsigned int* dst = reinterpret_cast<unsigned int*>(sL);
-        for (int w = tid; w < static_cast<int>(sizeof(LoopDev) / 4); w += kLoopThreads) dst[w] = src[w];
-        if (tid == 0)
-            {
-                s_tbl_cache[0] = s_tbl_cache[1] = s_tbl_cache_data[0] = s_tbl_cache_data[1] = 0;
-                s_data_channel = data ? data[i].channel : -1;
-            }
-    }
+    copy_words(sL, loops + i, tid, kLoopThreads);
+    if (tid == 0)
+        {
+            s_tbl_cache[0] = s_tbl_cache[1] = s_tbl_cache_data[0] = s_tbl_cache_data[1] = 0;
+            s_data_channel = data ? data[i].channel : -1;
+        }
     __syncthreads();
     const ChanDesc& ch = chans[sL->channel];
     const BandDesc bd = bands[ch.band];
@@ -603,19 +612,16 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                     //   warp 2 / lanes<5  the five magnitudes of the dump record
                     // The parts write disjoint members of the state.  When the lock verdict is "lost" (once per run at most) the
                     // state is put back from the copy taken below and the update is replayed in the reference's order.
-                    {
-                        const unsigned int* src = reinterpret_cast<const unsigned int*>(sL);
-                        unsigned int* dst = reinterpret_cast<unsigned int*>(sBackup);
-                        for (int w = tid; w < static_cast<int>(sizeof(LoopDev) / 4); w += kLoopThreads) dst[w] = src[w];
-                    }
+                    copy_words(sBackup, sL, tid, kLoopThreads);
                     __syncthreads();
                     PF_MARK(1)   // state copy + barrier
                     if (tid == 0)
                         {
                             loop_track_part(*sL, t);
                             s_stamp = loop_record_stamp(*sL);
-                            s_rec = (records && k_rec < rec_capacity) ? records + (static_cast<size_t>(i) * rec_capacity + k_rec) * kLoopRecordWords : nullptr;
-                            s_prm = (s_rec && prompts) ? prompts + static_cast<size_t>(i) * rec_capacity + k_rec : nullptr;
+                            float2* prm;
+                            s_rec = record_slot(records, prompts, rec_capacity, i, k_rec, prm);
+                            s_prm = prm;
                         }
                     else if (tid == 32)
                         {
@@ -642,13 +648,8 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                 {
                     if (have_taps)
                         {
-                            unsigned int* rec = nullptr;
-                            float2* prm = nullptr;
-                            if (records && k_rec < rec_capacity)
-                                {
-                                    rec = records + (static_cast<size_t>(i) * rec_capacity + k_rec) * kLoopRecordWords;
-                                    if (prompts) prm = prompts + static_cast<size_t>(i) * rec_capacity + k_rec;
-                                }
+                            float2* prm;
+                            unsigned int* rec = record_slot(records, prompts, rec_capacity, i, k_rec, prm);
                             if (s_lock_ok < 0)
                                 {
                                     if (loop_update(*sL, t, s_data_channel >= 0 ? &s_data_tap : nullptr, rec, prm)) k_rec++;
@@ -660,9 +661,7 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                                 }
                             else
                                 {
-                                    const unsigned int* src = reinterpret_cast<const unsigned int*>(sBackup);
-                                    unsigned int* dst = reinterpret_cast<unsigned int*>(sL);
-                                    for (int w = 0; w < static_cast<int>(sizeof(LoopDev) / 4); w++) dst[w] = src[w];
+                                    copy_words(sL, sBackup, 0, 1);
                                     if (loop_update(*sL, t, s_data_channel >= 0 ? &s_data_tap : nullptr, rec, prm)) k_rec++;
                                 }
                         }
@@ -714,11 +713,7 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
     __syncthreads();
     if (tid == 0) sL->pending = 0;
     __syncthreads();
-    {
-        unsigned int* dst = reinterpret_cast<unsigned int*>(loops + i);
-        const unsigned int* src = reinterpret_cast<const unsigned int*>(sL);
-        for (int w = tid; w < static_cast<int>(sizeof(LoopDev) / 4); w += kLoopThreads) dst[w] = src[w];
-    }
+    copy_words(loops + i, sL, tid, kLoopThreads);
     if (tid == 0 && n_records) n_records[i] = k_rec;
 }
 }  // namespace
@@ -733,7 +728,7 @@ static int launch_loop_persistent_width(LoopDev* loops, int n_loops, int max_epo
     const int once_dev = once.begin();
     if (once_dev >= 0)
         {
-            B200_CUDA_TRY(cudaFuncSetAttribute(trk_loop_persistent_kernel<THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+            B200_CUDA_TRY(cudaFuncSetAttribute(trk_loop_persistent_kernel<THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrkSmemMax));
             once.done(once_dev);
         }
     trk_loop_persistent_kernel<THREADS><<<n_loops, THREADS, smem_bytes, st>>>(loops, n_loops, max_epochs, avail, chans, bands, data, records,
@@ -743,13 +738,11 @@ static int launch_loop_persistent_width(LoopDev* loops, int n_loops, int max_epo
 }
 
 int launch_loop_persistent(LoopDev* loops, int n_loops, int max_epochs, const LoopAvail& avail, const ChanDesc* chans, const BandDesc* bands,
-    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, int max_code_len, cudaStream_t st)
+    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, int max_code_len, cudaStream_t st,
+    uint64_t& launched)
 {
     if (n_loops <= 0 || max_epochs <= 0) return B200_OK;
-    int tbl_cap = max_code_len + kTrkTablePad;
-    const int cap_limit = (200 * 1024 - 4096) / (data ? 8 : 4);   // one or two tables
-    if (tbl_cap > cap_limit) tbl_cap = cap_limit;
-    tbl_cap = (tbl_cap + 3) & ~3;
+    const int tbl_cap = trk_table_cap(max_code_len, data ? 2 : 1, 4096);   // one table, or two with the data channels'
     // width: each loop is a latency chain, so with no more loops than SMs a wide CTA is the faster one; beyond that two narrow
     // CTAs per SM overlap each other's serial sections.  On an H100 (400 W), us per epoch: 32 loops 10.1-10.5 at 512 threads,
     // 11.2 at 256; 256 loops 29.5-30.0 at 256 threads, 33.6-34.0 at 512.
@@ -759,21 +752,24 @@ int launch_loop_persistent(LoopDev* loops, int n_loops, int max_epochs, const Lo
     B200_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     bool wide = n_loops <= sms;
     if (const char* env = std::getenv("B200_LOOP_WIDTH")) wide = std::atoi(env) >= kLoopThreadsFew;
-    if (wide && kLoopThreadsMany < kLoopThreadsFew)
-        return launch_loop_persistent_width<kLoopThreadsFew>(loops, n_loops, max_epochs, avail, chans, bands, data, records, rec_capacity, n_records,
-            prompts, tbl_cap, st);
-    return launch_loop_persistent_width<kLoopThreadsMany>(loops, n_loops, max_epochs, avail, chans, bands, data, records, rec_capacity, n_records,
-        prompts, tbl_cap, st);
+    const int rc = (wide && kLoopThreadsMany < kLoopThreadsFew)
+                       ? launch_loop_persistent_width<kLoopThreadsFew>(loops, n_loops, max_epochs, avail, chans, bands, data, records, rec_capacity,
+                             n_records, prompts, tbl_cap, st)
+                       : launch_loop_persistent_width<kLoopThreadsMany>(loops, n_loops, max_epochs, avail, chans, bands, data, records, rec_capacity,
+                             n_records, prompts, tbl_cap, st);
+    if (rc == B200_OK) launched++;
+    return rc;
 }
 
 int launch_loop_cycle(LoopDev* loops, int n_loops, int mode, const LoopAvail& avail, b200_trk_item* items, const float2* taps,
-    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, cudaStream_t st)
+    const LoopData* data, unsigned int* records, int rec_capacity, int* n_records, float2* prompts, cudaStream_t st, uint64_t& launched)
 {
     if (n_loops <= 0) return B200_OK;
     const int threads = 32;  // one loop per thread, spread over SMs: the per-loop chain is latency-bound
     trk_loop_cycle_kernel<<<(n_loops + threads - 1) / threads, threads, 0, st>>>(loops, n_loops, mode, avail, items, taps, data, records,
         rec_capacity, n_records, prompts);
     B200_CUDA_TRY(cudaGetLastError());
+    launched++;
     return B200_OK;
 }
 }  // namespace b200

@@ -1,4 +1,5 @@
-// Device helpers shared by the tracking kernels (trk_kernels.cu, trk_shared_kernel.cu).
+// Device helpers shared by the tracking kernels (trk_kernels.cu, trk_shared_kernel.cu, trk_variants.cu and, through
+// trk_item.cuh, loop_kernels_nofma.cu).  Every contraction is written out, so they compute the same under --fmad=false.
 #pragma once
 
 #include "common.cuh"
@@ -36,10 +37,80 @@ __device__ __forceinline__ int chip_index_hd_avx(float step, float rate, float n
     return __float2int_rd(__fadd_rn(__fadd_rn(__fmul_rn(step, nf), __fmul_rn(rate, nn)), aux2));
 }
 
+// chip index of sample n of an epoch: the AVX association below body = 8*(N/8), the generic one in the tail
+__device__ __forceinline__ int chip_index_at(float step, int n, int body, float shift, float rem)
+{
+    const float nf = static_cast<float>(n);
+    return (n < body) ? chip_index_avx(step, nf, __fsub_rn(shift, rem)) : chip_index_generic(step, nf, shift, rem);
+}
+
+// [lo, hi] of the AVX-association chip indices of every tap over the samples n_first..n_last (monotone in n, so the ends
+// suffice); aux(t) = fl(shift_t - rem).
+template <int TAPS, class Aux>
+__device__ __forceinline__ void chip_range(float step, float n_first, float n_last, const Aux& aux, int& lo, int& hi)
+{
+    lo = 0x7fffffff;
+    hi = -0x7fffffff - 1;
+#pragma unroll
+    for (int t = 0; t < TAPS; t++)
+        {
+            const int i0 = chip_index_avx(step, n_first, aux(t));
+            const int i1 = chip_index_avx(step, n_last, aux(t));
+            lo = min(lo, min(i0, i1));
+            hi = max(hi, max(i0, i1));
+        }
+}
+
 __device__ __forceinline__ int mod_pos(int k, int L)
 {
     int r = k % L;
     return r < 0 ? r + L : r;
+}
+
+// Stages the code window [base, base + span) (indices modulo L) into a table: entries pos, pos + stride, ... are this
+// thread's, store(j, code + i) writes entry j from code value i.
+template <class Store>
+__device__ __forceinline__ void stage_code_window(const float* code, int L, int base, int span, int pos, int stride, const Store& store)
+{
+    int r = mod_pos(base + pos, L);
+    const int step = stride % L;
+    for (int j = pos; j < span; j += stride)
+        {
+            store(j, code + r);
+            r += step;
+            if (r >= L) r -= L;
+        }
+}
+
+// floor() by the 1.5*2^23 trick: fl_rd(x + kFloorMagic) has floor(x) in its low mantissa bits (exact for |x| < 2^22), so a
+// table entry's shared-memory address is one LEA, (bits << 2) + table_offset(table, base) for the entry floor(x) - base.
+constexpr float kFloorMagic = 12582912.0f;  // bit pattern 0x4B400000
+__device__ __forceinline__ unsigned int table_offset(const float* smem_tbl, int base)
+{
+    // computed inside an asm so the optimiser cannot split the constant back out of the per-lookup LEA
+    unsigned int off;
+    asm("sub.u32 %0, %1, %2;"
+        : "=r"(off)
+        : "r"(static_cast<unsigned int>(__cvta_generic_to_shared(smem_tbl))), "r"(4u * (static_cast<unsigned int>(base) + 0x4B400000u)));
+    return off;
+}
+
+template <class T>
+__device__ __forceinline__ T warp_sum(T v)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+__device__ __forceinline__ float2 warp_sum(float2 v)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+        {
+            v.x += __shfl_xor_sync(0xffffffffu, v.x, o);
+            v.y += __shfl_xor_sync(0xffffffffu, v.y, o);
+        }
+    return v;
 }
 
 // exp(j*2*pi*T/2^64)
@@ -58,6 +129,17 @@ __device__ __forceinline__ unsigned long long turns_from_rad(double rad)
     double t = rad * 0.15915494309189535;  // 1/(2*pi)
     t -= rint(t);
     return static_cast<unsigned long long>(__double2ll_rn(t * 18446744073709551616.0));
+}
+
+// carrier phase and step of an item in 64-bit turns (phase(n) = -(rem + n*step)), and body = 8*(N/8)
+struct ItemPhase
+{
+    unsigned long long T0, DT;
+    int body;
+};
+__device__ __forceinline__ ItemPhase item_phase(float rem_carrier_phase_rad, float phase_step_rad, int n)
+{
+    return ItemPhase{turns_from_rad(-static_cast<double>(rem_carrier_phase_rad)), turns_from_rad(-static_cast<double>(phase_step_rad)), (n / 8) * 8};
 }
 
 __device__ __forceinline__ float2 cmulf(float2 a, float2 b)
@@ -97,6 +179,34 @@ __device__ __forceinline__ float lds_f32(unsigned int addr)
     float v;
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
     return v;
+}
+
+// (zr, zi) *= (Dr2, Di2): the phasors of a sample pair (.x, .y) advance by one step D
+__device__ __forceinline__ void advance_pair(float2& zr, float2& zi, float2 Dr2, float2 Di2)
+{
+    const float2 t1 = mul2_rn(zi, Di2);
+    const float2 nzr = fma2_rn(zr, Dr2, make_float2(-t1.x, -t1.y));
+    zi = fma2_rn(zr, Di2, mul2_rn(zi, Dr2));
+    zr = nzr;
+}
+
+// The taps of one sample pair (.x = sample n, .y = n+1) with rotated samples (wr2, wi2) and m2 = fl(step * n): each tap's chip
+// is floor(fl(m2 + aux2[t])) by the kFloorMagic trick, looked up in the extended table (tbl_off = table_offset()).
+template <int TAPS>
+__device__ __forceinline__ void pair_taps(float2 m2, const float2 (&aux2)[TAPS], unsigned int tbl_off, float2 wr2, float2 wi2,
+    float2 (&are)[TAPS], float2 (&aim)[TAPS])
+{
+    const float2 magic2 = make_float2(kFloorMagic, kFloorMagic);
+#pragma unroll
+    for (int t = 0; t < TAPS; t++)
+        {
+            const float2 tt = add2_rd(add2_rn(m2, aux2[t]), magic2);
+            const float ca = lds_f32((__float_as_uint(tt.x) << 2) + tbl_off);
+            const float cb = lds_f32((__float_as_uint(tt.y) << 2) + tbl_off);
+            const float2 c2 = make_float2(ca, cb);
+            are[t] = fma2_rn(wr2, c2, are[t]);
+            aim[t] = fma2_rn(wi2, c2, aim[t]);
+        }
 }
 
 }  // namespace

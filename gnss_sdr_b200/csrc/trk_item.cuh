@@ -117,13 +117,10 @@ __device__ __forceinline__ void correlate_range(const ItemCtx& cx, const float (
                     const float2 z = phasor_from_turns(cx.T0 + cx.DT * static_cast<unsigned long long>(n));
                     const float wr = fmaf(x.x, z.x, -x.y * z.y);
                     const float wi = fmaf(x.x, z.y, x.y * z.x);
-                    const float nf = static_cast<float>(n);
 #pragma unroll
                     for (int t = 0; t < TAPS; t++)
                         {
-                            const int idx = (n < cx.body) ? chip_index_avx(cx.step, nf, aux2[t])
-                                                          : chip_index_generic(cx.step, nf, shifts[t], cx.rem);
-                            const float c = lut(idx);
+                            const float c = lut(chip_index_at(cx.step, n, cx.body, shifts[t], cx.rem));
                             acc[t].x = fmaf(wr, c, acc[t].x);
                             acc[t].y = fmaf(wi, c, acc[t].y);
                         }
@@ -133,10 +130,8 @@ __device__ __forceinline__ void correlate_range(const ItemCtx& cx, const float (
 
 
 // ---- main tiles, FAST path: arithmetic on sample pairs, no modulo, no F2I -----------------------------
-// Lane .x of every float2 value belongs to sample n0, lane .y to sample n0+1 (one LDG.128).
-// floor() uses the 1.5*2^23 trick: fl_rm(aux + 12582912.f) has floor(aux) in its low mantissa bits
-// (exact for |aux| < 2^22, guaranteed by the caller's range check), so the table address is one LEA:
-//   addr = (bits << 2) + tbl_off,  tbl_off = smem(table) - 4*(tbl_base + 0x4B400000)  (mod 2^32).
+// Lane .x of every float2 value belongs to sample n0, lane .y to sample n0+1 (one LDG.128).  The chip lookup is pair_taps'
+// floor trick (exact for |index| < 2^22, guaranteed by the caller's range check); tbl_off = table_offset().
 template <int TAPS, bool WRAPS, int THREADS = kTrkThreads>
 __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const float (&shifts)[TAPS], unsigned int tbl_off,
     int tile_begin, int tile_end, int head, float2 (&acc)[TAPS])
@@ -154,7 +149,6 @@ __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const fl
 #pragma unroll
     for (int t = 0; t < TAPS; t++) are[t] = aim[t] = make_float2(0.f, 0.f);
 
-    const float2 magic2 = make_float2(12582912.0f, 12582912.0f);
     const float2 D = phasor_from_turns(cx.DT * static_cast<unsigned long long>(kTile));
     const float2 Dr2 = make_float2(D.x, D.x), Di2 = make_float2(D.y, D.y);
     // group-to-group phasor step: kTrkReseed tiles
@@ -192,31 +186,15 @@ __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const fl
                     wr2.y = fmaf(v.z, zr.y, -v.w * zi.y);
                     wi2.y = fmaf(v.z, zi.y, v.w * zr.y);
                     const float2 m2 = make_float2(__fmul_rn(cx.step, nfa), __fmul_rn(cx.step, nfb));
-#pragma unroll
-                    for (int t = 0; t < TAPS; t++)
-                        {
-                            const float2 tt = add2_rd(add2_rn(m2, aux2[t]), magic2);
-                            const float ca = lds_f32((__float_as_uint(tt.x) << 2) + tbl_off);
-                            const float cb = lds_f32((__float_as_uint(tt.y) << 2) + tbl_off);
-                            const float2 c2 = make_float2(ca, cb);
-                            are[t] = fma2_rn(wr2, c2, are[t]);
-                            aim[t] = fma2_rn(wi2, c2, aim[t]);
-                        }
-                    // z *= D
-                    const float2 t1 = mul2_rn(zi, Di2);
-                    const float2 nzr = fma2_rn(zr, Dr2, make_float2(-t1.x, -t1.y));
-                    zi = fma2_rn(zr, Di2, mul2_rn(zi, Dr2));
-                    zr = nzr;
+                    pair_taps<TAPS>(m2, aux2, tbl_off, wr2, wi2, are, aim);
+                    advance_pair(zr, zi, Dr2, Di2);
                     nfa += static_cast<float>(kTile);
                     nfb += static_cast<float>(kTile);
                     n0 += kTile;
                     ptr += kTile;
                 }
             // group seed advances by G (few steps per epoch: error stays ~1e-7 per step)
-            const float2 t2 = mul2_rn(zi2, Gi2);
-            const float2 ngr = fma2_rn(zr2, Gr2, make_float2(-t2.x, -t2.y));
-            zi2 = fma2_rn(zr2, Gi2, mul2_rn(zi2, Gr2));
-            zr2 = ngr;
+            advance_pair(zr2, zi2, Gr2, Gi2);
         }
 #pragma unroll
     for (int t = 0; t < TAPS; t++)
@@ -283,16 +261,17 @@ __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const 
 {
     constexpr int kTile = 2 * THREADS;  // samples per CTA iteration (one LDG.128 per thread)
     const int tid = threadIdx.x;
+    const ItemPhase ph = item_phase(it.rem_carrier_phase_rad, it.phase_step_rad, it.n);
     ItemCtx cx;
     cx.base = bd.base;
     cx.mask = bd.mask;
     cx.s0 = it.sample_index - bd.first_index;
     cx.N = it.n;
-    cx.body = (it.n / 8) * 8;
+    cx.body = ph.body;
     cx.step = it.code_phase_step_chips;
     cx.rem = it.rem_code_phase_chips;
-    cx.T0 = turns_from_rad(-static_cast<double>(it.rem_carrier_phase_rad));
-    cx.DT = turns_from_rad(-static_cast<double>(it.phase_step_rad));
+    cx.T0 = ph.T0;
+    cx.DT = ph.DT;
     const int L = ch.code_len;
 
     float shifts[TAPS];
@@ -309,7 +288,7 @@ __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const 
             const bool in_smem = L <= tbl_cap;
             if (in_smem)
                 {
-                    for (int j = tid; j < L; j += THREADS) smem_tbl[j] = ch.code[j];
+                    stage_code_window(ch.code, L, 0, L, tid, THREADS, [&](int j, const float* src) { smem_tbl[j] = *src; });
                 }
             __syncthreads();
             LookupMod lut{in_smem ? smem_tbl : ch.code, L};
@@ -320,33 +299,23 @@ __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const 
         }
     else
         {
-            // index range over the epoch (monotone in n within each association)
-            long long lo = 0x7fffffff, hi = -0x7fffffff - 1LL;
-            const float nl_avx = static_cast<float>(max(cx.body - 1, 0));
+            // index range over the epoch (monotone in n within each association): the AVX association's ends, plus the
+            // generic association's at body, N-1 and 0 (epochs shorter than 8 samples)
+            int lo, hi;
+            chip_range<TAPS>(cx.step, 0.f, static_cast<float>(max(cx.body - 1, 0)), [&](int t) { return __fsub_rn(shifts[t], cx.rem); }, lo, hi);
             const float n_last = static_cast<float>(max(cx.N - 1, 0));
             const float n_body = static_cast<float>(cx.body);
 #pragma unroll
             for (int t = 0; t < TAPS; t++)
                 {
-                    const float a2 = __fsub_rn(shifts[t], cx.rem);
-                    int v[4];
-                    v[0] = chip_index_avx(cx.step, 0.f, a2);
-                    v[1] = chip_index_avx(cx.step, nl_avx, a2);
-                    v[2] = chip_index_generic(cx.step, n_body, shifts[t], cx.rem);
-                    v[3] = chip_index_generic(cx.step, n_last, shifts[t], cx.rem);
-                    // association 0 also evaluated at n = 0 (epochs shorter than 8 samples)
-                    const int v4 = chip_index_generic(cx.step, 0.f, shifts[t], cx.rem);
-#pragma unroll
-                    for (int q = 0; q < 4; q++)
-                        {
-                            lo = min(lo, static_cast<long long>(v[q]));
-                            hi = max(hi, static_cast<long long>(v[q]));
-                        }
-                    lo = min(lo, static_cast<long long>(v4));
-                    hi = max(hi, static_cast<long long>(v4));
+                    const int g0 = chip_index_generic(cx.step, n_body, shifts[t], cx.rem);
+                    const int g1 = chip_index_generic(cx.step, n_last, shifts[t], cx.rem);
+                    const int g2 = chip_index_generic(cx.step, 0.f, shifts[t], cx.rem);
+                    lo = min(lo, min(g0, min(g1, g2)));
+                    hi = max(hi, max(g0, max(g1, g2)));
                 }
-            const long long tbl_base = lo - 2;
-            const long long span = hi - lo + 5;
+            const long long tbl_base = static_cast<long long>(lo) - 2;
+            const long long span = static_cast<long long>(hi) - lo + 5;
 
             const int head = static_cast<int>(cx.s0 & 1ULL);
             const int ntiles = (cx.body > head) ? (cx.body - head) / kTile : 0;
@@ -377,17 +346,7 @@ __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const 
                                     span_st += 2 * margin;
                                 }
                         }
-                    if (stage)
-                        {
-                            int r = mod_pos(base_i + tid, L);
-                            const int stride = THREADS % L;
-                            for (int j = tid; j < span_st; j += THREADS)
-                                {
-                                    smem_tbl[j] = ch.code[r];
-                                    r += stride;
-                                    if (r >= L) r -= L;
-                                }
-                        }
+                    if (stage) stage_code_window(ch.code, L, base_i, span_st, tid, THREADS, [&](int j, const float* src) { smem_tbl[j] = *src; });
                     __syncthreads();
                     if (REUSE && stage && tid == 0)
                         {
@@ -395,15 +354,9 @@ __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const 
                             tbl_cache[1] = base_i + span_st;
                         }
                     LookupExt lut{smem_tbl - base_i};
-                    if (lo > -4000000LL && hi < 4000000LL)
+                    if (lo > -4000000 && hi < 4000000)
                         {
-                            // computed inside an asm so the optimiser cannot split the constant back out of
-                            // the per-lookup LEA
-                            unsigned int tbl_off;
-                            asm("sub.u32 %0, %1, %2;"
-                                : "=r"(tbl_off)
-                                : "r"(static_cast<unsigned int>(__cvta_generic_to_shared(smem_tbl))),
-                                  "r"(4u * (static_cast<unsigned int>(base_i) + 0x4B400000u)));
+                            const unsigned int tbl_off = table_offset(smem_tbl, base_i);
                             // ring wrap inside the epoch? (uniform per item)
                             const bool wraps = ((cx.s0 & cx.mask) + static_cast<unsigned long long>(cx.N)) > cx.mask;
                             if (wraps)
@@ -424,7 +377,7 @@ __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const 
                     if (REUSE && tid == 0) tbl_cache[1] = tbl_cache[0];  // smem_tbl no longer holds an extended window
                     if (in_smem)
                         {
-                            for (int j = tid; j < L; j += THREADS) smem_tbl[j] = ch.code[j];
+                            stage_code_window(ch.code, L, 0, L, tid, THREADS, [&](int j, const float* src) { smem_tbl[j] = *src; });
                         }
                     __syncthreads();
                     LookupMod lut{in_smem ? smem_tbl : ch.code, L};
@@ -434,15 +387,7 @@ __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const 
 
     // ---- CTA reduction: shuffles, then 8 warp partials through shared memory -------------------
 #pragma unroll
-    for (int t = 0; t < TAPS; t++)
-        {
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1)
-                {
-                    acc[t].x += __shfl_xor_sync(0xffffffffu, acc[t].x, o);
-                    acc[t].y += __shfl_xor_sync(0xffffffffu, acc[t].y, o);
-                }
-        }
+    for (int t = 0; t < TAPS; t++) acc[t] = warp_sum(acc[t]);
     const int warp = tid >> 5, lane = tid & 31;
     if (lane == 0)
         {

@@ -69,23 +69,24 @@ __device__ __forceinline__ void run_item(const b200_trk_item& it, const ChanDesc
         }
 }
 
-// TAPS_T > 0: every channel in the launch has exactly TAPS_T taps (specialised registers).
-// TAPS_T == 0: taps read per item.
-// No minimum-blocks hint by default.  sm_90a, no spills: <3> 64 registers (4 CTAs per SM), <1> 60, <5> 80 (3 CTAs), <0> 128.
+// One instantiation per tap count 1..8 (registers specialised to it).
+// No minimum-blocks hint by default.  sm_90a, no spills: <3> 64 registers (4 CTAs per SM), <1> 60, <5> 80 (3 CTAs).
 // TRK_MIN_BLOCKS builds the alternatives for tools/ab_item.sh.  On an H100 (400 W), ms per step: TRK_MIN_BLOCKS=4 (everything
-// at 64 registers; <0> spills 3.3 KB) C3 5.43-5.46 vs 5.52-5.53, but C3 + pilot 9.12-9.14 vs 8.93-8.98 and the C5 share
-// 2.73-2.80 vs 2.60-2.64; TRK_MIN_BLOCKS=3 slower on all four legs.  The default stays.
+// at 64 registers; the generic kernel then in use spilled 3.3 KB) C3 5.43-5.46 vs 5.52-5.53, but C3 + pilot 9.12-9.14 vs
+// 8.93-8.98 and the C5 share 2.73-2.80 vs 2.60-2.64; TRK_MIN_BLOCKS=3 slower on all four legs.  The default stays.
 #ifdef TRK_MIN_BLOCKS
 #define TRK_LAUNCH_BOUNDS __launch_bounds__(kTrkThreads, TRK_MIN_BLOCKS)
 #else
-#define TRK_LAUNCH_BOUNDS __launch_bounds__(kTrkThreads)
+// tap counts other than 1, 3 and 5 keep the register budget of two CTAs per SM (128) that the kernel which read the tap count
+// per item had: left to ptxas, <4>, <6> and <7> settle at 64-80 registers and spill
+#define TRK_LAUNCH_BOUNDS __launch_bounds__(kTrkThreads, (TAPS == 1 || TAPS == 3 || TAPS == 5) ? 0 : 2)
 #endif
-template <int TAPS_T>
+template <int TAPS>
 __global__ void TRK_LAUNCH_BOUNDS trk_correlate_kernel(const b200_trk_item* __restrict__ items, int n_items,
     const ChanDesc* __restrict__ chans, const BandDesc* __restrict__ bands, float2* __restrict__ out, int out_stride,
     int slices, float2* partial, unsigned int* counters, int tbl_cap, unsigned int only_mask)
 {
-    // only_mask != 0: a batch with several tap counts runs as one launch per specialisation; this launch serves the items whose
+    // only_mask != 0: a batch with several tap counts runs as one launch per tap count; this launch serves the items whose
     // channel has (1 << taps) in the mask and leaves the others to their own launch
     extern __shared__ __align__(16) float smem[];
     float* smem_tbl = smem;
@@ -106,36 +107,19 @@ __global__ void TRK_LAUNCH_BOUNDS trk_correlate_kernel(const b200_trk_item* __re
                     if (slice == 0 && threadIdx.x < ch.taps) out[static_cast<size_t>(item_id) * out_stride + threadIdx.x] = make_float2(0.f, 0.f);
                     continue;
                 }
-            if (TAPS_T > 0)
-                {
-                    run_item<(TAPS_T > 0 ? TAPS_T : 1)>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters);
-                }
-            else
-                {
-                    switch (ch.taps)
-                        {
-                        case 1: run_item<1>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters); break;
-                        case 2: run_item<2>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters); break;
-                        case 3: run_item<3>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters); break;
-                        case 4: run_item<4>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters); break;
-                        case 5: run_item<5>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters); break;
-                        case 6: run_item<6>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters); break;
-                        case 7: run_item<7>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters); break;
-                        default: run_item<8>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters); break;
-                        }
-                }
+            run_item<TAPS>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters);
         }
 }
 
 template <int T>
 int launch_one(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands, float2* out,
-    int out_stride, int slices, float2* partial, unsigned int* counters, int tbl_cap, size_t smem_bytes, cudaStream_t stream, unsigned int only_mask = 0u)
+    int out_stride, int slices, float2* partial, unsigned int* counters, int tbl_cap, size_t smem_bytes, cudaStream_t stream, unsigned int only_mask)
 {
     static DeviceOnce once;
     const int once_dev = once.begin();
     if (once_dev >= 0)
         {
-            B200_CUDA_TRY(cudaFuncSetAttribute(trk_correlate_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+            B200_CUDA_TRY(cudaFuncSetAttribute(trk_correlate_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrkSmemMax));
             once.done(once_dev);
         }
     const long long work = static_cast<long long>(n_items) * slices;
@@ -155,35 +139,31 @@ size_t trk_partial_elems(int n_items, int slices)
 
 int launch_trk_batch(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands,
     float2* out, int out_stride, int slices, float2* partial, unsigned int* counters,
-    int max_code_len, int taps_uniform, cudaStream_t stream, unsigned int taps_mask)
+    int max_code_len, unsigned int taps_mask, cudaStream_t stream, uint64_t& launched)
 {
     if (n_items <= 0) return B200_OK;
-    if (slices < 1) slices = 1;
-    int tbl_cap = max_code_len + kTrkTablePad;
-    const int cap_limit = (200 * 1024 - 1024) / 4;
-    if (tbl_cap > cap_limit) tbl_cap = cap_limit;
-    tbl_cap = (tbl_cap + 3) & ~3;
-    const size_t smem_bytes = static_cast<size_t>(tbl_cap) * 4 + (kTrkThreads / 32) * B200_MAX_TAPS * sizeof(float2) + 16;
-    switch (taps_uniform)
+    if (taps_mask == 0u)
         {
-        case 1: return launch_one<1>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap, smem_bytes, stream);
-        case 3: return launch_one<3>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap, smem_bytes, stream);
-        case 5: return launch_one<5>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap, smem_bytes, stream);
-        default: break;
+            set_error("tracking batch: no channel has a code table");
+            return B200_ERR_STATE;
         }
-    // Several tap counts in one batch (a tracked pilot's 5 + 1 taps, a multi-signal receiver): one launch per specialised
-    // kernel, each serving its own items - the generic kernel (tap count read per item) needs 128 registers and halves the
-    // occupancy (C5 share and C3 + pilot ran on it).  Tap counts without a specialisation still take the generic kernel.
-    if (taps_mask == 0u) return launch_one<0>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap, smem_bytes, stream);
-    int rc = B200_OK;
-    if (taps_mask & (1u << 1)) rc = launch_one<1>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap, smem_bytes, stream, 1u << 1);
-    if (rc == B200_OK && (taps_mask & (1u << 3)))
-        rc = launch_one<3>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap, smem_bytes, stream, 1u << 3);
-    if (rc == B200_OK && (taps_mask & (1u << 5)))
-        rc = launch_one<5>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap, smem_bytes, stream, 1u << 5);
-    const unsigned int others = taps_mask & ~((1u << 1) | (1u << 3) | (1u << 5));
-    if (rc == B200_OK && others) rc = launch_one<0>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap, smem_bytes, stream, others);
-    return rc;
+    if (slices < 1) slices = 1;
+    const int tbl_cap = trk_table_cap(max_code_len, 1, 1024);
+    const size_t smem_bytes = static_cast<size_t>(tbl_cap) * 4 + (kTrkThreads / 32) * B200_MAX_TAPS * sizeof(float2) + 16;
+    // Several tap counts in one batch (a tracked pilot's 5 + 1 taps, a multi-signal receiver): one launch per tap count, each
+    // serving its own items.  A kernel that read the tap count per item needed 128 registers and halved the occupancy.
+    const bool mixed = (taps_mask & (taps_mask - 1u)) != 0u;
+    for (int taps = 1; taps <= B200_MAX_TAPS; taps++)
+        {
+            if (!(taps_mask & (1u << taps))) continue;
+            const unsigned int only_mask = mixed ? 1u << taps : 0u;
+            const int rc = with_taps<1, 2, 3, 4, 5, 6, 7, 8>(taps, [&](auto tc) {
+                return launch_one<decltype(tc)::value>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap, smem_bytes, stream, only_mask);
+            });
+            if (rc) return rc;
+            launched++;
+        }
+    return B200_OK;
 }
 
 }  // namespace b200

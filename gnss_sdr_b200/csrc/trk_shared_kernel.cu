@@ -123,26 +123,23 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
 
 // Correct-for-anything fallback for one warp: direct global loads, exact phasor per sample, integer
 // modulo lookup in the global code table.  Used when an item cannot take the table path.
-// T0, DT: the item's carrier phase and phase step in 64-bit turns.
+// T0, DT, body: the item's item_phase().
 template <int TAPS>
 __device__ void warp_correlate_general(const b200_trk_item& it, const ChanDesc& ch, const BandDesc& bd, unsigned long long T0,
-    unsigned long long DT, float2 (&acc)[TAPS])
+    unsigned long long DT, int body, float2 (&acc)[TAPS])
 {
     const int lane = threadIdx.x & 31;
     const unsigned long long s0 = it.sample_index - bd.first_index;
-    const int body = (it.n / 8) * 8;
     for (int n = lane; n < it.n; n += 32)
         {
             const float2 x = ldg_stream8(bd.base + ((s0 + static_cast<unsigned long long>(n)) & bd.mask));
             const float2 z = phasor_from_turns(T0 + DT * static_cast<unsigned long long>(n));
             const float wr = fmaf(x.x, z.x, -x.y * z.y);
             const float wi = fmaf(x.x, z.y, x.y * z.x);
-            const float nf = static_cast<float>(n);
 #pragma unroll
             for (int t = 0; t < TAPS; t++)
                 {
-                    const int idx = (n < body) ? chip_index_avx(it.code_phase_step_chips, nf, __fsub_rn(ch.shifts[t], it.rem_code_phase_chips))
-                                               : chip_index_generic(it.code_phase_step_chips, nf, ch.shifts[t], it.rem_code_phase_chips);
+                    const int idx = chip_index_at(it.code_phase_step_chips, n, body, ch.shifts[t], it.rem_code_phase_chips);
                     const float c = ch.code[mod_pos(idx, ch.code_len)];
                     acc[t].x = fmaf(wr, c, acc[t].x);
                     acc[t].y = fmaf(wi, c, acc[t].y);
@@ -179,7 +176,6 @@ template <int TAPS, bool MASKED, class Loader>
 __device__ __forceinline__ void warp_tile(const Loader& load, float vlo, float vhi, float step, const float2 (&aux2)[TAPS],
     unsigned int tbl_off, float2 Dr2, float2 Di2, float& fa, float& fb, float2& zr, float2& zi, float2 (&are)[TAPS], float2 (&aim)[TAPS])
 {
-    const float2 magic2 = make_float2(12582912.0f, 12582912.0f);
 #pragma unroll
     for (int k = 0; k < kShTile / 64; k++)
         {
@@ -201,20 +197,8 @@ __device__ __forceinline__ void warp_tile(const Loader& load, float vlo, float v
             wr2.y = fmaf(xb.x, zr.y, -xb.y * zi.y);
             wi2.y = fmaf(xb.x, zi.y, xb.y * zr.y);
             const float2 m2 = make_float2(__fmul_rn(step, ua), __fmul_rn(step, ub));
-#pragma unroll
-            for (int t = 0; t < TAPS; t++)
-                {
-                    const float2 tt = add2_rd(add2_rn(m2, aux2[t]), magic2);
-                    const float ca = lds_f32((__float_as_uint(tt.x) << 2) + tbl_off);
-                    const float cb = lds_f32((__float_as_uint(tt.y) << 2) + tbl_off);
-                    const float2 c2 = make_float2(ca, cb);
-                    are[t] = fma2_rn(wr2, c2, are[t]);
-                    aim[t] = fma2_rn(wi2, c2, aim[t]);
-                }
-            const float2 t1 = mul2_rn(zi, Di2);
-            const float2 nzr = fma2_rn(zr, Dr2, make_float2(-t1.x, -t1.y));
-            zi = fma2_rn(zr, Di2, mul2_rn(zi, Dr2));
-            zr = nzr;
+            pair_taps<TAPS>(m2, aux2, tbl_off, wr2, wi2, are, aim);
+            advance_pair(zr, zi, Dr2, Di2);
             fa += 64.0f;
             fb += 64.0f;
         }
@@ -231,7 +215,6 @@ template <int TAPS, bool MASKED>
 __device__ __forceinline__ void warp_tile_chunks(const float4* x4, float4* pre4, const float4* rot4, float n0f, float vlo, float vhi,
     float step, const float2 (&aux2)[TAPS], unsigned int tbl_off, float2 z0, float2 (&acc_re)[TAPS], float2 (&acc_im)[TAPS])
 {
-    const float magic = 12582912.0f;
     float2 r = make_float2(0.f, 0.f);
 #pragma unroll
     for (int k = 0; k < kShChunk / 2; k++)
@@ -257,14 +240,14 @@ __device__ __forceinline__ void warp_tile_chunks(const float4* x4, float4* pre4,
     for (int t = 0; t < TAPS; t++)
         {
             const float a = aux2[t].x;
-            const float t0 = __fadd_rd(__fadd_rn(__fmul_rn(step, lo), a), magic);
+            const float t0 = __fadd_rd(__fadd_rn(__fmul_rn(step, lo), a), kFloorMagic);
             float q = n0f;  // last sample of the chunk known to keep index i0
 #pragma unroll
             for (int s = 8; s > 0; s >>= 1)
                 {
                     const float cand = q + static_cast<float>(s);
                     const float ce = MASKED ? fminf(fmaxf(cand, vlo), vhi) : cand;
-                    const float tc = __fadd_rd(__fadd_rn(__fmul_rn(step, ce), a), magic);
+                    const float tc = __fadd_rd(__fadd_rn(__fmul_rn(step, ce), a), kFloorMagic);
                     q = (tc == t0) ? cand : q;
                 }
             const float2 P = pre[__float2int_rz(q - n0f)];
@@ -407,11 +390,12 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
     unsigned long long T0 = 0, DT = 0;
     if (have_item && it.n > 0)
         {
-            body = (it.n / 8) * 8;
+            const ItemPhase ph = item_phase(it.rem_carrier_phase_rad, it.phase_step_rad, it.n);
+            T0 = ph.T0;
+            DT = ph.DT;
+            body = ph.body;
             step = it.code_phase_step_chips;
             const float rem = it.rem_code_phase_chips;
-            T0 = turns_from_rad(-static_cast<double>(it.rem_carrier_phase_rad));
-            DT = turns_from_rad(-static_cast<double>(it.phase_step_rad));
             float smin = ch->shifts[0], smax = ch->shifts[0];
 #pragma unroll
             for (int t = 0; t < TAPS; t++)
@@ -434,16 +418,9 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                     // whole-epoch table when the epoch's chip range fits the warp's storage (C/A at any rate):
                     // filled once, no per-tile work.  Range from the epoch ends (index monotone in n).
                     {
-                        int elo = 0x7fffffff, ehi = -0x7fffffff - 1;
+                        int elo, ehi;
                         const float nl = static_cast<float>(max(body - 1, 0));
-#pragma unroll
-                        for (int q = 0; q < TAPS; q++)
-                            {
-                                const int i0 = chip_index_avx(step, 0.f, aux2[q].x);
-                                const int i1 = chip_index_avx(step, nl, aux2[q].x);
-                                elo = min(elo, min(i0, i1));
-                                ehi = max(ehi, max(i0, i1));
-                            }
+                        chip_range<TAPS>(step, 0.f, nl, [&](int q) { return aux2[q].x; }, elo, ehi);
                         whole_table = (static_cast<long long>(ehi) - elo + 3) <= kShTblCap;
                         // Chunk path: the index a(n) = fl(fl(step n) + aux) of every tap may rise at most once over the
                         // 16 samples of a chunk.  Both roundings err by at most half an ulp of a value of magnitude
@@ -457,6 +434,9 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                             {
                                 const int wb = elo - 1;
                                 const int wspan = ehi - elo + 3;
+                                // This copy and stage_window's are written out instead of calling stage_code_window: with it,
+                                // ptxas laid the kernel out differently and the C2 step ran 0.8 % slower on an H100 80GB HBM3
+                                // at 700 W (1 088 000-1 095 000 against 1 098 000-1 099 000 Msamples/s, three alternating runs).
                                 const int L = ch->code_len;
                                 int r = mod_pos(wb + lane, L);
                                 const int stride = 32 % L;
@@ -466,7 +446,7 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                                         r += stride;
                                         if (r >= L) r -= L;
                                     }
-                                asm("sub.u32 %0, %1, %2;" : "=r"(tbl_off) : "r"(smem_u32(&sm.tbl[warp][0])), "r"(4u * (static_cast<unsigned int>(wb) + 0x4B400000u)));
+                                tbl_off = table_offset(&sm.tbl[warp][0], wb);
                                 __syncwarp();
                             }
                     }
@@ -521,15 +501,8 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                 auto stage_window = [&](int tt) {
                     const int m0 = tt * kShTile - a_i;
                     const float lo_f = static_cast<float>(max(m0, 0)), hi_f = static_cast<float>(min(m0 + kShTile, body) - 1);
-                    int wlo = 0x7fffffff, whi = -0x7fffffff - 1;
-#pragma unroll
-                    for (int q = 0; q < TAPS; q++)
-                        {
-                            const int i0 = chip_index_avx(step, lo_f, aux2[q].x);
-                            const int i1 = chip_index_avx(step, hi_f, aux2[q].x);
-                            wlo = min(wlo, min(i0, i1));
-                            whi = max(whi, max(i0, i1));
-                        }
+                    int wlo, whi;
+                    chip_range<TAPS>(step, lo_f, hi_f, [&](int q) { return aux2[q].x; }, wlo, whi);
                     const int wb = wlo - 1;
                     const int wspan = min(whi - wlo + 3, kShWin);  // <= kShWin by the span_bound test
                     const int L = ch->code_len;
@@ -549,7 +522,7 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                 asm volatile("cp.async.wait_all;" ::: "memory");
                 __syncwarp();
                 if (t + 1 < t_last) next_wb = stage_window(t + 1);
-                asm("sub.u32 %0, %1, %2;" : "=r"(tbl_off) : "r"(smem_u32(&sm.tbl[warp][(t & 1) * kShWin])), "r"(4u * (static_cast<unsigned int>(wb) + 0x4B400000u)));
+                tbl_off = table_offset(&sm.tbl[warp][(t & 1) * kShWin], wb);
             }
         if (interior)
             warp_tile<TAPS, false>(load, vlo, vhi, step, aux2, tbl_off, Dr2, Di2, fa, fb, zr, zi, are, aim);
@@ -559,10 +532,7 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
             {
                 // re-seed: the group seed advances by G = exp(j DT 64*kShReseed) and replaces the
                 // running phasor (bounds the drift of the 64 recurrence steps in between)
-                const float2 t2 = mul2_rn(zi2, Gi2);
-                const float2 ngr = fma2_rn(zr2, Gr2, make_float2(-t2.x, -t2.y));
-                zi2 = fma2_rn(zr2, Gi2, mul2_rn(zi2, Gr2));
-                zr2 = ngr;
+                advance_pair(zr2, zi2, Gr2, Gi2);
                 zr = zr2;
                 zi = zi2;
                 tiles_in_group = 0;
@@ -658,7 +628,7 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
 #pragma unroll
                             for (int t = 0; t < TAPS; t++)
                                 {
-                                    const int idx = chip_index_generic(step, static_cast<float>(n), ch->shifts[t], it.rem_code_phase_chips);
+                                    const int idx = chip_index_at(step, n, body, ch->shifts[t], it.rem_code_phase_chips);
                                     const float c = __ldg(ch->code + mod_pos(idx, ch->code_len));
                                     acc[t].x = fmaf(wr, c, acc[t].x);
                                     acc[t].y = fmaf(wi, c, acc[t].y);
@@ -667,18 +637,10 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
                 }
             else
                 {
-                    warp_correlate_general<TAPS>(it, *ch, bd, T0, DT, acc);
+                    warp_correlate_general<TAPS>(it, *ch, bd, T0, DT, body, acc);
                 }
 #pragma unroll
-            for (int t = 0; t < TAPS; t++)
-                {
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1)
-                        {
-                            acc[t].x += __shfl_xor_sync(0xffffffffu, acc[t].x, o);
-                            acc[t].y += __shfl_xor_sync(0xffffffffu, acc[t].y, o);
-                        }
-                }
+            for (int t = 0; t < TAPS; t++) acc[t] = warp_sum(acc[t]);
             if (lane < TAPS)
                 {
                     float2 r = acc[0];
@@ -693,32 +655,33 @@ __global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b
             out[static_cast<size_t>(item_id) * out_stride + lane] = make_float2(0.f, 0.f);
         }
 }
-}  // namespace
-
-int launch_trk_shared(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands, float2* out,
-    int out_stride, int taps_uniform, cudaStream_t stream)
+template <int TAPS>
+int launch_shared(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands, float2* out, int out_stride,
+    cudaStream_t stream)
 {
-    if (n_items <= 0) return B200_OK;
-    const int groups = (n_items + kShK - 1) / kShK;
     static DeviceOnce once;  // per device: a second engine on another GPU needs its own opt-in
     const int once_dev = once.begin();
     if (once_dev >= 0)
         {
-            B200_CUDA_TRY(cudaFuncSetAttribute(trk_shared_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(ShSmem))));
-            B200_CUDA_TRY(cudaFuncSetAttribute(trk_shared_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(ShSmem))));
-            B200_CUDA_TRY(cudaFuncSetAttribute(trk_shared_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(ShSmem))));
+            B200_CUDA_TRY(cudaFuncSetAttribute(trk_shared_kernel<TAPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(ShSmem))));
             once.done(once_dev);
         }
-    const size_t smem = sizeof(ShSmem);
-    switch (taps_uniform)
-        {
-        case 1: trk_shared_kernel<1><<<groups, kShThreads, smem, stream>>>(items, n_items, chans, bands, out, out_stride); break;
-        case 3: trk_shared_kernel<3><<<groups, kShThreads, smem, stream>>>(items, n_items, chans, bands, out, out_stride); break;
-        case 5: trk_shared_kernel<5><<<groups, kShThreads, smem, stream>>>(items, n_items, chans, bands, out, out_stride); break;
-        default: return B200_ERR_ARG;
-        }
+    const int groups = (n_items + kShK - 1) / kShK;
+    trk_shared_kernel<TAPS><<<groups, kShThreads, sizeof(ShSmem), stream>>>(items, n_items, chans, bands, out, out_stride);
     B200_CUDA_TRY(cudaGetLastError());
     return B200_OK;
+}
+}  // namespace
+
+int launch_trk_shared(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands, float2* out,
+    int out_stride, int taps, cudaStream_t stream, uint64_t& launched)
+{
+    if (n_items <= 0) return B200_OK;
+    const int rc = with_taps<1, 3, 5>(taps, [&](auto tc) {
+        return launch_shared<decltype(tc)::value>(items, n_items, chans, bands, out, out_stride, stream);
+    });
+    if (rc == B200_OK) launched++;
+    return rc;
 }
 
 // Longest code table for which every epoch takes the whole-table mode (faster than the per-item kernel on C2).

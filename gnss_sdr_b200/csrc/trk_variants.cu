@@ -29,20 +29,9 @@ struct VarArgs
     float shifts[B200_MAX_TAPS];
 };
 
-template <typename ACC>
-__device__ __forceinline__ ACC warp_sum(ACC v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 __device__ __forceinline__ int chip_of(const VarArgs& a, int n, int body, int t)
 {
-    const float nf = static_cast<float>(n);
-    const int idx = (n < body) ? chip_index_avx(a.code_phase_step_chips, nf, __fsub_rn(a.shifts[t], a.rem_code_phase_chips))
-                               : chip_index_generic(a.code_phase_step_chips, nf, a.shifts[t], a.rem_code_phase_chips);
-    return mod_pos(idx, a.L);
+    return mod_pos(chip_index_at(a.code_phase_step_chips, n, body, a.shifts[t], a.rem_code_phase_chips), a.L);
 }
 
 // result[t] = sum_n (x[n] * exp(-j(phi0 + n dphi))) * code[idx_t(n)]   (complex code)
@@ -50,21 +39,19 @@ __global__ void __launch_bounds__(kVarThreads) trk_cplx_code_kernel(const float2
     float2* __restrict__ out)
 {
     __shared__ float2 red[kVarThreads / 32][B200_MAX_TAPS];
-    const unsigned long long T0 = turns_from_rad(-static_cast<double>(a.rem_carrier_phase_rad));
-    const unsigned long long DT = turns_from_rad(-static_cast<double>(a.phase_step_rad));
-    const int body = (a.n / 8) * 8;
+    const ItemPhase ph = item_phase(a.rem_carrier_phase_rad, a.phase_step_rad, a.n);
     float2 acc[B200_MAX_TAPS];
 #pragma unroll
     for (int t = 0; t < B200_MAX_TAPS; t++) acc[t] = make_float2(0.f, 0.f);
     for (int n = threadIdx.x; n < a.n; n += kVarThreads)
         {
-            const float2 w = cmulf(x[n], phasor_from_turns(T0 + DT * static_cast<unsigned long long>(n)));
+            const float2 w = cmulf(x[n], phasor_from_turns(ph.T0 + ph.DT * static_cast<unsigned long long>(n)));
 #pragma unroll
             for (int t = 0; t < B200_MAX_TAPS; t++)
                 {
                     if (t < a.taps)
                         {
-                            const float2 c = __ldg(code + chip_of(a, n, body, t));
+                            const float2 c = __ldg(code + chip_of(a, n, ph.body, t));
                             acc[t].x += fmaf(w.x, c.x, -w.y * c.y);
                             acc[t].y += fmaf(w.x, c.y, w.y * c.x);
                         }
@@ -74,8 +61,8 @@ __global__ void __launch_bounds__(kVarThreads) trk_cplx_code_kernel(const float2
 #pragma unroll
     for (int t = 0; t < B200_MAX_TAPS; t++)
         {
-            const float sx = warp_sum(acc[t].x), sy = warp_sum(acc[t].y);
-            if (lane == 0) red[warp][t] = make_float2(sx, sy);
+            const float2 s = warp_sum(acc[t]);
+            if (lane == 0) red[warp][t] = s;
         }
     __syncthreads();
     if (threadIdx.x < a.taps)
@@ -99,24 +86,22 @@ __global__ void __launch_bounds__(kVarThreads) trk_16sc_kernel(const short2* __r
     short2* __restrict__ out)
 {
     __shared__ long long red[kVarThreads / 32][B200_MAX_TAPS][2];
-    const unsigned long long T0 = turns_from_rad(-static_cast<double>(a.rem_carrier_phase_rad));
-    const unsigned long long DT = turns_from_rad(-static_cast<double>(a.phase_step_rad));
     // the 16-bit resamplers have no AVX float association of their own in the tail; index sequence as for the float kernels
-    const int body = (a.n / 8) * 8;
+    const ItemPhase ph = item_phase(a.rem_carrier_phase_rad, a.phase_step_rad, a.n);
     long long ar[B200_MAX_TAPS], ai[B200_MAX_TAPS];
 #pragma unroll
     for (int t = 0; t < B200_MAX_TAPS; t++) ar[t] = ai[t] = 0;
     for (int n = threadIdx.x; n < a.n; n += kVarThreads)
         {
             const short2 s = x[n];
-            const float2 w = cmulf(make_float2(static_cast<float>(s.x), static_cast<float>(s.y)), phasor_from_turns(T0 + DT * static_cast<unsigned long long>(n)));
+            const float2 w = cmulf(make_float2(static_cast<float>(s.x), static_cast<float>(s.y)), phasor_from_turns(ph.T0 + ph.DT * static_cast<unsigned long long>(n)));
             const int wr = static_cast<short>(__float2int_rn(w.x)), wi = static_cast<short>(__float2int_rn(w.y));
 #pragma unroll
             for (int t = 0; t < B200_MAX_TAPS; t++)
                 {
                     if (t < a.taps)
                         {
-                            const short2 c = code[chip_of(a, n, body, t)];
+                            const short2 c = code[chip_of(a, n, ph.body, t)];
                             const short pr = static_cast<short>(wr * c.x - wi * c.y);
                             const short pi = static_cast<short>(wr * c.y + wi * c.x);
                             ar[t] += pr;
@@ -149,10 +134,8 @@ __global__ void __launch_bounds__(kVarThreads) trk_16sc_kernel(const short2* __r
             out[threadIdx.x] = make_short2(static_cast<short>(sr), static_cast<short>(si));
         }
 }
-}  // namespace
 
-int launch_trk_cplx_code(const float2* x, const float2* code, int n, int L, int taps, const float* shifts, float rem_carr, float dphi, float rem_code,
-    float step, float2* out, cudaStream_t st)
+VarArgs var_args(int n, int L, int taps, const float* shifts, float rem_carr, float dphi, float rem_code, float step)
 {
     VarArgs a{};
     a.n = n;
@@ -163,26 +146,26 @@ int launch_trk_cplx_code(const float2* x, const float2* code, int n, int L, int 
     a.rem_code_phase_chips = rem_code;
     a.code_phase_step_chips = step;
     for (int t = 0; t < taps; t++) a.shifts[t] = shifts[t];
-    trk_cplx_code_kernel<<<1, kVarThreads, 0, st>>>(x, code, a, out);
+    return a;
+}
+}  // namespace
+
+int launch_trk_cplx_code(const float2* x, const float2* code, int n, int L, int taps, const float* shifts, float rem_carr, float dphi, float rem_code,
+    float step, float2* out, cudaStream_t st, uint64_t& launched)
+{
+    trk_cplx_code_kernel<<<1, kVarThreads, 0, st>>>(x, code, var_args(n, L, taps, shifts, rem_carr, dphi, rem_code, step), out);
     B200_CUDA_TRY(cudaGetLastError());
+    launched++;
     return B200_OK;
 }
 
 int launch_trk_16sc(const short* x_iq, const short* code_iq, int n, int L, int taps, const float* shifts, float rem_carr, float dphi, float rem_code,
-    float step, short* out_iq, cudaStream_t st)
+    float step, short* out_iq, cudaStream_t st, uint64_t& launched)
 {
-    VarArgs a{};
-    a.n = n;
-    a.L = L;
-    a.taps = taps;
-    a.rem_carrier_phase_rad = rem_carr;
-    a.phase_step_rad = dphi;
-    a.rem_code_phase_chips = rem_code;
-    a.code_phase_step_chips = step;
-    for (int t = 0; t < taps; t++) a.shifts[t] = shifts[t];
-    trk_16sc_kernel<<<1, kVarThreads, 0, st>>>(reinterpret_cast<const short2*>(x_iq), reinterpret_cast<const short2*>(code_iq), a,
-        reinterpret_cast<short2*>(out_iq));
+    trk_16sc_kernel<<<1, kVarThreads, 0, st>>>(reinterpret_cast<const short2*>(x_iq), reinterpret_cast<const short2*>(code_iq),
+        var_args(n, L, taps, shifts, rem_carr, dphi, rem_code, step), reinterpret_cast<short2*>(out_iq));
     B200_CUDA_TRY(cudaGetLastError());
+    launched++;
     return B200_OK;
 }
 }  // namespace b200
