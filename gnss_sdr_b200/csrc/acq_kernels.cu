@@ -570,44 +570,38 @@ __global__ void acq_twiddle_kernel(float2* __restrict__ tw, FftPlan pl)
         }
 }
 
+// (statistic, PRN, bin, code phase) a comes before b: the larger statistic, then the lower PRN, bin and code phase
+__device__ __forceinline__ bool acq_peak_before(const b200_acq_peak& a, const b200_acq_peak& b)
+{
+    if (a.test_statistics != b.test_statistics) return a.test_statistics > b.test_statistics;
+    if (a.prn != b.prn) return a.prn < b.prn;
+    if (a.index_doppler != b.index_doppler) return a.index_doppler < b.index_doppler;
+    return a.index_time < b.index_time;
+}
+
 // Best satellite of one sweep as ONE 16-byte record {test statistic, PRN, Doppler bin, code phase}: what a rank
 // contributes to the multi-GPU peak exchange (an all-gather of N records; SURVEY 8e).  Ties go to the lowest
-// (slot order, bin, code phase) like the reference's strict '>' scans (pcps_acquisition.cc:417-426).
+// (PRN, bin, code phase), the rule of dist.best_peak and of the reference's strict '>' scans (pcps_acquisition.cc:417-426),
+// whatever order prn_of_result lists the PRNs in.
 __global__ void acq_sweep_best_kernel(const b200_acq_result* __restrict__ results, const unsigned int* __restrict__ prn_of_result, int n,
     b200_acq_peak* __restrict__ out)
 {
     const int lane = threadIdx.x;
-    float best = -1.0f;
-    int who = 0x7fffffff;
+    // statistic -1 with the lowest keys: only a record with a statistic above -1 replaces it
+    b200_acq_peak best{-1.0f, 0u, 0u, 0u};
     for (int i = lane; i < n; i += 32)
         {
-            const float v = results[i].test_statistics;
-            if (v > best)
-                {
-                    best = v;
-                    who = i;
-                }
+            const b200_acq_peak v{results[i].test_statistics, prn_of_result[i], results[i].index_doppler, results[i].index_time};
+            if (acq_peak_before(v, best)) best = v;
         }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1)
         {
-            const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-            const int ow = __shfl_xor_sync(0xffffffffu, who, o);
-            if (ov > best || (ov == best && ow < who))
-                {
-                    best = ov;
-                    who = ow;
-                }
+            const b200_acq_peak ov{__shfl_xor_sync(0xffffffffu, best.test_statistics, o), __shfl_xor_sync(0xffffffffu, best.prn, o),
+                __shfl_xor_sync(0xffffffffu, best.index_doppler, o), __shfl_xor_sync(0xffffffffu, best.index_time, o)};
+            if (acq_peak_before(ov, best)) best = ov;
         }
-    if (lane == 0)
-        {
-            b200_acq_peak p;
-            p.test_statistics = (n > 0 && who != 0x7fffffff) ? best : 0.0f;
-            p.prn = (n > 0 && who != 0x7fffffff) ? prn_of_result[who] : 0u;
-            p.index_doppler = (n > 0 && who != 0x7fffffff) ? results[who].index_doppler : 0u;
-            p.index_time = (n > 0 && who != 0x7fffffff) ? results[who].index_time : 0u;
-            *out = p;
-        }
+    if (lane == 0) *out = (best.test_statistics > -1.0f) ? best : b200_acq_peak{0.0f, 0u, 0u, 0u};
 }
 
 DeviceOnce g_attr_once;  // per device (a second engine on another GPU needs its own opt-in), thread-safe
