@@ -193,7 +193,8 @@ __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const fl
                     n0 += kTile;
                     ptr += kTile;
                 }
-            // group seed advances by G (few steps per epoch: error stays ~1e-7 per step)
+            // group seed advances by the rounded G, not re-seeded from the 64-bit phase: its error grows by about 1e-7
+            // per group (8192 samples); see the measured bound in trk_kernels.cu
             advance_pair(zr2, zi2, Gr2, Gi2);
         }
 #pragma unroll
