@@ -117,6 +117,9 @@ _SIGS.update({
     "b200_acq_set_step_two": ([_vp, C.c_float, C.c_float, C.c_uint32], C.c_int),
     "b200_acq_search_step_two": ([_vp, _vp, C.c_uint32, C.c_uint32, C.c_float, _vp], C.c_int),
     "b200_acq_search_dev": ([_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp], C.c_int),
+    "b200_acq_search_band": ([_vp, C.c_int, C.c_uint64, _vp, C.c_uint32, C.c_uint32, _vp], C.c_int),
+    "b200_acq_search_band_submit": ([_vp, C.c_int, C.c_uint64, _vp, C.c_uint32, C.c_uint32], C.c_int),
+    "b200_acq_search_step_two_band": ([_vp, C.c_int, C.c_uint64, C.c_uint32, C.c_uint32, C.c_float, _vp], C.c_int),
     "b200_acq_read_grid": ([_vp, C.c_uint32, _vp], C.c_int),
     "b200_acq_selftest_dft": ([_vp, _vp, _vp], C.c_int),
     "b200_acq_read_wipeoffs": ([_vp, _vp], C.c_int),
@@ -553,6 +556,28 @@ class PcpsAcquisition:
         slots = np.ascontiguousarray(slots, np.uint32)
         _chk(lib.b200_acq_search_dev(self.h, in_dev_ptr, slots.ctypes.data, slots.size, dwell_counter, results_dev_ptr),
              "b200_acq_search_dev")
+
+    def search_band(self, band: int, abs_index: int, slots, dwell_counter: int = 1) -> np.ndarray:
+        """search samples [abs_index, abs_index + consumed_samples) of one of the engine's bands; the result's sample stamp
+        for loop_start is abs_index + consumed_samples"""
+        slots = np.ascontiguousarray(slots, np.uint32)
+        res = np.zeros(slots.size, ACQ_RESULT_DTYPE)
+        _chk(lib.b200_acq_search_band(self.h, band, int(abs_index), slots.ctypes.data, slots.size, dwell_counter, res.ctypes.data),
+             "b200_acq_search_band")
+        return res
+
+    def search_band_submit(self, band: int, abs_index: int, slots, dwell_counter: int = 1):
+        """queue search_band's sweep; search_wait() collects its results"""
+        slots = np.ascontiguousarray(slots, np.uint32)
+        _chk(lib.b200_acq_search_band_submit(self.h, band, int(abs_index), slots.ctypes.data, slots.size, dwell_counter),
+             "b200_acq_search_band_submit")
+        self._pending_n = slots.size
+
+    def search_step_two_band(self, band: int, abs_index: int, slot: int, prev_input_power: float, dwell_counter: int = 1) -> np.ndarray:
+        res = np.zeros(1, ACQ_RESULT_DTYPE)
+        _chk(lib.b200_acq_search_step_two_band(self.h, band, int(abs_index), slot, dwell_counter, prev_input_power, res.ctypes.data),
+             "b200_acq_search_step_two_band")
+        return res[0]
 
     def sweep_best_dev(self, results_dev_ptr: int, prn_of_result_dev_ptr: int, n_results: int, peak_dev_ptr: int):
         """one 16-byte b200_acq_peak record of the sweep, written on the device (no host synchronisation)"""

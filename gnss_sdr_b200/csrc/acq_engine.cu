@@ -79,10 +79,10 @@ struct b200_acq
 
 namespace
 {
-int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev,
+int bluestein_search(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev,
     int step_two, float prev_input_power, uint64_t& launched);
 
-int mixed_radix_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
+int mixed_radix_search(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
     b200_acq_result* results_dev, int step_two, float prev_input_power, uint64_t& launched)
 {
     const b200_acq_conf& c = a->c;
@@ -101,7 +101,7 @@ int mixed_radix_search(b200_acq* a, const float2* in_dev, const uint32_t* slots,
     const float2* wipe = step_two ? a->wipe2 : a->wipe;
     const int ne = static_cast<int>(c.effective_fft_size);
     const int off = c.bit_transition_flag ? ne : 0;
-    int rc = acq_launch_fwd(in_dev, static_cast<int>(c.consumed_samples), wipe, a->X, bins, a->plan, a->tw, launched, st);
+    int rc = acq_launch_fwd(in, static_cast<int>(c.consumed_samples), wipe, a->X, bins, a->plan, a->tw, launched, st);
     if (rc) return rc;
     rc = acq_launch_row_stats(a->X, a->codes, a->slot_list, static_cast<int>(n_slots), bins, a->plan, a->tw, off, ne, a->grid,
         dwell_counter > 1 ? 1 : 0, a->rowstat, a->Z, a->partial, launched, st);
@@ -116,7 +116,7 @@ int mixed_radix_search(b200_acq* a, const float2* in_dev, const uint32_t* slots,
     return acq_launch_finish_second_peak(a->second_peak, static_cast<int>(n_slots), results_dev, launched, st);
 }
 
-int search_impl(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
+int search_impl(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
     b200_acq_result* results_dev, int step_two = 0, float prev_input_power = 0.f)
 {
     const b200_acq_conf& c = a->c;
@@ -143,8 +143,8 @@ int search_impl(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32
             return B200_ERR_STATE;
         }
     uint64_t launched = 0;
-    const int rc = a->bl ? bluestein_search(a, in_dev, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power, launched)
-                         : mixed_radix_search(a, in_dev, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power, launched);
+    const int rc = a->bl ? bluestein_search(a, in, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power, launched)
+                         : mixed_radix_search(a, in, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power, launched);
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(a->e->mu);
     a->e->launches += launched;
@@ -263,7 +263,7 @@ int bluestein_setup_queue(b200_acq* a, std::vector<float2> (&host)[6])
 
 // rows x N: out[r] = DFT_N(in[r * in_stride .. ] . mult[r * mult_stride ..])   (forward chirp-z, natural order); inputs past
 // `consumed` count as zeros (acquisition_core zero-pads the consumed samples to fft_size, :657-664)
-int bluestein_forward_rows(b200_acq* a, const float2* in, size_t in_stride, int consumed, const float2* mult, size_t mult_stride, int rows,
+int bluestein_forward_rows(b200_acq* a, AcqInput in, size_t in_stride, int consumed, const float2* mult, size_t mult_stride, int rows,
     float2* out, uint64_t& launched)
 {
     b200_acq::Bluestein* b = a->bl.get();
@@ -274,7 +274,7 @@ int bluestein_forward_rows(b200_acq* a, const float2* in, size_t in_stride, int 
         a->stream);
 }
 
-int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev,
+int bluestein_search(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev,
     int step_two, float prev_input_power, uint64_t& launched)
 {
     b200_acq::Bluestein* b = a->bl.get();
@@ -285,12 +285,12 @@ int bluestein_search(b200_acq* a, const float2* in_dev, const uint32_t* slots, u
     const int ne = static_cast<int>(c.effective_fft_size);
     const int off = c.bit_transition_flag ? ne : 0;
     // X_d = DFT_N(x . wipe_d) for every Doppler bin, once per sweep (x: the consumed samples, zero-padded to N)
-    int rc = bluestein_forward_rows(a, in_dev, 0, static_cast<int>(c.consumed_samples), mult, n, bins, b->Xs, launched);
+    int rc = bluestein_forward_rows(a, in, 0, static_cast<int>(c.consumed_samples), mult, n, bins, b->Xs, launched);
     if (rc) return rc;
     for (uint32_t i = 0; i < n_slots; i++)
         {
             // rows of this PRN: y = IDFT_N(X_d . C) = w . IFFT_M(FFT_M(pad(X_d . C . w)) . FFT_M(conj h)) / M ; |w| = 1
-            rc = acq_launch_fwd_rows(b->Xs, n, n, b->CW + static_cast<size_t>(slots[i]) * n, 0, b->A, bins, b->plM, b->twM, launched, a->stream);
+            rc = acq_launch_fwd_rows(AcqInput::linear(b->Xs), n, n, b->CW + static_cast<size_t>(slots[i]) * n, 0, b->A, bins, b->plM, b->twM, launched, a->stream);
             if (rc) return rc;
             // the correlation kernel addresses the grid by code-slot id, and the "code" here is filter slot 1; the grid rows are
             // [off, off + ne) of y, so slot s lands where the mixed-radix search puts it: (s * bins + bin) * ne
@@ -426,7 +426,7 @@ extern "C"
                 B200_CUDA_TRY(cudaMemcpyAsync(a->code_stage + place, code_host, sizeof(float2) * need, cudaMemcpyHostToDevice, a->stream));
                 // CW = conj(DFT_N(code)) . w / M  (volk_32fc_conjugate_32fc of set_local_code :250, then the inverse chirp-z pre-multiplier)
                 uint64_t setup_launches = 0;  // set-up, not counted
-                int rcb = bluestein_forward_rows(a, a->code_stage, 0, n, b->chirp_conj, 0, 1, b->Xs, setup_launches);
+                int rcb = bluestein_forward_rows(a, AcqInput::linear(a->code_stage), 0, n, b->chirp_conj, 0, 1, b->Xs, setup_launches);
                 if (rcb) return rcb;
                 rcb = acq_launch_rows_times_vector(b->Xs, n, b->chirp_M, n, 1, b->CW + static_cast<size_t>(slot) * n, n, 1, a->stream);
                 if (rcb) return rcb;
@@ -462,27 +462,37 @@ extern "C"
         return B200_OK;
     }
 
-    int b200_acq_search_submit(b200_acq* a, const b200_cf32* in_host, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter)
+    // B200_ERR_STATE while a submitted search still has results to collect
+    static int check_no_search_in_flight(const b200_acq* a)
     {
-        if (!a || !in_host) return B200_ERR_ARG;
-        if (a->pending)
-            {
-                set_error("a search is already in flight on this acquisition object: call b200_acq_search_wait");
-                return B200_ERR_STATE;
-            }
-        B200_ENTER_DEVICE(a->e->device);
-        if (!a->in_pin) B200_CUDA_TRY(a->in_pin.alloc(a->c.fft_size));
+        if (!a->pending) return B200_OK;
+        set_error("a search is already in flight on this acquisition object: call b200_acq_search_wait");
+        return B200_ERR_STATE;
+    }
+
+    // after a search queued on a->stream: its n_slots records follow into results_pin, for b200_acq_search_wait
+    static int queue_results(b200_acq* a, uint32_t n_slots)
+    {
         if (!a->done) B200_CUDA_TRY(a->done.create(cudaEventDisableTiming));
-        // the caller's buffer is free as soon as this returns: stage it in pinned memory so that the copy is truly asynchronous
-        std::memcpy(a->in_pin, in_host, sizeof(float2) * a->c.consumed_samples);
-        B200_CUDA_TRY(cudaMemcpyAsync(a->in_dev, a->in_pin, sizeof(float2) * a->c.consumed_samples, cudaMemcpyHostToDevice, a->stream));
-        int rc = search_impl(a, a->in_dev, slots, n_slots, dwell_counter, a->results_dev);
-        if (rc) return rc;
         B200_CUDA_TRY(cudaMemcpyAsync(a->results_pin, a->results_dev, sizeof(b200_acq_result) * n_slots, cudaMemcpyDeviceToHost, a->stream));
         B200_CUDA_TRY(cudaEventRecord(a->done, a->stream));
         a->pending = true;
         a->pending_slots = n_slots;
         return B200_OK;
+    }
+
+    int b200_acq_search_submit(b200_acq* a, const b200_cf32* in_host, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter)
+    {
+        if (!a || !in_host) return B200_ERR_ARG;
+        if (const int rc = check_no_search_in_flight(a)) return rc;
+        B200_ENTER_DEVICE(a->e->device);
+        if (!a->in_pin) B200_CUDA_TRY(a->in_pin.alloc(a->c.fft_size));
+        // the caller's buffer is free as soon as this returns: stage it in pinned memory so that the copy is truly asynchronous
+        std::memcpy(a->in_pin, in_host, sizeof(float2) * a->c.consumed_samples);
+        B200_CUDA_TRY(cudaMemcpyAsync(a->in_dev, a->in_pin, sizeof(float2) * a->c.consumed_samples, cudaMemcpyHostToDevice, a->stream));
+        const int rc = search_impl(a, AcqInput::linear(a->in_dev), slots, n_slots, dwell_counter, a->results_dev);
+        if (rc) return rc;
+        return queue_results(a, n_slots);
     }
 
     int b200_acq_search_wait(b200_acq* a, b200_acq_result* results_host)
@@ -528,11 +538,11 @@ extern "C"
         return rc;
     }
 
-    // search the samples in a->in_dev, then bring the n_slots result records back to the host
-    static int search_to_host(b200_acq* a, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, int step_two, float prev_input_power,
-        b200_acq_result* results_host)
+    // search the samples `in`, then bring the n_slots result records back to the host
+    static int search_to_host(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, int step_two,
+        float prev_input_power, b200_acq_result* results_host)
     {
-        const int rc = search_impl(a, a->in_dev, slots, n_slots, dwell_counter, a->results_dev, step_two, prev_input_power);
+        const int rc = search_impl(a, in, slots, n_slots, dwell_counter, a->results_dev, step_two, prev_input_power);
         if (rc) return rc;
         B200_CUDA_TRY(cudaMemcpyAsync(a->results_pin, a->results_dev, sizeof(b200_acq_result) * n_slots, cudaMemcpyDeviceToHost, a->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
@@ -544,15 +554,11 @@ extern "C"
         b200_acq_result* results_host)
     {
         if (!a || !in_host_iq || !results_host) return B200_ERR_ARG;
-        if (a->pending)
-            {
-                set_error("a search is already in flight on this acquisition object: call b200_acq_search_wait");
-                return B200_ERR_STATE;
-            }
+        if (const int rc = check_no_search_in_flight(a)) return rc;
         B200_ENTER_DEVICE(a->e->device);
         const int rc = upload_i16(a, in_host_iq);
         if (rc) return rc;
-        return search_to_host(a, slots, n_slots, dwell_counter, 0, 0.f, results_host);
+        return search_to_host(a, AcqInput::linear(a->in_dev), slots, n_slots, dwell_counter, 0, 0.f, results_host);
     }
 
     int b200_acq_search_step_two_i16(b200_acq* a, const int16_t* in_host_iq, uint32_t slot, uint32_t dwell_counter, float prev_input_power,
@@ -562,7 +568,7 @@ extern "C"
         B200_ENTER_DEVICE(a->e->device);
         const int rc = upload_i16(a, in_host_iq);
         if (rc) return rc;
-        return search_to_host(a, &slot, 1, dwell_counter, 1, prev_input_power, result_host);
+        return search_to_host(a, AcqInput::linear(a->in_dev), &slot, 1, dwell_counter, 1, prev_input_power, result_host);
     }
 
     int b200_acq_set_step_two(b200_acq* a, float doppler_center_step_two, float doppler_step2, uint32_t num_doppler_bins_step2)
@@ -607,7 +613,7 @@ extern "C"
         if (!a || !in_host || !result_host) return B200_ERR_ARG;
         B200_ENTER_DEVICE(a->e->device);
         B200_CUDA_TRY(cudaMemcpyAsync(a->in_dev, in_host, sizeof(float2) * a->c.consumed_samples, cudaMemcpyHostToDevice, a->stream));
-        return search_to_host(a, &slot, 1, dwell_counter, 1, prev_input_power, result_host);
+        return search_to_host(a, AcqInput::linear(a->in_dev), &slot, 1, dwell_counter, 1, prev_input_power, result_host);
     }
 
     int b200_acq_search_dev(b200_acq* a, const b200_cf32* in_dev, const uint32_t* slots_host, uint32_t n_slots,
@@ -617,7 +623,74 @@ extern "C"
         B200_ENTER_DEVICE(a->e->device);
         // (search_impl synchronises by itself when - and only when - the slot list changed and slot_pin must be rewritten; a
         // repeated sweep over the same slots issues no host synchronisation and can be captured in a CUDA graph)
-        return search_impl(a, reinterpret_cast<const float2*>(in_dev), slots_host, n_slots, dwell_counter, results_dev);
+        return search_impl(a, AcqInput::linear(reinterpret_cast<const float2*>(in_dev)), slots_host, n_slots, dwell_counter, results_dev);
+    }
+
+    // The view of samples [abs_index, abs_index + consumed_samples) of one of the engine's bands, with a->stream made to wait
+    // for every write to the band queued so far.  The window check and the waits share one critical section of e->mu, so no
+    // push can be queued between them.  Float pushes and refills are copies on the copy stream (copy_done marks the latest);
+    // integer pushes are converted on the compute stream, and raw_free[raw_last] follows the band's latest conversion.  The
+    // search waits for those two events only, not for the whole compute stream, so it never queues behind tracking batches.
+    static int band_input(b200_acq* a, int band, uint64_t abs_index, AcqInput* in)
+    {
+        if (band < 0 || band >= kMaxBands) return B200_ERR_ARG;
+        b200_engine* e = a->e;
+        const unsigned long long n = a->c.consumed_samples;
+        std::lock_guard<std::mutex> lk(e->mu);
+        const Band& b = e->bands[band];
+        if (!b.in_use)
+            {
+                set_error("band %d holds no samples (call b200_iq_create or b200_iq_attach_dev)", band);
+                return B200_ERR_STATE;
+            }
+        if (!b.holds(abs_index, n))
+            {
+                set_error("band %d: samples [%llu, %llu) are outside the band's window [%llu, %llu)", band, (unsigned long long)abs_index,
+                    (unsigned long long)abs_index + n, b.window_lo(), b.write_index);
+                return B200_ERR_RANGE;
+            }
+        B200_CUDA_TRY(cudaStreamWaitEvent(a->stream, e->copy_done, 0));
+        if (b.raw_last >= 0) B200_CUDA_TRY(cudaStreamWaitEvent(a->stream, b.raw_free[b.raw_last], 0));
+        // a ring window may wrap around the ring's end; an attached buffer is linear from first_index (mask ~0), and the
+        // window check keeps the window inside it
+        const unsigned long long off = (abs_index - b.first_index) & b.mask;
+        const unsigned long long run = b.capacity - off;
+        *in = AcqInput{b.base + off, static_cast<int>(n < run ? n : run), b.base};
+        return B200_OK;
+    }
+
+    int b200_acq_search_band_submit(b200_acq* a, int band, uint64_t abs_index, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter)
+    {
+        if (!a) return B200_ERR_ARG;
+        if (const int rc = check_no_search_in_flight(a)) return rc;
+        B200_ENTER_DEVICE(a->e->device);
+        AcqInput in{};
+        int rc = band_input(a, band, abs_index, &in);
+        if (rc) return rc;
+        rc = search_impl(a, in, slots, n_slots, dwell_counter, a->results_dev);
+        if (rc) return rc;
+        return queue_results(a, n_slots);
+    }
+
+    int b200_acq_search_band(b200_acq* a, int band, uint64_t abs_index, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
+        b200_acq_result* results_host)
+    {
+        if (!a || !results_host) return B200_ERR_ARG;
+        const int rc = b200_acq_search_band_submit(a, band, abs_index, slots, n_slots, dwell_counter);
+        if (rc) return rc;
+        return b200_acq_search_wait(a, results_host);
+    }
+
+    int b200_acq_search_step_two_band(b200_acq* a, int band, uint64_t abs_index, uint32_t slot, uint32_t dwell_counter, float prev_input_power,
+        b200_acq_result* result_host)
+    {
+        if (!a || !result_host) return B200_ERR_ARG;
+        if (const int rc = check_no_search_in_flight(a)) return rc;
+        B200_ENTER_DEVICE(a->e->device);
+        AcqInput in{};
+        const int rc = band_input(a, band, abs_index, &in);
+        if (rc) return rc;
+        return search_to_host(a, in, &slot, 1, dwell_counter, 1, prev_input_power, result_host);
     }
 
     int b200_acq_sweep_best_dev(b200_acq* a, const b200_acq_result* results_dev, const uint32_t* prn_of_result_dev, uint32_t n_results,
@@ -644,7 +717,7 @@ extern "C"
         const size_t n = a->c.fft_size;
         B200_CUDA_TRY(cudaMemcpyAsync(a->code_stage, in_host, sizeof(float2) * n, cudaMemcpyHostToDevice, a->stream));
         uint64_t selftest_launches = 0;  // a self-test, not a search: not counted
-        const int rc = bluestein_forward_rows(a, a->code_stage, 0, static_cast<int>(n), a->bl->chirp_conj, 0, 1, a->bl->Xs, selftest_launches);
+        const int rc = bluestein_forward_rows(a, AcqInput::linear(a->code_stage), 0, static_cast<int>(n), a->bl->chirp_conj, 0, 1, a->bl->Xs, selftest_launches);
         if (rc) return rc;
         B200_CUDA_TRY(cudaMemcpyAsync(out_host, a->bl->Xs, sizeof(float2) * n, cudaMemcpyDeviceToHost, a->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(a->stream));

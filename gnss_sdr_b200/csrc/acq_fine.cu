@@ -189,7 +189,7 @@ extern "C"
         B200_CUDA_TRY(cudaGetLastError());
         uint64_t launched = 1;  // acq_fine_modulate_kernel
         // volk_32fc_x2_multiply_32fc (:347) fused into the transform's load, then the 8 M-point FFTs
-        int rc = acq_launch_fwd(f->in_dev, f->m, f->rows, f->X, kZeroPadding, f->plan, f->tw, launched, f->stream);
+        int rc = acq_launch_fwd(AcqInput::linear(f->in_dev), f->m, f->rows, f->X, kZeroPadding, f->plan, f->tw, launched, f->stream);
         if (rc) return rc;
         acq_fine_argmax_kernel<<<1, kArgmaxThreads, 0, f->stream>>>(f->X, f->plan, f->best_dev);
         B200_CUDA_TRY(cudaGetLastError());

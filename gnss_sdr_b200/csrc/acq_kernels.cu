@@ -146,7 +146,7 @@ __global__ void __launch_bounds__(THREADS, 1) acq_code_fft_kernel(const float2* 
 
 // ---- forward: wipe-off + FFT, one CTA per Doppler bin ------------------------------------------------
 template <int THREADS>
-__global__ void __launch_bounds__(THREADS, 1) acq_fwd_kernel(const float2* __restrict__ in, int consumed,
+__global__ void __launch_bounds__(THREADS, 1) acq_fwd_kernel(AcqInput in, int consumed,
     const float2* __restrict__ wipe, float2* __restrict__ X, FftPlan pl, const float2* __restrict__ tw)
 {
     extern __shared__ __align__(16) float2 s[];
@@ -157,7 +157,7 @@ __global__ void __launch_bounds__(THREADS, 1) acq_fwd_kernel(const float2* __res
     for (int i = threadIdx.x; i < n; i += blockDim.x)
         {
             // acquisition_core zero-pads beyond consumed samples (:657-664); volk_32fc_x2_multiply_32fc (:531)
-            s[i] = (i < consumed) ? cmul_rn(in[i], w[i]) : make_float2(0.f, 0.f);
+            s[i] = (i < consumed) ? cmul_rn(in(i), w[i]) : make_float2(0.f, 0.f);
         }
     fft_forward_to_global<false, THREADS == kAcqThreads25>(s, pl, tw, X + static_cast<size_t>(d) * n);
 }
@@ -287,18 +287,19 @@ __global__ void __launch_bounds__(THREADS, 1) acq_corr_kernel(const float2* __re
 // Forward: one radix-n1 DIF stage through global memory (block length n_total, sub-length n), then the
 // in-shared-memory plan on each of the n1 blocks.  Inverse: the blocks first, then the radix-n1 DIT stage,
 // whose natural-order outputs feed the statistics directly.  Layout stays "digit reversed" end to end.
-__device__ __forceinline__ float2 acq_source(const float2* __restrict__ in, const float2* __restrict__ wipe, int i, int consumed,
+__device__ __forceinline__ float2 acq_source(const AcqInput& in, const float2* __restrict__ wipe, int i, int consumed,
     int layout, int n_total)
 {
     // wipe != nullptr: signal * wipe-off, zero-padded beyond consumed (acquisition_core :657-664, :531)
-    // wipe == nullptr: local code placed by `layout`
-    if (wipe != nullptr) return (i < consumed) ? cmul_rn(in[i], wipe[i]) : make_float2(0.f, 0.f);
-    return acq_code_sample(in, i, n_total, consumed, layout);
+    // wipe == nullptr: local code placed by `layout`, from the linear buffer in.a
+    if (wipe != nullptr) return (i < consumed) ? cmul_rn(in(i), wipe[i]) : make_float2(0.f, 0.f);
+    return acq_code_sample(in.a, i, n_total, consumed, layout);
 }
 
-// in_stride / wipe_stride: elements between the inputs / multiplier tables of consecutive rows (0 = one shared by all rows)
+// in_stride / wipe_stride: elements between the inputs / multiplier tables of consecutive rows (0 = one shared by all rows;
+// in_stride > 0 only with a linear input)
 template <int R>
-__global__ void acq_global_fwd_stage(const float2* __restrict__ in, int consumed, int layout, const float2* __restrict__ wipe,
+__global__ void acq_global_fwd_stage(AcqInput in, int consumed, int layout, const float2* __restrict__ wipe,
     float2* __restrict__ X, FftPlan pl, const float2* __restrict__ tw, size_t in_stride, size_t wipe_stride)
 {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -306,7 +307,7 @@ __global__ void acq_global_fwd_stage(const float2* __restrict__ in, int consumed
     if (j >= n2) return;
     const int d = blockIdx.y;
     const float2* w = wipe ? wipe + static_cast<size_t>(d) * wipe_stride : nullptr;
-    in += static_cast<size_t>(d) * in_stride;
+    in.a += static_cast<size_t>(d) * in_stride;
     float2 v[R];
 #pragma unroll
     for (int q = 0; q < R; q++) v[q] = acq_source(in, w, j + q * n2, consumed, layout, pl.n_total);
@@ -796,7 +797,7 @@ int acq_launch_code_fft(const float2* code, int consumed, int layout, float2* ou
     else
         {
             const dim3 g((pl.n + 255) / 256, 1);
-            rc = dispatch_radix(pl.n1, [&](auto R) { acq_global_fwd_stage<decltype(R)::value><<<g, 256, 0, st>>>(code, consumed, layout, nullptr, out, pl, tw, 0, 0); });
+            rc = dispatch_radix(pl.n1, [&](auto R) { acq_global_fwd_stage<decltype(R)::value><<<g, 256, 0, st>>>(AcqInput::linear(code), consumed, layout, nullptr, out, pl, tw, 0, 0); });
             if (rc) return rc;
             acq_block_fft_kernel<<<dim3(pl.n1, 1), kAcqThreads, pl.n * sizeof(float2), st>>>(out, pl, tw, 1);
         }
@@ -804,7 +805,7 @@ int acq_launch_code_fft(const float2* code, int consumed, int layout, float2* ou
     return B200_OK;
 }
 
-int acq_launch_fwd(const float2* in, int consumed, const float2* wipe, float2* X, int bins, const FftPlan& pl, const float2* tw,
+int acq_launch_fwd(AcqInput in, int consumed, const float2* wipe, float2* X, int bins, const FftPlan& pl, const float2* tw,
     uint64_t& launched, cudaStream_t st)
 {
     int rc = set_attrs();
@@ -905,8 +906,8 @@ int acq_launch_sweep_best(const b200_acq_result* results, const unsigned int* pr
 }
 
 // ---- Bluestein building blocks (acq_engine.cu composes them) --------------------------------------------------------
-// X[r] = FFT_M( pad( in[r * in_stride + i] * mult[r * mult_stride + i], i < consumed ) ), rows r < rows (two-level plan)
-int acq_launch_fwd_rows(const float2* in, size_t in_stride, int consumed, const float2* mult, size_t mult_stride, float2* X, int rows,
+// X[r] = FFT_M( pad( in(r * in_stride + i) * mult[r * mult_stride + i], i < consumed ) ), rows r < rows (two-level plan)
+int acq_launch_fwd_rows(AcqInput in, size_t in_stride, int consumed, const float2* mult, size_t mult_stride, float2* X, int rows,
     const FftPlan& pl, const float2* tw, uint64_t& launched, cudaStream_t st)
 {
     int rc = set_attrs();

@@ -70,6 +70,17 @@ struct BandDesc
     unsigned long long limit;  // samples addressable from base (ring capacity or attached length)
 };
 
+// The samples an acquisition forward stage reads: x(i) = a[i] for i < na, b[i - na] from there on.  A window of a band is at
+// most two linear runs (it may wrap around the ring's end); a linear buffer is one run, with na past every index.
+struct AcqInput
+{
+    const float2* a;
+    int na;
+    const float2* b;
+    static AcqInput linear(const float2* p) { return AcqInput{p, 0x7fffffff, nullptr}; }
+    __device__ __forceinline__ float2 operator()(int i) const { return __ldg(i < na ? a + i : b + (i - na)); }
+};
+
 // One tracking channel registration: code table (device), its length, taps and shifts.
 struct ChanDesc
 {
@@ -209,7 +220,7 @@ int acq_launch_twiddles(float2* tw, const FftPlan& pl, cudaStream_t st);
 int acq_launch_wipeoff(float2* wipe, int n, int bins, int doppler_max, int doppler_center, int doppler_step,
     int doppler_bias, long long fs_in, int step_two, float center2, float step2, cudaStream_t st);
 int acq_launch_code_fft(const float2* code, int consumed, int layout, float2* out, const FftPlan& pl, const float2* tw, cudaStream_t st);
-int acq_launch_fwd(const float2* in, int consumed, const float2* wipe, float2* X, int bins, const FftPlan& pl, const float2* tw,
+int acq_launch_fwd(AcqInput in, int consumed, const float2* wipe, float2* X, int bins, const FftPlan& pl, const float2* tw,
     uint64_t& launched, cudaStream_t st);
 // rowstat[slot_pos * bins + bin] for every (slot, bin) row over [off, off + ne) of the correlation; grid != nullptr: each row's
 // |y|^2 is stored there (accumulate: added to what is there)
@@ -225,7 +236,8 @@ int acq_launch_stats(const AcqRowStat* rowstat, int n_slots, int bins, int ne, i
     int doppler_step, unsigned int dwell_counter, int use_cfar, AcqBest* best, b200_acq_result* results, int step_two, float center2,
     float step2, float prev_input_power, uint64_t& launched, cudaStream_t st);
 int acq_launch_finish_second_peak(const float* second_peak, int n_slots, b200_acq_result* results, uint64_t& launched, cudaStream_t st);
-int acq_launch_fwd_rows(const float2* in, size_t in_stride, int consumed, const float2* mult, size_t mult_stride, float2* X, int rows,
+// in_stride > 0 (rows of one linear buffer) needs a linear view
+int acq_launch_fwd_rows(AcqInput in, size_t in_stride, int consumed, const float2* mult, size_t mult_stride, float2* X, int rows,
     const FftPlan& pl, const float2* tw, uint64_t& launched, cudaStream_t st);
 int acq_launch_inverse_store_rows(const float2* X, const float2* filt, const int* one_slot_dev, int rows, const FftPlan& pl, const float2* tw,
     float2* Z, const float2* post, int n_out, float2* out, size_t out_stride, uint64_t& launched, cudaStream_t st);

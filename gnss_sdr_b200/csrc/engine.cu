@@ -296,6 +296,7 @@ extern "C"
                 if (rc) return rc;
                 e->launches++;
                 B200_CUDA_TRY(cudaEventRecord(b.raw_free[k], e->stream));
+                b.raw_last = k;
             }
         b.write_index += n;
         return B200_OK;
@@ -314,7 +315,7 @@ extern "C"
             Band& b = e->bands[band];
             if (const int rc = b.check_owned_ring(band)) return rc;
             // what the ring holds right now
-            const unsigned long long lo = std::max(b.valid_from, b.oldest());
+            const unsigned long long lo = b.window_lo();
             if (abs_index >= lo && abs_index + n <= b.write_index) return B200_OK;  // every sample of this block is already in the band
             if (abs_index > b.write_index || abs_index < lo)
                 {
@@ -348,7 +349,7 @@ extern "C"
         std::lock_guard<std::mutex> lk(e->mu);
         const Band& b = e->bands[band];
         if (!b.in_use) return B200_ERR_STATE;
-        if (valid_from) *valid_from = std::max(b.valid_from, b.oldest());
+        if (valid_from) *valid_from = b.window_lo();
         if (write_index) *write_index = b.write_index;
         return B200_OK;
     }
@@ -651,11 +652,11 @@ extern "C"
                 const Band& b = e->bands[e->chans[ch].desc.band];
                 if (b.in_use && !b.attached && items_host[i].n > 0)
                     {
-                        const unsigned long long s0 = items_host[i].sample_index, s1 = s0 + static_cast<unsigned long long>(items_host[i].n);
-                        const unsigned long long lo = std::max(b.valid_from, b.oldest());
-                        if (s0 < lo || s1 > b.write_index)
+                        const unsigned long long s0 = items_host[i].sample_index, n = static_cast<unsigned long long>(items_host[i].n);
+                        if (!b.holds(s0, n))
                             {
-                                set_error("item %d: samples [%llu, %llu) are outside the band's window [%llu, %llu)", i, s0, s1, lo, b.write_index);
+                                set_error("item %d: samples [%llu, %llu) are outside the band's window [%llu, %llu)", i, s0, s0 + n, b.window_lo(),
+                                    b.write_index);
                                 return B200_ERR_RANGE;
                             }
                     }

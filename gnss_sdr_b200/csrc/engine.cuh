@@ -5,6 +5,7 @@
 #include "cuda_owned.cuh"
 #include "loop.cuh"
 
+#include <algorithm>
 #include <mutex>
 #include <vector>
 
@@ -28,6 +29,7 @@ struct Band
     DevBuf<unsigned char> raw_stage[2];
     CudaEvent raw_free[2];  // conversion that read the buffer has finished
     int raw_next{0};
+    int raw_last{-1};       // raw_free[raw_last] is recorded right after the band's latest conversion (-1: none yet)
 
     // B200_OK, or B200_ERR_STATE with the error text when this is not a ring made by b200_iq_create
     int check_owned_ring(int band) const
@@ -38,6 +40,10 @@ struct Band
     }
     // oldest absolute index still held: an owned ring (first_index 0) keeps the last `capacity` samples pushed
     unsigned long long oldest() const { return (!attached && write_index > capacity) ? write_index - capacity : first_index; }
+    // the band's readable window is [window_lo(), write_index) (what b200_iq_window reports)
+    unsigned long long window_lo() const { return std::max(valid_from, oldest()); }
+    // samples [s0, s0 + n) all lie inside that window; the test cannot wrap around 2^64
+    bool holds(unsigned long long s0, unsigned long long n) const { return s0 >= window_lo() && s0 <= write_index && n <= write_index - s0; }
 };
 
 struct Channel

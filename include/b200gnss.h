@@ -83,7 +83,8 @@ extern "C"
      * rest is already there.  abs_index beyond the write index opens a gap: the band restarts there
      * (b200_iq_window reports the new oldest valid sample).  Thread-safe. */
     int b200_iq_push_at(b200_engine* e, int band, uint64_t abs_index, const b200_cf32* host, uint64_t n, uint64_t* n_new);
-    /* [valid_from, write_index): absolute indices of the samples a work item may address right now */
+    /* [valid_from, write_index): absolute indices of the samples a work item or a band search (b200_acq_search_band) may
+     * address right now */
     int b200_iq_window(b200_engine* e, int band, uint64_t* valid_from, uint64_t* write_index);
     /* Declare what the band holds stale (the window becomes empty; the write index stays).  For hosts that start a new
      * stream whose indices overlap the previous one's (a flowgraph restarted inside one process): without this,
@@ -418,6 +419,33 @@ extern "C"
     /* same with the input already on the device and results left on the device (asynchronous) */
     int b200_acq_search_dev(b200_acq* a, const b200_cf32* in_dev, const uint32_t* slots_host, uint32_t n_slots,
         uint32_t dwell_counter, b200_acq_result* results_dev);
+    /* Search straight from a band of the acquisition object's engine: the input is samples [abs_index, abs_index +
+     * consumed_samples) of `band`, the buffer the reference's block copies its d_consumed_samples from
+     * (pcps_acquisition.cc:790-815).  The same samples a host would otherwise keep a second copy of, in host memory, for
+     * b200_acq_search; the forward stage reads them where they lie in the ring (a window may wrap around the ring's end),
+     * with no extra copy or launch, so a band search issues exactly the kernels b200_acq_search_dev does and computes
+     * bit for bit what b200_acq_search computes on the same samples.
+     *  - The window must lie inside [valid_from, write_index) as b200_iq_window reports it (the rule b200_trk_submit
+     *    applies to work items); attached bands are linear from their first_index.  Otherwise B200_ERR_RANGE, with the
+     *    window and the band's window in b200_last_error(), and nothing is launched.  An unused band is B200_ERR_STATE.
+     *  - The search is ordered after every b200_iq_push* / b200_iq_refill of the band made before the call, without a host
+     *    synchronisation and without waiting for tracking work queued on the engine.
+     *  - A later push that laps the ring over a window still queued for a search overwrites what it reads: sizing the
+     *    ring so that this cannot happen is the caller's responsibility, as for tracking.
+     *  - Successive dwells and step two take the following windows (abs_index + k * consumed_samples), as the block's
+     *    successive input buffers.
+     *  - The result's sample stamp (Acq_samplestamp_samples, :594) for b200_trk_loop_start is abs_index + consumed_samples.
+     *  - The window is resolved when the call is made: these calls are not meant for CUDA-graph capture (that is what
+     *    b200_acq_search_dev is for).
+     * b200_acq_search_band replaces b200_acq_search (synchronous); b200_acq_search_band_submit replaces
+     * b200_acq_search_submit (results through b200_acq_search_wait, one search in flight per object);
+     * b200_acq_search_step_two_band replaces b200_acq_search_step_two. */
+    int b200_acq_search_band(b200_acq* a, int band, uint64_t abs_index, const uint32_t* slots, uint32_t n_slots,
+        uint32_t dwell_counter, b200_acq_result* results_host);
+    int b200_acq_search_band_submit(b200_acq* a, int band, uint64_t abs_index, const uint32_t* slots, uint32_t n_slots,
+        uint32_t dwell_counter);
+    int b200_acq_search_step_two_band(b200_acq* a, int band, uint64_t abs_index, uint32_t slot, uint32_t dwell_counter,
+        float prev_input_power, b200_acq_result* result_host);
     /* Multi-GPU cold start (SURVEY 8e): the PRN x Doppler grid is sharded by PRN; each rank reduces its sweep to ONE
      * 16-byte record on the device and the ranks exchange the records (an all-gather of N x 16 bytes over NVLink; the
      * host or a peer then takes the best, ties to the lowest PRN / bin / code phase as the reference's strict '>' scans).
