@@ -146,7 +146,6 @@ int search_impl(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slot
     const int rc = a->bl ? bluestein_search(a, in, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power, launched)
                          : mixed_radix_search(a, in, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power, launched);
     if (rc) return rc;
-    std::lock_guard<std::mutex> lk(a->e->mu);
     a->e->launches += launched;
     return B200_OK;
 }
@@ -530,11 +529,7 @@ extern "C"
         std::memcpy(a->in_pin, in_host_iq, sizeof(int16_t) * 2 * n);
         B200_CUDA_TRY(cudaMemcpyAsync(a->raw_dev, a->in_pin, sizeof(int16_t) * 2 * n, cudaMemcpyHostToDevice, a->stream));
         const int rc = launch_convert_i16(a->raw_dev, a->in_dev, ~0ULL, 0ULL, n, a->stream);
-        if (rc == B200_OK)
-            {
-                std::lock_guard<std::mutex> lk(a->e->mu);
-                a->e->launches++;
-            }
+        if (rc == B200_OK) a->e->launches++;
         return rc;
     }
 
@@ -700,7 +695,6 @@ extern "C"
         uint64_t launched = 0;
         const int rc = acq_launch_sweep_best(results_dev, prn_of_result_dev, static_cast<int>(n_results), peak_dev, launched, a->stream);
         if (rc) return rc;
-        std::lock_guard<std::mutex> lk(a->e->mu);
         a->e->launches += launched;
         return B200_OK;
     }

@@ -196,7 +196,7 @@ extern "C"
         launched += 1;
         B200_CUDA_TRY(cudaMemcpyAsync(f->best_pin, f->best_dev, sizeof(FineBest), cudaMemcpyDeviceToHost, f->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(f->stream));
-        f->e->launches += launched;  // (under e->mu, held for the whole estimate)
+        f->e->launches += launched;
         *index_freq = f->best_pin->index;
         if (peak) *peak = f->best_pin->peak;
         return B200_OK;

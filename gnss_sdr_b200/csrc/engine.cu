@@ -195,22 +195,28 @@ extern "C"
     int b200_engine_launch_count(b200_engine* e, uint64_t* n)
     {
         if (!e || !n) return B200_ERR_ARG;
-        *n = e->launches;
+        *n = e->launches.load();
         return B200_OK;
     }
 
     // ---- bands -----------------------------------------------------------------------------
+    // caller holds e->mu; before the band is re-created or attached: queued launches may still read its owned ring
+    static int release_owned_ring(b200_engine* e, Band& b)
+    {
+        if (!b.dev) return B200_OK;
+        B200_ENTER_DEVICE(e->device);
+        B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
+        B200_CUDA_TRY(b.dev.reset());
+        return B200_OK;
+    }
+
     int b200_iq_create(b200_engine* e, int band, uint64_t capacity_samples)
     {
         if (!e || band < 0 || band >= kMaxBands || capacity_samples == 0) return B200_ERR_ARG;
         std::lock_guard<std::mutex> lk(e->mu);
         B200_ENTER_DEVICE(e->device);
         Band& b = e->bands[band];
-        if (b.dev)
-            {
-                B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
-                B200_CUDA_TRY(b.dev.reset());
-            }
+        if (const int rc = release_owned_ring(e, b)) return rc;
         const unsigned long long cap = next_pow2(capacity_samples);
         cudaError_t err = b.dev.alloc(cap);
         if (err != cudaSuccess)
@@ -230,34 +236,36 @@ extern "C"
         return B200_OK;
     }
 
-    int b200_iq_push(b200_engine* e, int band, const b200_cf32* host, uint64_t n, uint64_t* first_index)
+    // n items of item_bytes from host into the slots [off, off + n) of a device ring of cap items (split at its end), on the
+    // copy stream; copy_done marks the copy and the compute stream waits for it, so every later launch sees the samples and a
+    // band search (acq_engine.cu, band_input) can wait for them alone.  n == 0 queues nothing.
+    static int copy_in(b200_engine* e, void* ring, unsigned long long cap, unsigned long long off, const void* host, unsigned long long n,
+        size_t item_bytes)
     {
-        if (!e || band < 0 || band >= kMaxBands || (!host && n)) return B200_ERR_ARG;
-        std::lock_guard<std::mutex> lk(e->mu);
-        Band& b = e->bands[band];
-        if (const int rc = b.check_owned_ring(band)) return rc;
-        if (n > b.capacity)
-            {
-                set_error("push of %llu samples exceeds ring capacity %llu", (unsigned long long)n, b.capacity);
-                return B200_ERR_RANGE;
-            }
-        B200_ENTER_DEVICE(e->device);
-        if (first_index) *first_index = b.write_index;
-        // copies run on the copy stream; later launches on the compute stream wait on copy_done.
-        // (Overwriting samples that an in-flight launch still reads is the caller's ring-sizing
-        // responsibility, exactly as with any circular sample buffer.)
-        const unsigned long long off = b.write_index & b.mask;
-        const unsigned long long first = (n < b.capacity - off) ? n : (b.capacity - off);
-        if (first) B200_CUDA_TRY(cudaMemcpyAsync(b.dev + off, host, first * sizeof(float2), cudaMemcpyHostToDevice, e->copy_stream));
-        if (n > first) B200_CUDA_TRY(cudaMemcpyAsync(b.dev, host + first, (n - first) * sizeof(float2), cudaMemcpyHostToDevice, e->copy_stream));
+        if (n == 0) return B200_OK;
+        char* const dst = static_cast<char*>(ring);
+        const char* const src = static_cast<const char*>(host);
+        const unsigned long long first = std::min(n, cap - off);
+        B200_CUDA_TRY(cudaMemcpyAsync(dst + off * item_bytes, src, first * item_bytes, cudaMemcpyHostToDevice, e->copy_stream));
+        if (n > first) B200_CUDA_TRY(cudaMemcpyAsync(dst, src + first * item_bytes, (n - first) * item_bytes, cudaMemcpyHostToDevice, e->copy_stream));
         B200_CUDA_TRY(cudaEventRecord(e->copy_done, e->copy_stream));
         B200_CUDA_TRY(cudaStreamWaitEvent(e->stream, e->copy_done, 0));
-        b.write_index += n;
         return B200_OK;
     }
 
-    // shared implementation of the integer-sample pushes: raw bytes H2D, then conversion into the ring
-    static int push_raw(b200_engine* e, int band, const void* host, uint64_t n, uint64_t* first_index, int bytes_per_component)
+    // the host sample formats of a band, by bytes per component: b200_cf32, and interleaved (I, Q) int16 / int8 pairs
+    enum SampleFormat
+    {
+        kI8 = 1,
+        kI16 = 2,
+        kCf32 = 4,
+    };
+
+    // The one write path of an owned ring: n host samples of format fmt at the band's write index.  Float samples are copied
+    // into the ring; integers cross PCIe as they are and are converted into the ring on the device.  (Overwriting samples
+    // that an in-flight launch still reads is the caller's ring-sizing responsibility, exactly as with any circular sample
+    // buffer.)
+    static int push_samples(b200_engine* e, int band, const void* host, uint64_t n, SampleFormat fmt, uint64_t* first_index)
     {
         if (!e || band < 0 || band >= kMaxBands || (!host && n)) return B200_ERR_ARG;
         std::lock_guard<std::mutex> lk(e->mu);
@@ -270,29 +278,33 @@ extern "C"
             }
         B200_ENTER_DEVICE(e->device);
         if (first_index) *first_index = b.write_index;
-        const unsigned long long bytes = n * 2ULL * static_cast<unsigned long long>(bytes_per_component);
-        const int k = b.raw_next;
-        b.raw_next ^= 1;
-        if (!b.raw_free[k]) B200_CUDA_TRY(b.raw_free[k].create(cudaEventDisableTiming));
-        if (!b.raw_stage[k].fits(bytes))
+        if (n == 0) return B200_OK;
+        if (fmt == kCf32)
             {
-                B200_CUDA_TRY(cudaStreamSynchronize(e->copy_stream));
-                B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
-                B200_CUDA_TRY(b.raw_stage[k].alloc(bytes + bytes / 4 + 256));
-                B200_CUDA_TRY(cudaEventRecord(b.raw_free[k], e->stream));
+                const int rc = copy_in(e, b.dev, b.capacity, b.write_index & b.mask, host, n, sizeof(float2));
+                if (rc) return rc;
             }
-        if (n)
+        else
             {
                 // raw integers cross PCIe on the copy stream; the conversion into the float ring runs on the compute
                 // stream (ordered before every later correlator launch), so the copy engine goes straight on to the
                 // next block, which lands in the other staging buffer
+                const unsigned long long bytes = n * 2ULL * static_cast<unsigned long long>(fmt);
+                const int k = b.raw_next;
+                b.raw_next ^= 1;
+                if (!b.raw_free[k]) B200_CUDA_TRY(b.raw_free[k].create(cudaEventDisableTiming));
+                if (!b.raw_stage[k].fits(bytes))
+                    {
+                        B200_CUDA_TRY(cudaStreamSynchronize(e->copy_stream));
+                        B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
+                        B200_CUDA_TRY(b.raw_stage[k].alloc(bytes + bytes / 4 + 256));
+                        B200_CUDA_TRY(cudaEventRecord(b.raw_free[k], e->stream));
+                    }
                 B200_CUDA_TRY(cudaStreamWaitEvent(e->copy_stream, b.raw_free[k], 0));
-                B200_CUDA_TRY(cudaMemcpyAsync(b.raw_stage[k], host, bytes, cudaMemcpyHostToDevice, e->copy_stream));
-                B200_CUDA_TRY(cudaEventRecord(e->copy_done, e->copy_stream));
-                B200_CUDA_TRY(cudaStreamWaitEvent(e->stream, e->copy_done, 0));
-                int rc = (bytes_per_component == 2)
-                             ? launch_convert_i16(reinterpret_cast<const short*>(b.raw_stage[k].get()), b.dev, b.mask, b.write_index, n, e->stream)
-                             : launch_convert_i8(reinterpret_cast<const signed char*>(b.raw_stage[k].get()), b.dev, b.mask, b.write_index, n, e->stream);
+                int rc = copy_in(e, b.raw_stage[k], n, 0, host, n, 2 * static_cast<size_t>(fmt));
+                if (rc) return rc;
+                rc = (fmt == kI16) ? launch_convert_i16(reinterpret_cast<const short*>(b.raw_stage[k].get()), b.dev, b.mask, b.write_index, n, e->stream)
+                                   : launch_convert_i8(reinterpret_cast<const signed char*>(b.raw_stage[k].get()), b.dev, b.mask, b.write_index, n, e->stream);
                 if (rc) return rc;
                 e->launches++;
                 B200_CUDA_TRY(cudaEventRecord(b.raw_free[k], e->stream));
@@ -302,12 +314,27 @@ extern "C"
         return B200_OK;
     }
 
+    int b200_iq_push(b200_engine* e, int band, const b200_cf32* host, uint64_t n, uint64_t* first_index)
+    {
+        return push_samples(e, band, host, n, kCf32, first_index);
+    }
+
+    int b200_iq_push_i16(b200_engine* e, int band, const int16_t* host_iq, uint64_t n, uint64_t* first_index)
+    {
+        return push_samples(e, band, host_iq, n, kI16, first_index);
+    }
+
+    int b200_iq_push_i8(b200_engine* e, int band, const int8_t* host_iq, uint64_t n, uint64_t* first_index)
+    {
+        return push_samples(e, band, host_iq, n, kI8, first_index);
+    }
+
     int b200_iq_push_at(b200_engine* e, int band, uint64_t abs_index, const b200_cf32* host, uint64_t n, uint64_t* n_new)
     {
         if (!e || band < 0 || band >= kMaxBands || (!host && n)) return B200_ERR_ARG;
         if (n_new) *n_new = 0;
         // competing producers of one band (every tracking block of a flowgraph sees the same stream and offers the same
-        // samples) are serialised here; e->mu itself is only held for the bookkeeping and inside b200_iq_push
+        // samples) are serialised here; e->mu itself is only held for the bookkeeping and inside push_samples
         std::lock_guard<std::mutex> plk(e->push_mu[band]);
         uint64_t skip = 0;
         {
@@ -326,8 +353,7 @@ extern "C"
                 }
             skip = b.write_index - abs_index;
         }
-        uint64_t first = 0;
-        const int rc = b200_iq_push(e, band, host + skip, n - skip, &first);
+        const int rc = push_samples(e, band, host + skip, n - skip, kCf32, nullptr);
         if (rc == B200_OK && n_new) *n_new = n - skip;
         return rc;
     }
@@ -354,28 +380,18 @@ extern "C"
         return B200_OK;
     }
 
-    int b200_iq_push_i16(b200_engine* e, int band, const int16_t* host_iq, uint64_t n, uint64_t* first_index)
-    {
-        return push_raw(e, band, host_iq, n, first_index, 2);
-    }
-
-    int b200_iq_push_i8(b200_engine* e, int band, const int8_t* host_iq, uint64_t n, uint64_t* first_index)
-    {
-        return push_raw(e, band, host_iq, n, first_index, 1);
-    }
-
     int b200_iq_push_file(b200_engine* e, int band, const char* path, const char* item_type, uint64_t header_bytes, uint64_t skip_samples,
         uint64_t max_samples, uint64_t chunk_samples, uint64_t* first_index, uint64_t* samples_pushed)
     {
         if (!e || !path || !item_type || band < 0 || band >= kMaxBands) return B200_ERR_ARG;
         // FileSourceBase::itemTypeToSize (file_source_base.cc:340-378): complex samples as interleaved (I, Q) pairs
-        int bytes_per_component;
+        SampleFormat fmt;
         if (std::strcmp(item_type, "gr_complex") == 0)
-            bytes_per_component = 4;
+            fmt = kCf32;
         else if (std::strcmp(item_type, "ishort") == 0)
-            bytes_per_component = 2;
+            fmt = kI16;
         else if (std::strcmp(item_type, "ibyte") == 0)
-            bytes_per_component = 1;
+            fmt = kI8;
         else
             {
                 set_error("iq_push_file: item type %s is not an interleaved complex type (gr_complex, ishort, ibyte)", item_type);
@@ -397,7 +413,7 @@ extern "C"
                 set_error("iq_push_file: cannot open %s", path);
                 return B200_ERR_STATE;
             }
-        const size_t sample_bytes = 2u * static_cast<size_t>(bytes_per_component);
+        const size_t sample_bytes = 2u * static_cast<size_t>(fmt);
         // samplesToSkip (:385-414): header, then whole samples
         if (std::fseek(f, static_cast<long>(header_bytes + skip_samples * sample_bytes), SEEK_SET) != 0)
             {
@@ -431,12 +447,7 @@ extern "C"
                 const size_t got = std::fread(stage[k], sample_bytes, static_cast<size_t>(want), f);
                 if (got == 0) break;
                 uint64_t first = 0;
-                if (bytes_per_component == 4)
-                    rc = b200_iq_push(e, band, reinterpret_cast<const b200_cf32*>(stage[k].get()), got, &first);
-                else if (bytes_per_component == 2)
-                    rc = b200_iq_push_i16(e, band, reinterpret_cast<const int16_t*>(stage[k].get()), got, &first);
-                else
-                    rc = b200_iq_push_i8(e, band, reinterpret_cast<const int8_t*>(stage[k].get()), got, &first);
+                rc = push_samples(e, band, stage[k], got, fmt, &first);
                 if (rc != B200_OK) break;
                 if (cudaEventRecord(freed[k], e->copy_stream) != cudaSuccess) rc = B200_ERR_CUDA;
                 if (!have_first)
@@ -463,12 +474,7 @@ extern "C"
             }
         std::lock_guard<std::mutex> lk(e->mu);
         Band& b = e->bands[band];
-        if (b.dev)
-            {
-                B200_ENTER_DEVICE(e->device);
-                B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
-                B200_CUDA_TRY(b.dev.reset());
-            }
+        if (const int rc = release_owned_ring(e, b)) return rc;
         b.base = reinterpret_cast<const float2*>(dev);
         b.capacity = n_samples;
         b.mask = ~0ULL;
@@ -497,11 +503,9 @@ extern "C"
                 return B200_ERR_RANGE;
             }
         B200_ENTER_DEVICE(e->device);
-        // same ordering as b200_iq_push: the copy runs on the copy stream, later launches on the compute stream wait for it;
         // overwriting samples an in-flight launch still reads is the caller's double-buffering responsibility
-        if (n) B200_CUDA_TRY(cudaMemcpyAsync(const_cast<float2*>(b.base), host, n * sizeof(float2), cudaMemcpyHostToDevice, e->copy_stream));
-        B200_CUDA_TRY(cudaEventRecord(e->copy_done, e->copy_stream));
-        B200_CUDA_TRY(cudaStreamWaitEvent(e->stream, e->copy_done, 0));
+        const int rc = copy_in(e, const_cast<float2*>(b.base), b.capacity, 0, host, n, sizeof(float2));
+        if (rc) return rc;
         if (b.first_index != first_index)
             {
                 b.first_index = first_index;
@@ -841,6 +845,34 @@ struct b200_trk
     }
 };
 
+namespace
+{
+// a local code table of n elements into buf: the launches that read the old table finish first, buf is reallocated when it
+// must grow, and the copy has landed on return (the caller's buffer may go away)
+template <typename T>
+int load_code(b200_trk* t, DevBuf<T>& buf, const void* host, size_t n)
+{
+    B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
+    if (!buf.fits(n)) B200_CUDA_TRY(buf.alloc(n));
+    B200_CUDA_TRY(cudaMemcpyAsync(buf, host, sizeof(T) * n, cudaMemcpyHostToDevice, t->stream));
+    B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
+    return B200_OK;
+}
+
+// the signal of one correlate call: n samples of sample_bytes from host into dev, queued on t->stream
+int stage_signal(b200_trk* t, void* dev, const void* host, int n, size_t sample_bytes)
+{
+    if (n < 0 || n > t->max_len)
+        {
+            set_error("signal_length_samples %d outside 0..%d", n, t->max_len);
+            return B200_ERR_RANGE;
+        }
+    B200_ENTER_DEVICE(t->e->device);
+    if (n > 0) B200_CUDA_TRY(cudaMemcpyAsync(dev, host, sample_bytes * n, cudaMemcpyHostToDevice, t->stream));
+    return B200_OK;
+}
+}  // namespace
+
 extern "C"
 {
     int b200_trk_create(b200_engine* e, b200_trk** out, int max_signal_length_samples, int n_correlators)
@@ -880,14 +912,8 @@ extern "C"
     {
         if (!t || !local_code_in || !shifts_chips || code_length_chips < 1) return B200_ERR_ARG;
         B200_ENTER_DEVICE(t->e->device);
-        B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
-        if (!t->code_dev.fits(code_length_chips))
-            {
-                t->have_code = false;  // the old table is released here
-                B200_CUDA_TRY(t->code_dev.alloc(code_length_chips));
-            }
-        B200_CUDA_TRY(cudaMemcpyAsync(t->code_dev, local_code_in, sizeof(float) * code_length_chips, cudaMemcpyHostToDevice, t->stream));
-        B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
+        if (!t->code_dev.fits(code_length_chips)) t->have_code = false;  // load_code releases the old table
+        if (const int rc = load_code(t, t->code_dev, local_code_in, code_length_chips)) return rc;
         ChanDesc& c = t->ctl->chan;
         c.code = t->code_dev;
         c.code_len = code_length_chips;
@@ -918,14 +944,8 @@ extern "C"
                 set_error("correlate before set_local_code_and_taps");
                 return B200_ERR_STATE;
             }
-        if (signal_length_samples < 0 || signal_length_samples > t->max_len)
-            {
-                set_error("signal_length_samples %d outside 0..%d", signal_length_samples, t->max_len);
-                return B200_ERR_RANGE;
-            }
-        B200_ENTER_DEVICE(t->e->device);
         const int n = signal_length_samples;
-        if (n > 0) B200_CUDA_TRY(cudaMemcpyAsync(t->sig_dev, sig_in_host, sizeof(float2) * n, cudaMemcpyHostToDevice, t->stream));
+        if (const int rc = stage_signal(t, t->sig_dev, sig_in_host, n, sizeof(float2))) return rc;
         b200_trk::Ctl* c = t->ctl;
         c->chan.high_dyn = t->high_dyn;
         c->band.base = t->sig_dev;
@@ -948,10 +968,7 @@ extern "C"
         int rc = launch_trk_batch(&c->item, 1, &c->chan, &c->band, c->out, B200_MAX_TAPS, slices, t->partial, t->counter,
             c->chan.code_len, 1u << t->taps, t->stream, launched);
         if (rc) return rc;
-        {
-            std::lock_guard<std::mutex> lk(t->e->mu);
-            t->e->launches += launched;
-        }
+        t->e->launches += launched;
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
         for (int k = 0; k < t->taps; k++)
             {
@@ -966,13 +983,10 @@ extern "C"
     {
         if (!t || !local_code_in || !shifts_chips || code_length_chips < 1) return B200_ERR_ARG;
         B200_ENTER_DEVICE(t->e->device);
-        B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
         // the code table last: b200_trk_correlate_cplx takes a code table to mean that the output buffer exists
         if (!t->out_cplx_dev) B200_CUDA_TRY(t->out_cplx_dev.alloc(B200_MAX_TAPS));
-        if (code_length_chips > t->cplx_code_len) B200_CUDA_TRY(t->cplx_code_dev.alloc(code_length_chips));
+        if (const int rc = load_code(t, t->cplx_code_dev, local_code_in, code_length_chips)) return rc;
         t->cplx_code_len = code_length_chips;
-        B200_CUDA_TRY(cudaMemcpyAsync(t->cplx_code_dev, local_code_in, sizeof(float2) * code_length_chips, cudaMemcpyHostToDevice, t->stream));
-        B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
         for (int k = 0; k < t->taps; k++) t->var_shifts[k] = shifts_chips[k];
         return B200_OK;
     }
@@ -987,21 +1001,12 @@ extern "C"
                 return B200_ERR_STATE;
             }
         const int n = signal_length_samples;
-        if (n < 0 || n > t->max_len)
-            {
-                set_error("signal_length_samples %d outside 0..%d", n, t->max_len);
-                return B200_ERR_RANGE;
-            }
-        B200_ENTER_DEVICE(t->e->device);
-        if (n > 0) B200_CUDA_TRY(cudaMemcpyAsync(t->sig_dev, sig_in_host, sizeof(float2) * n, cudaMemcpyHostToDevice, t->stream));
+        if (const int rc = stage_signal(t, t->sig_dev, sig_in_host, n, sizeof(float2))) return rc;
         uint64_t launched = 0;
         const int rc = launch_trk_cplx_code(t->sig_dev, t->cplx_code_dev, n, t->cplx_code_len, t->taps, t->var_shifts, rem_carrier_phase_in_rad,
             phase_step_rad, rem_code_phase_chips, code_phase_step_chips, t->out_cplx_dev, t->stream, launched);
         if (rc) return rc;
-        {
-            std::lock_guard<std::mutex> lk(t->e->mu);
-            t->e->launches += launched;
-        }
+        t->e->launches += launched;
         B200_CUDA_TRY(cudaMemcpyAsync(corr_out_host, t->out_cplx_dev, sizeof(float2) * t->taps, cudaMemcpyDeviceToHost, t->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
         return B200_OK;
@@ -1012,14 +1017,11 @@ extern "C"
     {
         if (!t || !local_code_iq || !shifts_chips || code_length_chips < 1) return B200_ERR_ARG;
         B200_ENTER_DEVICE(t->e->device);
-        B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
         // the code table last: b200_trk_correlate_16sc takes a code table to mean that all three buffers exist
         if (!t->sig16_dev) B200_CUDA_TRY(t->sig16_dev.alloc(2 * (static_cast<size_t>(t->max_len) + 2)));
         if (!t->out16_dev) B200_CUDA_TRY(t->out16_dev.alloc(2 * B200_MAX_TAPS));
-        if (code_length_chips > t->code16_len) B200_CUDA_TRY(t->code16_dev.alloc(2 * code_length_chips));
+        if (const int rc = load_code(t, t->code16_dev, local_code_iq, 2 * static_cast<size_t>(code_length_chips))) return rc;
         t->code16_len = code_length_chips;
-        B200_CUDA_TRY(cudaMemcpyAsync(t->code16_dev, local_code_iq, sizeof(short) * 2 * code_length_chips, cudaMemcpyHostToDevice, t->stream));
-        B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
         for (int k = 0; k < t->taps; k++) t->var_shifts[k] = shifts_chips[k];
         return B200_OK;
     }
@@ -1034,21 +1036,12 @@ extern "C"
                 return B200_ERR_STATE;
             }
         const int n = signal_length_samples;
-        if (n < 0 || n > t->max_len)
-            {
-                set_error("signal_length_samples %d outside 0..%d", n, t->max_len);
-                return B200_ERR_RANGE;
-            }
-        B200_ENTER_DEVICE(t->e->device);
-        if (n > 0) B200_CUDA_TRY(cudaMemcpyAsync(t->sig16_dev, sig_in_iq_host, sizeof(short) * 2 * n, cudaMemcpyHostToDevice, t->stream));
+        if (const int rc = stage_signal(t, t->sig16_dev, sig_in_iq_host, n, 2 * sizeof(short))) return rc;
         uint64_t launched = 0;
         const int rc = launch_trk_16sc(t->sig16_dev, t->code16_dev, n, t->code16_len, t->taps, t->var_shifts, rem_carrier_phase_in_rad, phase_step_rad,
             rem_code_phase_chips, code_phase_step_chips, t->out16_dev, t->stream, launched);
         if (rc) return rc;
-        {
-            std::lock_guard<std::mutex> lk(t->e->mu);
-            t->e->launches += launched;
-        }
+        t->e->launches += launched;
         B200_CUDA_TRY(cudaMemcpyAsync(corr_out_iq_host, t->out16_dev, sizeof(short) * 2 * t->taps, cudaMemcpyDeviceToHost, t->stream));
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));
         return B200_OK;

@@ -6,6 +6,7 @@
 #include "loop.cuh"
 
 #include <algorithm>
+#include <atomic>
 #include <mutex>
 #include <vector>
 
@@ -75,7 +76,7 @@ struct b200_engine
     int shared_mode{-1};   // -1 auto, 0 never, 1 always-when-legal (env B200_TRK_SHARED)
     b200::DevBuf<float2> partial;
     b200::DevBuf<unsigned int> counters;
-    uint64_t launches{0};
+    std::atomic<uint64_t> launches{0};  // kernels issued (b200_engine_launch_count); counted without e->mu
     // asynchronous batches (b200_trk_submit / b200_trk_wait)
     struct Slot
     {

@@ -135,8 +135,9 @@ int ensure_loop_buffers(b200_engine* e, int rec_capacity)
     return B200_OK;
 }
 
-// what the bands hold right now: [valid_from, write_index) of an owned ring, as b200_iq_window, b200_iq_push_at and
-// b200_trk_submit see it (ring slots below valid_from still hold the stream from before a gap, restart or forget)
+// what the bands hold right now: [window_lo, write_index), the window b200_iq_window reports (ring slots below valid_from
+// still hold the stream from before a gap, restart or forget; an attached buffer refilled with fewer samples than it
+// holds still has the previous fill's past write_index)
 LoopAvail snapshot_avail(const b200_engine* e)
 {
     LoopAvail a{};
@@ -144,8 +145,8 @@ LoopAvail snapshot_avail(const b200_engine* e)
         {
             const Band& b = e->bands[i];
             if (!b.in_use) continue;
-            a.lo[i] = b.attached ? b.first_index : std::max(b.valid_from, b.oldest());
-            a.hi[i] = b.attached ? b.first_index + b.capacity : b.write_index;
+            a.lo[i] = b.window_lo();
+            a.hi[i] = b.write_index;
         }
     return a;
 }
