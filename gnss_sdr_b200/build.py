@@ -35,7 +35,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False, ptxas_v: bool = False, extra=(), out: str = None) -> str:
-    """extra: additional nvcc flags (e.g. -DTRK_PREFETCH=2) and out: alternative output path, for A/B variants."""
+    """extra: additional nvcc flags (e.g. -DSH_STAGES=8) and out: alternative output path, for A/B variants."""
     if out:
         force = True
     if not force and not needs_build():

@@ -594,11 +594,6 @@ extern "C"
         if (slices < 1) slices = 1;
         rc = ensure_partials(e, n_items, slices);
         if (rc) return rc;
-        if (e->shared_mode < 0)
-            {
-                const char* env = std::getenv("B200_TRK_SHARED");
-                e->shared_mode = env ? std::atoi(env) : 2;  // 2 = automatic
-            }
         // the shared-window kernel takes batches whose channels all have 1, 3 or 5 taps
         const unsigned int mask = e->taps_mask;
         const bool shared_legal = (mask == (1u << 1) || mask == (1u << 3) || mask == (1u << 5)) && !e->any_high_dyn && slices == 1;
@@ -620,7 +615,7 @@ extern "C"
     {
         if (!e || mode < -1 || mode > 2) return B200_ERR_ARG;
         std::lock_guard<std::mutex> lk(e->mu);
-        e->shared_mode = mode;
+        e->shared_mode = mode < 0 ? 2 : mode;
         return B200_OK;
     }
 

@@ -73,7 +73,7 @@ struct b200_engine
     int max_code_len{0};
     unsigned int taps_mask{0};   // bit t set: some channel with a code table has t taps (a batch runs one launch per tap count)
     bool any_high_dyn{false};
-    int shared_mode{-1};   // -1 auto, 0 never, 1 always-when-legal (env B200_TRK_SHARED)
+    int shared_mode{2};    // shared-window kernel: 2 auto, 0 never, 1 always-when-legal (b200_trk_kernel_choice)
     b200::DevBuf<float2> partial;
     b200::DevBuf<unsigned int> counters;
     std::atomic<uint64_t> launches{0};  // kernels issued (b200_engine_launch_count); counted without e->mu
@@ -107,7 +107,7 @@ struct b200_engine
     std::vector<b200::LoopData> loop_data;      // data channel of each loop (b200_trk_loop_set_data_channel)
     int loop_n_data{0};                         // loops that have one
     b200::DevBuf<b200::LoopData> loop_data_dev;
-    int loop_mode{-1};       // 0 persistent kernel (default), 1 one launch pair per epoch with slices = 1, 2 same with automatic slices
+    int loop_mode{0};        // 0 persistent kernel (default), 1 one launch pair per epoch with slices = 1, 2 same with automatic slices
 
     ~b200_engine()
     {

@@ -360,11 +360,6 @@ extern "C"
                 prompts = e->loop_prm_dev;
             }
         const LoopData* data = loop_data_dev(e);
-        if (e->loop_mode < 0)
-            {
-                const char* env = std::getenv("B200_LOOP_MODE");
-                e->loop_mode = env ? std::atoi(env) : 0;
-            }
         const LoopAvail avail = snapshot_avail(e);
         B200_CUDA_TRY(cudaMemsetAsync(e->loop_nrec_dev, 0, sizeof(int) * n, e->stream));
         uint64_t launched = 0;

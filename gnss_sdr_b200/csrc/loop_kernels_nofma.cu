@@ -17,11 +17,6 @@
 //   lock_detectors.cc:99-147,160-181     exponential_smoother.cc:86-115
 #include <cstdlib>
 #include "loop.cuh"
-// A persistent CTA has the SM to itself (8-16 warps): its tile loop may want more loads in flight than the batch kernel's, which
-// shares the SM with three other CTAs.  B200_LOOP_TILE_UNROLL sets it for this translation unit only (tools/loop_ab.sh).
-#ifdef B200_LOOP_TILE_UNROLL
-#define TRK_TILE_UNROLL_3 B200_LOOP_TILE_UNROLL
-#endif
 #include "trk_item.cuh"
 
 namespace b200
@@ -508,17 +503,10 @@ __global__ void trk_loop_cycle_kernel(LoopDev* loops, int n_loops, int mode, Loo
 // kLoopThreads threads with the batch kernel's per-item templates, slices = 1).  Loops are independent, so there is no
 // grid-wide dependency and no launch per epoch; a CTA ends when its loop has run max_epochs cycles, loses lock, or
 // finds its next vector_length samples not resident (stall).
-// Each channel is a latency chain (epoch k+1's NCO commands need epoch k's taps); the CTA width is a build parameter.  The
-// serial double-precision loop update, not the correlation, dominates the epoch time, and wider CTAs cost residency when
-// many loops run.
-#ifndef B200_LOOP_THREADS
-#define B200_LOOP_THREADS 256
-#endif
-#ifndef B200_LOOP_SERIAL_UPDATE
-#define B200_LOOP_SERIAL_UPDATE 0
-#endif
-constexpr int kLoopThreadsMany = B200_LOOP_THREADS;   // CTA width when loops outnumber the SMs (two CTAs per SM)
-constexpr int kLoopThreadsFew = 512;                  // one loop per SM at most: wider CTAs shorten the correlation
+// Each channel is a latency chain (epoch k+1's NCO commands need epoch k's taps).  The serial double-precision loop update,
+// not the correlation, dominates the epoch time, and wider CTAs cost residency when many loops run.
+constexpr int kLoopThreadsMany = 256;   // CTA width when loops outnumber the SMs (two CTAs per SM)
+constexpr int kLoopThreadsFew = 512;    // one loop per SM at most: wider CTAs shorten the correlation
 
 // The data pass of a loop with a data channel: its own function, not inlined, so that the pilot's code in the persistent
 // kernel stays laid out as without it (inlined, the 1-tap correlation made every epoch of a loop without a data channel about
@@ -543,7 +531,7 @@ __device__ __forceinline__ void copy_words(LoopDev* dst, const LoopDev* src, int
 // data: nullptr when no loop of the launch has a data channel; otherwise the data channel of every loop (-1: none), and the
 // dynamic shared memory holds a second code table of tbl_cap entries for it, right after the pilot's.
 template <int kLoopThreads>
-__global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / kLoopThreads : 1) trk_loop_persistent_kernel(LoopDev* loops, int n_loops, int max_epochs, LoopAvail avail,
+__global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads) trk_loop_persistent_kernel(LoopDev* loops, int n_loops, int max_epochs, LoopAvail avail,
     const ChanDesc* __restrict__ chans, const BandDesc* __restrict__ bands, const LoopData* __restrict__ data, unsigned int* records,
     int rec_capacity, int* n_records, float2* prompts, int tbl_cap)
 {
@@ -583,27 +571,8 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
     bool have_taps = false;
     float2 t[B200_MAX_TAPS];
 
-#ifdef B200_LOOP_PROFILE
-    long long pf[8] = {0, 0, 0, 0, 0, 0, 0, 0}, pc = 0;
-    __shared__ long long s_pf_lock;
-#define PF_MARK(slot)                 \
-    if (tid == 0)                     \
-        {                             \
-            const long long now_ = clock64(); \
-            pf[slot] += now_ - pc;    \
-            pc = now_;                \
-        }
-    if (tid == 0) pc = clock64();
-    if (tid == 32) s_pf_lock = 0;
-#else
-#define PF_MARK(slot)
-#endif
     for (int k = 0; k <= max_epochs; k++)
         {
-            PF_MARK(0)   // correlation of the previous iteration (incl. its barrier)
-#if B200_LOOP_SERIAL_UPDATE
-            if (have_taps && tid == 0) s_lock_ok = -1;   // A/B build: the whole update on thread 0, as before
-#else
             if (have_taps)
                 {
                     // Loop update of epoch k-1 on three warps at once (every thread holds the taps t[]):
@@ -614,7 +583,6 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                     // state is put back from the copy taken below and the update is replayed in the reference's order.
                     copy_words(sBackup, sL, tid, kLoopThreads);
                     __syncthreads();
-                    PF_MARK(1)   // state copy + barrier
                     if (tid == 0)
                         {
                             loop_track_part(*sL, t);
@@ -624,26 +592,15 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                             s_prm = prm;
                         }
                     else if (tid == 32)
-                        {
-#ifdef B200_LOOP_PROFILE
-                            const long long a_ = clock64();
-#endif
-                            s_lock_ok = loop_lock_part(*sL, t) ? 1 : 0;
-#ifdef B200_LOOP_PROFILE
-                            s_pf_lock += clock64() - a_;
-#endif
-                        }
+                        s_lock_ok = loop_lock_part(*sL, t) ? 1 : 0;
                     else if (tid >= 64 && tid < 69)
                         s_mags[tid - 64] = loop_record_magnitude(sL->c, t, tid - 64);
-                    PF_MARK(2)   // track part (thread 0 alone)
                     __syncthreads();
-                    PF_MARK(3)   // waiting for the lock part / magnitudes
                     // the dump record goes out from warp 1 while thread 0 consumes the epoch and prepares the next one: in the
                     // tracking state neither of those writes a member the record reads (the sample stamp was taken above)
                     if (tid == 32 && s_lock_ok > 0 && s_rec != nullptr) loop_record_part(*sL, t, s_data_channel >= 0 ? &s_data_tap : nullptr, s_mags, s_stamp, s_rec,
                                                                                           s_prm);
                 }
-#endif
             if (tid == 0)
                 {
                     if (have_taps)
@@ -665,7 +622,6 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                                     if (loop_update(*sL, t, s_data_channel >= 0 ? &s_data_tap : nullptr, rec, prm)) k_rec++;
                                 }
                         }
-                    PF_MARK(4)   // record + consume
                     int go = 0;
                     if (k < max_epochs)
                         {
@@ -677,9 +633,7 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                         }
                     s_go = go;
                 }
-            PF_MARK(5)   // prepare
             __syncthreads();
-            PF_MARK(6)   // barrier
             if (!s_go) break;
             if (taps == 3)
                 {
@@ -704,12 +658,6 @@ __global__ void __launch_bounds__(kLoopThreads, 512 / kLoopThreads > 0 ? 512 / k
                 }
             have_taps = true;
         }
-#ifdef B200_LOOP_PROFILE
-    if (tid == 0 && i == 0)
-        printf("LOOP_PROFILE loop 0, %d epochs, cycles per epoch: correlation %lld | state copy %lld | track part %lld | wait for lock part %lld (lock part itself %lld) | "
-               "record %lld | prepare %lld | barrier %lld\n", k_rec, pf[0] / k_rec, pf[1] / k_rec, pf[2] / k_rec, pf[3] / k_rec, s_pf_lock / k_rec, pf[4] / k_rec,
-            pf[5] / k_rec, pf[6] / k_rec);
-#endif
     __syncthreads();
     if (tid == 0) sL->pending = 0;
     __syncthreads();
@@ -752,7 +700,7 @@ int launch_loop_persistent(LoopDev* loops, int n_loops, int max_epochs, const Lo
     B200_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     bool wide = n_loops <= sms;
     if (const char* env = std::getenv("B200_LOOP_WIDTH")) wide = std::atoi(env) >= kLoopThreadsFew;
-    const int rc = (wide && kLoopThreadsMany < kLoopThreadsFew)
+    const int rc = wide
                        ? launch_loop_persistent_width<kLoopThreadsFew>(loops, n_loops, max_epochs, avail, chans, bands, data, records, rec_capacity,
                              n_records, prompts, tbl_cap, st)
                        : launch_loop_persistent_width<kLoopThreadsMany>(loops, n_loops, max_epochs, avail, chans, bands, data, records, rec_capacity,

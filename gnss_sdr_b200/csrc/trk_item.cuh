@@ -8,28 +8,18 @@
 #include "common.cuh"
 #include "trk_device.cuh"
 
-// tiles of the main loop unrolled per thread (one 16-byte load each): memory-level parallelism vs registers.  With five taps
-// (C3, Galileo E1) and one tap (the data correlator of a tracked pilot) the kernel waits on L2, so 16 = a whole re-seed group
-// of loads in flight; three taps (C2) take 4.  tools/ab_item.sh compares builds with other values.  On an H100 (400 W), ms per
-// step, default vs 8: five taps C3 5.52 vs 5.94; three taps C2 distinct-IQ 1.165 vs 1.178; one tap C3 + pilot 8.93-8.98 vs
-// 8.84 (within the spread of repeated runs of one build).
-#ifndef TRK_TILE_UNROLL_3
-#define TRK_TILE_UNROLL_3 4
-#endif
-#ifndef TRK_TILE_UNROLL_5
-#define TRK_TILE_UNROLL_5 16
-#endif
-#ifndef TRK_TILE_UNROLL_1
-#define TRK_TILE_UNROLL_1 16
-#endif
-
 namespace b200
 {
 namespace
 {
-constexpr int kTileUnroll3 = TRK_TILE_UNROLL_3;   // (#pragma unroll takes constant expressions, not macros)
-constexpr int kTileUnroll5 = TRK_TILE_UNROLL_5;
-constexpr int kTileUnroll1 = TRK_TILE_UNROLL_1;   // one tap: the data prompt of a tracked pilot
+// tiles of the main loop unrolled per thread (one 16-byte load each): memory-level parallelism vs registers.  With five taps
+// (C3, Galileo E1) and one tap (the data correlator of a tracked pilot) the kernel waits on L2, so 16 = a whole re-seed group
+// of loads in flight; three taps (C2) take 4.  On an H100 (400 W), ms per step, these values vs 8: five taps C3 5.52 vs 5.94;
+// three taps C2 distinct-IQ 1.165 vs 1.178; one tap C3 + pilot 8.93-8.98 vs 8.84 (within the spread of repeated runs of one
+// build).
+constexpr int kTileUnroll3 = 4;
+constexpr int kTileUnroll5 = 16;
+constexpr int kTileUnroll1 = 16;   // one tap: the data prompt of a tracked pilot
 
 struct ItemCtx
 {

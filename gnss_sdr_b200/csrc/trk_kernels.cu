@@ -76,20 +76,15 @@ __device__ __forceinline__ void run_item(const b200_trk_item& it, const ChanDesc
 }
 
 // One instantiation per tap count 1..8 (registers specialised to it).
-// No minimum-blocks hint by default.  sm_90a, no spills: <3> 64 registers (4 CTAs per SM), <1> 60, <5> 80 (3 CTAs).
-// TRK_MIN_BLOCKS builds the alternatives for tools/ab_item.sh.  On an H100 (400 W), ms per step: TRK_MIN_BLOCKS=4 (everything
-// at 64 registers; the generic kernel then in use spilled 3.3 KB) C3 5.43-5.46 vs 5.52-5.53, but C3 + pilot 9.12-9.14 vs
-// 8.93-8.98 and the C5 share 2.73-2.80 vs 2.60-2.64; TRK_MIN_BLOCKS=3 slower on all four legs.  The default stays.
-#ifdef TRK_MIN_BLOCKS
-#define TRK_LAUNCH_BOUNDS __launch_bounds__(kTrkThreads, TRK_MIN_BLOCKS)
-#else
-// tap counts other than 1, 3 and 5 keep the register budget of two CTAs per SM (128) that the kernel which read the tap count
-// per item had: left to ptxas, <4>, <6> and <7> settle at 64-80 registers and spill
-#define TRK_LAUNCH_BOUNDS __launch_bounds__(kTrkThreads, (TAPS == 1 || TAPS == 3 || TAPS == 5) ? 0 : 2)
-#endif
+// No minimum-blocks hint for 1, 3 and 5 taps.  sm_90a, no spills: <3> 64 registers (4 CTAs per SM), <1> 60, <5> 80 (3 CTAs).
+// On an H100 (400 W), ms per step: a minimum of 4 blocks (everything at 64 registers; the generic kernel then in use spilled
+// 3.3 KB) C3 5.43-5.46 vs 5.52-5.53, but C3 + pilot 9.12-9.14 vs 8.93-8.98 and the C5 share 2.73-2.80 vs 2.60-2.64; a minimum
+// of 3 blocks slower on all four legs.
+// Other tap counts keep the register budget of two CTAs per SM (128) that the kernel which read the tap count per item had:
+// left to ptxas, <4>, <6> and <7> settle at 64-80 registers and spill.
 template <int TAPS>
-__global__ void TRK_LAUNCH_BOUNDS trk_correlate_kernel(const b200_trk_item* __restrict__ items, int n_items,
-    const ChanDesc* __restrict__ chans, const BandDesc* __restrict__ bands, float2* __restrict__ out, int out_stride,
+__global__ void __launch_bounds__(kTrkThreads, (TAPS == 1 || TAPS == 3 || TAPS == 5) ? 0 : 2)
+    trk_correlate_kernel(const b200_trk_item* __restrict__ items, int n_items, const ChanDesc* __restrict__ chans, const BandDesc* __restrict__ bands, float2* __restrict__ out, int out_stride,
     int slices, float2* partial, unsigned int* counters, int tbl_cap, unsigned int only_mask)
 {
     // only_mask != 0: a batch with several tap counts runs as one launch per tap count; this launch serves the items whose

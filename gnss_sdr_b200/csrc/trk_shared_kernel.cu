@@ -30,14 +30,12 @@ constexpr int kShTile = 512;     // samples per tile (4 KB)
 #ifndef SH_STAGES
 #define SH_STAGES 4
 #endif
+constexpr int kShStages = SH_STAGES;
 // Minimum resident CTAs per SM (__launch_bounds__).  sm_90a, 288 threads: 3 caps the kernel at 72 registers and spills
 // (<3>: 166 B stores / 248 B loads), 2 gives 96 registers (<3>: 8 B / 8 B), 1 no spills at 127-152.  On an H100 (400 W), ms
 // per C2 step: 2 -> 0.969-0.970, 3 -> 1.051-1.058, 1 -> 1.189-1.191, 4 -> 1.179; distinct-IQ through this kernel 1.237 at 2,
 // 1.393 at 3.  With the chunk path's scratch a CTA takes about 92 KB of shared memory, so three no longer fit on an SM.
-#ifndef SH_MINB
-#define SH_MINB 2
-#endif
-constexpr int kShStages = SH_STAGES;
+constexpr int kShMinBlocks = 2;
 // SH_STRESS (test builds only, tests/test_ring_stress_gpu.py): pseudo-random delays in the producer and in every consumer
 // warp, before the tile is read and before the slot is released, so that warps drift apart by several tiles and every
 // full/empty hand-over of the TMA ring is exercised with 2, 4 and 8 stages.
@@ -261,7 +259,7 @@ __device__ __forceinline__ void warp_tile_chunks(const float4* x4, float4* pre4,
 }
 
 template <int TAPS>
-__global__ void __launch_bounds__(kShThreads, SH_MINB) trk_shared_kernel(const b200_trk_item* __restrict__ items, int n_items,
+__global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(const b200_trk_item* __restrict__ items, int n_items,
     const ChanDesc* __restrict__ chans, const BandDesc* __restrict__ bands, float2* __restrict__ out, int out_stride)
 {
     extern __shared__ __align__(128) unsigned char sh_raw[];

@@ -195,7 +195,7 @@ extern "C"
     /* Which correlator kernel a batch runs on.  2 (default): the shared-window kernel (one TMA-staged sample window per group
      * of 8 items) for batches of >= 1024 items with C/A-sized code tables whose consecutive items overlap in the band -
      * known for b200_trk_submit, which sees the items; assumed for b200_trk_batch_dev - and the per-item kernel otherwise.
-     * 1: shared-window whenever legal; 0: always per-item; -1: back to the B200_TRK_SHARED environment variable / default. */
+     * 1: shared-window whenever legal; 0: always per-item; -1: same as 2. */
     int b200_trk_kernel_choice(b200_engine* e, int mode);
     int b200_trk_submit(b200_engine* e, const b200_trk_item* items_host, int n_items, int out_stride, uint64_t* ticket);
     int b200_trk_wait(b200_engine* e, uint64_t ticket, b200_cf32* out_host);
@@ -325,7 +325,7 @@ extern "C"
     /* How b200_trk_loop_run schedules the work: 0 (default) one persistent kernel, one CTA per loop, free-running
      * for max_epochs cycles with no launch per epoch; 1 a correlator launch + a loop-update launch per epoch with
      * one CTA per loop (same integers as mode 0, floats within an ulp of atanf/log10f: the correlator sums in a different order); 2 the same with each epoch split over several CTAs
-     * (lowest latency for a handful of channels).  Env B200_LOOP_MODE sets the initial value. */
+     * (lowest latency for a handful of channels). */
     int b200_trk_loop_set_mode(b200_engine* e, int mode);
     /* Prepare (if not already pending) and return the next work item of every loop: the seven scalars
      * do_correlation_step would pass, for hosts that correlate elsewhere.  n == 0 marks a loop in standby.

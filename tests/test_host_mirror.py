@@ -9,7 +9,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EXE = os.path.join(ROOT, "tests", "host", "test_host_mirror")
 
 
-def build():
+def build(exe=EXE):
+    """the host program, by default into tests/host/ where bench.py runs it; the tests build their own copy under tmp_path,
+    so that they also run from a read-only tree"""
     libdir = os.path.join(ROOT, "gnss_sdr_b200")
     ref = os.path.join(ROOT, "oracle", "_ref", "liboracle_ref.so")
     cmd = ["g++", "-std=c++20", "-O2", os.path.join(ROOT, "tests", "host", "test_host_mirror.cc"),
@@ -20,24 +22,24 @@ def build():
            os.path.join(libdir, "host", "b200_pcps_acquisition_fine_doppler_core.cc"),
            os.path.join(libdir, "host", "b200_dll_pll_veml_loop.cc"),
            "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(libdir, "host"),
-           "-L" + libdir, "-lb200gnss", "-Wl,-rpath," + libdir, "-lpthread", "-o", EXE]
+           "-L" + libdir, "-lb200gnss", "-Wl,-rpath," + libdir, "-lpthread", "-o", str(exe)]
     if os.path.exists(ref):
         cmd += ["-DHAVE_REF", ref, "-Wl,-rpath," + os.path.dirname(ref)]
     subprocess.check_call(cmd)
-    return EXE
+    return str(exe)
 
 
-def test_host_mirror_builds_and_links():
+def test_host_mirror_builds_and_links(tmp_path):
     import gnss_sdr_b200.capi  # noqa: F401  (library must exist)
-    exe = build()
+    exe = build(tmp_path / "test_host_mirror")
     assert os.path.exists(exe)
 
 
-def test_coalescer_logic_against_a_fake_engine():
+def test_coalescer_logic_against_a_fake_engine(tmp_path):
     """b200::Trk_Coalescer linked against a fake engine (tests/host/test_coalescer_cpu.cc): 24 block threads on one stream
     (right answers, one copy of the samples, shared batches), a restarted stream with overlapping indices, two bands with a
     straggler, a wrapping ring with a slow channel - no GPU needed."""
-    exe = os.path.join(ROOT, "tests", "host", "test_coalescer_cpu")
+    exe = str(tmp_path / "test_coalescer_cpu")
     libdir = os.path.join(ROOT, "gnss_sdr_b200")
     subprocess.check_call(["g++", "-std=c++20", "-O2", "-Wall", "-Wextra", os.path.join(ROOT, "tests", "host", "test_coalescer_cpu.cc"),
                            os.path.join(libdir, "host", "b200_trk_coalescer.cc"), "-I" + os.path.join(ROOT, "include"),
@@ -47,11 +49,11 @@ def test_coalescer_logic_against_a_fake_engine():
         assert r.returncode == 0 and "COALESCER_CPU OK" in r.stdout, r.stdout + r.stderr
 
 
-def test_compute_threshold_matches_boost_formula():
+def test_compute_threshold_matches_boost_formula(tmp_path):
     """compute_threshold (pcps_acquisition.cc:52-56) on the host, no GPU: against scipy's gammaincinv
     (== boost::math::gamma_p_inv) through the oracle's restatement."""
     from oracle.acq_np import compute_threshold
-    exe = build()
+    exe = build(tmp_path / "test_host_mirror")
     r = subprocess.run([exe, "--thresholds"], capture_output=True, text=True, timeout=60)
     assert r.returncode == 0
     lines = [ln.split() for ln in r.stdout.splitlines() if ln.startswith("THRESH")]
@@ -62,8 +64,8 @@ def test_compute_threshold_matches_boost_formula():
 
 
 @pytest.mark.gpu
-def test_host_mirror_runs_and_matches_reference():
-    exe = build()
+def test_host_mirror_runs_and_matches_reference(tmp_path):
+    exe = build(tmp_path / "test_host_mirror")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
     print(r.stdout)
     assert r.returncode == 0, r.stdout + r.stderr
@@ -134,12 +136,12 @@ int main()
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("threads,epochs", [(32, 300), (256, 100)])
-def test_class_interface_through_the_coalescer(threads, epochs):
+def test_class_interface_through_the_coalescer(threads, epochs, tmp_path):
     """N std::threads drive B200_Multicorrelator_Real_Codes in coalesced mode on one band (C2 sizes: 25 000 samples per
     epoch): every correlation succeeds, the samples cross PCIe once (copy ratio ~ 1/N) and the epochs share launches.
     The throughput / per-call latency line is what bench.py reports as `coalesced_class_interface`."""
     import json
-    exe = build()
+    exe = build(tmp_path / "test_host_mirror")
     r = subprocess.run([exe, "--coalescer", str(threads), str(epochs), "200"], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout + r.stderr
     line = [ln for ln in r.stdout.splitlines() if ln.startswith("COALESCED ")][0]

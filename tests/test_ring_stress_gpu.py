@@ -39,7 +39,7 @@ for c in range(n_ch):
         items.append((cid, n, off + k * n, 0.0, 0.0, 0.0, float(rng.uniform(0, 1)), step, 0.0))
 items = np.array(items, dtype=capi.TRK_ITEM_DTYPE)
 items = items[np.argsort(items["sample_index"], kind="stable")]
-os.environ["B200_TRK_SHARED"] = "1"
+eng.trk_kernel_choice(1)                        # 960 items: below the automatic choice's 1024
 first = None
 bad = 0
 for it in range(launches):
@@ -86,7 +86,7 @@ def build_variant(stages, stress):
 def run_worker(lib, launches, tmp_path):
     script = tmp_path / "ring_worker.py"
     script.write_text(WORKER)
-    env = dict(os.environ, B200_ROOT=ROOT, B200_LIB=lib, B200_TRK_SHARED="1")
+    env = dict(os.environ, B200_ROOT=ROOT, B200_LIB=lib)
     r = subprocess.run([sys.executable, str(script), str(launches)], env=env, capture_output=True, text=True, timeout=1500)
     assert r.returncode == 0, r.stdout + r.stderr
     line = [ln for ln in r.stdout.splitlines() if ln.startswith("RESULT ")][0]

@@ -441,7 +441,6 @@ def test_shared_window_groups_staggered_integer_exact(capi, oracle, L, taps_shif
     where every channel is aligned to its own code period), item count not a multiple of 8, different
     code tables and code phases per channel.  Integer data => results must be EXACT.  Run with the
     shared kernel forced on and forced off: both must equal the integer oracle."""
-    import os
     rng = np.random.default_rng(L + n)
     n_ch, n_ep = 11, 3
     total = n * (n_ep + 1) + 4096
@@ -457,8 +456,8 @@ def test_shared_window_groups_staggered_integer_exact(capi, oracle, L, taps_shif
             want[(k, c)] = int_oracle(x_int[s0:s0 + n], codes[c], idx)
     results = {}
     for mode in ("1", "0"):
-        os.environ["B200_TRK_SHARED"] = mode
         e = capi.Engine(0)
+        e.trk_kernel_choice(int(mode))
         e.iq_create(0, total)
         first = e.iq_push(0, x_int.astype(np.complex64))
         cids = []
@@ -489,7 +488,6 @@ def test_shared_window_groups_staggered_integer_exact(capi, oracle, L, taps_shif
             assert np.array_equal(got[i, :, 0].astype(np.int64), want[key]), (mode, key)
             assert np.all(got[i, :, 1] == 0)
         e.close()
-    os.environ.pop("B200_TRK_SHARED", None)
     assert np.array_equal(results["0"], results["1"])
 
 
@@ -497,7 +495,6 @@ def test_shared_kernel_groups_that_cannot_share(capi, oracle):
     """Groups of 8 items whose sample ranges are far apart (channel-major order: 8 consecutive epochs of one
     channel) or that sit on different bands cannot share a window; each warp then streams its own samples
     with the same arithmetic.  Integer-exact."""
-    import os
     import torch
     n, L, shifts, step = 6000, 1023, [-0.5, 0.0, 0.5], 0.1705
     rng = np.random.default_rng(4242)
@@ -505,8 +502,8 @@ def test_shared_kernel_groups_that_cannot_share(capi, oracle):
     total = n * n_ep + 1001
     xs = [rng.integers(-7, 8, total) for _ in range(2)]           # two bands
     codes = [(((np.arange(L) * (7919 + 2 * c)) % 31) - 15) for c in range(n_ch)]
-    os.environ["B200_TRK_SHARED"] = "1"
     e = capi.Engine(0)
+    e.trk_kernel_choice(1)
     firsts = []
     for b in range(2):
         e.iq_create(b, total)
@@ -533,13 +530,65 @@ def test_shared_kernel_groups_that_cannot_share(capi, oracle):
     e.sync()
     got = out_t.cpu().numpy()
     e.close()
-    os.environ.pop("B200_TRK_SHARED", None)
     for i, (c, k) in enumerate(order):
         _, idx = oracle.port.resampler(1, codes[c].astype(np.float32), 0.3 + c, step, shifts, n, return_idx=True)
         s0 = 37 * c + k * n + (k % 2)
         want = int_oracle(xs[c % 2][s0:s0 + n], codes[c], idx)
         assert np.array_equal(got[i, :, 0].astype(np.int64), want), (c, k)
         assert np.all(got[i, :, 1] == 0)
+
+
+def test_kernel_choice_only_through_the_api(capi, oracle, monkeypatch):
+    """The engine picks the correlator kernel from b200_trk_kernel_choice alone; B200_TRK_SHARED in the environment
+    changes nothing.  1024 overlapping C/A-like float items at 25 Msps on the device entry point: by default they take the
+    shared-window kernel, byte for byte what forcing it (1) gives, and -1 means the default.  These items take its chunk
+    path, whose float sums differ from the per-item kernel's in the last bits, so the per-item result (0) must differ."""
+    import torch
+    monkeypatch.setenv("B200_TRK_SHARED", "0")
+    fs, n, n_ch, n_ep = 25e6, 25000, 32, 32
+    rng = np.random.default_rng(1024)
+    total = n * (n_ep + 1)
+    e = capi.Engine(0)
+    e.iq_create(0, 1 << 20)
+    first = e.iq_push(0, (rng.normal(size=total) + 1j * rng.normal(size=total)).astype(np.complex64))
+    cids = []
+    for c in range(n_ch):
+        cid = e.channel_create(0, 3)
+        e.channel_set_code(cid, oracle.port.gps_ca_code(c + 1), [-0.5, 0.0, 0.5])
+        cids.append(cid)
+    starts = np.sort(rng.integers(0, n, n_ch))
+    dopplers = rng.uniform(-4000.0, 4000.0, n_ch)
+    items = np.zeros(n_ch * n_ep, capi.TRK_ITEM_DTYPE)
+    for k in range(n_ep):                                          # epoch-major: a group's 8 items overlap in the band
+        for c in range(n_ch):
+            it = items[k * n_ch + c]
+            it["channel"] = cids[c]
+            it["n"] = n
+            it["sample_index"] = first + int(starts[c]) + k * n
+            it["rem_carrier_phase_rad"] = 0.1 * c
+            it["phase_step_rad"] = 2 * np.pi * dopplers[c] / fs
+            it["rem_code_phase_chips"] = 0.01 * c
+            it["code_phase_step_chips"] = 1.023e6 * (1 + dopplers[c] / 1575.42e6) / fs
+    items_t = torch.from_numpy(items.view(np.uint8)).cuda()
+    out_t = torch.zeros(len(items), 3, 2, dtype=torch.float32, device="cuda")
+
+    def run():
+        out_t.zero_()
+        e.trk_batch_dev(items_t.data_ptr(), len(items), out_t.data_ptr(), 3, 1)
+        e.sync()
+        return out_t.cpu().numpy().tobytes()
+
+    default = run()
+    e.trk_kernel_choice(1)
+    forced = run()
+    e.trk_kernel_choice(-1)
+    minus_one = run()
+    e.trk_kernel_choice(0)
+    per_item = run()
+    e.close()
+    assert default == forced
+    assert minus_one == forced
+    assert per_item != forced
 
 
 @pytest.mark.parametrize("layout", ["shared", "distinct"])

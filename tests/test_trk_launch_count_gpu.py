@@ -102,3 +102,18 @@ def test_loop_run_counts_its_launches(capi, monkeypatch, mode, with_data, launch
     e.loop_run(n_ep)
     assert e.launch_count() - k0 == launches(n_ep)
     e.close()
+
+
+def test_loop_mode_only_through_the_api(capi, monkeypatch):
+    """B200_LOOP_MODE in the environment selects nothing: an engine whose mode was never set runs the persistent kernel,
+    one launch per run (mode 1 would issue 1 + 2 per epoch)."""
+    n_ep = 5
+    monkeypatch.setenv("B200_LOOP_MODE", "1")
+    sp, _ = pd.pilot_data_spec(5, 25, 1234.0, 1777, n_ep)
+    e, ids, _ = pd.make_engine(capi, [sp], [None], {0: len(sp.stream.x) + 16})
+    tl.push_all(e, [sp])
+    tl.start_all(e, ids, [sp])
+    k0 = e.launch_count()
+    e.loop_run(n_ep)
+    assert e.launch_count() - k0 == 1
+    e.close()
