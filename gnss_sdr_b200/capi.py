@@ -6,6 +6,9 @@ import os
 
 import numpy as np
 
+from .abi import (ACQ_RESULT_DTYPE, TRK_DUMP_RECORD_DTYPE, TRK_ITEM_DTYPE, AcqConf, AcqDump, AcqResult,  # noqa: F401
+                  TrkDumpRecord, TrkItem, TrkLoopConf, TrkLoopStatus)
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200_LIB selects an alternative build of the SAME library (A/B kernel experiments); default = in-tree build
 LIB_PATH = os.environ.get("B200_LIB") or os.path.join(_HERE, "libb200gnss.so")
@@ -27,19 +30,6 @@ class B200Error(RuntimeError):
         msg = lib.b200_last_error()
         super().__init__(f"{where}: {ERRORS.get(code, code)}: {msg.decode() if msg else ''}")
 
-
-class TrkItem(C.Structure):
-    _fields_ = [("channel", C.c_int32), ("n", C.c_int32), ("sample_index", C.c_uint64),
-                ("rem_carrier_phase_rad", C.c_float), ("phase_step_rad", C.c_float), ("phase_rate_step_rad", C.c_float),
-                ("rem_code_phase_chips", C.c_float), ("code_phase_step_chips", C.c_float),
-                ("code_phase_rate_step_chips", C.c_float)]
-
-
-TRK_ITEM_DTYPE = np.dtype([("channel", "<i4"), ("n", "<i4"), ("sample_index", "<u8"),
-                           ("rem_carrier_phase_rad", "<f4"), ("phase_step_rad", "<f4"), ("phase_rate_step_rad", "<f4"),
-                           ("rem_code_phase_chips", "<f4"), ("code_phase_step_chips", "<f4"),
-                           ("code_phase_rate_step_chips", "<f4")])
-assert TRK_ITEM_DTYPE.itemsize == 40 and C.sizeof(TrkItem) == 40
 
 lib.b200_last_error.restype = C.c_char_p
 _vp = C.c_void_p
@@ -85,29 +75,6 @@ _SIGS = {
     "b200_trk_batch_dev": ([_vp, _vp, C.c_int, _vp, C.c_int, C.c_int], C.c_int),
     "b200_trk_submit": ([_vp, _vp, C.c_int, C.c_int, C.POINTER(C.c_uint64)], C.c_int),
     "b200_trk_wait": ([_vp, C.c_uint64, _vp], C.c_int),
-}
-
-
-class AcqConf(C.Structure):
-    _fields_ = [("fft_size", C.c_uint32), ("effective_fft_size", C.c_uint32), ("consumed_samples", C.c_uint32),
-                ("num_doppler_bins", C.c_uint32), ("doppler_max", C.c_int32), ("doppler_step", C.c_int32),
-                ("fs_in", C.c_int64), ("samples_per_chip", C.c_uint32), ("code_layout", C.c_uint32),
-                ("bit_transition_flag", C.c_int32), ("use_cfar", C.c_int32), ("max_dwells", C.c_uint32),
-                ("n_code_slots", C.c_uint32), ("keep_grid", C.c_int32)]
-
-
-class AcqResult(C.Structure):
-    _fields_ = [("index_time", C.c_uint32), ("index_doppler", C.c_uint32), ("doppler", C.c_int32),
-                ("test_statistics", C.c_float), ("grid_maximum", C.c_float), ("input_power", C.c_float),
-                ("second_peak", C.c_float)]
-
-
-ACQ_RESULT_DTYPE = np.dtype([("index_time", "<u4"), ("index_doppler", "<u4"), ("doppler", "<i4"),
-                             ("test_statistics", "<f4"), ("grid_maximum", "<f4"), ("input_power", "<f4"),
-                             ("second_peak", "<f4")])
-assert ACQ_RESULT_DTYPE.itemsize == C.sizeof(AcqResult) == 28
-
-_SIGS.update({
     "b200_acq_create": ([_vp, C.POINTER(AcqConf), C.POINTER(_vp)], C.c_int),
     "b200_acq_set_local_code": ([_vp, C.c_uint32, _vp], C.c_int),
     "b200_acq_set_doppler_center": ([_vp, C.c_int32, C.c_int32], C.c_int),
@@ -124,49 +91,6 @@ _SIGS.update({
     "b200_acq_selftest_dft": ([_vp, _vp, _vp], C.c_int),
     "b200_acq_read_wipeoffs": ([_vp, _vp], C.c_int),
     "b200_acq_destroy": ([_vp], C.c_int),
-})
-
-
-
-class TrkLoopConf(C.Structure):
-    """b200_trk_loop_conf: Dll_Pll_Conf / dll_pll_veml_tracking members the device loop needs."""
-    _fields_ = [
-        ("fs_in", C.c_double), ("code_chip_rate", C.c_double), ("signal_carrier_freq", C.c_double),
-        ("code_period", C.c_double), ("carrier_lock_th", C.c_double),
-        ("code_length_chips", C.c_uint32), ("vector_length", C.c_uint32), ("pull_in_time_s", C.c_uint32),
-        ("bit_synchronization_time_limit_s", C.c_uint32), ("prn", C.c_uint32),
-        ("code_samples_per_chip", C.c_int32), ("pll_filter_order", C.c_int32), ("dll_filter_order", C.c_int32),
-        ("cn0_samples", C.c_int32), ("cn0_min", C.c_int32), ("max_code_lock_fail", C.c_int32),
-        ("max_carrier_lock_fail", C.c_int32), ("cn0_smoother_samples", C.c_int32),
-        ("carrier_lock_test_smoother_samples", C.c_int32), ("veml", C.c_int32), ("cloop", C.c_int32),
-        ("carrier_aiding", C.c_int32), ("enable_fll_pull_in", C.c_int32), ("enable_fll_steady_state", C.c_int32),
-        ("pll_bw_hz", C.c_float), ("dll_bw_hz", C.c_float), ("fll_bw_hz", C.c_float),
-        ("early_late_space_chips", C.c_float), ("slope", C.c_float), ("y_intercept", C.c_float),
-        ("cn0_smoother_alpha", C.c_float), ("carrier_lock_test_smoother_alpha", C.c_float),
-    ]
-
-
-class TrkLoopStatus(C.Structure):
-    _fields_ = [
-        ("state", C.c_int32), ("loss_of_lock", C.c_int32), ("sample_counter", C.c_uint64), ("epochs", C.c_uint64),
-        ("carrier_doppler_hz", C.c_double), ("code_freq_chips", C.c_double), ("rem_code_phase_samples", C.c_double),
-        ("acc_carrier_phase_rad", C.c_double), ("CN0_SNV_dB_Hz", C.c_double), ("carrier_lock_test", C.c_double),
-    ]
-
-
-# b200_trk_dump_record: one epoch of the reference's tracking dump file (108 bytes, unpadded)
-TRK_DUMP_RECORD_DTYPE = np.dtype([
-    ("abs_VE", "<f4"), ("abs_E", "<f4"), ("abs_P", "<f4"), ("abs_L", "<f4"), ("abs_VL", "<f4"),
-    ("prompt_I", "<f4"), ("prompt_Q", "<f4"), ("PRN_start_sample_count", "<u8"),
-    ("acc_carrier_phase_rad", "<f4"), ("carrier_doppler_hz", "<f4"), ("carrier_doppler_rate_hz_s", "<f4"),
-    ("code_freq_chips", "<f4"), ("code_freq_rate_chips", "<f4"), ("carr_error_hz", "<f4"),
-    ("carr_error_filt_hz", "<f4"), ("code_error_chips", "<f4"), ("code_error_filt_chips", "<f4"),
-    ("CN0_SNV_dB_Hz", "<f4"), ("carrier_lock_test", "<f4"), ("aux1", "<f4"), ("aux2", "<f8"),
-    ("PRN", "<u4"), ("TOW_ms", "<u8"), ("WN", "<u4"),
-])
-assert TRK_DUMP_RECORD_DTYPE.itemsize == 108 and C.sizeof(TrkLoopConf) == 152
-
-_SIGS.update({
     "b200_trk_loop_create": ([_vp, C.c_int, C.POINTER(TrkLoopConf), C.POINTER(C.c_int)], C.c_int),
     "b200_trk_loop_start": ([_vp, C.c_int, C.c_double, C.c_double, C.c_uint64, C.c_uint64], C.c_int),
     "b200_trk_loop_run": ([_vp, C.c_int, _vp, _vp], C.c_int),
@@ -177,27 +101,13 @@ _SIGS.update({
     "b200_trk_loop_step_taps": ([_vp, _vp, _vp, _vp], C.c_int),
     "b200_trk_loop_status_get": ([_vp, C.c_int, C.POINTER(TrkLoopStatus)], C.c_int),
     "b200_trk_dump_write": ([C.c_char_p, _vp, C.c_int, C.c_int], C.c_int),
-})
-
-
-
-class AcqDump(C.Structure):
-    _fields_ = [("acq_grid", _vp), ("acq_grid_narrow", _vp), ("effective_fft_size", C.c_uint32), ("num_doppler_bins", C.c_uint32),
-                ("num_doppler_bins_step2", C.c_uint32), ("doppler_max", C.c_int32), ("doppler_step", C.c_int32),
-                ("positive_acq", C.c_int32), ("num_dwells", C.c_int32), ("prn", C.c_uint32), ("acq_doppler_hz", C.c_float),
-                ("acq_delay_samples", C.c_float), ("test_statistic", C.c_float), ("threshold", C.c_float),
-                ("input_power", C.c_float), ("doppler_step_narrow", C.c_float), ("doppler_grid_narrow_min", C.c_float),
-                ("sample_counter", C.c_uint64)]
-
-
-_SIGS.update({
     "b200_acq_fine_create": ([_vp, C.c_uint32, C.POINTER(_vp)], C.c_int),
     "b200_acq_fine_estimate": ([_vp, _vp, _vp, C.POINTER(C.c_uint32), C.POINTER(C.c_float)], C.c_int),
     "b200_acq_fine_read_spectrum": ([_vp, _vp], C.c_int),
     "b200_acq_fine_destroy": ([_vp], C.c_int),
     "b200_acq_dump_write": ([C.c_char_p, C.POINTER(AcqDump)], C.c_int),
     "b200_acq_dump_filename": ([C.c_char_p, C.c_char, C.c_char_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t], C.c_int),
-})
+}
 
 for _name, (_args, _res) in _SIGS.items():
     _fn = getattr(lib, _name)

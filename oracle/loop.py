@@ -4,7 +4,8 @@
 * ``RefLoop``  -> oracle/ref_loop.cc over the reference's own tracking libs (oracle/_ref/liboracle_ref_loop.so)
 * ``ref_dump_read`` -> the reference's own Tracking_Dump_Reader
 
-The structures restate include/b200gnss.h (b200_trk_loop_conf, b200_trk_dump_record, b200_trk_loop_status).
+The structures are include/b200gnss.h's (b200_trk_loop_conf, b200_trk_dump_record, b200_trk_loop_status), from
+gnss_sdr_b200.abi, which declares them without loading the product library: the C port includes the same header.
 """
 from __future__ import annotations
 
@@ -13,52 +14,20 @@ import os
 
 import numpy as np
 
+from gnss_sdr_b200.abi import TRK_DUMP_RECORD_DTYPE, TrkLoopConf, TrkLoopStatus
+
+# the names this module has always exported, for the code that still uses them: the same objects, not copies
+LoopConf, LoopStatus, DUMP_RECORD_DTYPE = TrkLoopConf, TrkLoopStatus, TRK_DUMP_RECORD_DTYPE
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _REF_LOOP_SO = os.path.join(_HERE, "_ref", "liboracle_ref_loop.so")
 _PORT_SO = os.path.join(_HERE, "liboracle_port.so")
 
 
-class LoopConf(C.Structure):
-    _fields_ = [
-        ("fs_in", C.c_double), ("code_chip_rate", C.c_double), ("signal_carrier_freq", C.c_double),
-        ("code_period", C.c_double), ("carrier_lock_th", C.c_double),
-        ("code_length_chips", C.c_uint32), ("vector_length", C.c_uint32), ("pull_in_time_s", C.c_uint32),
-        ("bit_synchronization_time_limit_s", C.c_uint32), ("prn", C.c_uint32),
-        ("code_samples_per_chip", C.c_int32), ("pll_filter_order", C.c_int32), ("dll_filter_order", C.c_int32),
-        ("cn0_samples", C.c_int32), ("cn0_min", C.c_int32), ("max_code_lock_fail", C.c_int32),
-        ("max_carrier_lock_fail", C.c_int32), ("cn0_smoother_samples", C.c_int32),
-        ("carrier_lock_test_smoother_samples", C.c_int32), ("veml", C.c_int32), ("cloop", C.c_int32),
-        ("carrier_aiding", C.c_int32), ("enable_fll_pull_in", C.c_int32), ("enable_fll_steady_state", C.c_int32),
-        ("pll_bw_hz", C.c_float), ("dll_bw_hz", C.c_float), ("fll_bw_hz", C.c_float),
-        ("early_late_space_chips", C.c_float), ("slope", C.c_float), ("y_intercept", C.c_float),
-        ("cn0_smoother_alpha", C.c_float), ("carrier_lock_test_smoother_alpha", C.c_float),
-    ]
-
-
-class LoopStatus(C.Structure):
-    _fields_ = [
-        ("state", C.c_int32), ("loss_of_lock", C.c_int32), ("sample_counter", C.c_uint64), ("epochs", C.c_uint64),
-        ("carrier_doppler_hz", C.c_double), ("code_freq_chips", C.c_double), ("rem_code_phase_samples", C.c_double),
-        ("acc_carrier_phase_rad", C.c_double), ("CN0_SNV_dB_Hz", C.c_double), ("carrier_lock_test", C.c_double),
-    ]
-
-
-DUMP_RECORD_DTYPE = np.dtype([
-    ("abs_VE", "<f4"), ("abs_E", "<f4"), ("abs_P", "<f4"), ("abs_L", "<f4"), ("abs_VL", "<f4"),
-    ("prompt_I", "<f4"), ("prompt_Q", "<f4"), ("PRN_start_sample_count", "<u8"),
-    ("acc_carrier_phase_rad", "<f4"), ("carrier_doppler_hz", "<f4"), ("carrier_doppler_rate_hz_s", "<f4"),
-    ("code_freq_chips", "<f4"), ("code_freq_rate_chips", "<f4"), ("carr_error_hz", "<f4"),
-    ("carr_error_filt_hz", "<f4"), ("code_error_chips", "<f4"), ("code_error_filt_chips", "<f4"),
-    ("CN0_SNV_dB_Hz", "<f4"), ("carrier_lock_test", "<f4"), ("aux1", "<f4"), ("aux2", "<f8"),
-    ("PRN", "<u4"), ("TOW_ms", "<u8"), ("WN", "<u4"),
-])
-assert DUMP_RECORD_DTYPE.itemsize == 108
-
-
-def default_conf(fs_in=4e6, prn=1, **kw) -> LoopConf:
+def default_conf(fs_in=4e6, prn=1, **kw) -> TrkLoopConf:
     """GPS L1 C/A defaults of Dll_Pll_Conf (dll_pll_conf.h:32-89, gnss_sdr_flags.cc:44-53) with
     early_late_space_chips = 0.5 as gps_l1_ca_dll_pll_tracking_test.cc:291 sets it."""
-    c = LoopConf()
+    c = TrkLoopConf()
     c.fs_in = fs_in
     c.code_chip_rate = 1.023e6
     c.signal_carrier_freq = 1575.42e6
@@ -99,16 +68,16 @@ def default_conf(fs_in=4e6, prn=1, **kw) -> LoopConf:
 
 
 class _Loop:
-    def __init__(self, lib, prefix, conf: LoopConf):
+    def __init__(self, lib, prefix, conf: TrkLoopConf):
         self.lib, self.p = lib, prefix
         f = lambda name: getattr(lib, prefix + name)
         f("create").restype = C.c_void_p
-        f("create").argtypes = [C.POINTER(LoopConf)]
+        f("create").argtypes = [C.POINTER(TrkLoopConf)]
         f("destroy").argtypes = [C.c_void_p]
         f("start").argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_uint64, C.c_uint64]
         f("prepare").argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.POINTER(C.c_float)]
         f("update").argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_void_p]
-        f("status").argtypes = [C.c_void_p, C.POINTER(LoopStatus)]
+        f("status").argtypes = [C.c_void_p, C.POINTER(TrkLoopStatus)]
         self.conf = conf
         self.h = f("create")(C.byref(conf))
         if not self.h:
@@ -127,12 +96,12 @@ class _Loop:
     def update(self, taps):
         """taps complex64[3 or 5] -> (logged, record)"""
         t = np.ascontiguousarray(taps, np.complex64)
-        rec = np.zeros(1, DUMP_RECORD_DTYPE)
+        rec = np.zeros(1, TRK_DUMP_RECORD_DTYPE)
         logged = getattr(self.lib, self.p + "update")(self.h, t.ctypes.data_as(C.POINTER(C.c_float)), rec.ctypes.data)
         return bool(logged), rec[0]
 
-    def status(self) -> LoopStatus:
-        s = LoopStatus()
+    def status(self) -> TrkLoopStatus:
+        s = TrkLoopStatus()
         getattr(self.lib, self.p + "status")(self.h, C.byref(s))
         return s
 
@@ -190,11 +159,11 @@ def ref_lib():
     return _ref_lib
 
 
-def PortLoop(conf: LoopConf) -> _Loop:
+def PortLoop(conf: TrkLoopConf) -> _Loop:
     return _Loop(port_lib(), "port_loop_", conf)
 
 
-def RefLoop(conf: LoopConf) -> _Loop:
+def RefLoop(conf: TrkLoopConf) -> _Loop:
     lib = ref_lib()
     if lib is None:
         raise RuntimeError("oracle/_ref/liboracle_ref_loop.so not built")

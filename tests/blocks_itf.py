@@ -12,6 +12,7 @@ import os
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+E1C_SECONDARY = "0011100000001010110110010"  # GALILEO_E1_C_SECONDARY_CODE, src/core/system_parameters/Galileo_E1.h
 
 
 class Synchro(C.Structure):

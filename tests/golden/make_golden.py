@@ -92,6 +92,7 @@ def main():
     np.savez(os.path.join(HERE, "acq_ref_golden.npz"), **acq)
     # DLL/PLL loop: records and item scalars produced by the reference's own loop-filter / discriminator /
     # lock-detector / smoother objects (oracle/_ref/liboracle_ref_loop.so) for seeded correlator outputs
+    from gnss_sdr_b200.abi import TRK_DUMP_RECORD_DTYPE
     from oracle import loop as ol
     import loop_harness as lh
     lp = {}
@@ -107,7 +108,7 @@ def main():
             ok, r = R.update(taps[k])
             assert ok
             recs.append(r)
-        lp[f"{name}/records"] = np.frombuffer(np.array(recs, ol.DUMP_RECORD_DTYPE).tobytes(), np.uint8)
+        lp[f"{name}/records"] = np.frombuffer(np.array(recs, TRK_DUMP_RECORD_DTYPE).tobytes(), np.uint8)
         lp[f"{name}/items"] = np.array(items, np.uint64)
     np.savez_compressed(os.path.join(HERE, "loop_ref_golden.npz"), **lp)
     # SHA-256 of the reference kernels' outputs behind tests/test_oracle_port_vs_ref.py

@@ -2,7 +2,7 @@
 and the closed loop `prepare -> correlate -> update` over a host sample buffer."""
 import numpy as np
 
-from oracle import loop as ol
+from gnss_sdr_b200.abi import TRK_DUMP_RECORD_DTYPE
 
 
 def synthetic_taps(n_epochs, n_taps, seed, amp=4000.0, weak_from=None):
@@ -62,4 +62,4 @@ def run_closed_loop(loop, correlate, iq, n_epochs):
         logged, r = loop.update(taps)
         if logged:
             recs.append(r)
-    return np.array(recs, ol.DUMP_RECORD_DTYPE)
+    return np.array(recs, TRK_DUMP_RECORD_DTYPE)

@@ -13,23 +13,11 @@ import numpy as np
 import pytest
 
 import gnss_synth as gs
+from gpu_fixtures import capi, engine  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 ERR_ARG, ERR_STATE, ERR_RANGE = -1, -4, -5
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
-
-
-@pytest.fixture(scope="module")
-def engine(capi):
-    e = capi.Engine(0)
-    yield e
-    e.close()
 
 
 def _pow2(n):
@@ -305,21 +293,12 @@ def test_band_search_launches_what_search_dev_launches(capi, engine, spms, opts)
 
 
 # ---- cold start on the device ------------------------------------------------------------------------------------------
-# The loop configuration of tests/test_loop_gpu.py (GPS L1 C/A defaults of Dll_Pll_Conf), copied.
-def _loop_conf(capi, fs, prn):
-    from oracle import loop as ol
-    c = ol.default_conf(fs_in=fs, prn=prn, pull_in_time_s=1)
-    out = capi.TrkLoopConf()
-    for name, _ in ol.LoopConf._fields_:
-        setattr(out, name, getattr(c, name))
-    return out
-
-
 def test_cold_start_from_a_pushed_file_into_device_loops(capi, tmp_path):
     """GPS L1 C/A at 4 Msps written as an ishort file and pushed into a band once; PRNs 1-32 swept from the band in one call
     and judged against the reference's CFAR threshold; a device loop started for each detection from the acquisition result
     (code phase, Doppler, sample stamp abs_index + consumed_samples) tracks its satellite on the same band."""
     from scipy.special import gammaincinv
+    from oracle import loop as ol
     fs, spms, n_ep, pfa, scale = 4e6, 4000, 1000, 0.001, 64.0
     # 46-48 dB-Hz: with one 1 ms dwell the reference's threshold (pfa 1e-3 over 4000 x 100 cells) is a statistic of 46; a
     # satellite at 46 dB-Hz peaks near 80 on average, the strongest absent PRN of this seed reaches 35
@@ -356,7 +335,7 @@ def test_cold_start_from_a_pushed_file_into_device_loops(capi, tmp_path):
         r = res[sv["prn"] - 1]
         ch = e.channel_create(0, 3)
         e.channel_set_code(ch, codes[sv["prn"]], [-0.5, 0.0, 0.5])
-        lid = e.loop_create(ch, _loop_conf(capi, fs, sv["prn"]))
+        lid = e.loop_create(ch, ol.default_conf(fs_in=fs, prn=sv["prn"], pull_in_time_s=1))
         e.loop_start(lid, math.fmod(float(r["index_time"]), float(spms)), float(r["doppler"]), stamp, stamp)
         assert abs(r["doppler"] - sv["doppler"]) <= 150            # a 1 ms peak spans several 100 Hz bins
         assert abs(int(r["index_time"]) - (sv["delay"] - abs_index) % spms) <= 1

@@ -15,19 +15,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from gnss_synth import make_iq  # noqa: E402
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
-
-
-@pytest.fixture(scope="module")
-def engine(capi):
-    e = capi.Engine(0)
-    yield e
-    e.close()
+from gpu_fixtures import capi, engine  # noqa: E402,F401
 
 
 def _bits(a):

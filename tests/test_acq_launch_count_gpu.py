@@ -10,20 +10,9 @@ checked in test_acq_chirpz_modes_gpu.py.
 import numpy as np
 import pytest
 
+from gpu_fixtures import capi, engine  # noqa: F401
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
-
-
-@pytest.fixture(scope="module")
-def engine(capi):
-    e = capi.Engine(0)
-    yield e
-    e.close()
 
 
 @pytest.mark.parametrize("fs,sampled_ms,cfar,keep_grid,launches", [

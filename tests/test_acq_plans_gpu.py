@@ -14,24 +14,13 @@ Inputs are random +-1 (I and Q) codes at one sample per symbol on carriers at th
 import numpy as np
 import pytest
 
+from gpu_fixtures import capi, engine  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
 GRID_TOL = 2e-5
 STAT_TOL = 1e-4
 MARGIN = 1e-3
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
-
-
-@pytest.fixture(scope="module")
-def engine(capi):
-    e = capi.Engine(0)
-    yield e
-    e.close()
 
 
 def _params(n, *, spc=None, cfar=True, keep_grid=False, slots=3, **kw):

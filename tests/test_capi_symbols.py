@@ -32,6 +32,9 @@ def test_struct_layouts_match_header():
     assert ctypes.sizeof(capi.TrkItem) == 40
     assert ctypes.sizeof(capi.AcqResult) == 28
     assert ctypes.sizeof(capi.AcqConf) == 64
+    assert ctypes.sizeof(capi.TrkLoopConf) == 152
+    assert ctypes.sizeof(capi.TrkLoopStatus) == 72
+    assert ctypes.sizeof(capi.TrkDumpRecord) == capi.TRK_DUMP_RECORD_DTYPE.itemsize == 108
 
 
 def test_no_gpu_means_loud_failure_not_fallback():

@@ -8,16 +8,11 @@ import numpy as np
 import pytest
 
 from gnss_synth import make_iq, trk_params_for
+from gpu_fixtures import capi  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 FS, N, NCH, NEP = 25e6, 25000, 32, 1000
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
 
 
 @pytest.fixture(scope="module")

@@ -21,7 +21,6 @@ from gnss_synth import make_iq
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FS = 4_000_000
-E1C_SECONDARY = "0011100000001010110110010"  # GALILEO_E1_C_SECONDARY_CODE, src/core/system_parameters/Galileo_E1.h
 
 
 def base_conf(**over):
@@ -293,7 +292,7 @@ def test_b200_galileo_e1_pilot_veml_matches_reference(reflib, b200lib):
     e1b = bi.code_table(reflib, "E", "1B", prn)
     e1c = bi.code_table(reflib, "E", "1C", prn)
     data = rng.choice([-1.0, 1.0], 300)
-    sec = np.array([1.0 if c == "0" else -1.0 for c in E1C_SECONDARY])
+    sec = np.array([1.0 if c == "0" else -1.0 for c in bi.E1C_SECONDARY])
     fs = FS
     n = int(fs * 1.9)
     delay = 1234

@@ -30,13 +30,6 @@ ATOL = dict(acc_carrier_phase_rad=2e-3, carrier_doppler_hz=1e-3, carrier_doppler
             code_error_filt_chips=1e-5, CN0_SNV_dB_Hz=2e-4, carrier_lock_test=1e-6, aux1=1e-6)
 
 
-def conf_to_capi(capi, c):
-    out = capi.TrkLoopConf()
-    for name, _ in ol.LoopConf._fields_:
-        setattr(out, name, getattr(c, name))
-    return out
-
-
 def assert_records_match(got, want, what=""):
     assert got.dtype == want.dtype and got.shape == want.shape
     for f in EXACT_FIELDS:
@@ -67,7 +60,7 @@ def make_engine_with_loops(capi, oracle, confs, fs, band_samples=None, prns=None
                 code = np.repeat(code, 2)
         ch = e.channel_create(0, taps)
         e.channel_set_code(ch, code, shifts)
-        ids.append(e.loop_create(ch, conf_to_capi(capi, c)))
+        ids.append(e.loop_create(ch, c))
     return e, ids
 
 
@@ -129,7 +122,7 @@ def test_cycle_with_supplied_taps_matches_oracle(oracle):
                 got[i].append(rec[i])
                 want[i].append(r)
     for i, c in enumerate(confs):
-        g, w = np.array(got[i], capi.TRK_DUMP_RECORD_DTYPE), np.array(want[i], ol.DUMP_RECORD_DTYPE)
+        g, w = np.array(got[i], capi.TRK_DUMP_RECORD_DTYPE), np.array(want[i], capi.TRK_DUMP_RECORD_DTYPE)
         assert_records_match(g, w, what=f"conf {i}")
         sd, so = e.loop_status(ids[i]), orc[i].status()
         assert (sd.state, sd.loss_of_lock, sd.sample_counter, sd.epochs) == (so.state, so.loss_of_lock, so.sample_counter, so.epochs), i
@@ -166,7 +159,7 @@ def test_cycle_matches_reference_golden(oracle):
         recs.append(r)
     recs = np.array(recs, capi.TRK_DUMP_RECORD_DTYPE)
     for i, (name, _, _) in enumerate(mg.LOOP_CASES):
-        want = np.frombuffer(gold[f"{name}/records"].tobytes(), ol.DUMP_RECORD_DTYPE)
+        want = np.frombuffer(gold[f"{name}/records"].tobytes(), capi.TRK_DUMP_RECORD_DTYPE)
         assert_records_match(recs[:, i], want, what=name)
     e.close()
 
@@ -355,7 +348,7 @@ def test_streaming_through_a_small_ring_is_identical(oracle):
     for c, sv in zip(confs, svs):
         ch = e.channel_create(0, 3)
         e.channel_set_code(ch, codes[sv["prn"]], [-0.5, 0.0, 0.5])
-        ids.append(e.loop_create(ch, conf_to_capi(capi, c)))
+        ids.append(e.loop_create(ch, c))
     start_all(e, ids)
     got = [[] for _ in ids]
     step = 400_000
@@ -426,12 +419,12 @@ def test_loop_api_rejects_inconsistent_requests(oracle):
     ch_hd = e.channel_create(0, 3)
     e.channel_set_code(ch_hd, code, [-0.5, 0.0, 0.5], high_dyn=True)
     ch_empty = e.channel_create(0, 3)
-    good = conf_to_capi(capi, ol.default_conf())
+    good = ol.default_conf()
     with pytest.raises(capi.B200Error) as ei:
         e.loop_create(ch_empty, good)                      # no code table
     assert ei.value.code == -4
     with pytest.raises(capi.B200Error) as ei:
-        e.loop_create(ch3, conf_to_capi(capi, ol.default_conf(veml=1)))   # five taps wanted, three registered
+        e.loop_create(ch3, ol.default_conf(veml=1))   # five taps wanted, three registered
     assert ei.value.code == -1
     with pytest.raises(capi.B200Error) as ei:
         e.loop_create(ch_hd, good)                          # high-dynamics resampler: not in the device loop
@@ -439,7 +432,7 @@ def test_loop_api_rejects_inconsistent_requests(oracle):
     for bad in (dict(cn0_samples=65), dict(cn0_samples=0), dict(pll_filter_order=4), dict(dll_filter_order=0), dict(slope=0.0),
                 dict(code_period=0.0004)):
         with pytest.raises(capi.B200Error) as ei:
-            e.loop_create(ch3, conf_to_capi(capi, ol.default_conf(**bad)))
+            e.loop_create(ch3, ol.default_conf(**bad))
         assert ei.value.code == -5, bad
     rec, cnt = e.loop_run(5)                                # no loops yet: nothing to do, no error
     assert rec.shape == (0, 5) and cnt.size == 0

@@ -3,7 +3,8 @@
 A loop with a data channel correlates each epoch's item against the data code too, with the pilot's NCO values; its record
 carries the data prompt as prompt_I / prompt_Q (log_data, dll_pll_veml_tracking.cc:1614-1617), every other field comes from
 the pilot taps, and run_prompts hands back the pilot prompt of every record.  The checks follow
-tests/test_loop_correlator_gpu.py (peek -> run(1) -> compare, in mode 0 at both CTA widths, mode 1 and mode 2):
+tests/test_loop_correlator_gpu.py on its rig, tests/loop_rig.py (peek -> run(1) -> compare, in mode 0 at both CTA widths,
+mode 1 and mode 2):
 
   * integer samples with a zero carrier: the data prompt equals the integer oracle of the data table, every abs_* and the
     returned pilot prompt equal the oracle of the pilot taps;
@@ -12,44 +13,16 @@ tests/test_loop_correlator_gpu.py (peek -> run(1) -> compare, in mode 0 at both 
     the pilot prompts the data-carrying run returned (also through a loss of lock);
   * the persistent kernel's taps, data tap in its slot, replayed through b200_trk_loop_step_taps reproduce it byte for byte;
   * a synthetic pilot + data signal: the recorded data prompts carry the transmitted symbols, the pilot prompts do not."""
-import types
-
 import numpy as np
 import pytest
 
-import test_loop_correlator_gpu as tl
-from oracle import loop as ol
+from gpu_fixtures import capi  # noqa: F401
+import loop_rig as tl
 
 pytestmark = pytest.mark.gpu
 
 MODES = list(tl.MODES)
 N_EP = 150
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
-
-
-def data_view(sp, table):
-    """the data correlator as the oracle sees it: one tap at the prompt's shift (0), the loop's stream"""
-    return types.SimpleNamespace(table=np.asarray(table, np.float32), shifts=[0.0], taps=1, stream=sp.stream)
-
-
-def make_engine(capi, specs, data_tables, caps):
-    """tl.make_engine plus a 1-tap data channel for every spec whose data table is not None -> (engine, loop ids, data ids)"""
-    e, ids = tl.make_engine(capi, specs, caps)
-    dids = []
-    for lid, sp, dt in zip(ids, specs, data_tables):
-        if dt is None:
-            dids.append(None)
-            continue
-        dch = e.channel_create(sp.band, 1)
-        e.channel_set_code(dch, dt, [0.0])
-        e.loop_set_data_channel(lid, dch)
-        dids.append(dch)
-    return e, ids, dids
 
 
 def run_per_epoch(e, ids, n_ep, feed=None):
@@ -77,7 +50,7 @@ def check_int_epoch(sp, dt, item, r, pilot, what):
     if dt is None:
         tl.check_int_epoch(sp, item, r, what)
         return
-    want_d = tl.int_taps(data_view(sp, dt), item)[0]
+    want_d = tl.int_taps(tl.data_view(sp, dt), item)[0]
     assert r["prompt_I"] == want_d and r["prompt_Q"] == 0.0, (what, r["prompt_I"], r["prompt_Q"], want_d)
     assert np.array_equal(tl.rec_mags(sp, r), np.abs(want).astype(np.float64)), (what, tl.rec_mags(sp, r), want)
     if sp.taps == 3:
@@ -108,7 +81,7 @@ def int_configs(n_ep):
 
 def run_config(capi, monkeypatch, specs, data, caps, ring, mode, n_ep):
     caps = tl.capacities_for(specs, caps)
-    e, ids, _ = make_engine(capi, specs, data, caps)
+    e, ids, _ = tl.make_engine_with_data(capi, specs, data, caps)
     tl.set_mode(monkeypatch, e, mode)
     if ring:
         feeder = tl.RingFeeder(e, 0, specs[0].stream)
@@ -143,35 +116,11 @@ def test_integer_data_prompt_equals_the_integer_oracle(capi, monkeypatch, config
 # ---------------------------------------------------------------------------------------------------------------------
 # float data: a pilot and a data component on one carrier
 
-FS = tl.FS
-
-
-def pilot_data_spec(prn, data_prn, doppler, delay, n_ep, veml=0, symbols=None, cn0=55.0, pull_in_now=False):
-    """GPS-like pilot (code prn) + data (code data_prn) with the same Doppler and code phase; symbols (+-1, one per code
-    period) modulate the data.  pull_in_now: the acquisition stamp lies a second before the first sample, so the loop
-    leaves its pull-in transitory at once and the PLL (not the FLL alone) steers from the first epoch."""
-    from gnss_synth import make_iq
-    port = tl.ol_port()
-    spc = 2 if veml else 1
-    pilot = np.repeat(port.gps_ca_code(prn), spc)
-    data = np.repeat(port.gps_ca_code(data_prn), spc)
-    n = 4000 * (n_ep + 2) + delay
-    cp = (-delay * spc * tl.CA_RATE / FS) % len(pilot)
-    common = dict(doppler=doppler, code_phase_chips=cp, cn0=cn0, phase0=0.7)
-    iq = make_iq({prn: pilot, data_prn: data}, FS, n, [dict(prn=prn, **common), dict(prn=data_prn, symbols=symbols, **common)],
-                 seed=prn, chips_per_table_chip=spc)
-    kw = dict(veml=1, code_samples_per_chip=2, early_late_space_chips=0.15) if veml else {}
-    base = 4_000_000 if pull_in_now else 0       # 4e6 samples are exactly 1000 code periods: same code phase
-    conf = ol.default_conf(fs_in=FS, prn=prn, pull_in_time_s=0 if pull_in_now else 1, cloop=0, **kw)
-    sp = tl.LoopSpec(0, pilot, conf, (delay + 0.2, doppler - (0.0 if pull_in_now else 6.0), 0, base), tl.Stream(iq, base))
-    return sp, data
-
-
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("veml", [0, 1])
 def test_float_data_prompt_within_the_float64_truth(capi, monkeypatch, veml, mode):
-    sp, dt = pilot_data_spec(5, 25, 1234.0 if not veml else -2710.0, 1777, N_EP, veml=veml)
-    e, ids, _ = make_engine(capi, [sp], [dt], {0: len(sp.stream.x) + 16})
+    sp, dt = tl.pilot_data_spec(5, 25, 1234.0 if not veml else -2710.0, 1777, N_EP, veml=veml)
+    e, ids, _ = tl.make_engine_with_data(capi, [sp], [dt], {0: len(sp.stream.x) + 16})
     tl.set_mode(monkeypatch, e, mode)
     tl.push_all(e, [sp])
     tl.start_all(e, ids, [sp])
@@ -180,7 +129,7 @@ def test_float_data_prompt_within_the_float64_truth(capi, monkeypatch, veml, mod
     assert len(recs) == N_EP and np.all(items["phase_step_rad"] != 0.0)
     p = sp.taps // 2
     for k in range(N_EP):
-        truth_d = tl.f64_taps(data_view(sp, dt), items[k])[0]
+        truth_d = tl.f64_taps(tl.data_view(sp, dt), items[k])[0]
         got = complex(float(recs[k]["prompt_I"]), float(recs[k]["prompt_Q"]))
         assert abs(got - truth_d) <= tl.TRUTH_RTOL * abs(truth_d), (mode, k, got, truth_d)
         truth = tl.f64_taps(sp, items[k])
@@ -195,7 +144,7 @@ def twin_configs():
     port = tl.ol_port()
     lost = tl.lock_loss_case(rng)
     gal = tl.int_configs(N_EP)["galileo_like"][0][0]
-    sp, dt = pilot_data_spec(14, 29, 2222.0, 909, 300)
+    sp, dt = tl.pilot_data_spec(14, 29, 2222.0, 909, 300)
     return {
         "gps_float_3taps": (sp, dt, 300),
         "veml_sinboc_int": (gal, port.sinboc11((2 * rng.integers(0, 2, 4092) - 1).astype(np.int32)), N_EP),
@@ -213,7 +162,7 @@ def test_a_data_channel_changes_nothing_but_the_record_prompt(capi, monkeypatch,
     caps = {0: len(sp.stream.x) + 16}
     out = []
     for data in ([dt], [None]):
-        e, ids, _ = make_engine(capi, [sp], data, caps)
+        e, ids, _ = tl.make_engine_with_data(capi, [sp], data, caps)
         tl.set_mode(monkeypatch, e, mode)
         tl.push_all(e, [sp])
         tl.start_all(e, ids, [sp])
@@ -243,7 +192,7 @@ def test_persistent_taps_replay_through_step_taps(capi, monkeypatch, config, mod
     slot after the pilot taps, fed to the sequential update of a twin reproduce every item, record and the final status"""
     sp, dt, n_ep = twin_configs()[config]
     caps = {0: len(sp.stream.x) + 16}
-    e, ids, _ = make_engine(capi, [sp], [dt], caps)
+    e, ids, _ = tl.make_engine_with_data(capi, [sp], [dt], caps)
     tl.set_mode(monkeypatch, e, mode)
     tl.push_all(e, [sp])
     tl.start_all(e, ids, [sp])
@@ -253,7 +202,7 @@ def test_persistent_taps_replay_through_step_taps(capi, monkeypatch, config, mod
     lost = config == "gps_int_lock_loss"
     assert (st.state == 0 and st.loss_of_lock == 1) if lost else len(recs) == n_ep
 
-    t, tids, _ = make_engine(capi, [sp], [dt], caps)
+    t, tids, _ = tl.make_engine_with_data(capi, [sp], [dt], caps)
     tl.push_all(t, [sp])
     tl.start_all(t, tids, [sp])
     for k in range(len(recs)):
@@ -285,8 +234,8 @@ def test_data_prompts_carry_the_symbols(capi, monkeypatch, mode):
     n_ep, settle = 400, 100
     rng = np.random.default_rng(3)
     sym = (2 * rng.integers(0, 2, n_ep + 8) - 1).astype(np.float64)
-    sp, dt = pilot_data_spec(7, 22, 1500.0, 1234, n_ep, symbols=sym, cn0=50.0, pull_in_now=True)
-    e, ids, _ = make_engine(capi, [sp], [dt], {0: len(sp.stream.x) + 16})
+    sp, dt = tl.pilot_data_spec(7, 22, 1500.0, 1234, n_ep, symbols=sym, cn0=50.0, pull_in_now=True)
+    e, ids, _ = tl.make_engine_with_data(capi, [sp], [dt], {0: len(sp.stream.x) + 16})
     tl.set_mode(monkeypatch, e, mode)
     tl.push_all(e, [sp])
     tl.start_all(e, ids, [sp])
@@ -297,8 +246,8 @@ def test_data_prompts_carry_the_symbols(capi, monkeypatch, mode):
     # the code period each record integrated over, as make_iq numbers them: the one under the middle of the epoch, which
     # ends about at PRN_start_sample_count
     mid = r["PRN_start_sample_count"].astype(np.float64) - sp.stream.x0 - 2000.0
-    rate = tl.CA_RATE * (1.0 + 1500.0 / 1575.42e6) / FS
-    cp = (-1234 * tl.CA_RATE / FS) % 1023
+    rate = tl.CA_RATE * (1.0 + 1500.0 / 1575.42e6) / tl.FS
+    cp = (-1234 * tl.CA_RATE / tl.FS) % 1023
     period = np.floor((cp + mid * rate) / 1023).astype(np.int64)
     want = sym[period % len(sym)]
     got = np.sign(r["prompt_I"])
@@ -347,7 +296,7 @@ def test_replacing_the_data_channel_between_runs(capi, monkeypatch, mode):
     sp = tl.gps_int_case(rng, 2 * n_ep)
     port = tl.ol_port()
     tables = [port.gps_ca_code(11), port.gps_ca_code(12)]
-    e, ids, dids = make_engine(capi, [sp], [tables[0]], {0: len(sp.stream.x) + 16})
+    e, ids, dids = tl.make_engine_with_data(capi, [sp], [tables[0]], {0: len(sp.stream.x) + 16})
     second = e.channel_create(0, 1)
     e.channel_set_code(second, tables[1], [0.0])
     tl.set_mode(monkeypatch, e, mode)

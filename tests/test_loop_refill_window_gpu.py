@@ -2,20 +2,16 @@
 
 b200_iq_refill with fewer samples than the attached buffer holds moves write_index to first_index + n; the buffer's slots
 past it still hold the previous fill.  A loop must track the refilled samples exactly and stall where they end, never
-correlating what the buffer held before.  Helpers and configurations are those of test_loop_correlator_gpu.py."""
+correlating what the buffer held before.  Helpers and configurations are those of test_loop_correlator_gpu.py, from
+tests/loop_rig.py."""
 import numpy as np
 import pytest
 
-import test_loop_correlator_gpu as tl
+from gpu_fixtures import capi  # noqa: F401
+import loop_rig as tl
 from oracle import loop as ol
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
 
 
 @pytest.mark.parametrize("mode", list(tl.MODES))

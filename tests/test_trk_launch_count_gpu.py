@@ -8,18 +8,12 @@ count: a loop with a data channel has 3- or 5-tap pilot items and 1-tap data ite
 import numpy as np
 import pytest
 
-import test_loop_correlator_gpu as tl
-import test_loop_pilot_data_gpu as pd
+from gpu_fixtures import capi  # noqa: F401
+import loop_rig as tl
 
 pytestmark = pytest.mark.gpu
 
 N = 4000
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
 
 
 def batch_engine(capi, taps_list):
@@ -93,8 +87,8 @@ def test_single_correlators_count_one_launch_each(capi):
 ])
 def test_loop_run_counts_its_launches(capi, monkeypatch, mode, with_data, launches):
     n_ep = 5
-    sp, dt = pd.pilot_data_spec(5, 25, 1234.0, 1777, n_ep)
-    e, ids, _ = pd.make_engine(capi, [sp], [dt if with_data else None], {0: len(sp.stream.x) + 16})
+    sp, dt = tl.pilot_data_spec(5, 25, 1234.0, 1777, n_ep)
+    e, ids, _ = tl.make_engine_with_data(capi, [sp], [dt if with_data else None], {0: len(sp.stream.x) + 16})
     tl.set_mode(monkeypatch, e, mode)
     tl.push_all(e, [sp])
     tl.start_all(e, ids, [sp])
@@ -109,8 +103,8 @@ def test_loop_mode_only_through_the_api(capi, monkeypatch):
     one launch per run (mode 1 would issue 1 + 2 per epoch)."""
     n_ep = 5
     monkeypatch.setenv("B200_LOOP_MODE", "1")
-    sp, _ = pd.pilot_data_spec(5, 25, 1234.0, 1777, n_ep)
-    e, ids, _ = pd.make_engine(capi, [sp], [None], {0: len(sp.stream.x) + 16})
+    sp, _ = tl.pilot_data_spec(5, 25, 1234.0, 1777, n_ep)
+    e, ids, _ = tl.make_engine_with_data(capi, [sp], [None], {0: len(sp.stream.x) + 16})
     tl.push_all(e, [sp])
     tl.start_all(e, ids, [sp])
     k0 = e.launch_count()

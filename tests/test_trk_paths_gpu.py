@@ -28,6 +28,8 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from gnss_synth import make_iq, trk_params_for  # noqa: E402
+from gpu_fixtures import capi  # noqa: E402,F401
+from trk_ref import int_code, int_oracle  # noqa: E402
 
 RING = 1 << 18          # ring bands of the per-item tests: 262 144 samples ...
 WRAP_AT = 60000         # ... whose end falls between data samples WRAP_AT - 1 and WRAP_AT
@@ -53,26 +55,9 @@ def _report_worst():
 
 
 @pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
-
-
-@pytest.fixture(scope="module")
 def torch():
     import torch as t
     return t
-
-
-def int_oracle(x_int, code_int, idx):
-    """exact integer correlation given chip indices (taps x n)."""
-    return np.array([np.sum(x_int * code_int[idx[t]]) for t in range(idx.shape[0])], dtype=np.int64)
-
-
-def _int_code(L, salt):
-    c = ((np.arange(L) * (7919 + 2 * salt)) % 31) - 15
-    c[c == 0] = 16
-    return c
 
 
 def _shifts(taps, spread):
@@ -189,7 +174,7 @@ def test_every_per_item_path_at_every_tap_count(capi, torch, oracle, taps):
     near = _shifts(taps, 0.6)
     carrier = (1.1, 0.2 + 0.013 * taps, 0.0)
     small = Rig(capi, oracle, 100 + taps)
-    code = _int_code(1023, taps)
+    code = int_code(1023, taps, nonzero=True)
     small.add("fast", code, near, 25000, 1000, 0.37, ST25, carrier=carrier)
     small.add("fast, ring wrap, even start", code, near, 25000, WRAP_AT - 10000, -0.81, ST25, carrier=carrier)
     small.add("fast, ring wrap, odd start", code, near, 25001, WRAP_AT - 9999, 1.93, ST25, carrier=carrier)
@@ -202,7 +187,7 @@ def test_every_per_item_path_at_every_tap_count(capi, torch, oracle, taps):
     small.add("high dynamics, smem", code, _shifts(taps, 0.5), 100000, 9000, 0.37, 0.04092, hd=True, rate=3e-12,
               carrier=(0.7, 1.1e-3, 2e-9))
     big = Rig(capi, oracle, 200 + taps)
-    code_b = _int_code(60000, taps)
+    code_b = int_code(60000, taps, nonzero=True)
     big.add("modulo, gmem", code_b, near, 100000, 1000, 0.37, 0.7, carrier=carrier)
     big.add("high dynamics, gmem", code_b, _shifts(taps, 0.5), 70001, 2001, 0.37, 0.7, hd=True, rate=1e-11,
             carrier=(0.7, -1.3e-3, -3e-9))
@@ -223,7 +208,7 @@ def test_single_correlator_six_and_seven_taps_integer_exact(capi, oracle, n, L, 
     rng = np.random.default_rng(n + L)
     x_int = rng.integers(-7, 8, n)
     x_int[x_int == 0] = 1
-    code_int = _int_code(L, 0)
+    code_int = int_code(L, 0, nonzero=True)
     _, idx = oracle.port.resampler(1, code_int.astype(np.float32), rem, step, shifts, n, return_idx=True)
     e = capi.Engine(0)
     mc = capi.Multicorrelator(e, n, len(shifts))
@@ -242,7 +227,7 @@ def test_edge_lengths_at_every_tap_count(capi, torch, oracle, taps):
     """No main tile (n < 512 + head), one tile plus remainder, the tails of the generic association and the ends of the
     16-tile re-seed groups, at both sample parities; an empty epoch gives zeros."""
     rig = Rig(capi, oracle, 300 + taps)
-    code = _int_code(1023, taps + 8)
+    code = int_code(1023, taps + 8, nonzero=True)
     shifts = _shifts(taps, 0.5)
     for n in EDGE_NS:
         for parity in (0, 1):
@@ -261,7 +246,7 @@ def test_slices_at_every_tap_count(capi, torch, oracle, taps):
     slices than tiles (64 over 7), the modulo and high-dynamics paths.  Integer items stay exact, float items stay within
     2e-5 of the one-slice result and of the truth, and three launches give the same bits."""
     rig = Rig(capi, oracle, 400 + taps)
-    code = _int_code(1023, taps + 16)
+    code = int_code(1023, taps + 16, nonzero=True)
     shifts = _shifts(taps, 0.5)
     rig.add("48 tiles", code, shifts, 25000, 1000, 0.2, ST25)
     rig.add("7 tiles", code, shifts, 7 * 512 + 5, 30000, 0.7, ST25 * 2)
@@ -295,7 +280,7 @@ def test_mixed_tap_counts_with_slices(capi, torch, oracle, slices):
     its own reference, and the columns past its taps must stay untouched."""
     rig = Rig(capi, oracle, 500 + slices)
     for taps in (1, 2, 5, 8):
-        code = _int_code(1023 if taps != 5 else 2046, taps + 24)
+        code = int_code(1023 if taps != 5 else 2046, taps + 24, nonzero=True)
         shifts = _shifts(taps, 0.6)
         rig.add(f"{taps} taps", code, shifts, 25000 + taps, 1000 * taps, 0.3, ST25)
         rig.add(f"{taps} taps, ring wrap", code, shifts, 9000 + taps, WRAP_AT - 3001, -1.3, ST25)
@@ -409,7 +394,7 @@ def test_shared_kernel_paths_integer_exact(capi, torch, oracle, taps):
     pos = 1
     for b, (path, L, n, step, rem0, sp) in enumerate(blocks):
         for j in range(8):
-            code = _int_code(L, 8 * b + j)
+            code = int_code(L, 8 * b + j, nonzero=True)
             cid = e.channel_create(0, taps)
             e.channel_set_code(cid, code.astype(np.float32), shifts)
             s0 = pos + j * sp
@@ -453,7 +438,7 @@ def test_shared_kernel_linear_band_to_its_last_sample(capi, torch, oracle, total
         for j in range(8):
             n = ns[j]
             s0 = total - n - gap * max(6 - j, 0)   # items 6 and 7 end at the band's last sample
-            code = _int_code(1023, 8 * g + j)
+            code = int_code(1023, 8 * g + j, nonzero=True)
             cid = e.channel_create(0, 3)
             e.channel_set_code(cid, code.astype(np.float32), shifts)
             rem = float(np.float32(rng.uniform(-3, 3)))

@@ -2,27 +2,21 @@
 contiguous 16-sample chunk and splits it at the one exact chip boundary per tap.  All through the C ABI with the shared
 kernel forced on.  Integer samples and codes with a zero carrier keep every sum exact, so these runs must EQUAL the
 integer oracle built from the reference's chip indices; float data stays within the bounds of test_trk_gpu.py."""
-import os
-
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
 
+from gnss_sdr_b200.build import LIB, build_variant  # noqa: E402
 from gnss_synth import make_iq, trk_params_for  # noqa: E402
-from test_trk_gpu import _ref_or_port_avx, int_oracle  # noqa: E402
-import test_ring_stress_gpu as ring  # noqa: E402
+from gpu_fixtures import capi  # noqa: E402,F401
+from ring_worker import run_worker  # noqa: E402
+from trk_ref import int_oracle, ref_or_port_avx  # noqa: E402
 
 SHIFTS = [-0.5, 0.0, 0.5]
 CA_16368 = 1023.0 / 16368
 CA_25 = 1.023e6 * (1 + 3000 / 1575.42e6) / 25e6
 CA_50 = 1.023e6 * (1 - 4500 / 1575.42e6) / 50e6
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import gnss_sdr_b200.capi as c
-    return c
 
 
 def run_shared(capi, x_int, chans, epochs, filler=0, capacity=None):
@@ -168,7 +162,7 @@ def test_float_signal_full_epochs_within_bounds(capi, oracle):
         seg = iq[int(it["sample_index"]) - first: int(it["sample_index"]) - first + n]
         a = (float(it["rem_carrier_phase_rad"]), float(it["phase_step_rad"]), float(it["rem_code_phase_chips"]),
              float(it["code_phase_step_chips"]))
-        want = _ref_or_port_avx(oracle, seg, codes[sv["prn"]], SHIFTS, *a)
+        want = ref_or_port_avx(oracle, seg, codes[sv["prn"]], SHIFTS, *a)
         truth = oracle.port.multicorrelator_f64(1, seg, codes[sv["prn"]], SHIFTS, *a)
         assert np.abs(truth[1]) > 3 * np.sqrt(n)
         worst_ref = max(worst_ref, float(np.max(np.abs(got[i] - want) / np.abs(want))))
@@ -177,17 +171,13 @@ def test_float_signal_full_epochs_within_bounds(capi, oracle):
     assert worst_truth < 1e-5
 
 
-# test_ring_stress_gpu.py's worker at a C2-like step (its own step, about 0.17, runs warp_tile only)
-CHUNK_WORKER = ring.WORKER.replace("step = 1023.0 / n *", "step = 1.023e6 / 25e6 *")
-
-
 @pytest.mark.parametrize("stages", [2, 4, 8])
-def test_ring_under_injected_delays_chunk_path(stages, tmp_path, monkeypatch):
+def test_ring_under_injected_delays_chunk_path(stages):
     """The -DSH_STRESS=1 builds (delays injected into producer and consumers) at a chunk-path step: 500 launches bitwise
-    stable and equal to the production build on integer-exact inputs."""
-    assert CHUNK_WORKER != ring.WORKER
-    monkeypatch.setattr(ring, "WORKER", CHUNK_WORKER)
-    prod = ring.run_worker(os.path.join(ring.ROOT, "gnss_sdr_b200", "libb200gnss.so"), 3, tmp_path)
-    got = ring.run_worker(ring.build_variant(stages, stress=True), 500, tmp_path)
+    stable and equal to the production build on integer-exact inputs.  test_ring_stress_gpu.py runs the same worker at
+    its own step (about 0.17, warp_tile only); this one at a C2-like step, 25 Msps."""
+    step = 1.023e6 / 25e6
+    prod = run_worker(LIB, 3, step)
+    got = run_worker(build_variant(stages, stress=True), 500, step)
     assert got["bad"] == 0, got
     assert got["sha"] == prod["sha"], (got, prod)

@@ -11,8 +11,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import blocks_itf as bi  # noqa: E402
 from gnss_synth import make_iq  # noqa: E402
-from oracle.loop import DUMP_RECORD_DTYPE  # noqa: E402
-import test_integration_blocks as tib  # noqa: E402
+from gnss_sdr_b200.abi import TRK_DUMP_RECORD_DTYPE  # noqa: E402
 
 
 def run(which, coalesce):
@@ -23,7 +22,7 @@ def run(which, coalesce):
         e1b = bi.code_table(reflib, "E", "1B", prn)
         e1c = bi.code_table(reflib, "E", "1C", prn)
         data = rng.choice([-1.0, 1.0], 300)
-        sec = np.array([1.0 if c == "0" else -1.0 for c in tib.E1C_SECONDARY])
+        sec = np.array([1.0 if c == "0" else -1.0 for c in bi.E1C_SECONDARY])
         n, delay = int(fs * 1.9), 1234
         cp = (-delay * 2 * 1.023e6 / fs) % 8184
         svs = [dict(prn="b", doppler=-850.0, code_phase_chips=cp, cn0=43.0, symbols=data, periods_per_symbol=1),
@@ -68,7 +67,7 @@ def run(which, coalesce):
         print(name, "outputs", len(out), "events", ch.events("trk"))
         ch.close()
         fn = os.path.join(tmp, name + "_0.dat")
-        dumps[name] = np.fromfile(fn, DUMP_RECORD_DTYPE)
+        dumps[name] = np.fromfile(fn, TRK_DUMP_RECORD_DTYPE)
     r, g = dumps["ref"], dumps["b200"]
     print(which, "coalesce", coalesce, "records", len(r), len(g))
     m = min(len(r), len(g))

@@ -8,7 +8,7 @@ Each loop: 8184-entry sinBOC(1,1) pilot table, VEML taps, 4 ms epochs of 16 000 
 kernel) at both CTA widths (B200_LOOP_WIDTH = 256 | 512).  The samples are noise: the lock detectors are switched off so
 that every loop runs every epoch.
 
---baseline DIR: a checkout of another version with its library built.  Each round then runs both libraries, one after
+--baseline DIR: a checkout of another version with its library and oracle built.  Each round then runs both libraries, one after
 the other, each in a fresh process; the baseline's legs without a data channel are timed if it has no
 b200_trk_loop_set_data_channel.  One JSON line per measurement, and the card's name, power limit and SM clocks first."""
 from __future__ import annotations
@@ -28,11 +28,11 @@ REPEATS = 5
 
 def child(root: str, label: str):
     sys.path.insert(0, ROOT)
+    sys.path.insert(0, root)   # the library under test, its binding and its oracle: this tree's or the baseline's
     import numpy as np
+    import gnss_sdr_b200.capi as capi
     from oracle import loop as ol
     import oracle
-    sys.path.insert(0, root)   # the library under test: this tree's or the baseline's
-    import gnss_sdr_b200.capi as capi
 
     has_data = hasattr(capi.lib, "b200_trk_loop_set_data_channel")
     rng = np.random.default_rng(1)
@@ -53,10 +53,7 @@ def child(root: str, label: str):
                     conf = ol.default_conf(fs_in=fs, prn=j + 1, code_length_chips=4092, code_period=0.004, vector_length=n_ep_samples,
                                            code_samples_per_chip=2, veml=1, early_late_space_chips=0.15, cn0_min=-1000,
                                            max_code_lock_fail=1 << 30, max_carrier_lock_fail=1 << 30, cloop=0)
-                    cc = capi.TrkLoopConf()
-                    for name, _ in ol.LoopConf._fields_:
-                        setattr(cc, name, getattr(conf, name))
-                    lid = e.loop_create(ch, cc)
+                    lid = e.loop_create(ch, capi.TrkLoopConf.from_buffer_copy(conf))   # an older tree's oracle has its own class
                     if data:
                         dch = e.channel_create(0, 1)
                         e.channel_set_code(dch, tables[2 * j + 1], [0.0])

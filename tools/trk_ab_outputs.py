@@ -151,21 +151,13 @@ def main(out_path):
     e.close()
 
     # ---- device loops
-    import test_loop_correlator_gpu as tl
-    import test_loop_pilot_data_gpu as pd
-
-    class Env:  # the monkeypatch the loop helpers take
-        def setenv(self, k, v):
-            os.environ[k] = v
-
-        def delenv(self, k, raising=True):
-            os.environ.pop(k, None)
+    import loop_rig as tl
 
     for mode in tl.MODES:
         for with_data in (False, True):
-            sp, dt = pd.pilot_data_spec(5, 25, 1234.0, 1777, 60)
-            e, ids, _ = pd.make_engine(capi, [sp], [dt if with_data else None], {0: len(sp.stream.x) + 16})
-            tl.set_mode(Env(), e, mode)
+            sp, dt = tl.pilot_data_spec(5, 25, 1234.0, 1777, 60)
+            e, ids, _ = tl.make_engine_with_data(capi, [sp], [dt if with_data else None], {0: len(sp.stream.x) + 16})
+            tl.set_mode(None, e, mode)
             tl.push_all(e, [sp])
             tl.start_all(e, ids, [sp])
             rec, cnt, prm = e.loop_run_prompts(60)
