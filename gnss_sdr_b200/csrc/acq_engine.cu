@@ -79,80 +79,6 @@ struct b200_acq
 
 namespace
 {
-int bluestein_search(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev,
-    int step_two, float prev_input_power, uint64_t& launched);
-
-int mixed_radix_search(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
-    b200_acq_result* results_dev, int step_two, float prev_input_power, uint64_t& launched)
-{
-    const b200_acq_conf& c = a->c;
-    cudaStream_t st = a->stream;
-    bool same = a->slots_on_device.size() == n_slots;
-    for (uint32_t i = 0; same && i < n_slots; i++) same = a->slots_on_device[i] == static_cast<int>(slots[i]);
-    if (!same)
-        {
-            // slot_pin is read by the asynchronous copy: wait for a previous upload's reader before rewriting it
-            B200_CUDA_TRY(cudaStreamSynchronize(st));
-            for (uint32_t i = 0; i < n_slots; i++) a->slot_pin[i] = static_cast<int>(slots[i]);
-            B200_CUDA_TRY(cudaMemcpyAsync(a->slot_list, a->slot_pin, sizeof(int) * n_slots, cudaMemcpyHostToDevice, st));
-            a->slots_on_device.assign(a->slot_pin.get(), a->slot_pin.get() + n_slots);
-        }
-    const int bins = step_two ? static_cast<int>(a->bins2) : static_cast<int>(c.num_doppler_bins);
-    const float2* wipe = step_two ? a->wipe2 : a->wipe;
-    const int ne = static_cast<int>(c.effective_fft_size);
-    const int off = c.bit_transition_flag ? ne : 0;
-    int rc = acq_launch_fwd(in, static_cast<int>(c.consumed_samples), wipe, a->X, bins, a->plan, a->tw, launched, st);
-    if (rc) return rc;
-    rc = acq_launch_row_stats(a->X, a->codes, a->slot_list, static_cast<int>(n_slots), bins, a->plan, a->tw, off, ne, a->grid,
-        dwell_counter > 1 ? 1 : 0, a->rowstat, a->Z, a->partial, launched, st);
-    if (rc) return rc;
-    rc = acq_launch_stats(a->rowstat, static_cast<int>(n_slots), bins, ne, c.doppler_max, a->doppler_center, c.doppler_step,
-        dwell_counter, c.use_cfar, a->best, results_dev, step_two, a->center2, a->step2, prev_input_power, launched, st);
-    if (rc) return rc;
-    if (c.use_cfar) return B200_OK;
-    rc = acq_launch_second_peak(a->X, a->codes, a->slot_list, static_cast<int>(n_slots), bins, a->plan, a->tw, off, ne, a->grid, a->best,
-        static_cast<int>(c.samples_per_chip), a->second_peak, a->Z, a->partial, launched, st);
-    if (rc) return rc;
-    return acq_launch_finish_second_peak(a->second_peak, static_cast<int>(n_slots), results_dev, launched, st);
-}
-
-int search_impl(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
-    b200_acq_result* results_dev, int step_two = 0, float prev_input_power = 0.f)
-{
-    const b200_acq_conf& c = a->c;
-    if (n_slots == 0) return B200_OK;
-    if (n_slots > c.n_code_slots || !slots) return B200_ERR_ARG;
-    if (dwell_counter < 1) dwell_counter = 1;
-    if (dwell_counter > 1 && !a->grid)
-        {
-            set_error("dwell_counter %u needs the magnitude grid (create with max_dwells > 1 or keep_grid)", dwell_counter);
-            return B200_ERR_STATE;
-        }
-    for (uint32_t i = 0; i < n_slots; i++)
-        {
-            if (slots[i] >= c.n_code_slots || !a->slot_set[slots[i]])
-                {
-                    set_error("slot %u has no local code", slots[i]);
-                    return B200_ERR_STATE;
-                }
-        }
-    const float2* rows2 = a->bl ? a->bl->mult2.get() : a->wipe2.get();  // the step-two rows b200_acq_set_step_two built
-    if (step_two && (a->bins2 == 0 || !rows2 || n_slots != 1))
-        {
-            set_error("step two needs b200_acq_set_step_two first and exactly one slot");
-            return B200_ERR_STATE;
-        }
-    uint64_t launched = 0;
-    const int rc = a->bl ? bluestein_search(a, in, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power, launched)
-                         : mixed_radix_search(a, in, slots, n_slots, dwell_counter, results_dev, step_two, prev_input_power, launched);
-    if (rc) return rc;
-    a->e->launches += launched;
-    return B200_OK;
-}
-}  // namespace
-
-namespace
-{
 // smallest M >= 2N - 1 that the two-level planner accepts
 int bluestein_size(int n, FftPlan* pl)
 {
@@ -167,12 +93,21 @@ int bluestein_size(int n, FftPlan* pl)
     return 0;
 }
 
-int bluestein_refresh_mult(b200_acq* a)
+// The Doppler rows a search multiplies its input by: the wipe-off rows (wipe, or wipe2 for step two) from the object's
+// Doppler settings, and on a chirp-z object their chirped copy, mult[d][i] = wipe[d][i] * conj(w[i]) (mult2 from wipe2):
+// the wipe-off grid keeps the reference's float32 sincos values, the chirp is extra.  The chirped copy reads chirp_conj,
+// so it needs bluestein_setup first.
+int build_rows(b200_acq* a, bool step_two)
 {
-    // mult[d][i] = wipe[d][i] * conj(w[i]): the wipe-off grid keeps the reference's float32 sincos values, the chirp is extra
-    b200_acq::Bluestein* b = a->bl.get();
-    const int n = static_cast<int>(a->c.fft_size);
-    return acq_launch_rows_times_vector(a->wipe, n, b->chirp_conj, n, 0, b->mult, n, static_cast<int>(a->c.num_doppler_bins), a->stream);
+    const b200_acq_conf& c = a->c;
+    const int n = static_cast<int>(c.fft_size);
+    const int bins = step_two ? static_cast<int>(a->bins2) : static_cast<int>(c.num_doppler_bins);
+    float2* wipe = step_two ? a->wipe2 : a->wipe;
+    const int rc = step_two ? acq_launch_wipeoff(wipe, n, bins, 0, 0, 0, a->doppler_bias, c.fs_in, 1, a->center2, a->step2, a->stream)
+                            : acq_launch_wipeoff(wipe, n, bins, c.doppler_max, a->doppler_center, c.doppler_step, a->doppler_bias, c.fs_in,
+                                  0, 0.f, 0.f, a->stream);
+    if (rc || !a->bl) return rc;
+    return acq_launch_rows_times_vector(wipe, n, a->bl->chirp_conj, n, 0, step_two ? a->bl->mult2 : a->bl->mult, n, bins, a->stream);
 }
 
 int bluestein_setup_queue(b200_acq* a, std::vector<float2> (&host)[6]);
@@ -273,34 +208,102 @@ int bluestein_forward_rows(b200_acq* a, AcqInput in, size_t in_stride, int consu
         a->stream);
 }
 
-int bluestein_search(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, b200_acq_result* results_dev,
-    int step_two, float prev_input_power, uint64_t& launched)
+// One sweep over n_slots code slots on the samples `in`, records into results_dev; launches counted on success only
+int search_impl(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
+    b200_acq_result* results_dev, int step_two = 0, float prev_input_power = 0.f)
 {
-    b200_acq::Bluestein* b = a->bl.get();
     const b200_acq_conf& c = a->c;
-    const int n = static_cast<int>(c.fft_size);
-    const int bins = step_two ? static_cast<int>(a->bins2) : static_cast<int>(c.num_doppler_bins);
-    const float2* mult = step_two ? b->mult2 : b->mult;
-    const int ne = static_cast<int>(c.effective_fft_size);
-    const int off = c.bit_transition_flag ? ne : 0;
-    // X_d = DFT_N(x . wipe_d) for every Doppler bin, once per sweep (x: the consumed samples, zero-padded to N)
-    int rc = bluestein_forward_rows(a, in, 0, static_cast<int>(c.consumed_samples), mult, n, bins, b->Xs, launched);
-    if (rc) return rc;
+    if (n_slots == 0) return B200_OK;
+    if (n_slots > c.n_code_slots || !slots) return B200_ERR_ARG;
+    if (dwell_counter < 1) dwell_counter = 1;
+    if (dwell_counter > 1 && !a->grid)
+        {
+            set_error("dwell_counter %u needs the magnitude grid (create with max_dwells > 1 or keep_grid)", dwell_counter);
+            return B200_ERR_STATE;
+        }
     for (uint32_t i = 0; i < n_slots; i++)
         {
-            // rows of this PRN: y = IDFT_N(X_d . C) = w . IFFT_M(FFT_M(pad(X_d . C . w)) . FFT_M(conj h)) / M ; |w| = 1
-            rc = acq_launch_fwd_rows(AcqInput::linear(b->Xs), n, n, b->CW + static_cast<size_t>(slots[i]) * n, 0, b->A, bins, b->plM, b->twM, launched, a->stream);
+            if (slots[i] >= c.n_code_slots || !a->slot_set[slots[i]])
+                {
+                    set_error("slot %u has no local code", slots[i]);
+                    return B200_ERR_STATE;
+                }
+        }
+    b200_acq::Bluestein* b = a->bl.get();
+    const float2* rows = b ? (step_two ? b->mult2 : b->mult) : (step_two ? a->wipe2 : a->wipe);  // what build_rows built
+    if (step_two && (a->bins2 == 0 || !rows || n_slots != 1))
+        {
+            set_error("step two needs b200_acq_set_step_two first and exactly one slot");
+            return B200_ERR_STATE;
+        }
+    const int bins = step_two ? static_cast<int>(a->bins2) : static_cast<int>(c.num_doppler_bins);
+    const int ne = static_cast<int>(c.effective_fft_size);
+    const int off = c.bit_transition_flag ? ne : 0;
+    const int accumulate = dwell_counter > 1 ? 1 : 0;
+    cudaStream_t st = a->stream;
+    uint64_t launched = 0;
+    int rc;
+    if (b)
+        {
+            // X_d = DFT_N(x . wipe_d) for every Doppler bin, once per sweep (x: the consumed samples, zero-padded to N)
+            const int n = static_cast<int>(c.fft_size);
+            rc = bluestein_forward_rows(a, in, 0, static_cast<int>(c.consumed_samples), rows, n, bins, b->Xs, launched);
             if (rc) return rc;
-            // the correlation kernel addresses the grid by code-slot id, and the "code" here is filter slot 1; the grid rows are
-            // [off, off + ne) of y, so slot s lands where the mixed-radix search puts it: (s * bins + bin) * ne
-            float* grid = a->grid ? a->grid + (static_cast<ptrdiff_t>(slots[i]) - 1) * static_cast<ptrdiff_t>(bins) * ne : nullptr;
-            rc = acq_launch_row_stats(b->A, b->filt, b->slot_ids + 1, 1, bins, b->plM, b->twM, off, ne, grid, dwell_counter > 1 ? 1 : 0,
-                a->rowstat + static_cast<size_t>(i) * bins, b->Zw, b->partial, launched, a->stream);
+            for (uint32_t i = 0; i < n_slots; i++)
+                {
+                    // rows of this PRN: y = IDFT_N(X_d . C) = w . IFFT_M(FFT_M(pad(X_d . C . w)) . FFT_M(conj h)) / M ; |w| = 1
+                    rc = acq_launch_fwd_rows(AcqInput::linear(b->Xs), n, n, b->CW + static_cast<size_t>(slots[i]) * n, 0, b->A, bins, b->plM, b->twM, launched, st);
+                    if (rc) return rc;
+                    // the correlation kernel addresses the grid by code-slot id, and the "code" here is filter slot 1; the grid rows are
+                    // [off, off + ne) of y, so slot s lands where the mixed-radix search puts it: (s * bins + bin) * ne
+                    float* grid = a->grid ? a->grid + (static_cast<ptrdiff_t>(slots[i]) - 1) * static_cast<ptrdiff_t>(bins) * ne : nullptr;
+                    rc = acq_launch_row_stats(b->A, b->filt, b->slot_ids + 1, 1, bins, b->plM, b->twM, off, ne, grid, accumulate,
+                        a->rowstat + static_cast<size_t>(i) * bins, b->Zw, b->partial, launched, st);
+                    if (rc) return rc;
+                }
+        }
+    else
+        {
+            bool same = a->slots_on_device.size() == n_slots;
+            for (uint32_t i = 0; same && i < n_slots; i++) same = a->slots_on_device[i] == static_cast<int>(slots[i]);
+            if (!same)
+                {
+                    // slot_pin is read by the asynchronous copy: wait for a previous upload's reader before rewriting it
+                    B200_CUDA_TRY(cudaStreamSynchronize(st));
+                    for (uint32_t i = 0; i < n_slots; i++) a->slot_pin[i] = static_cast<int>(slots[i]);
+                    B200_CUDA_TRY(cudaMemcpyAsync(a->slot_list, a->slot_pin, sizeof(int) * n_slots, cudaMemcpyHostToDevice, st));
+                    a->slots_on_device.assign(a->slot_pin.get(), a->slot_pin.get() + n_slots);
+                }
+            rc = acq_launch_fwd(in, static_cast<int>(c.consumed_samples), rows, a->X, bins, a->plan, a->tw, launched, st);
+            if (rc) return rc;
+            rc = acq_launch_row_stats(a->X, a->codes, a->slot_list, static_cast<int>(n_slots), bins, a->plan, a->tw, off, ne, a->grid,
+                accumulate, a->rowstat, a->Z, a->partial, launched, st);
             if (rc) return rc;
         }
-    return acq_launch_stats(a->rowstat, static_cast<int>(n_slots), bins, ne, c.doppler_max, a->doppler_center, c.doppler_step, dwell_counter,
-        c.use_cfar, a->best, results_dev, step_two, a->center2, a->step2, prev_input_power, launched, a->stream);
+    rc = acq_launch_stats(a->rowstat, static_cast<int>(n_slots), bins, ne, c.doppler_max, a->doppler_center, c.doppler_step, dwell_counter,
+        c.use_cfar, a->best, results_dev, step_two, a->center2, a->step2, prev_input_power, launched, st);
+    if (rc) return rc;
+    if (!c.use_cfar)  // mixed radix only: b200_acq_create takes the chirp-z path with use_cfar only
+        {
+            rc = acq_launch_second_peak(a->X, a->codes, a->slot_list, static_cast<int>(n_slots), bins, a->plan, a->tw, off, ne, a->grid,
+                a->best, static_cast<int>(c.samples_per_chip), a->second_peak, a->Z, a->partial, launched, st);
+            if (rc) return rc;
+            rc = acq_launch_finish_second_peak(a->second_peak, static_cast<int>(n_slots), results_dev, launched, st);
+            if (rc) return rc;
+        }
+    a->e->launches += launched;
+    return B200_OK;
 }
+
+// The samples of one search that returns its records to the host: consumed_samples complex values in the caller's memory,
+// as b200_cf32 or as I,Q-interleaved int16, or samples [abs_index, abs_index + consumed_samples) of one of the engine's bands
+struct SearchSource
+{
+    enum Kind { kHostF32, kHostI16, kBand } kind;
+    const void* host;
+    int band;
+    uint64_t abs_index;
+};
 }  // namespace
 
 extern "C"
@@ -387,22 +390,10 @@ extern "C"
                     }
                 B200_CUDA_TRY(cudaMemsetAsync(a->grid, 0, sizeof(float) * ne * bins * slots, a->stream));
             }
-        if (use_bluestein)
-            {
-                rc = acq_launch_wipeoff(a->wipe, static_cast<int>(n), static_cast<int>(bins), c.doppler_max, 0, c.doppler_step, 0, c.fs_in, 0, 0.f, 0.f, a->stream);
-                if (rc) return rc;
-                rc = bluestein_setup(a.get());
-                if (rc) return rc;
-                rc = bluestein_refresh_mult(a.get());
-                if (rc) return rc;
-            }
-        else
-            {
-                rc = acq_launch_twiddles(a->tw, a->plan, a->stream);
-                if (rc) return rc;
-                rc = acq_launch_wipeoff(a->wipe, static_cast<int>(n), static_cast<int>(bins), c.doppler_max, 0, c.doppler_step, 0, c.fs_in, 0, 0.f, 0.f, a->stream);
-                if (rc) return rc;
-            }
+        rc = use_bluestein ? bluestein_setup(a.get()) : acq_launch_twiddles(a->tw, a->plan, a->stream);
+        if (rc) return rc;
+        rc = build_rows(a.get(), false);
+        if (rc) return rc;
         B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
         *out = a.release();
         return B200_OK;
@@ -448,15 +439,8 @@ extern "C"
         B200_ENTER_DEVICE(a->e->device);
         a->doppler_center = doppler_center;
         a->doppler_bias = doppler_bias;
-        const b200_acq_conf& c = a->c;
-        int rc = acq_launch_wipeoff(a->wipe, static_cast<int>(c.fft_size), static_cast<int>(c.num_doppler_bins), c.doppler_max,
-            doppler_center, c.doppler_step, doppler_bias, c.fs_in, 0, 0.f, 0.f, a->stream);
+        const int rc = build_rows(a, false);
         if (rc) return rc;
-        if (a->bl)
-            {
-                rc = bluestein_refresh_mult(a);
-                if (rc) return rc;
-            }
         B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
         return B200_OK;
     }
@@ -469,156 +453,24 @@ extern "C"
         return B200_ERR_STATE;
     }
 
-    // after a search queued on a->stream: its n_slots records follow into results_pin, for b200_acq_search_wait
-    static int queue_results(b200_acq* a, uint32_t n_slots)
-    {
-        if (!a->done) B200_CUDA_TRY(a->done.create(cudaEventDisableTiming));
-        B200_CUDA_TRY(cudaMemcpyAsync(a->results_pin, a->results_dev, sizeof(b200_acq_result) * n_slots, cudaMemcpyDeviceToHost, a->stream));
-        B200_CUDA_TRY(cudaEventRecord(a->done, a->stream));
-        a->pending = true;
-        a->pending_slots = n_slots;
-        return B200_OK;
-    }
-
-    int b200_acq_search_submit(b200_acq* a, const b200_cf32* in_host, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter)
-    {
-        if (!a || !in_host) return B200_ERR_ARG;
-        if (const int rc = check_no_search_in_flight(a)) return rc;
-        B200_ENTER_DEVICE(a->e->device);
-        if (!a->in_pin) B200_CUDA_TRY(a->in_pin.alloc(a->c.fft_size));
-        // the caller's buffer is free as soon as this returns: stage it in pinned memory so that the copy is truly asynchronous
-        std::memcpy(a->in_pin, in_host, sizeof(float2) * a->c.consumed_samples);
-        B200_CUDA_TRY(cudaMemcpyAsync(a->in_dev, a->in_pin, sizeof(float2) * a->c.consumed_samples, cudaMemcpyHostToDevice, a->stream));
-        const int rc = search_impl(a, AcqInput::linear(a->in_dev), slots, n_slots, dwell_counter, a->results_dev);
-        if (rc) return rc;
-        return queue_results(a, n_slots);
-    }
-
-    int b200_acq_search_wait(b200_acq* a, b200_acq_result* results_host)
-    {
-        if (!a || !results_host) return B200_ERR_ARG;
-        if (!a->pending)
-            {
-                set_error("no search in flight on this acquisition object");
-                return B200_ERR_STATE;
-            }
-        B200_ENTER_DEVICE(a->e->device);
-        B200_CUDA_TRY(cudaEventSynchronize(a->done));
-        std::memcpy(results_host, a->results_pin, sizeof(b200_acq_result) * a->pending_slots);
-        a->pending = false;
-        return B200_OK;
-    }
-
-    int b200_acq_search(b200_acq* a, const b200_cf32* in_host, const uint32_t* slots, uint32_t n_slots,
-        uint32_t dwell_counter, b200_acq_result* results_host)
-    {
-        if (!a || !in_host || !results_host) return B200_ERR_ARG;
-        const int rc = b200_acq_search_submit(a, in_host, slots, n_slots, dwell_counter);
-        if (rc) return rc;
-        return b200_acq_search_wait(a, results_host);
-    }
-
-    // cshort input (pcps_acquisition.cc:653-656 converts with volk_gnsssdr_16ic_convert_32fc on the host): the raw 16-bit
-    // pairs cross PCIe (half the bytes) and become float2 on the device; int -> float is exact, so results are those
-    // of the float path on the converted samples.
-    static int upload_i16(b200_acq* a, const int16_t* in_host_iq)
+    // Host input of either format crosses the same way: into pinned memory (the caller's buffer is free as soon as the call
+    // returns, and the copy is truly asynchronous), then one copy on a->stream.  cshort input (pcps_acquisition.cc:653-656
+    // converts with volk_gnsssdr_16ic_convert_32fc on the host): the raw 16-bit pairs cross PCIe (half the bytes) and become
+    // float2 on the device; int -> float is exact, so results are those of the float path on the converted samples.
+    static int stage_host(b200_acq* a, const SearchSource& src)
     {
         const size_t n = a->c.consumed_samples;
+        const bool i16 = src.kind == SearchSource::kHostI16;
+        const size_t bytes = i16 ? sizeof(int16_t) * 2 * n : sizeof(float2) * n;
         if (!a->in_pin) B200_CUDA_TRY(a->in_pin.alloc(a->c.fft_size));
-        if (!a->raw_dev) B200_CUDA_TRY(a->raw_dev.alloc(2 * a->c.fft_size));
-        std::memcpy(a->in_pin, in_host_iq, sizeof(int16_t) * 2 * n);
-        B200_CUDA_TRY(cudaMemcpyAsync(a->raw_dev, a->in_pin, sizeof(int16_t) * 2 * n, cudaMemcpyHostToDevice, a->stream));
+        if (i16 && !a->raw_dev) B200_CUDA_TRY(a->raw_dev.alloc(2 * a->c.fft_size));
+        std::memcpy(a->in_pin, src.host, bytes);
+        void* dst = i16 ? static_cast<void*>(a->raw_dev.get()) : static_cast<void*>(a->in_dev.get());
+        B200_CUDA_TRY(cudaMemcpyAsync(dst, a->in_pin, bytes, cudaMemcpyHostToDevice, a->stream));
+        if (!i16) return B200_OK;
         const int rc = launch_convert_i16(a->raw_dev, a->in_dev, ~0ULL, 0ULL, n, a->stream);
         if (rc == B200_OK) a->e->launches++;
         return rc;
-    }
-
-    // search the samples `in`, then bring the n_slots result records back to the host
-    static int search_to_host(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter, int step_two,
-        float prev_input_power, b200_acq_result* results_host)
-    {
-        const int rc = search_impl(a, in, slots, n_slots, dwell_counter, a->results_dev, step_two, prev_input_power);
-        if (rc) return rc;
-        B200_CUDA_TRY(cudaMemcpyAsync(a->results_pin, a->results_dev, sizeof(b200_acq_result) * n_slots, cudaMemcpyDeviceToHost, a->stream));
-        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-        std::memcpy(results_host, a->results_pin, sizeof(b200_acq_result) * n_slots);
-        return B200_OK;
-    }
-
-    int b200_acq_search_i16(b200_acq* a, const int16_t* in_host_iq, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
-        b200_acq_result* results_host)
-    {
-        if (!a || !in_host_iq || !results_host) return B200_ERR_ARG;
-        if (const int rc = check_no_search_in_flight(a)) return rc;
-        B200_ENTER_DEVICE(a->e->device);
-        const int rc = upload_i16(a, in_host_iq);
-        if (rc) return rc;
-        return search_to_host(a, AcqInput::linear(a->in_dev), slots, n_slots, dwell_counter, 0, 0.f, results_host);
-    }
-
-    int b200_acq_search_step_two_i16(b200_acq* a, const int16_t* in_host_iq, uint32_t slot, uint32_t dwell_counter, float prev_input_power,
-        b200_acq_result* result_host)
-    {
-        if (!a || !in_host_iq || !result_host) return B200_ERR_ARG;
-        B200_ENTER_DEVICE(a->e->device);
-        const int rc = upload_i16(a, in_host_iq);
-        if (rc) return rc;
-        return search_to_host(a, AcqInput::linear(a->in_dev), &slot, 1, dwell_counter, 1, prev_input_power, result_host);
-    }
-
-    int b200_acq_set_step_two(b200_acq* a, float doppler_center_step_two, float doppler_step2, uint32_t num_doppler_bins_step2)
-    {
-        if (!a || num_doppler_bins_step2 < 1) return B200_ERR_ARG;
-        if (num_doppler_bins_step2 > a->c.num_doppler_bins)
-            {
-                set_error("step-two bins %u exceed the grid's %u rows", num_doppler_bins_step2, a->c.num_doppler_bins);
-                return B200_ERR_RANGE;
-            }
-        B200_ENTER_DEVICE(a->e->device);
-        if (!a->wipe2 || a->bins2 < num_doppler_bins_step2)
-            {
-                B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-                B200_CUDA_TRY(a->wipe2.alloc(a->c.fft_size * num_doppler_bins_step2));
-            }
-        if (a->bl && !a->bl->mult2.fits(a->c.fft_size * num_doppler_bins_step2))
-            {
-                B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-                B200_CUDA_TRY(a->bl->mult2.alloc(a->c.fft_size * num_doppler_bins_step2));
-            }
-        a->bins2 = num_doppler_bins_step2;
-        a->center2 = doppler_center_step_two;
-        a->step2 = doppler_step2;
-        int rc = acq_launch_wipeoff(a->wipe2, static_cast<int>(a->c.fft_size), static_cast<int>(a->bins2), 0, 0, 0, a->doppler_bias, a->c.fs_in, 1,
-            doppler_center_step_two, doppler_step2, a->stream);
-        if (rc) return rc;
-        if (a->bl)
-            {
-                // chirped step-two rows, as bluestein_refresh_mult builds the step-one rows
-                const int n = static_cast<int>(a->c.fft_size);
-                rc = acq_launch_rows_times_vector(a->wipe2, n, a->bl->chirp_conj, n, 0, a->bl->mult2, n, static_cast<int>(a->bins2), a->stream);
-                if (rc) return rc;
-            }
-        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
-        return B200_OK;
-    }
-
-    int b200_acq_search_step_two(b200_acq* a, const b200_cf32* in_host, uint32_t slot, uint32_t dwell_counter, float prev_input_power,
-        b200_acq_result* result_host)
-    {
-        if (!a || !in_host || !result_host) return B200_ERR_ARG;
-        B200_ENTER_DEVICE(a->e->device);
-        B200_CUDA_TRY(cudaMemcpyAsync(a->in_dev, in_host, sizeof(float2) * a->c.consumed_samples, cudaMemcpyHostToDevice, a->stream));
-        return search_to_host(a, AcqInput::linear(a->in_dev), &slot, 1, dwell_counter, 1, prev_input_power, result_host);
-    }
-
-    int b200_acq_search_dev(b200_acq* a, const b200_cf32* in_dev, const uint32_t* slots_host, uint32_t n_slots,
-        uint32_t dwell_counter, b200_acq_result* results_dev)
-    {
-        if (!a || !in_dev || !results_dev) return B200_ERR_ARG;
-        B200_ENTER_DEVICE(a->e->device);
-        // (search_impl synchronises by itself when - and only when - the slot list changed and slot_pin must be rewritten; a
-        // repeated sweep over the same slots issues no host synchronisation and can be captured in a CUDA graph)
-        return search_impl(a, AcqInput::linear(reinterpret_cast<const float2*>(in_dev)), slots_host, n_slots, dwell_counter, results_dev);
     }
 
     // The view of samples [abs_index, abs_index + consumed_samples) of one of the engine's bands, with a->stream made to wait
@@ -654,38 +506,138 @@ extern "C"
         return B200_OK;
     }
 
-    int b200_acq_search_band_submit(b200_acq* a, int band, uint64_t abs_index, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter)
+    // Every search that returns its records to the host goes through here: refused while a sweep is in flight, it stages
+    // the input, queues the search on a->stream and its n_slots records into results_pin, and records `done` for
+    // b200_acq_search_wait.
+    static int submit_search(b200_acq* a, const SearchSource& src, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
+        int step_two, float prev_input_power)
     {
-        if (!a) return B200_ERR_ARG;
+        if (!a || (src.kind != SearchSource::kBand && !src.host)) return B200_ERR_ARG;
         if (const int rc = check_no_search_in_flight(a)) return rc;
         B200_ENTER_DEVICE(a->e->device);
-        AcqInput in{};
-        int rc = band_input(a, band, abs_index, &in);
+        AcqInput in = AcqInput::linear(a->in_dev);
+        int rc = src.kind == SearchSource::kBand ? band_input(a, src.band, src.abs_index, &in) : stage_host(a, src);
         if (rc) return rc;
-        rc = search_impl(a, in, slots, n_slots, dwell_counter, a->results_dev);
+        rc = search_impl(a, in, slots, n_slots, dwell_counter, a->results_dev, step_two, prev_input_power);
         if (rc) return rc;
-        return queue_results(a, n_slots);
+        if (!a->done) B200_CUDA_TRY(a->done.create(cudaEventDisableTiming));
+        B200_CUDA_TRY(cudaMemcpyAsync(a->results_pin, a->results_dev, sizeof(b200_acq_result) * n_slots, cudaMemcpyDeviceToHost, a->stream));
+        B200_CUDA_TRY(cudaEventRecord(a->done, a->stream));
+        a->pending = true;
+        a->pending_slots = n_slots;
+        return B200_OK;
+    }
+
+    // the synchronous searches: submit_search, then b200_acq_search_wait
+    static int search_and_wait(b200_acq* a, const SearchSource& src, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
+        int step_two, float prev_input_power, b200_acq_result* results_host)
+    {
+        if (!results_host) return B200_ERR_ARG;
+        const int rc = submit_search(a, src, slots, n_slots, dwell_counter, step_two, prev_input_power);
+        return rc ? rc : b200_acq_search_wait(a, results_host);
+    }
+
+    int b200_acq_search_submit(b200_acq* a, const b200_cf32* in_host, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter)
+    {
+        return submit_search(a, SearchSource{SearchSource::kHostF32, in_host}, slots, n_slots, dwell_counter, 0, 0.f);
+    }
+
+    int b200_acq_search_wait(b200_acq* a, b200_acq_result* results_host)
+    {
+        if (!a || !results_host) return B200_ERR_ARG;
+        if (!a->pending)
+            {
+                set_error("no search in flight on this acquisition object");
+                return B200_ERR_STATE;
+            }
+        B200_ENTER_DEVICE(a->e->device);
+        B200_CUDA_TRY(cudaEventSynchronize(a->done));
+        std::memcpy(results_host, a->results_pin, sizeof(b200_acq_result) * a->pending_slots);
+        a->pending = false;
+        return B200_OK;
+    }
+
+    int b200_acq_search(b200_acq* a, const b200_cf32* in_host, const uint32_t* slots, uint32_t n_slots,
+        uint32_t dwell_counter, b200_acq_result* results_host)
+    {
+        return search_and_wait(a, SearchSource{SearchSource::kHostF32, in_host}, slots, n_slots, dwell_counter, 0, 0.f, results_host);
+    }
+
+    int b200_acq_search_i16(b200_acq* a, const int16_t* in_host_iq, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
+        b200_acq_result* results_host)
+    {
+        return search_and_wait(a, SearchSource{SearchSource::kHostI16, in_host_iq}, slots, n_slots, dwell_counter, 0, 0.f, results_host);
+    }
+
+    int b200_acq_search_step_two_i16(b200_acq* a, const int16_t* in_host_iq, uint32_t slot, uint32_t dwell_counter, float prev_input_power,
+        b200_acq_result* result_host)
+    {
+        return search_and_wait(a, SearchSource{SearchSource::kHostI16, in_host_iq}, &slot, 1, dwell_counter, 1, prev_input_power, result_host);
+    }
+
+    int b200_acq_set_step_two(b200_acq* a, float doppler_center_step_two, float doppler_step2, uint32_t num_doppler_bins_step2)
+    {
+        if (!a || num_doppler_bins_step2 < 1) return B200_ERR_ARG;
+        if (num_doppler_bins_step2 > a->c.num_doppler_bins)
+            {
+                set_error("step-two bins %u exceed the grid's %u rows", num_doppler_bins_step2, a->c.num_doppler_bins);
+                return B200_ERR_RANGE;
+            }
+        B200_ENTER_DEVICE(a->e->device);
+        if (!a->wipe2 || a->bins2 < num_doppler_bins_step2)
+            {
+                B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
+                B200_CUDA_TRY(a->wipe2.alloc(a->c.fft_size * num_doppler_bins_step2));
+            }
+        if (a->bl && !a->bl->mult2.fits(a->c.fft_size * num_doppler_bins_step2))
+            {
+                B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
+                B200_CUDA_TRY(a->bl->mult2.alloc(a->c.fft_size * num_doppler_bins_step2));
+            }
+        a->bins2 = num_doppler_bins_step2;
+        a->center2 = doppler_center_step_two;
+        a->step2 = doppler_step2;
+        const int rc = build_rows(a, true);
+        if (rc) return rc;
+        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
+        return B200_OK;
+    }
+
+    int b200_acq_search_step_two(b200_acq* a, const b200_cf32* in_host, uint32_t slot, uint32_t dwell_counter, float prev_input_power,
+        b200_acq_result* result_host)
+    {
+        return search_and_wait(a, SearchSource{SearchSource::kHostF32, in_host}, &slot, 1, dwell_counter, 1, prev_input_power, result_host);
+    }
+
+    // Not a submit_search path, and not refused while a sweep is in flight: the input is on the device and the records stay
+    // there, so it touches neither in_pin nor results_pin, and it must stay capturable in a CUDA graph.  (search_impl
+    // synchronises by itself when - and only when - the slot list changed and slot_pin must be rewritten; a repeated sweep
+    // over the same slots issues no host synchronisation.)
+    int b200_acq_search_dev(b200_acq* a, const b200_cf32* in_dev, const uint32_t* slots_host, uint32_t n_slots,
+        uint32_t dwell_counter, b200_acq_result* results_dev)
+    {
+        if (!a || !in_dev || !results_dev) return B200_ERR_ARG;
+        B200_ENTER_DEVICE(a->e->device);
+        return search_impl(a, AcqInput::linear(reinterpret_cast<const float2*>(in_dev)), slots_host, n_slots, dwell_counter, results_dev);
+    }
+
+    int b200_acq_search_band_submit(b200_acq* a, int band, uint64_t abs_index, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter)
+    {
+        return submit_search(a, SearchSource{SearchSource::kBand, nullptr, band, abs_index}, slots, n_slots, dwell_counter, 0, 0.f);
     }
 
     int b200_acq_search_band(b200_acq* a, int band, uint64_t abs_index, const uint32_t* slots, uint32_t n_slots, uint32_t dwell_counter,
         b200_acq_result* results_host)
     {
-        if (!a || !results_host) return B200_ERR_ARG;
-        const int rc = b200_acq_search_band_submit(a, band, abs_index, slots, n_slots, dwell_counter);
-        if (rc) return rc;
-        return b200_acq_search_wait(a, results_host);
+        return search_and_wait(a, SearchSource{SearchSource::kBand, nullptr, band, abs_index}, slots, n_slots, dwell_counter, 0, 0.f,
+            results_host);
     }
 
     int b200_acq_search_step_two_band(b200_acq* a, int band, uint64_t abs_index, uint32_t slot, uint32_t dwell_counter, float prev_input_power,
         b200_acq_result* result_host)
     {
-        if (!a || !result_host) return B200_ERR_ARG;
-        if (const int rc = check_no_search_in_flight(a)) return rc;
-        B200_ENTER_DEVICE(a->e->device);
-        AcqInput in{};
-        const int rc = band_input(a, band, abs_index, &in);
-        if (rc) return rc;
-        return search_to_host(a, in, &slot, 1, dwell_counter, 1, prev_input_power, result_host);
+        return search_and_wait(a, SearchSource{SearchSource::kBand, nullptr, band, abs_index}, &slot, 1, dwell_counter, 1, prev_input_power,
+            result_host);
     }
 
     int b200_acq_sweep_best_dev(b200_acq* a, const b200_acq_result* results_dev, const uint32_t* prn_of_result_dev, uint32_t n_results,

@@ -413,7 +413,9 @@ extern "C"
     /* Asynchronous form: submit returns once the sweep is queued (the input is copied first, the caller's buffer
      * is free again), wait blocks for its results.  One sweep may be in flight per acquisition object; objects own
      * their stream, so the sweeps of different channels' blocks overlap on the device as the reference's
-     * acquisition threads overlap on the host. */
+     * acquisition threads overlap on the host.  While a sweep is in flight, every search that returns results to the
+     * host (b200_acq_search, _i16, _step_two, _step_two_i16, _submit and the band forms below) is refused with
+     * B200_ERR_STATE and queues nothing; b200_acq_search_dev is not refused. */
     int b200_acq_search_submit(b200_acq* a, const b200_cf32* in_host, const uint32_t* slots_host, uint32_t n_slots, uint32_t dwell_counter);
     int b200_acq_search_wait(b200_acq* a, b200_acq_result* results_host);
     /* same with the input already on the device and results left on the device (asynchronous) */

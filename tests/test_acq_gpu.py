@@ -400,3 +400,49 @@ def test_async_search_matches_synchronous_and_guards_misuse(oracle):
     a.close()
     b.close()
     e.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("entry", ["search", "search_i16", "search_step_two", "search_step_two_i16",
+                                   "search_submit", "search_band", "search_band_submit", "search_step_two_band"])
+def test_host_searches_refused_while_a_sweep_is_in_flight(entry):
+    """Every search that returns results to the host is B200_ERR_STATE while a submitted sweep is in flight, and the
+    sweep's results are still the synchronous search's."""
+    import ctypes as C
+    from gnss_sdr_b200 import capi
+    import gnss_synth as gs
+    fs, n, band = 4e6, 4000, 0
+    iq = gs.make_iq({3: gs.gps_ca_code(3)}, fs, n, [dict(prn=3, doppler=2100.0, code_phase_chips=400.0, cn0=48.0)], seed=8)
+    raw = np.round(iq.view(np.float32) * 100).astype(np.int16)
+    e = capi.Engine()
+    e.iq_create(band, 8192)
+    e.iq_push(band, iq)
+    a = capi.PcpsAcquisition(e, fs_in=int(fs), samples_per_ms=float(n), samples_per_chip=4, doppler_max=5000, doppler_step=250, n_code_slots=2)
+    a.set_local_code(0, gs.gps_ca_code_complex_sampled(3, int(fs)))
+    a.set_local_code(1, gs.gps_ca_code_complex_sampled(4, int(fs)))
+    a.set_step_two(2100.0, 125.0, 4)   # so that a step-two call is otherwise legal
+    want = a.search(iq, [0, 1])
+    res, slot = np.zeros(1, capi.ACQ_RESULT_DTYPE), np.zeros(1, np.uint32)
+
+    def i16(name, *args):
+        rc = getattr(capi.lib, name)(a.h, raw.ctypes.data, *args, res.ctypes.data)
+        if rc:
+            raise capi.B200Error(rc, name)
+
+    calls = {
+        "search": lambda: a.search(iq, [0]),
+        "search_i16": lambda: i16("b200_acq_search_i16", slot.ctypes.data, 1, 1),
+        "search_step_two": lambda: a.search_step_two(iq, 0, 1.0),
+        "search_step_two_i16": lambda: i16("b200_acq_search_step_two_i16", 0, 1, C.c_float(1.0)),
+        "search_submit": lambda: a.search_submit(iq, [0]),
+        "search_band": lambda: a.search_band(band, 0, [0]),
+        "search_band_submit": lambda: a.search_band_submit(band, 0, [0]),
+        "search_step_two_band": lambda: a.search_step_two_band(band, 0, 0, 1.0),
+    }
+    a.search_submit(iq, [0, 1])
+    with pytest.raises(capi.B200Error) as ei:
+        calls[entry]()
+    assert ei.value.code == -4
+    assert a.search_wait().tobytes() == want.tobytes()
+    a.close()
+    e.close()
