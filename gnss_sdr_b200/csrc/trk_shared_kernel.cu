@@ -13,7 +13,7 @@
 //                   samples with conflict-free LDS.128, correlates them against a warp-private shared-memory
 //                   code table, releases the tile.  warp_tile looks every tap's chip up per sample;
 //                   warp_tile_chunks (C/A-like steps) splits 16-sample chunks at their one exact chip
-//                   boundary per tap and multiplies two chip values into chunk sums.
+//                   boundary per tap and multiplies two chip values into chunk sums kept in registers.
 //
 // Both use the chip-index float sequence and the 64-bit fixed-point carrier phase of trk_kernels.cu, so
 // indices are bit-exact and results follow the same contract.  Items of a group need
@@ -34,7 +34,9 @@ constexpr int kShStages = SH_STAGES;
 // Minimum resident CTAs per SM (__launch_bounds__).  sm_90a, 288 threads: 3 caps the kernel at 72 registers and spills
 // (<3>: 166 B stores / 248 B loads), 2 gives 96 registers (<3>: 8 B / 8 B), 1 no spills at 127-152.  On an H100 (400 W), ms
 // per C2 step: 2 -> 0.969-0.970, 3 -> 1.051-1.058, 1 -> 1.189-1.191, 4 -> 1.179; distinct-IQ through this kernel 1.237 at 2,
-// 1.393 at 3.  With the chunk path's scratch a CTA takes about 92 KB of shared memory, so three no longer fit on an SM.
+// 1.393 at 3.  Since the chunk path keeps its running sums in registers, a CTA takes about 54 KB of shared memory and three
+// fit again; at 3 the kernel is capped at 72 registers and <3> spills 134 B / 268 B.  On an H100 80GB HBM3 (700 W, 1980 MHz),
+// ms per C2 step, two runs each: 2 -> 0.6946-0.6950, 3 -> 0.6988-0.6989.
 constexpr int kShMinBlocks = 2;
 // SH_STRESS (test builds only, tests/test_ring_stress_gpu.py): pseudo-random delays in the producer and in every consumer
 // warp, before the tile is read and before the slot is released, so that warps drift apart by several tiles and every
@@ -63,7 +65,6 @@ constexpr int kShChunk = 16;
 constexpr int kShRun = 4 * kShChunk;          // samples per bulk copy
 constexpr int kShRunStride = kShRun + 2;      // float2 per run slot
 constexpr int kShTileSlot = kShTile / kShRun * kShRunStride;
-constexpr int kShChunkStride = kShChunk + 2;  // float2 per lane in the prefix scratch (144 B: conflict-free STS.128)
 __device__ __forceinline__ int lane_chunk(int lane) { return 4 * (lane & 7) + (lane >> 3); }
 
 namespace
@@ -72,11 +73,11 @@ struct __align__(128) ShSmem
 {
     float2 tiles[kShStages][kShTileSlot];
     float tbl[kShK][kShTblCap];
-    float2 prefix[kShK][32 * kShChunkStride];  // chunk path: each lane's running sums of its rotated chunk
     float2 rot[kShK][kShChunk];                // chunk path: D^j, j = 0..15, D = the item's per-sample phasor
     unsigned long long full[kShStages];
     unsigned long long empty[kShStages];
     unsigned long long item_start[kShK];  // offset of the item's first sample in the band (band-relative)
+    unsigned long long item_turns[kShK][2];  // the item's T0 and DT (item_phase()), read back after the set-up
     int item_n[kShK];
     int item_band[kShK];
     unsigned long long hull_start;
@@ -202,17 +203,38 @@ __device__ __forceinline__ void warp_tile(const Loader& load, float vlo, float v
         }
 }
 
-// Chunk path: one tile for one warp, lane l owns the 16 contiguous samples of chunk lane_chunk(l) of the tile, n0f is
-// the epoch index of the first of them.  The lane rotates its chunk in the chunk frame, u_j = x_j D^j, and stores the
-// running sums R_j = u_0 + ... + u_j.  Every tap's chip index rises at most once inside a chunk (the step test at the
-// item set-up), so with i0 the index of the first sample and m the number of samples that keep it, the tap gets
-//     z0 (c[i0] R_{m-1} + c[i0+1] (S - R_{m-1})),   S = R_15,   z0 = the phasor of the chunk's first sample.
-// m comes from a 4-step binary search on the exact index formula floor(fl(fl(step n) + aux)), which is non-decreasing
-// in n for step > 0: no sample's index is estimated.  MASKED as in warp_tile.  Accumulates into acc_re / acc_im.
-template <int TAPS, bool MASKED>
-__device__ __forceinline__ void warp_tile_chunks(const float4* x4, float4* pre4, const float4* rot4, float n0f, float vlo, float vhi,
-    float step, const float2 (&aux2)[TAPS], unsigned int tbl_off, float2 z0, float2 (&acc_re)[TAPS], float2 (&acc_im)[TAPS])
+// R[m] for a lane-dependent m in [0, 15] without indexing registers (which would put R in local memory): a 4-level tree
+// of selects on the bits of m.
+__device__ __forceinline__ float2 select16(const float2 (&R)[kShChunk], int m)
 {
+    float2 a[8], b[4], c[2];
+#pragma unroll
+    for (int i = 0; i < 8; i++) a[i] = (m & 1) ? R[2 * i + 1] : R[2 * i];
+#pragma unroll
+    for (int i = 0; i < 4; i++) b[i] = (m & 2) ? a[2 * i + 1] : a[2 * i];
+#pragma unroll
+    for (int i = 0; i < 2; i++) c[i] = (m & 4) ? b[2 * i + 1] : b[2 * i];
+    return (m & 8) ? c[1] : c[0];
+}
+
+// Chunk path: one tile for one warp, lane l owns the 16 contiguous samples of chunk lane_chunk(l) of the tile, n0f is
+// the epoch index of the first of them.  The lane rotates its chunk in the chunk frame, u_j = x_j D^j, and forms the
+// running sums R_j = u_0 + ... + u_j.  Every tap's chip index rises at most once inside a chunk (the step test at the
+// item set-up), so with i0 the index of the first sample and m the last sample that keeps it, the tap gets
+//     z0 (c[i0] R_m + c[i0+1] (S - R_m)),   S = R_15,   z0 = the phasor of the chunk's first sample.
+// m comes from an estimate that the exact index formula a(n) = fl(fl(step n) + aux), i(n) = floor(a(n)), then decides
+// (item set-up: the bound there keeps the estimate within one sample).  From the chunk's first valid sample lo, the
+// index rises at b = lo + j, j >= 1 the first with a(b) >= i0 + 1; with e = (i0 + 1) - a(lo) in (0, 1] that is near
+// lo + e / step, and c = fl(fl(e) inv_step + 1/2) puts b in {lo + k, lo + k + 1}, k = floor(c) (c clamped to 16.5: m is
+// 15 for any b >= lo + 16).  One evaluation of i(lo + k) picks the one: m = b - 1.  The formula is non-decreasing in n
+// for step > 0, and it alone decides, so no sample's index is estimated.
+// MASKED as in warp_tile: lo is the first sample of the chunk inside the epoch; masked samples add zero to R, so every m
+// past the epoch's last sample selects the same sum.  Accumulates into acc_re / acc_im.
+template <int TAPS, bool MASKED>
+__device__ __forceinline__ void warp_tile_chunks(const float4* x4, const float4* rot4, float n0f, float vlo, float vhi,
+    float step, float inv_step, const float2 (&aux2)[TAPS], unsigned int tbl_off, float2 z0, float2 (&acc_re)[TAPS], float2 (&acc_im)[TAPS])
+{
+    float2 R[kShChunk];
     float2 r = make_float2(0.f, 0.f);
 #pragma unroll
     for (int k = 0; k < kShChunk / 2; k++)
@@ -225,31 +247,39 @@ __device__ __forceinline__ void warp_tile_chunks(const float4* x4, float4* pre4,
                     if (na < vlo || na > vhi) v.x = v.y = 0.f;
                     if (nb < vlo || nb > vhi) v.z = v.w = 0.f;
                 }
-            r.x += fmaf(v.x, d.x, -v.y * d.y);
-            r.y += fmaf(v.x, d.y, v.y * d.x);
-            const float2 ra = r;
-            r.x += fmaf(v.z, d.z, -v.w * d.w);
-            r.y += fmaf(v.z, d.w, v.w * d.z);
-            pre4[k] = make_float4(ra.x, ra.y, r.x, r.y);
+            // two chained FFMA per component: with a zero carrier D^j = (1, 0) and integer data stays exact
+            r.x = fmaf(-v.y, d.y, fmaf(v.x, d.x, r.x));
+            r.y = fmaf(v.y, d.x, fmaf(v.x, d.y, r.y));
+            R[2 * k] = r;
+            r.x = fmaf(-v.w, d.w, fmaf(v.z, d.z, r.x));
+            r.y = fmaf(v.w, d.z, fmaf(v.z, d.w, r.y));
+            R[2 * k + 1] = r;
         }
-    const float2* pre = reinterpret_cast<const float2*>(pre4);
     const float lo = MASKED ? fminf(fmaxf(n0f, vlo), vhi) : n0f;
+    const float lo_m = lo - kFloorMagic;  // exact: lo + k = t_k + lo_m below
+    // m relative to the chunk start is (lo - n0f) + (b - lo) - 1
+    const int lo_off = MASKED ? __float2int_rn(lo - n0f) : 0;
+    float t0[TAPS];
+    int m[TAPS];
 #pragma unroll
     for (int t = 0; t < TAPS; t++)
         {
             const float a = aux2[t].x;
-            const float t0 = __fadd_rd(__fadd_rn(__fmul_rn(step, lo), a), kFloorMagic);
-            float q = n0f;  // last sample of the chunk known to keep index i0
+            const float g = __fadd_rn(__fmul_rn(step, lo), a);
+            t0[t] = __fadd_rd(g, kFloorMagic);                                      // kFloorMagic + i0
+            const float e = __fsub_rn(__fsub_rn(t0[t], kFloorMagic - 1.0f), g);    // (i0 + 1) - a(lo)
+            const float c = fminf(__fmaf_rn(e, inv_step, 0.5f), 16.5f);
+            const float tk = __fadd_rd(c, kFloorMagic);                             // kFloorMagic + k
+            const float tb = __fadd_rd(__fadd_rn(__fmul_rn(step, __fadd_rn(tk, lo_m)), a), kFloorMagic);
+            const int k = __float_as_int(tk) - __float_as_int(kFloorMagic);
+            const int mt = lo_off + k - (tb != t0[t] ? 1 : 0);
+            m[t] = MASKED ? min(max(mt, 0), kShChunk - 1) : min(mt, kShChunk - 1);
+        }
 #pragma unroll
-            for (int s = 8; s > 0; s >>= 1)
-                {
-                    const float cand = q + static_cast<float>(s);
-                    const float ce = MASKED ? fminf(fmaxf(cand, vlo), vhi) : cand;
-                    const float tc = __fadd_rd(__fadd_rn(__fmul_rn(step, ce), a), kFloorMagic);
-                    q = (tc == t0) ? cand : q;
-                }
-            const float2 P = pre[__float2int_rz(q - n0f)];
-            const unsigned int addr = (__float_as_uint(t0) << 2) + tbl_off;
+    for (int t = 0; t < TAPS; t++)
+        {
+            const float2 P = select16(R, m[t]);
+            const unsigned int addr = (__float_as_uint(t0[t]) << 2) + tbl_off;
             const float c0 = lds_f32(addr), c1 = lds_f32(addr + 4u);
             const float dc = c0 - c1;
             const float vr = fmaf(dc, P.x, c1 * r.x), vi = fmaf(dc, P.y, c1 * r.y);
@@ -391,6 +421,14 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
             const ItemPhase ph = item_phase(it.rem_carrier_phase_rad, it.phase_step_rad, it.n);
             T0 = ph.T0;
             DT = ph.DT;
+            // The chunk path's re-seeds and the epilogue read T0 and DT back from here, so that the two 64-bit words do
+            // not hold registers through the tile loops (with them, ptxas spilled a flag word of <3> at 96 registers).
+            if (lane == 0)
+                {
+                    sm.item_turns[warp][0] = T0;
+                    sm.item_turns[warp][1] = DT;
+                }
+            __syncwarp();
             body = ph.body;
             step = it.code_phase_step_chips;
             const float rem = it.rem_code_phase_chips;
@@ -425,13 +463,22 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
                         chip_range<TAPS>(step, 0.f, nl, [&](int q) { return aux2[q].x; }, elo, ehi);
                         whole_table = (static_cast<long long>(ehi) - elo + 3) <= kShTblCap;
                         // Chunk path: the index a(n) = fl(fl(step n) + aux) of every tap may rise at most once over the
-                        // 16 samples of a chunk.  Both roundings err by at most half an ulp of a value of magnitude
-                        // <= M = step (body - 1) + max(|elo|, |ehi|) + 1, so a(n + 15) - a(n) <= 15 step + 2 ulp(M)
-                        // <= 15 step + M 2^-22; below 1, floor(a) rises at most once.  Only a shared window is laid
-                        // out in per-lane chunks, so items that stream their own tiles keep warp_tile.
-                        const double M = static_cast<double>(step) * nl + static_cast<double>(max(abs(elo), abs(ehi))) + 1.0;
+                        // 16 samples of a chunk.  warp_tile_chunks evaluates a(n) for 0 <= n <= body - 1 + 16, where
+                        // |step n| + |a(n)| <= M = step (body + 15) + max(|elo|, |ehi|) + 3 (16 step < 2).  Both roundings
+                        // err by at most half an ulp of their result, so |a(n) - (step n + aux)| <= eps = M 2^-24, and
+                        // a(n + 15) - a(n) <= 15 step + 2 eps < 15 step + M 2^-22; below 1, floor(a) rises at most once.
+                        // The boundary estimate of warp_tile_chunks: the first j >= 1 with a(lo + j) >= i0 + 1 lies in
+                        // [(e - 2 eps) / step, (e + 2 eps) / step + 1), e = (i0 + 1) - a(lo).  fl(e) is within 2^-25 of e
+                        // (e <= 1), inv_step = fl(1 / step) within 2^-24 / step, and the FMA rounds c < 17.5 by at most
+                        // 2^-20, so |c - (e / step + 1/2)| <= 2^-23 / step + 2^-20.  With
+                        // tau = (2 eps + 2^-23) / step + 2^-20 < 1/2, that is (M + 1/2) 2^-22 < step (1 - 2^-19), the first
+                        // j lies in (c - 1, c + 1): it is floor(c) or floor(c) + 1.  (C/A at 25 Msps and 1 ms: tau < 0.013;
+                        // at 100 Msps and 20 ms: tau < 0.26.)  Only a shared window is laid out in per-lane chunks, so
+                        // items that stream their own tiles keep warp_tile.
+                        const double M = static_cast<double>(step) * (nl + 16.0) + static_cast<double>(max(abs(elo), abs(ehi))) + 3.0;
                         chunked = whole_table && sm.share && step > 0.f &&
-                                  static_cast<double>(kShChunk - 1) * static_cast<double>(step) + M * 0x1p-22 < 1.0;
+                                  static_cast<double>(kShChunk - 1) * static_cast<double>(step) + M * 0x1p-22 < 1.0 &&
+                                  (M + 1.0) * 0x1p-22 < static_cast<double>(step) * (1.0 - 0x1p-18);
                         if (whole_table)
                             {
                                 const int wb = elo - 1;
@@ -567,22 +614,22 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
     // The two paths walk the ring in separate loops, so that none of warp_tile's lane state is live on the chunk path.
     if (chunked)
         {
+            const float inv_step = __frcp_rn(step);  // for the boundary estimate (bound at the chunked test)
             for_each_ring_tile([&](int t, int s) {
                 const int n_tile0 = t * kShTile - a_i;
                 const float n0f = static_cast<float>(n_tile0 + kShChunk * lane_chunk(lane));
                 const float vlo = static_cast<float>(max(n_tile0, 0)), vhi = static_cast<float>(min(n_tile0 + kShTile, body) - 1);
                 const float4* x4 = reinterpret_cast<const float4*>(&sm.tiles[s][(lane & 7) * kShRunStride + (lane >> 3) * kShChunk]);
-                float4* pre4 = reinterpret_cast<float4*>(&sm.prefix[warp][lane * kShChunkStride]);
                 const float4* rot4 = reinterpret_cast<const float4*>(&sm.rot[warp][0]);
                 if (n_tile0 >= 0 && n_tile0 + kShTile <= body)
-                    warp_tile_chunks<TAPS, false>(x4, pre4, rot4, n0f, vlo, vhi, step, aux2, tbl_off, z0, are, aim);
+                    warp_tile_chunks<TAPS, false>(x4, rot4, n0f, vlo, vhi, step, inv_step, aux2, tbl_off, z0, are, aim);
                 else
-                    warp_tile_chunks<TAPS, true>(x4, pre4, rot4, n0f, vlo, vhi, step, aux2, tbl_off, z0, are, aim);
+                    warp_tile_chunks<TAPS, true>(x4, rot4, n0f, vlo, vhi, step, inv_step, aux2, tbl_off, z0, are, aim);
                 if ((t - t_first + 1) % (kShReseed / 8) == 0)
                     {
                         // exact re-seed from the 64-bit phase of the lane's next chunk start, every 4096 samples
                         const long long n_next = static_cast<long long>(t + 1) * kShTile + kShChunk * lane_chunk(lane) - a_i;
-                        z0 = phasor_from_turns(T0 + DT * static_cast<unsigned long long>(n_next));
+                        z0 = phasor_from_turns(sm.item_turns[warp][0] + sm.item_turns[warp][1] * static_cast<unsigned long long>(n_next));
                     }
                 else
                     {
@@ -612,6 +659,8 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
         }
     if (have_item && it.n > 0)
         {
+            T0 = sm.item_turns[warp][0];
+            DT = sm.item_turns[warp][1];
             if (table_path)
                 {
 #pragma unroll
