@@ -20,7 +20,6 @@
 #include "acq_fft.cuh"
 #include "common.cuh"
 
-#include <cstdlib>
 #include <type_traits>
 
 namespace b200
@@ -655,11 +654,9 @@ int acq_plan_make(int n_total, FftPlan* pl)
     if (n_total < 2) return B200_ERR_RANGE;
     if (n_total <= kAcqMaxSmemPoints)
         {
-            // radix-25 stages (one shared-memory pass instead of two radix-5 passes) on 512-thread CTAs;
-            // B200_ACQ_RADIX25=0 keeps the radix <= 8 plan on 1024 threads
-            const char* env = std::getenv("B200_ACQ_RADIX25");
-            const bool allow25 = env ? std::atoi(env) != 0 : true;
-            const int rc = acq_plan_make_smem(n_total, pl, allow25);
+            // radix-25 stages (one shared-memory pass instead of two radix-5 passes) on 512-thread CTAs wherever
+            // acq_plan_make_smem can place them; every other size keeps the radix <= 8 plan on 1024 threads
+            const int rc = acq_plan_make_smem(n_total, pl, true);
             pl->n1 = 1;
             pl->n_total = n_total;
             pl->tw_goff = 0;

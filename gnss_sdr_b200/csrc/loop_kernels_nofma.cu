@@ -15,7 +15,6 @@
 //   tracking_discriminators.cc:26-39,69-77,86-89,100-107,119-129,142-153
 //   tracking_FLL_PLL_filter.cc:72-104    tracking_loop_filter.cc:62-96
 //   lock_detectors.cc:99-147,160-181     exponential_smoother.cc:86-115
-#include <cstdlib>
 #include "loop.cuh"
 #include "trk_item.cuh"
 
@@ -694,13 +693,10 @@ int launch_loop_persistent(LoopDev* loops, int n_loops, int max_epochs, const Lo
     // width: each loop is a latency chain, so with no more loops than SMs a wide CTA is the faster one; beyond that two narrow
     // CTAs per SM overlap each other's serial sections.  On an H100 (400 W), us per epoch: 32 loops 10.1-10.5 at 512 threads,
     // 11.2 at 256; 256 loops 29.5-30.0 at 256 threads, 33.6-34.0 at 512.
-    // B200_LOOP_WIDTH = 256 | 512 forces one (A/B runs).
     int sms = 0, dev = 0;
     B200_CUDA_TRY(cudaGetDevice(&dev));
     B200_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    bool wide = n_loops <= sms;
-    if (const char* env = std::getenv("B200_LOOP_WIDTH")) wide = std::atoi(env) >= kLoopThreadsFew;
-    const int rc = wide
+    const int rc = n_loops <= sms
                        ? launch_loop_persistent_width<kLoopThreadsFew>(loops, n_loops, max_epochs, avail, chans, bands, data, records, rec_capacity,
                              n_records, prompts, tbl_cap, st)
                        : launch_loop_persistent_width<kLoopThreadsMany>(loops, n_loops, max_epochs, avail, chans, bands, data, records, rec_capacity,

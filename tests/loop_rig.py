@@ -2,7 +2,6 @@
 built from them in each loop mode, ring feeding, the integer cases and configurations, the exact references of a peeked
 item (integer taps, float64 taps) and the per-epoch runner peek -> run(1).  The pilot + data helpers at the end give a
 loop a 1-tap data channel beside its pilot."""
-import os
 import types
 
 import numpy as np
@@ -12,24 +11,24 @@ from oracle import loop as ol
 FS = 4e6
 CA_RATE = 1.023e6
 TRUTH_RTOL = 1e-5
-# (mode, B200_LOOP_WIDTH)
-MODES = {"persistent256": (0, "256"), "persistent512": (0, "512"), "per_epoch": (1, None), "sliced": (2, None)}
+# name -> (loop mode, standby loops?).  Mode 0 runs 512-thread CTAs up to one loop per SM and 256-thread CTAs beyond.
+MODES = {"persistent256": (0, True), "persistent512": (0, False), "per_epoch": (1, False), "sliced": (2, False)}
 PERSISTENT = ["persistent256", "persistent512"]
 
 
-def set_mode(monkeypatch, e, name):
-    """loop mode `name` of MODES on engine e.  B200_LOOP_WIDTH goes through monkeypatch when a test passes one (undone
-    after the test), else straight into os.environ (scripts without pytest)."""
-    mode, width = MODES[name]
-    if monkeypatch is None:
-        if width is None:
-            os.environ.pop("B200_LOOP_WIDTH", None)
-        else:
-            os.environ["B200_LOOP_WIDTH"] = width
-    elif width is None:
-        monkeypatch.delenv("B200_LOOP_WIDTH", raising=False)
-    else:
-        monkeypatch.setenv("B200_LOOP_WIDTH", width)
+def set_mode(e, name, sp):
+    """loop mode `name` of MODES on engine e, whose channel 0 is sp's pilot channel (make_engine creates it first).
+    persistent256 adds one standby loop per SM there, never started: in state 0 it leaves the persistent kernel at its first
+    prepare, so the started loops' taps and records do not change.  Standby rows follow the started loops' in every
+    per-loop array and hold nothing defined."""
+    import torch
+    mode, standby = MODES[name]
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    for _ in range(sms if standby else 0):
+        e.loop_create(0, sp.conf)
+    if mode == 0:
+        n_loops = len(e.loop_run(0)[1])          # a run of no epochs launches nothing and returns one count per loop
+        assert (n_loops > sms) == standby, (name, n_loops, sms)
     e.loop_set_mode(mode)
 
 
@@ -257,9 +256,9 @@ def gps_stream(rng, prn, x0, n):
     return code, Stream(int_signal(rng, code, n, 3.0, (-DELAY * rate) % 1023, rate), x0)
 
 
-def window_engine(capi, monkeypatch, mode, specs, caps):
+def window_engine(capi, mode, specs, caps):
     e, ids = make_engine(capi, specs, caps)
-    set_mode(monkeypatch, e, mode)
+    set_mode(e, mode, specs[0])
     return e, ids
 
 

@@ -162,24 +162,41 @@ def test_two_level_radices_against_float64(capi, engine, n, cfar, keep_grid):
 
 
 @pytest.mark.parametrize("n", [
-    25000,    # [8, 25, 25, 5] on 512 threads; [8, 5, 5, 5, 5, 5] on 1024
-    3125,     # [25, 25, 5]; [5, 5, 5, 5, 5]
-    15625,    # [5, 5, 5, 5, 5, 5] either way: six radix-5 stages
+    25000,    # [8, 25, 25, 5] on 512 threads
+    3125,     # [25, 25, 5] on 512 threads
+    15625,    # [5, 5, 5, 5, 5, 5] on 1024 threads: six radix-5 stages
     27648,    # [8, 8, 8, 2, 3, 3, 3]: seven stages, the single-CTA maximum
     4802,     # [2, 7, 7, 7, 7]
     210,      # [2, 3, 7, 5]
 ])
-@pytest.mark.parametrize("radix25", ["1", "0"])
-def test_single_cta_plans_against_float64(capi, engine, monkeypatch, n, radix25):
-    monkeypatch.setenv("B200_ACQ_RADIX25", radix25)   # read when the plan is made, in b200_acq_create
+def test_single_cta_plans_against_float64(capi, engine, n):
     for cfar, keep_grid in ((True, True), (False, True), (False, False)):
         _plan_case(capi, engine, n, cfar, keep_grid, seed=n + 1)
 
 
+def test_fft_plan_only_from_the_size(capi, engine, monkeypatch):
+    """B200_ACQ_RADIX25 in the environment selects nothing: with B200_ACQ_RADIX25=0 a 25 000-point search still plans
+    [8, 25, 25, 5], so its records and grids, which [8, 5, 5, 5, 5, 5] would sum in another order, are the same bytes."""
+    p = _params(25000, keep_grid=True)
+    rng = np.random.default_rng(25)
+    codes = _codes(rng, 3, 25000)
+    iq = _signal(rng, codes, _oracle(p).c, p["fs_in"], [(0, 1.0, 777, 500.0), (1, 0.8, 12345, -1000.0)])
+
+    def search():
+        acq = capi.PcpsAcquisition(engine, **p)
+        for s, code in enumerate(codes):
+            acq.set_local_code(s, code)
+        out = acq.search(iq, [0, 1, 2]).tobytes() + b"".join(acq.read_grid(s).tobytes() for s in range(3))
+        acq.close()
+        return out
+
+    want = search()
+    monkeypatch.setenv("B200_ACQ_RADIX25", "0")
+    assert search() == want
+
+
 @pytest.mark.parametrize("n", [7, 8, 25])   # one stage of 7, one of 8, two of 5
-@pytest.mark.parametrize("radix25", ["1", "0"])
-def test_smallest_sizes_search_right_or_refuse(capi, engine, monkeypatch, n, radix25):
-    monkeypatch.setenv("B200_ACQ_RADIX25", radix25)
+def test_smallest_sizes_search_right_or_refuse(capi, engine, n):
     try:
         capi.PcpsAcquisition(engine, **_params(n, slots=1)).close()
     except capi.B200Error:

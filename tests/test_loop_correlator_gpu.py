@@ -4,7 +4,8 @@ In the tracking state b200_trk_loop_peek_items is a pure function of the loop st
 that item and logs one record carrying the P tap's bits (prompt_I, prompt_Q) and hypotf of every tap (abs_*).  So
 peek -> run(1) -> compare checks every epoch a loop actually produced, in each way the loops can run:
 
-  * mode 0, the persistent CTA per loop, at both widths (B200_LOOP_WIDTH = 256 | 512; the launcher reads it per launch);
+  * mode 0, the persistent CTA per loop, at both widths (512 threads while the engine holds no more loops than the device
+    has SMs, else 256: the narrow case adds loops that are never started);
   * mode 1, the batch correlator with one slice per item and a loop-update launch per epoch;
   * mode 2, the same with each epoch split over several CTAs (batch_slices).
 
@@ -31,11 +32,11 @@ pytestmark = pytest.mark.gpu
 # ---------------------------------------------------------------------------------------------------------------------
 # configurations with integer data
 
-def run_config(capi, monkeypatch, specs, caps, ring, mode, n_ep):
+def run_config(capi, specs, caps, ring, mode, n_ep):
     """-> per-epoch results (run_per_epoch), records of the multi-epoch twin, final status of both"""
     caps = capacities_for(specs, caps)
     e, ids = make_engine(capi, specs, caps)
-    set_mode(monkeypatch, e, mode)
+    set_mode(e, mode, specs[0])
     if ring:
         assert len(specs) == 1
         feeder = RingFeeder(e, 0, specs[0].stream)
@@ -50,7 +51,7 @@ def run_config(capi, monkeypatch, specs, caps, ring, mode, n_ep):
 
     # the twin: the same loops in launches of many epochs
     e, ids = make_engine(capi, specs, caps)
-    set_mode(monkeypatch, e, mode)
+    set_mode(e, mode, specs[0])
     if ring:
         feeder = RingFeeder(e, 0, specs[0].stream)
         start_all(e, ids, specs)
@@ -76,11 +77,11 @@ N_EP = 300
 
 @pytest.mark.parametrize("mode", list(MODES))
 @pytest.mark.parametrize("config", ["gps_ring", "veml_2spc", "galileo_like", "two_bands"])
-def test_integer_epochs_equal_the_integer_oracle(capi, monkeypatch, config, mode):
+def test_integer_epochs_equal_the_integer_oracle(capi, config, mode):
     """(a) every epoch's taps equal the integer oracle exactly, and (c) one launch of many epochs gives the same records,
     byte for byte, as one launch per epoch."""
     specs, caps, ring = int_configs(N_EP)[config]
-    per, multi, st, st2 = run_config(capi, monkeypatch, specs, caps, ring, mode, N_EP)
+    per, multi, st, st2 = run_config(capi, specs, caps, ring, mode, N_EP)
     for i, sp in enumerate(specs):
         items, recs = per[i]
         assert len(recs) == N_EP, (config, i, len(recs))
@@ -131,11 +132,11 @@ def float_configs(n_ep):
 
 @pytest.mark.parametrize("mode", list(MODES))
 @pytest.mark.parametrize("config", ["gps_3taps", "veml_5taps"])
-def test_float_epochs_within_the_float64_truth(capi, monkeypatch, config, mode):
+def test_float_epochs_within_the_float64_truth(capi, config, mode):
     """(b) complex samples with a real Doppler: every epoch's P and |tap| within 1e-5 |P| of the float64 correlation of the
     peeked item, and (c) one launch of many epochs equals one launch per epoch byte for byte."""
     sp = float_configs(N_EP)[config]
-    per, multi, st, st2 = run_config(capi, monkeypatch, [sp], None, False, mode, N_EP)
+    per, multi, st, st2 = run_config(capi, [sp], None, False, mode, N_EP)
     items, recs = per[0]
     assert len(recs) == N_EP
     assert np.all(items["phase_step_rad"] != 0.0)
@@ -144,6 +145,25 @@ def test_float_epochs_within_the_float64_truth(capi, monkeypatch, config, mode):
     assert abs(np.mean(recs["carrier_doppler_hz"][-100:]) - (1234.0 if config == "gps_3taps" else -2710.0)) < 2.0
     assert len(multi[0]) == N_EP and multi[0].tobytes() == recs.tobytes(), (config, mode)
     assert (st[0].sample_counter, st[0].epochs) == (st2[0].sample_counter, st2[0].epochs)
+
+
+def test_loop_width_only_from_the_loop_count(capi, monkeypatch):
+    """B200_LOOP_WIDTH in the environment selects nothing: with B200_LOOP_WIDTH=256 one loop still runs on 512-thread CTAs,
+    so its records on float data, where a 256-thread CTA sums the taps in another order, are the same bytes."""
+    sp = float_configs(N_EP)["gps_3taps"]
+
+    def run():
+        e, ids = make_engine(capi, [sp], capacities_for([sp], None))
+        push_all(e, [sp])
+        start_all(e, ids, [sp])
+        rec, cnt = e.loop_run(N_EP)
+        e.close()
+        assert cnt[0] == N_EP
+        return rec[0].tobytes()
+
+    want = run()
+    monkeypatch.setenv("B200_LOOP_WIDTH", "256")
+    assert run() == want
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -160,7 +180,7 @@ def split_configs():
 
 @pytest.mark.parametrize("mode", PERSISTENT)
 @pytest.mark.parametrize("config", ["gps_float_3taps", "veml_int_5taps", "gps_int_lock_loss"])
-def test_split_update_equals_the_sequential_update(capi, monkeypatch, config, mode):
+def test_split_update_equals_the_sequential_update(capi, config, mode):
     """(d) The persistent kernel updates the loop on three warps at once and, on a lost-lock verdict, restores its backup
     and replays the update.  Feeding its taps to b200_trk_loop_step_taps (the sequential update) on a twin started
     identically must reproduce every peeked item and every record byte for byte; the lock-loss configuration also
@@ -168,7 +188,7 @@ def test_split_update_equals_the_sequential_update(capi, monkeypatch, config, mo
     sp, n_ep = split_configs()[config]
     caps = {0: len(sp.stream.x) + 16}
     e, ids = make_engine(capi, [sp], caps)
-    set_mode(monkeypatch, e, mode)
+    set_mode(e, mode, sp)
     push_all(e, [sp])
     start_all(e, ids, [sp])
     items, recs = run_per_epoch(e, ids, n_ep)[0]
@@ -204,7 +224,7 @@ def test_split_update_equals_the_sequential_update(capi, monkeypatch, config, mo
 # the loops' sample window is [valid_from, write_index)
 
 @pytest.mark.parametrize("mode", list(MODES))
-def test_loops_below_valid_from_stall_after_a_gap(capi, monkeypatch, mode):
+def test_loops_below_valid_from_stall_after_a_gap(capi, mode):
     """iq_push_at(0, A[:60000]) then iq_push_at(1_000_000, B[:30000]) into a 2^16 ring: ring slots below valid_from still
     hold A.  A loop whose epochs lie below 1_000_000 must stall (no record, sample counter frozen after its first
     prepare); a loop started at 1_000_000 tracks B exactly; a loop on another band is unaffected."""
@@ -214,7 +234,7 @@ def test_loops_below_valid_from_stall_after_a_gap(capi, monkeypatch, mode):
     low = LoopSpec(0, code, ol.default_conf(fs_in=FS, prn=3), (DELAY + 0.3, 0.0, 990_000, 990_000), None)
     high = LoopSpec(0, code, ol.default_conf(fs_in=FS, prn=3), (DELAY + 0.3, 0.0, 1_000_000, 1_000_000), b)
     oth = other_band(rng, 12)
-    e, ids = window_engine(capi, monkeypatch, mode, [low, high, oth], {0: 1 << 16, 1: len(oth.stream.x) + 16})
+    e, ids = window_engine(capi, mode, [low, high, oth], {0: 1 << 16, 1: len(oth.stream.x) + 16})
     e.iq_push_at(0, 0, a.x.astype(np.complex64))
     e.iq_push_at(0, 1_000_000, b.x.astype(np.complex64))
     push_all(e, [oth])
@@ -232,7 +252,7 @@ def test_loops_below_valid_from_stall_after_a_gap(capi, monkeypatch, mode):
 
 
 @pytest.mark.parametrize("mode", list(MODES))
-def test_loops_stall_after_iq_forget(capi, monkeypatch, mode):
+def test_loops_stall_after_iq_forget(capi, mode):
     """After b200_iq_forget every sample in the band is history: both of its loops stall, although the ring still holds
     those samples and more arrive behind them; the loop on the other band keeps running."""
     rng = np.random.default_rng(6)
@@ -240,7 +260,7 @@ def test_loops_stall_after_iq_forget(capi, monkeypatch, mode):
     l0 = LoopSpec(0, code, ol.default_conf(fs_in=FS, prn=8), (DELAY + 0.3, 0.0, 0, 0), s)
     l1 = LoopSpec(0, code, ol.default_conf(fs_in=FS, prn=8, early_late_space_chips=0.25), (DELAY - 0.2, 0.0, 0, 0), s)
     oth = other_band(rng, 10)
-    e, ids = window_engine(capi, monkeypatch, mode, [l0, l1, oth], {0: 1 << 17, 1: len(oth.stream.x) + 16})
+    e, ids = window_engine(capi, mode, [l0, l1, oth], {0: 1 << 17, 1: len(oth.stream.x) + 16})
     e.iq_push_at(0, 0, s.x[:60_000].astype(np.complex64))
     push_all(e, [oth])
     start_all(e, ids, [l0, l1, oth])
@@ -259,7 +279,7 @@ def test_loops_stall_after_iq_forget(capi, monkeypatch, mode):
 
 
 @pytest.mark.parametrize("mode", list(MODES))
-def test_loops_follow_a_restarted_stream(capi, monkeypatch, mode):
+def test_loops_follow_a_restarted_stream(capi, mode):
     """A stream at 1_000_000 into a 2^16 ring, then a restart iq_push_at at the older index 500_000.  The loop on the old
     stream stalls, a loop started at 500_000 runs on the new samples exactly, and one started at 480_000 (below the new
     valid_from, yet inside what the ring's slots span) stalls instead of correlating the old stream."""
@@ -272,7 +292,7 @@ def test_loops_follow_a_restarted_stream(capi, monkeypatch, mode):
     below = LoopSpec(0, code, conf, (DELAY + 0.3, 0.0, 480_000, 480_000), None)
     oth = other_band(rng, 12)
     specs = [old, new, below, oth]
-    e, ids = window_engine(capi, monkeypatch, mode, specs, {0: 1 << 16, 1: len(oth.stream.x) + 16})
+    e, ids = window_engine(capi, mode, specs, {0: 1 << 16, 1: len(oth.stream.x) + 16})
     e.iq_push_at(0, 1_000_000, s1.x.astype(np.complex64))
     push_all(e, [oth])
     e.loop_start(ids[0], *old.start)

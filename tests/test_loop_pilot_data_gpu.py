@@ -79,10 +79,10 @@ def int_configs(n_ep):
     }
 
 
-def run_config(capi, monkeypatch, specs, data, caps, ring, mode, n_ep):
+def run_config(capi, specs, data, caps, ring, mode, n_ep):
     caps = tl.capacities_for(specs, caps)
     e, ids, _ = tl.make_engine_with_data(capi, specs, data, caps)
-    tl.set_mode(monkeypatch, e, mode)
+    tl.set_mode(e, mode, specs[0])
     if ring:
         feeder = tl.RingFeeder(e, 0, specs[0].stream)
         tl.start_all(e, ids, specs)
@@ -97,9 +97,9 @@ def run_config(capi, monkeypatch, specs, data, caps, ring, mode, n_ep):
 
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("config", ["epl_1023_ring", "veml_sinboc_8184", "two_bands_one_data"])
-def test_integer_data_prompt_equals_the_integer_oracle(capi, monkeypatch, config, mode):
+def test_integer_data_prompt_equals_the_integer_oracle(capi, config, mode):
     specs, data, caps, ring = int_configs(N_EP)[config]
-    per = run_config(capi, monkeypatch, specs, data, caps, ring, mode, N_EP)
+    per = run_config(capi, specs, data, caps, ring, mode, N_EP)
     for i, (sp, dt) in enumerate(zip(specs, data)):
         items, recs, pilots = per[i]
         assert len(recs) == N_EP, (config, i, len(recs))
@@ -118,10 +118,10 @@ def test_integer_data_prompt_equals_the_integer_oracle(capi, monkeypatch, config
 
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("veml", [0, 1])
-def test_float_data_prompt_within_the_float64_truth(capi, monkeypatch, veml, mode):
+def test_float_data_prompt_within_the_float64_truth(capi, veml, mode):
     sp, dt = tl.pilot_data_spec(5, 25, 1234.0 if not veml else -2710.0, 1777, N_EP, veml=veml)
     e, ids, _ = tl.make_engine_with_data(capi, [sp], [dt], {0: len(sp.stream.x) + 16})
-    tl.set_mode(monkeypatch, e, mode)
+    tl.set_mode(e, mode, sp)
     tl.push_all(e, [sp])
     tl.start_all(e, ids, [sp])
     items, recs, pilots = run_per_epoch(e, ids, N_EP)[0]
@@ -157,13 +157,13 @@ PROMPT_FIELDS = ("prompt_I", "prompt_Q")   # zeroed on copies: a multi-field vie
 
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("config", ["gps_float_3taps", "veml_sinboc_int", "gps_int_lock_loss"])
-def test_a_data_channel_changes_nothing_but_the_record_prompt(capi, monkeypatch, config, mode):
+def test_a_data_channel_changes_nothing_but_the_record_prompt(capi, config, mode):
     sp, dt, n_ep = twin_configs()[config]
     caps = {0: len(sp.stream.x) + 16}
     out = []
     for data in ([dt], [None]):
         e, ids, _ = tl.make_engine_with_data(capi, [sp], data, caps)
-        tl.set_mode(monkeypatch, e, mode)
+        tl.set_mode(e, mode, sp)
         tl.push_all(e, [sp])
         tl.start_all(e, ids, [sp])
         rec, cnt, prm = e.loop_run_prompts(n_ep)
@@ -187,13 +187,13 @@ def test_a_data_channel_changes_nothing_but_the_record_prompt(capi, monkeypatch,
 
 @pytest.mark.parametrize("mode", tl.PERSISTENT)
 @pytest.mark.parametrize("config", ["gps_float_3taps", "veml_sinboc_int", "gps_int_lock_loss"])
-def test_persistent_taps_replay_through_step_taps(capi, monkeypatch, config, mode):
+def test_persistent_taps_replay_through_step_taps(capi, config, mode):
     """the persistent kernel's pilot taps (rebuilt from the record and the returned pilot prompt) and its data tap, in the
     slot after the pilot taps, fed to the sequential update of a twin reproduce every item, record and the final status"""
     sp, dt, n_ep = twin_configs()[config]
     caps = {0: len(sp.stream.x) + 16}
     e, ids, _ = tl.make_engine_with_data(capi, [sp], [dt], caps)
-    tl.set_mode(monkeypatch, e, mode)
+    tl.set_mode(e, mode, sp)
     tl.push_all(e, [sp])
     tl.start_all(e, ids, [sp])
     items, recs, pilots = run_per_epoch(e, ids, n_ep)[0]
@@ -230,13 +230,13 @@ def test_persistent_taps_replay_through_step_taps(capi, monkeypatch, config, mod
 # navigation symbols come out of the records
 
 @pytest.mark.parametrize("mode", MODES)
-def test_data_prompts_carry_the_symbols(capi, monkeypatch, mode):
+def test_data_prompts_carry_the_symbols(capi, mode):
     n_ep, settle = 400, 100
     rng = np.random.default_rng(3)
     sym = (2 * rng.integers(0, 2, n_ep + 8) - 1).astype(np.float64)
     sp, dt = tl.pilot_data_spec(7, 22, 1500.0, 1234, n_ep, symbols=sym, cn0=50.0, pull_in_now=True)
     e, ids, _ = tl.make_engine_with_data(capi, [sp], [dt], {0: len(sp.stream.x) + 16})
-    tl.set_mode(monkeypatch, e, mode)
+    tl.set_mode(e, mode, sp)
     tl.push_all(e, [sp])
     tl.start_all(e, ids, [sp])
     rec, cnt, prm = e.loop_run_prompts(n_ep)
@@ -290,7 +290,7 @@ def test_set_data_channel_refuses_each_broken_rule(capi, rule):
 
 
 @pytest.mark.parametrize("mode", MODES)
-def test_replacing_the_data_channel_between_runs(capi, monkeypatch, mode):
+def test_replacing_the_data_channel_between_runs(capi, mode):
     n_ep = 40
     rng = np.random.default_rng(12)
     sp = tl.gps_int_case(rng, 2 * n_ep)
@@ -299,7 +299,7 @@ def test_replacing_the_data_channel_between_runs(capi, monkeypatch, mode):
     e, ids, dids = tl.make_engine_with_data(capi, [sp], [tables[0]], {0: len(sp.stream.x) + 16})
     second = e.channel_create(0, 1)
     e.channel_set_code(second, tables[1], [0.0])
-    tl.set_mode(monkeypatch, e, mode)
+    tl.set_mode(e, mode, sp)
     tl.push_all(e, [sp])
     tl.start_all(e, ids, [sp])
     for table in tables:

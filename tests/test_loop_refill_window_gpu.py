@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("mode", list(tl.MODES))
-def test_loops_stall_past_a_partial_refill(capi, monkeypatch, mode):
+def test_loops_stall_past_a_partial_refill(capi, mode):
     """A device buffer of 60_000 samples attached at 2_000_000 and filled with stream A, then b200_iq_refill of B[:30_000] at
     the same index.  A loop started at 2_000_000 tracks B exactly for the epochs inside the refill, then stalls (no record,
     sample counter frozen); a loop on another band is unaffected."""
@@ -26,7 +26,7 @@ def test_loops_stall_past_a_partial_refill(capi, monkeypatch, mode):
     code, b = tl.gps_stream(rng, 3, x0, 30_000)
     loop = tl.LoopSpec(0, code, ol.default_conf(fs_in=tl.FS, prn=3), (tl.DELAY + 0.3, 0.0, x0, x0), b)
     oth = tl.other_band(rng, 16)
-    e, ids = tl.window_engine(capi, monkeypatch, mode, [loop, oth], {1: len(oth.stream.x) + 16})
+    e, ids = tl.window_engine(capi, mode, [loop, oth], {1: len(oth.stream.x) + 16})
     buf = torch.zeros(2 * len(a.x), dtype=torch.float32, device="cuda")
     torch.cuda.synchronize()
     e.iq_attach_dev(0, buf.data_ptr(), len(a.x), x0)

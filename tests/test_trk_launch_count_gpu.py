@@ -85,11 +85,11 @@ def test_single_correlators_count_one_launch_each(capi):
     ("per_epoch", True, lambda ep: 1 + ep * 3),   # pilot items and data items: two correlator launches per epoch
     ("sliced", True, lambda ep: 1 + ep * 3),
 ])
-def test_loop_run_counts_its_launches(capi, monkeypatch, mode, with_data, launches):
+def test_loop_run_counts_its_launches(capi, mode, with_data, launches):
     n_ep = 5
     sp, dt = tl.pilot_data_spec(5, 25, 1234.0, 1777, n_ep)
     e, ids, _ = tl.make_engine_with_data(capi, [sp], [dt if with_data else None], {0: len(sp.stream.x) + 16})
-    tl.set_mode(monkeypatch, e, mode)
+    tl.set_mode(e, mode, sp)
     tl.push_all(e, [sp])
     tl.start_all(e, ids, [sp])
     k0 = e.launch_count()

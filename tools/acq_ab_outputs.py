@@ -5,9 +5,9 @@
   python tools/acq_ab_outputs.py --compare a.npz b.npz         # names the first array that differs
 
 Inputs are random +-1 codes and noisy code-modulated carriers from numpy's seeded generator.  The cases reach every plan
-family: single-level N = 4000, 16 000 and 25 000 (radix-25 stages on 512 threads, and without them on 1024), two-level
-N with each global radix 2, 3, 4, 5, 7, 8, 10, chirp-z sizes, and the fine Doppler estimate at a single- and a two-level
-size.  On one single-level and one two-level size every search option runs as well.
+family: single-level N = 4000, 16 000 and 25 000, two-level N with each global radix 2, 3, 4, 5, 7, 8, 10, chirp-z sizes,
+and the fine Doppler estimate at a single- and a two-level size.  On one single-level and one two-level size every search
+option runs as well.
 """
 import ctypes as C
 import os
@@ -55,13 +55,11 @@ def main(out_path):
         return rng.integers(-200, 200, 2 * n).astype(np.int16)
 
     def case(name, spms, *, cfar=True, keep_grid=True, dwells=1, bits=False, ms_per_code=1, sampled_ms=1, center=0, step_two=False,
-             i16_search=False, dev=False, selftest=False, radix25=True):
-        os.environ["B200_ACQ_RADIX25"] = "1" if radix25 else "0"  # read when the plan is made
+             i16_search=False, dev=False, selftest=False):
         fs = int(spms * 1000)
         acq = capi.PcpsAcquisition(eng, fs_in=fs, samples_per_ms=float(spms), samples_per_chip=max(1, int(fs / 1.023e6)), doppler_max=1000,
                                    doppler_step=500, use_CFAR_algorithm_flag=cfar, keep_grid=keep_grid, max_dwells=dwells, n_code_slots=2,
                                    bit_transition_flag=bits, sampled_ms=sampled_ms, ms_per_code=ms_per_code)
-        os.environ.pop("B200_ACQ_RADIX25")
         c = acq.conf
         need = c.fft_size // 2 if c.code_layout == 1 else c.consumed_samples
         codes = [rng.choice([-1.0, 1.0], need).astype(np.complex64) for _ in range(2)]
@@ -105,7 +103,6 @@ def main(out_path):
 
     for n in SINGLE + TWO_LEVEL:
         case(f"n{n}", n)
-    case("n25000_radix25_off", 25000, radix25=False)
     for name, spms in (("single", 4000), ("two_level", 50000)):
         half = spms // 2  # bit transition and layout 2 keep fft_size = spms
         case(f"{name}_nocfar_grid", spms, cfar=False)

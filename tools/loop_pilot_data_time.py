@@ -4,9 +4,10 @@ data channel.
     python tools/loop_pilot_data_time.py [--baseline DIR] [--rounds 3] [--out FILE]
 
 Each loop: 8184-entry sinBOC(1,1) pilot table, VEML taps, 4 ms epochs of 16 000 samples (4 Msps) or 200 000 samples
-(50 Msps); each loop with a data channel also has its own 8184-entry data table.  32 and 64 loops, mode 0 (the persistent
-kernel) at both CTA widths (B200_LOOP_WIDTH = 256 | 512).  The samples are noise: the lock detectors are switched off so
-that every loop runs every epoch.
+(50 Msps); each loop with a data channel also has its own 8184-entry data table.  32, 64 and 256 loops in mode 0, the
+persistent kernel, which takes 512-thread CTAs while the loops are no more than the SMs and 256-thread CTAs beyond that: on
+a 132-SM H100 the first two counts time the wide CTA, the third the narrow one.  The samples are noise: the lock detectors
+are switched off so that every loop runs every epoch.
 
 --baseline DIR: a checkout of another version with its library and oracle built.  Each round then runs both libraries, one after
 the other, each in a fresh process; the baseline's legs without a data channel are timed if it has no
@@ -22,6 +23,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EPOCHS = {16000: (4e6, 100), 200000: (50e6, 30)}   # samples per epoch -> (fs, timed epochs per run)
+LOOPS = (32, 64, 256)
 WARM = 2
 REPEATS = 5
 
@@ -36,12 +38,12 @@ def child(root: str, label: str):
 
     has_data = hasattr(capi.lib, "b200_trk_loop_set_data_channel")
     rng = np.random.default_rng(1)
-    tables = [oracle.port.sinboc11((2 * rng.integers(0, 2, 4092) - 1).astype(np.int32)) for _ in range(128)]
+    tables = [oracle.port.sinboc11((2 * rng.integers(0, 2, 4092) - 1).astype(np.int32)) for _ in range(2 * LOOPS[-1])]
     shifts = [-1.0, -0.3, 0.0, 0.3, 1.0]
     for n_ep_samples, (fs, k) in EPOCHS.items():
         n_iq = n_ep_samples * (WARM + k + 2)
         iq = (rng.standard_normal(n_iq) + 1j * rng.standard_normal(n_iq)).astype(np.complex64)
-        for n_loops in (32, 64):
+        for n_loops in LOOPS:
             for data in ((False, True) if has_data else (False,)):
                 e = capi.Engine(0)
                 e.iq_create(0, n_iq + 16)
@@ -60,25 +62,23 @@ def child(root: str, label: str):
                         e.loop_set_data_channel(lid, dch)
                     ids.append(lid)
                 e.loop_set_mode(0)
-                for width in ("256", "512"):
-                    os.environ["B200_LOOP_WIDTH"] = width
-                    times = []
-                    for _ in range(REPEATS + 1):
-                        for j, lid in enumerate(ids):
-                            e.loop_start(lid, 100.0 + 37 * j, 0.0, 0, 0)
-                        rc = capi.lib.b200_trk_loop_run(e.h, WARM, None, None)
-                        assert rc == 0
-                        e.timer_start()
-                        rc = capi.lib.b200_trk_loop_run(e.h, k, None, None)
-                        ms = e.timer_stop_ms()
-                        assert rc == 0
-                        times.append(ms)
-                    st = [e.loop_status(lid) for lid in ids]
-                    assert all(s.state == 2 for s in st), "a loop stopped"
-                    times = sorted(times[1:])
-                    print(json.dumps(dict(lib=label, samples_per_epoch=n_ep_samples, loops=n_loops, data_channel=data, width=int(width),
-                                          us_per_epoch_median=round(1000.0 * times[len(times) // 2] / k, 3),
-                                          us_per_epoch_min=round(1000.0 * times[0] / k, 3))), flush=True)
+                times = []
+                for _ in range(REPEATS + 1):
+                    for j, lid in enumerate(ids):
+                        e.loop_start(lid, 100.0 + 37 * j, 0.0, 0, 0)
+                    rc = capi.lib.b200_trk_loop_run(e.h, WARM, None, None)
+                    assert rc == 0
+                    e.timer_start()
+                    rc = capi.lib.b200_trk_loop_run(e.h, k, None, None)
+                    ms = e.timer_stop_ms()
+                    assert rc == 0
+                    times.append(ms)
+                st = [e.loop_status(lid) for lid in ids]
+                assert all(s.state == 2 for s in st), "a loop stopped"
+                times = sorted(times[1:])
+                print(json.dumps(dict(lib=label, samples_per_epoch=n_ep_samples, loops=n_loops, data_channel=data,
+                                      us_per_epoch_median=round(1000.0 * times[len(times) // 2] / k, 3),
+                                      us_per_epoch_min=round(1000.0 * times[0] / k, 3))), flush=True)
                 e.close()
 
 

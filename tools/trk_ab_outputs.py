@@ -23,8 +23,8 @@ Each case is sized for the path it names (STEP = 1.023 Mchip/s at 4 Msps, 0.2558
     off_table            rem = 2e6 chips: warp_correlate_general
     linear_band          an attached band whose last tiles are clipped at its end
   and the same items through the per-item kernel with a single tap count (only_mask = 0), two slices;
-  the three single correlators; the device loops in modes 0, 1 and 2 with and without a data channel (records, pilot
-  prompts, final status).
+  the three single correlators; the device loops in modes 0 (at both CTA widths), 1 and 2 with and without a data channel
+  (records, pilot prompts, final status).
 """
 import os
 import sys
@@ -157,10 +157,10 @@ def main(out_path):
         for with_data in (False, True):
             sp, dt = tl.pilot_data_spec(5, 25, 1234.0, 1777, 60)
             e, ids, _ = tl.make_engine_with_data(capi, [sp], [dt if with_data else None], {0: len(sp.stream.x) + 16})
-            tl.set_mode(None, e, mode)
+            tl.set_mode(e, mode, sp)
             tl.push_all(e, [sp])
             tl.start_all(e, ids, [sp])
-            rec, cnt, prm = e.loop_run_prompts(60)
+            rec, cnt, prm = (a[:len(ids)] for a in e.loop_run_prompts(60))   # the started loop, not the standby ones
             name = f"loop.{mode}.{'data' if with_data else 'pilot'}"
             out[name + ".records"] = rec
             out[name + ".n_records"] = np.asarray(cnt)
