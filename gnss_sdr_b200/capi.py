@@ -44,6 +44,7 @@ _SIGS = {
     "b200_engine_timer_stop_ms": ([_vp, C.POINTER(C.c_float)], C.c_int),
     "b200_engine_launch_count": ([_vp, C.POINTER(C.c_uint64)], C.c_int),
     "b200_iq_create": ([_vp, C.c_int, C.c_uint64], C.c_int),
+    "b200_iq_create_typed": ([_vp, C.c_int, C.c_uint64, C.c_char_p], C.c_int),
     "b200_iq_push": ([_vp, C.c_int, _vp, C.c_uint64, C.POINTER(C.c_uint64)], C.c_int),
     "b200_iq_push_at": ([_vp, C.c_int, C.c_uint64, _vp, C.c_uint64, C.POINTER(C.c_uint64)], C.c_int),
     "b200_iq_window": ([_vp, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)], C.c_int),
@@ -168,8 +169,10 @@ class Engine:
         return n.value
 
     # bands
-    def iq_create(self, band: int, capacity: int):
-        _chk(lib.b200_iq_create(self.h, band, capacity), "b200_iq_create")
+    def iq_create(self, band: int, capacity: int, item_type: str = "gr_complex"):
+        """item_type: "gr_complex" (float samples), "ishort" or "ibyte" (interleaved int16 / int8 I,Q kept at their own
+        width; such a band takes only iq_push_int / iq_push_file pushes of its own type)"""
+        _chk(lib.b200_iq_create_typed(self.h, band, capacity, item_type.encode()), "b200_iq_create_typed")
 
     def iq_push(self, band: int, iq: np.ndarray) -> int:
         iq = np.ascontiguousarray(iq, np.complex64)

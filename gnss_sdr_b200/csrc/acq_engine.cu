@@ -499,10 +499,10 @@ extern "C"
         B200_CUDA_TRY(cudaStreamWaitEvent(a->stream, e->copy_done, 0));
         if (b.raw_last >= 0) B200_CUDA_TRY(cudaStreamWaitEvent(a->stream, b.raw_free[b.raw_last], 0));
         // a ring window may wrap around the ring's end; an attached buffer is linear from first_index (mask ~0), and the
-        // window check keeps the window inside it
+        // window check keeps the window inside it.  A narrow band is read at its own width (AcqInput::at widens on load).
         const unsigned long long off = (abs_index - b.first_index) & b.mask;
         const unsigned long long run = b.capacity - off;
-        *in = AcqInput{b.base + off, static_cast<int>(n < run ? n : run), b.base};
+        *in = AcqInput{static_cast<const char*>(b.base) + off * 2ULL * b.fmt, static_cast<int>(n < run ? n : run), b.base, b.fmt};
         return B200_OK;
     }
 

@@ -144,7 +144,8 @@ __global__ void __launch_bounds__(THREADS, 1) acq_code_fft_kernel(const float2* 
 }
 
 // ---- forward: wipe-off + FFT, one CTA per Doppler bin ------------------------------------------------
-template <int THREADS>
+// FMT: the SampleFormat of the input (in.fmt); narrow samples are widened to float on load, exactly
+template <int THREADS, int FMT>
 __global__ void __launch_bounds__(THREADS, 1) acq_fwd_kernel(AcqInput in, int consumed,
     const float2* __restrict__ wipe, float2* __restrict__ X, FftPlan pl, const float2* __restrict__ tw)
 {
@@ -156,7 +157,7 @@ __global__ void __launch_bounds__(THREADS, 1) acq_fwd_kernel(AcqInput in, int co
     for (int i = threadIdx.x; i < n; i += blockDim.x)
         {
             // acquisition_core zero-pads beyond consumed samples (:657-664); volk_32fc_x2_multiply_32fc (:531)
-            s[i] = (i < consumed) ? cmul_rn(in(i), w[i]) : make_float2(0.f, 0.f);
+            s[i] = (i < consumed) ? cmul_rn(in.at<FMT>(i), w[i]) : make_float2(0.f, 0.f);
         }
     fft_forward_to_global<false, THREADS == kAcqThreads25>(s, pl, tw, X + static_cast<size_t>(d) * n);
 }
@@ -286,18 +287,19 @@ __global__ void __launch_bounds__(THREADS, 1) acq_corr_kernel(const float2* __re
 // Forward: one radix-n1 DIF stage through global memory (block length n_total, sub-length n), then the
 // in-shared-memory plan on each of the n1 blocks.  Inverse: the blocks first, then the radix-n1 DIT stage,
 // whose natural-order outputs feed the statistics directly.  Layout stays "digit reversed" end to end.
+template <int FMT>
 __device__ __forceinline__ float2 acq_source(const AcqInput& in, const float2* __restrict__ wipe, int i, int consumed,
     int layout, int n_total)
 {
     // wipe != nullptr: signal * wipe-off, zero-padded beyond consumed (acquisition_core :657-664, :531)
-    // wipe == nullptr: local code placed by `layout`, from the linear buffer in.a
-    if (wipe != nullptr) return (i < consumed) ? cmul_rn(in(i), wipe[i]) : make_float2(0.f, 0.f);
-    return acq_code_sample(in.a, i, n_total, consumed, layout);
+    // wipe == nullptr: local code placed by `layout`, from the linear float buffer in.a
+    if (wipe != nullptr) return (i < consumed) ? cmul_rn(in.at<FMT>(i), wipe[i]) : make_float2(0.f, 0.f);
+    return acq_code_sample(static_cast<const float2*>(in.a), i, n_total, consumed, layout);
 }
 
 // in_stride / wipe_stride: elements between the inputs / multiplier tables of consecutive rows (0 = one shared by all rows;
-// in_stride > 0 only with a linear input)
-template <int R>
+// in_stride > 0 only with a linear float input); FMT: the SampleFormat of the input (in.fmt)
+template <int R, int FMT>
 __global__ void acq_global_fwd_stage(AcqInput in, int consumed, int layout, const float2* __restrict__ wipe,
     float2* __restrict__ X, FftPlan pl, const float2* __restrict__ tw, size_t in_stride, size_t wipe_stride)
 {
@@ -306,10 +308,10 @@ __global__ void acq_global_fwd_stage(AcqInput in, int consumed, int layout, cons
     if (j >= n2) return;
     const int d = blockIdx.y;
     const float2* w = wipe ? wipe + static_cast<size_t>(d) * wipe_stride : nullptr;
-    in.a += static_cast<size_t>(d) * in_stride;
+    in.a = static_cast<const float2*>(in.a) + static_cast<size_t>(d) * in_stride;
     float2 v[R];
 #pragma unroll
-    for (int q = 0; q < R; q++) v[q] = acq_source(in, w, j + q * n2, consumed, layout, pl.n_total);
+    for (int q = 0; q < R; q++) v[q] = acq_source<FMT>(in, w, j + q * n2, consumed, layout, pl.n_total);
     Bfly<R>::fwd(v);
     const float2 w1 = __ldg(tw + pl.tw_goff + j);
     float2 wp = w1;
@@ -611,10 +613,14 @@ int set_attrs()
     if (once_dev < 0) return B200_OK;
     const int bytes = kAcqMaxSmemPoints * static_cast<int>(sizeof(float2));
     B200_CUDA_TRY(cudaFuncSetAttribute(acq_code_fft_kernel<kAcqThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-    B200_CUDA_TRY(cudaFuncSetAttribute(acq_fwd_kernel<kAcqThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    B200_CUDA_TRY(cudaFuncSetAttribute(acq_fwd_kernel<kAcqThreads, kCf32>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    B200_CUDA_TRY(cudaFuncSetAttribute(acq_fwd_kernel<kAcqThreads, kI16>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    B200_CUDA_TRY(cudaFuncSetAttribute(acq_fwd_kernel<kAcqThreads, kI8>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     B200_CUDA_TRY(cudaFuncSetAttribute(acq_corr_kernel<kAcqThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     B200_CUDA_TRY(cudaFuncSetAttribute(acq_code_fft_kernel<kAcqThreads25>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-    B200_CUDA_TRY(cudaFuncSetAttribute(acq_fwd_kernel<kAcqThreads25>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    B200_CUDA_TRY(cudaFuncSetAttribute(acq_fwd_kernel<kAcqThreads25, kCf32>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    B200_CUDA_TRY(cudaFuncSetAttribute(acq_fwd_kernel<kAcqThreads25, kI16>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    B200_CUDA_TRY(cudaFuncSetAttribute(acq_fwd_kernel<kAcqThreads25, kI8>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     B200_CUDA_TRY(cudaFuncSetAttribute(acq_corr_kernel<kAcqThreads25>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     B200_CUDA_TRY(cudaFuncSetAttribute(acq_block_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     B200_CUDA_TRY(cudaFuncSetAttribute(acq_corr_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
@@ -794,7 +800,7 @@ int acq_launch_code_fft(const float2* code, int consumed, int layout, float2* ou
     else
         {
             const dim3 g((pl.n + 255) / 256, 1);
-            rc = dispatch_radix(pl.n1, [&](auto R) { acq_global_fwd_stage<decltype(R)::value><<<g, 256, 0, st>>>(AcqInput::linear(code), consumed, layout, nullptr, out, pl, tw, 0, 0); });
+            rc = dispatch_radix(pl.n1, [&](auto R) { acq_global_fwd_stage<decltype(R)::value, kCf32><<<g, 256, 0, st>>>(AcqInput::linear(code), consumed, layout, nullptr, out, pl, tw, 0, 0); });
             if (rc) return rc;
             acq_block_fft_kernel<<<dim3(pl.n1, 1), kAcqThreads, pl.n * sizeof(float2), st>>>(out, pl, tw, 1);
         }
@@ -809,14 +815,24 @@ int acq_launch_fwd(AcqInput in, int consumed, const float2* wipe, float2* X, int
     if (rc) return rc;
     if (pl.n1 == 1)
         {
-            dispatch_threads(pl, [&](auto T) {
-                acq_fwd_kernel<decltype(T)::value><<<bins, decltype(T)::value, pl.n * sizeof(float2), st>>>(in, consumed, wipe, X, pl, tw);
+            rc = with_format(in.fmt, [&](auto F) {
+                dispatch_threads(pl, [&](auto T) {
+                    acq_fwd_kernel<decltype(T)::value, decltype(F)::value><<<bins, decltype(T)::value, pl.n * sizeof(float2), st>>>(in, consumed, wipe,
+                        X, pl, tw);
+                });
+                return B200_OK;
             });
+            if (rc) return rc;
         }
     else
         {
             const dim3 g((pl.n + 255) / 256, bins);
-            rc = dispatch_radix(pl.n1, [&](auto R) { acq_global_fwd_stage<decltype(R)::value><<<g, 256, 0, st>>>(in, consumed, 0, wipe, X, pl, tw, 0, static_cast<size_t>(pl.n_total)); });
+            rc = with_format(in.fmt, [&](auto F) {
+                return dispatch_radix(pl.n1, [&](auto R) {
+                    acq_global_fwd_stage<decltype(R)::value, decltype(F)::value><<<g, 256, 0, st>>>(in, consumed, 0, wipe, X, pl, tw, 0,
+                        static_cast<size_t>(pl.n_total));
+                });
+            });
             if (rc) return rc;
             acq_block_fft_kernel<<<dim3(pl.n1, bins), kAcqThreads, pl.n * sizeof(float2), st>>>(X, pl, tw, 0);
         }
@@ -911,7 +927,12 @@ int acq_launch_fwd_rows(AcqInput in, size_t in_stride, int consumed, const float
     if (rc) return rc;
     if (pl.n1 < 2) return B200_ERR_ARG;
     const dim3 g((pl.n + 255) / 256, rows);
-    rc = dispatch_radix(pl.n1, [&](auto R) { acq_global_fwd_stage<decltype(R)::value><<<g, 256, 0, st>>>(in, consumed, 0, mult, X, pl, tw, in_stride, mult_stride); });
+    rc = with_format(in.fmt, [&](auto F) {
+        return dispatch_radix(pl.n1, [&](auto R) {
+            acq_global_fwd_stage<decltype(R)::value, decltype(F)::value><<<g, 256, 0, st>>>(in, consumed, 0, mult, X, pl, tw, in_stride,
+                mult_stride);
+        });
+    });
     if (rc) return rc;
     acq_block_fft_kernel<<<dim3(pl.n1, rows), kAcqThreads, pl.n * sizeof(float2), st>>>(X, pl, tw, 0);
     B200_CUDA_TRY(cudaGetLastError());

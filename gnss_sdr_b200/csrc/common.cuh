@@ -60,25 +60,86 @@ struct DeviceOnce
     }
 };
 
-// One conditioned IQ stream resident in HBM.  Sample with absolute index i lives at
-// base[(i - first_index) & mask]; attach-mode (linear) bands use mask = ~0.
+// A band's sample type, by bytes per component: gr_complex (float I, Q), and interleaved (I, Q) int16 (lv_16sc_t, the
+// reference's "ishort") and int8 ("ibyte") pairs.  A sample takes 2 * format bytes.
+enum SampleFormat
+{
+    kI8 = 1,
+    kI16 = 2,
+    kCf32 = 4,
+};
+
+// f(std::integral_constant<int, F>{}) for the SampleFormat F that equals fmt; B200_ERR_ARG when there is none
+template <class F>
+int with_format(int fmt, const F& f)
+{
+    switch (fmt)
+        {
+        case kCf32: return f(std::integral_constant<int, kCf32>{});
+        case kI16: return f(std::integral_constant<int, kI16>{});
+        case kI8: return f(std::integral_constant<int, kI8>{});
+        default: set_error("unknown sample format %d", fmt); return B200_ERR_ARG;
+        }
+}
+
+// int -> float of narrow sample components (I2F; exact for every int16 and int8).  w holds (I, Q) of one int16 sample, or of
+// int8 samples in bytes (2K, 2K + 1).  The exact I2F-free alternative (the biased component permuted into the mantissa of
+// 2^23, then one FADD) was measured against it on an H100 80GB HBM3 (700 W), per-item kernel, ms per step: C2 distinct-IQ
+// ishort 0.707 vs 0.689 (I2F), ibyte 0.638 vs 0.648; C2 shared layout ishort 1.224 vs 1.186, ibyte 1.214 vs 1.223.  Neither
+// wins on both widths, and only I2F keeps every instantiation spill-free (the permute form spilled at 8 taps on ishort).
+__device__ __forceinline__ float2 widen_i16(unsigned int w)
+{
+    return make_float2(static_cast<float>(static_cast<short>(w & 0xffffu)), static_cast<float>(static_cast<short>(w >> 16)));
+}
+template <int K>
+__device__ __forceinline__ float2 widen_i8(unsigned int w)
+{
+    return make_float2(static_cast<float>(static_cast<signed char>((w >> (16 * K)) & 0xffu)),
+        static_cast<float>(static_cast<signed char>((w >> (16 * K + 8)) & 0xffu)));
+}
+
+// the raw element of one sample of SampleFormat FMT, and that element widened to float
+template <int FMT>
+using SampleRaw = std::conditional_t<FMT == kCf32, float2, std::conditional_t<FMT == kI16, unsigned int, unsigned short>>;
+template <int FMT>
+__device__ __forceinline__ float2 widen(SampleRaw<FMT> v)
+{
+    if constexpr (FMT == kCf32)
+        return v;
+    else if constexpr (FMT == kI16)
+        return widen_i16(v);
+    else
+        return widen_i8<0>(v);
+}
+
+// One conditioned IQ stream resident in HBM.  Sample with absolute index i lives at sample slot (i - first_index) & mask
+// from base, each slot 2 * fmt bytes; attach-mode (linear) bands use mask = ~0.
 struct BandDesc
 {
-    const float2* base;
+    const void* base;
     unsigned long long mask;
     unsigned long long first_index;
     unsigned long long limit;  // samples addressable from base (ring capacity or attached length)
+    int fmt;                   // SampleFormat
 };
 
-// The samples an acquisition forward stage reads: x(i) = a[i] for i < na, b[i - na] from there on.  A window of a band is at
-// most two linear runs (it may wrap around the ring's end); a linear buffer is one run, with na past every index.
+// The samples an acquisition forward stage reads: x(i) = a[i] for i < na, b[i - na] from there on, in format fmt.  A window
+// of a band is at most two linear runs (it may wrap around the ring's end); a linear buffer is one run of float2, with na
+// past every index.
 struct AcqInput
 {
-    const float2* a;
+    const void* a;
     int na;
-    const float2* b;
-    static AcqInput linear(const float2* p) { return AcqInput{p, 0x7fffffff, nullptr}; }
-    __device__ __forceinline__ float2 operator()(int i) const { return __ldg(i < na ? a + i : b + (i - na)); }
+    const void* b;
+    int fmt;  // SampleFormat
+    static AcqInput linear(const float2* p) { return AcqInput{p, 0x7fffffff, nullptr, kCf32}; }
+    // x(i) for an input of format FMT (== fmt), widened to float on load
+    template <int FMT>
+    __device__ __forceinline__ float2 at(int i) const
+    {
+        using Raw = SampleRaw<FMT>;
+        return widen<FMT>(__ldg(i < na ? static_cast<const Raw*>(a) + i : static_cast<const Raw*>(b) + (i - na)));
+    }
 };
 
 // One tracking channel registration: code table (device), its length, taps and shifts.
@@ -117,12 +178,14 @@ int with_taps(int taps, const F& f)
 }
 
 // Launchers (trk_kernels.cu).  All pointers are device-accessible.  Each adds the number of kernels it issued to `launched`.
-// taps_mask: bit t set when some channel with a code table has t taps (one launch per tap count; an empty mask is an error)
+// taps_mask: bit t set when some channel with a code table has t taps; fmt_mask: bit f set when some such channel is on a band
+// of SampleFormat f.  One launch per (tap count, format) pair; an empty mask is an error.
 int launch_trk_batch(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands,
     float2* out, int out_stride, int slices, float2* partial, unsigned int* counters,
-    int max_code_len, unsigned int taps_mask, cudaStream_t stream, uint64_t& launched);
+    int max_code_len, unsigned int taps_mask, unsigned int fmt_mask, cudaStream_t stream, uint64_t& launched);
 size_t trk_partial_elems(int n_items, int slices);
 // shared-window kernel (trk_shared_kernel.cu): groups of 8 items share one copy of the samples; every channel has `taps` taps
+// and sits on a float band (it reads samples as float2)
 int launch_trk_shared(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands, float2* out,
     int out_stride, int taps, cudaStream_t stream, uint64_t& launched);
 int trk_shared_max_code_len();

@@ -45,12 +45,14 @@ int upload_tables(b200_engine* e)
             bd[i].mask = e->bands[i].mask;
             bd[i].first_index = e->bands[i].first_index;
             bd[i].limit = e->bands[i].capacity;
+            bd[i].fmt = e->bands[i].fmt;
         }
     B200_CUDA_TRY(cudaMemcpyAsync(e->bands_dev, bd, sizeof(bd), cudaMemcpyHostToDevice, e->stream));
     const int n = static_cast<int>(e->chans.size());
     B200_CUDA_TRY(e->chans_dev.grow(n, n + 64));
     e->max_code_len = 0;
     e->taps_mask = 0u;
+    e->fmt_mask = 0u;
     e->any_high_dyn = false;
     if (n > 0)
         {
@@ -62,6 +64,7 @@ int upload_tables(b200_engine* e)
                     if (cd[i].code == nullptr) continue;
                     if (cd[i].high_dyn) e->any_high_dyn = true;
                     e->taps_mask |= 1u << cd[i].taps;
+                    e->fmt_mask |= 1u << e->bands[cd[i].band].fmt;
                 }
             // synchronous-safe: source is a temporary, so block until the copy has been staged
             B200_CUDA_TRY(cudaMemcpyAsync(e->chans_dev, cd.data(), sizeof(ChanDesc) * n, cudaMemcpyHostToDevice, e->stream));
@@ -98,6 +101,33 @@ unsigned long long next_pow2(unsigned long long v)
     unsigned long long p = 2;
     while (p < v) p <<= 1;
     return p;
+}
+
+// FileSourceBase::itemTypeToSize (file_source_base.cc:340-378): the complex item types, as interleaved (I, Q) pairs
+const char* const kItemTypes[] = {nullptr, "ibyte", "ishort", nullptr, "gr_complex"};
+
+const char* item_type_name(SampleFormat f) { return kItemTypes[f]; }
+
+// B200_OK and *f, or B200_ERR_ARG with the error text for a type that is not one of kItemTypes
+int parse_item_type(const char* item_type, const char* caller, SampleFormat* f)
+{
+    for (const SampleFormat k : {kCf32, kI16, kI8})
+        if (item_type && std::strcmp(item_type, kItemTypes[k]) == 0)
+            {
+                *f = k;
+                return B200_OK;
+            }
+    set_error("%s: item type %s is not an interleaved complex type (gr_complex, ishort, ibyte)", caller, item_type ? item_type : "(null)");
+    return B200_ERR_ARG;
+}
+
+// A float band takes every push (integers are widened on the way in); a narrow band only pushes of its own type, which are
+// copied as they are.  Otherwise B200_ERR_STATE with the error text.
+int check_push_format(const Band& b, int band, SampleFormat f)
+{
+    if (b.fmt == kCf32 || f == b.fmt) return B200_OK;
+    set_error("band %d holds %s samples: a %s push cannot be written into it", band, item_type_name(b.fmt), item_type_name(f));
+    return B200_ERR_STATE;
 }
 }  // namespace
 
@@ -212,19 +242,27 @@ extern "C"
 
     int b200_iq_create(b200_engine* e, int band, uint64_t capacity_samples)
     {
+        return b200_iq_create_typed(e, band, capacity_samples, "gr_complex");
+    }
+
+    int b200_iq_create_typed(b200_engine* e, int band, uint64_t capacity_samples, const char* item_type)
+    {
         if (!e || band < 0 || band >= kMaxBands || capacity_samples == 0) return B200_ERR_ARG;
+        SampleFormat fmt;
+        if (const int rc = parse_item_type(item_type, "iq_create_typed", &fmt)) return rc;
         std::lock_guard<std::mutex> lk(e->mu);
         B200_ENTER_DEVICE(e->device);
         Band& b = e->bands[band];
         if (const int rc = release_owned_ring(e, b)) return rc;
         const unsigned long long cap = next_pow2(capacity_samples);
-        cudaError_t err = b.dev.alloc(cap);
+        cudaError_t err = b.dev.alloc(cap * 2ULL * fmt);
         if (err != cudaSuccess)
             {
-                set_error("band %d: device allocation of %llu samples: %s", band, cap, cudaGetErrorString(err));
+                set_error("band %d: device allocation of %llu %s samples: %s", band, cap, item_type, cudaGetErrorString(err));
                 return B200_ERR_NOMEM;
             }
         b.base = b.dev;
+        b.fmt = fmt;
         b.capacity = cap;
         b.mask = cap - 1;
         b.first_index = 0;
@@ -253,16 +291,9 @@ extern "C"
         return B200_OK;
     }
 
-    // the host sample formats of a band, by bytes per component: b200_cf32, and interleaved (I, Q) int16 / int8 pairs
-    enum SampleFormat
-    {
-        kI8 = 1,
-        kI16 = 2,
-        kCf32 = 4,
-    };
-
-    // The one write path of an owned ring: n host samples of format fmt at the band's write index.  Float samples are copied
-    // into the ring; integers cross PCIe as they are and are converted into the ring on the device.  (Overwriting samples
+    // The one write path of an owned ring: n host samples of format fmt at the band's write index.  Samples of the ring's own
+    // format are copied into it; integers pushed into a float ring cross PCIe as they are and are converted into the ring on
+    // the device; anything else is refused before a byte is written (check_push_format).  (Overwriting samples
     // that an in-flight launch still reads is the caller's ring-sizing responsibility, exactly as with any circular sample
     // buffer.)
     static int push_samples(b200_engine* e, int band, const void* host, uint64_t n, SampleFormat fmt, uint64_t* first_index)
@@ -271,6 +302,7 @@ extern "C"
         std::lock_guard<std::mutex> lk(e->mu);
         Band& b = e->bands[band];
         if (const int rc = b.check_owned_ring(band)) return rc;
+        if (const int rc = check_push_format(b, band, fmt)) return rc;
         if (n > b.capacity)
             {
                 set_error("push of %llu samples exceeds ring capacity %llu", (unsigned long long)n, b.capacity);
@@ -279,9 +311,9 @@ extern "C"
         B200_ENTER_DEVICE(e->device);
         if (first_index) *first_index = b.write_index;
         if (n == 0) return B200_OK;
-        if (fmt == kCf32)
+        if (fmt == b.fmt)
             {
-                const int rc = copy_in(e, b.dev, b.capacity, b.write_index & b.mask, host, n, sizeof(float2));
+                const int rc = copy_in(e, b.dev, b.capacity, b.write_index & b.mask, host, n, 2 * static_cast<size_t>(fmt));
                 if (rc) return rc;
             }
         else
@@ -303,8 +335,9 @@ extern "C"
                 B200_CUDA_TRY(cudaStreamWaitEvent(e->copy_stream, b.raw_free[k], 0));
                 int rc = copy_in(e, b.raw_stage[k], n, 0, host, n, 2 * static_cast<size_t>(fmt));
                 if (rc) return rc;
-                rc = (fmt == kI16) ? launch_convert_i16(reinterpret_cast<const short*>(b.raw_stage[k].get()), b.dev, b.mask, b.write_index, n, e->stream)
-                                   : launch_convert_i8(reinterpret_cast<const signed char*>(b.raw_stage[k].get()), b.dev, b.mask, b.write_index, n, e->stream);
+                float2* const ring = reinterpret_cast<float2*>(b.dev.get());
+                rc = (fmt == kI16) ? launch_convert_i16(reinterpret_cast<const short*>(b.raw_stage[k].get()), ring, b.mask, b.write_index, n, e->stream)
+                                   : launch_convert_i8(reinterpret_cast<const signed char*>(b.raw_stage[k].get()), ring, b.mask, b.write_index, n, e->stream);
                 if (rc) return rc;
                 e->launches++;
                 B200_CUDA_TRY(cudaEventRecord(b.raw_free[k], e->stream));
@@ -341,6 +374,7 @@ extern "C"
             std::lock_guard<std::mutex> lk(e->mu);
             Band& b = e->bands[band];
             if (const int rc = b.check_owned_ring(band)) return rc;
+            if (const int rc = check_push_format(b, band, kCf32)) return rc;
             // what the ring holds right now
             const unsigned long long lo = b.window_lo();
             if (abs_index >= lo && abs_index + n <= b.write_index) return B200_OK;  // every sample of this block is already in the band
@@ -384,24 +418,14 @@ extern "C"
         uint64_t max_samples, uint64_t chunk_samples, uint64_t* first_index, uint64_t* samples_pushed)
     {
         if (!e || !path || !item_type || band < 0 || band >= kMaxBands) return B200_ERR_ARG;
-        // FileSourceBase::itemTypeToSize (file_source_base.cc:340-378): complex samples as interleaved (I, Q) pairs
         SampleFormat fmt;
-        if (std::strcmp(item_type, "gr_complex") == 0)
-            fmt = kCf32;
-        else if (std::strcmp(item_type, "ishort") == 0)
-            fmt = kI16;
-        else if (std::strcmp(item_type, "ibyte") == 0)
-            fmt = kI8;
-        else
-            {
-                set_error("iq_push_file: item type %s is not an interleaved complex type (gr_complex, ishort, ibyte)", item_type);
-                return B200_ERR_ARG;
-            }
+        if (const int rc = parse_item_type(item_type, "iq_push_file", &fmt)) return rc;
         unsigned long long capacity;
         {
             std::lock_guard<std::mutex> lk(e->mu);
             const Band& b = e->bands[band];
             if (const int rc = b.check_owned_ring(band)) return rc;
+            if (const int rc = check_push_format(b, band, fmt)) return rc;
             capacity = b.capacity;
         }
         if (chunk_samples == 0) chunk_samples = 1ULL << 20;
@@ -475,7 +499,8 @@ extern "C"
         std::lock_guard<std::mutex> lk(e->mu);
         Band& b = e->bands[band];
         if (const int rc = release_owned_ring(e, b)) return rc;
-        b.base = reinterpret_cast<const float2*>(dev);
+        b.base = dev;
+        b.fmt = kCf32;
         b.capacity = n_samples;
         b.mask = ~0ULL;
         b.first_index = first_index;
@@ -492,6 +517,8 @@ extern "C"
         if (!e || band < 0 || band >= kMaxBands || (!host && n)) return B200_ERR_ARG;
         std::lock_guard<std::mutex> lk(e->mu);
         Band& b = e->bands[band];
+        if (b.in_use)
+            if (const int rc = check_push_format(b, band, kCf32)) return rc;
         if (!b.in_use || !b.attached)
             {
                 set_error("band %d is not an attached device buffer (call b200_iq_attach_dev)", band);
@@ -504,7 +531,7 @@ extern "C"
             }
         B200_ENTER_DEVICE(e->device);
         // overwriting samples an in-flight launch still reads is the caller's double-buffering responsibility
-        const int rc = copy_in(e, const_cast<float2*>(b.base), b.capacity, 0, host, n, sizeof(float2));
+        const int rc = copy_in(e, const_cast<void*>(b.base), b.capacity, 0, host, n, sizeof(float2));
         if (rc) return rc;
         if (b.first_index != first_index)
             {
@@ -594,9 +621,11 @@ extern "C"
         if (slices < 1) slices = 1;
         rc = ensure_partials(e, n_items, slices);
         if (rc) return rc;
-        // the shared-window kernel takes batches whose channels all have 1, 3 or 5 taps
+        // the shared-window kernel takes batches whose channels all have 1, 3 or 5 taps and sit on float bands (it reads float2
+        // samples: a narrow ring would be read past its end)
         const unsigned int mask = e->taps_mask;
-        const bool shared_legal = (mask == (1u << 1) || mask == (1u << 3) || mask == (1u << 5)) && !e->any_high_dyn && slices == 1;
+        const bool shared_legal = (mask == (1u << 1) || mask == (1u << 3) || mask == (1u << 5)) && !e->any_high_dyn && slices == 1 &&
+                                  e->fmt_mask == (1u << kCf32);
         const bool use_shared = shared_legal && (e->shared_mode == 1 || (e->shared_mode == 2 && n_items >= 1024 && layout_hint != 0 &&
                                                                             e->max_code_len <= trk_shared_max_code_len()));
         uint64_t launched = 0;
@@ -605,7 +634,7 @@ extern "C"
                 __builtin_ctz(mask), e->stream, launched);
         else
             rc = launch_trk_batch(items_dev, n_items, e->chans_dev, e->bands_dev, reinterpret_cast<float2*>(out_dev), out_stride,
-                slices, e->partial, e->counters, e->max_code_len, mask, e->stream, launched);
+                slices, e->partial, e->counters, e->max_code_len, mask, e->fmt_mask, e->stream, launched);
         if (rc) return rc;
         e->launches += launched;
         return B200_OK;
@@ -947,6 +976,7 @@ extern "C"
         c->band.mask = ~0ULL;
         c->band.first_index = 0;
         c->band.limit = static_cast<unsigned long long>(t->max_len) + 2ULL;
+        c->band.fmt = kCf32;
         c->item.channel = 0;
         c->item.n = n;
         c->item.sample_index = 0;
@@ -961,7 +991,7 @@ extern "C"
         if (slices > t->slices_cap) slices = t->slices_cap;
         uint64_t launched = 0;
         int rc = launch_trk_batch(&c->item, 1, &c->chan, &c->band, c->out, B200_MAX_TAPS, slices, t->partial, t->counter,
-            c->chan.code_len, 1u << t->taps, t->stream, launched);
+            c->chan.code_len, 1u << t->taps, 1u << kCf32, t->stream, launched);
         if (rc) return rc;
         t->e->launches += launched;
         B200_CUDA_TRY(cudaStreamSynchronize(t->stream));

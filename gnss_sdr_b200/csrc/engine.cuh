@@ -16,8 +16,9 @@ constexpr int kMaxBands = 16;
 
 struct Band
 {
-    DevBuf<float2> dev;        // owned ring (empty when attached)
-    const float2* base{nullptr};
+    DevBuf<unsigned char> dev;  // owned ring (empty when attached)
+    const void* base{nullptr};
+    SampleFormat fmt{kCf32};    // what the ring holds (b200_iq_create_typed); attached buffers are float
     unsigned long long mask{0};
     unsigned long long first_index{0};
     unsigned long long capacity{0};
@@ -72,6 +73,7 @@ struct b200_engine
     bool tables_dirty{true};
     int max_code_len{0};
     unsigned int taps_mask{0};   // bit t set: some channel with a code table has t taps (a batch runs one launch per tap count)
+    unsigned int fmt_mask{0};    // bit f set: some channel with a code table is on a band of SampleFormat f (and one per format)
     bool any_high_dyn{false};
     int shared_mode{2};    // shared-window kernel: 2 auto, 0 never, 1 always-when-legal (b200_trk_kernel_choice)
     b200::DevBuf<float2> partial;

@@ -166,10 +166,22 @@ int upload_loop_data(b200_engine* e)
 // the kernels' view: nullptr while no loop has a data channel
 const LoopData* loop_data_dev(const b200_engine* e) { return e->loop_n_data ? e->loop_data_dev.get() : nullptr; }
 
+// the loops read float bands only (narrow_band_refusal keeps them there), so only the float instantiations run
 int correlate_loop_items(b200_engine* e, int n, int slices, uint64_t& launched)
 {
     return launch_trk_batch(e->loop_items_dev, n, e->chans_dev, e->bands_dev, e->loop_taps_dev, kLoopTapStride, slices, e->partial,
-        e->counters, e->max_code_len, e->taps_mask, e->stream, launched);
+        e->counters, e->max_code_len, e->taps_mask, 1u << kCf32, e->stream, launched);
+}
+
+// B200_ERR_STATE with the error text when channel sits on a narrow band: the loop kernels read their bands as float2, so a
+// narrow ring would be read past its end
+int narrow_band_refusal(const b200_engine* e, int channel, const char* caller)
+{
+    const int band = e->chans[channel].desc.band;
+    if (e->bands[band].fmt == kCf32) return B200_OK;
+    set_error("%s: channel %d is on band %d, which holds narrow (integer) samples; the device loops read gr_complex bands only",
+        caller, channel, band);
+    return B200_ERR_STATE;
 }
 }  // namespace
 
@@ -184,6 +196,7 @@ extern "C"
                 set_error("loop_create: channel %d has no code table", channel);
                 return B200_ERR_STATE;
             }
+        if (const int rc = narrow_band_refusal(e, channel, "loop_create")) return rc;
         const int need_taps = conf->veml ? 5 : 3;
         if (e->chans[channel].desc.taps != need_taps)
             {
@@ -254,6 +267,7 @@ extern "C"
                 set_error("loop_set_data_channel: channel %d has no code table", data_channel);
                 return B200_ERR_ARG;
             }
+        if (const int rc = narrow_band_refusal(e, data_channel, "loop_set_data_channel")) return rc;
         const ChanDesc& d = e->chans[data_channel].desc;
         if (d.taps != 1)
             {
@@ -347,6 +361,14 @@ extern "C"
         std::lock_guard<std::mutex> lk(e->mu);
         const int n = static_cast<int>(e->loops.size());
         if (n == 0 || max_epochs == 0) return B200_OK;
+        // a band may have been re-created narrow after its loops were made
+        for (int i = 0; i < n; i++)
+            {
+                if (e->loops[i].state == 0) continue;
+                if (const int rc = narrow_band_refusal(e, e->loops[i].channel, "loop_run")) return rc;
+                if (e->loop_data[i].channel >= 0)
+                    if (const int rc = narrow_band_refusal(e, e->loop_data[i].channel, "loop_run")) return rc;
+            }
         B200_ENTER_DEVICE(e->device);
         int rc = upload_tables(e);
         if (rc) return rc;

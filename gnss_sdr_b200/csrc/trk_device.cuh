@@ -163,6 +163,58 @@ __device__ __forceinline__ float2 ldg_stream8(const float2* p)
     return v;
 }
 
+// Streaming loads of band samples of SampleFormat FMT, widened to float on load (widen_i16 / widen_i8 of common.cuh):
+// sample slot k of a band starts at byte 2 * FMT * k of its base.
+template <int FMT>
+__device__ __forceinline__ const char* sample_ptr(const void* base, unsigned long long k)
+{
+    return static_cast<const char*>(base) + k * (2ULL * FMT);
+}
+// samples k and k + 1 (k even) as (re, im, re, im): one 16-, 8- or 4-byte load
+template <int FMT>
+__device__ __forceinline__ float4 ldg_stream_pair(const char* p)
+{
+    if constexpr (FMT == kCf32)
+        {
+            return ldg_stream16(reinterpret_cast<const float2*>(p));
+        }
+    else if constexpr (FMT == kI16)
+        {
+            unsigned int w0, w1;
+            asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(w0), "=r"(w1) : "l"(p));
+            const float2 a = widen_i16(w0), b = widen_i16(w1);
+            return make_float4(a.x, a.y, b.x, b.y);
+        }
+    else
+        {
+            unsigned int w;
+            asm volatile("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(w) : "l"(p));
+            const float2 a = widen_i8<0>(w), b = widen_i8<1>(w);
+            return make_float4(a.x, a.y, b.x, b.y);
+        }
+}
+// one sample: an 8-, 4- or 2-byte load
+template <int FMT>
+__device__ __forceinline__ float2 ldg_stream_one(const char* p)
+{
+    if constexpr (FMT == kCf32)
+        {
+            return ldg_stream8(reinterpret_cast<const float2*>(p));
+        }
+    else if constexpr (FMT == kI16)
+        {
+            unsigned int w;
+            asm volatile("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(w) : "l"(p));
+            return widen_i16(w);
+        }
+    else
+        {
+            unsigned short h;
+            asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=h"(h) : "l"(p));
+            return widen_i8<0>(h);
+        }
+}
+
 
 // ---- lane-wise float2 arithmetic on sample pairs (.x = sample n, .y = sample n+1).  Hopper has no
 // packed FP32 instructions, so each is two scalar operations with an explicit rounding mode: ptxas

@@ -12,7 +12,7 @@ namespace b200
 {
 namespace
 {
-// tiles of the main loop unrolled per thread (one 16-byte load each): memory-level parallelism vs registers.  With five taps
+// tiles of the main loop unrolled per thread (one 16-byte load each on a float band): memory-level parallelism vs registers.  With five taps
 // (C3, Galileo E1) and one tap (the data correlator of a tracked pilot) the kernel waits on L2, so 16 = a whole re-seed group
 // of loads in flight; three taps (C2) take 4.  On an H100 (400 W), ms per step, these values vs 8: five taps C3 5.52 vs 5.94;
 // three taps C2 distinct-IQ 1.165 vs 1.178; one tap C3 + pilot 8.93-8.98 vs 8.84 (within the spread of repeated runs of one
@@ -23,7 +23,7 @@ constexpr int kTileUnroll1 = 16;   // one tap: the data prompt of a tracked pilo
 
 struct ItemCtx
 {
-    const float2* base;
+    const void* base;       // the band's samples (sample_ptr)
     unsigned long long mask;
     unsigned long long s0;  // offset of the epoch's first sample in the band
     unsigned long long T0;  // -rem_carrier in turns
@@ -64,7 +64,7 @@ __device__ __forceinline__ void accumulate_sample(float2 x, float2 z, float m, c
         }
 }
 
-template <int TAPS, class Lookup, int THREADS = kTrkThreads>
+template <int TAPS, class Lookup, int THREADS = kTrkThreads, int FMT = kCf32>
 __device__ __forceinline__ void correlate_range(const ItemCtx& cx, const float (&shifts)[TAPS], const Lookup& lut,
     int tile_begin, int tile_end, int head, bool do_remainder, int n_main_end, float2 (&acc)[TAPS])
 {
@@ -86,7 +86,7 @@ __device__ __forceinline__ void correlate_range(const ItemCtx& cx, const float (
 #pragma unroll 4
             for (int tile = tg; tile < tg_end; tile++)
                 {
-                    const float4 v = ldg_stream16(cx.base + ((cx.s0 + static_cast<unsigned long long>(n0)) & cx.mask));
+                    const float4 v = ldg_stream_pair<FMT>(sample_ptr<FMT>(cx.base, (cx.s0 + static_cast<unsigned long long>(n0)) & cx.mask));
                     accumulate_sample<TAPS>(make_float2(v.x, v.y), za, __fmul_rn(cx.step, nf), aux2, lut, acc);
                     accumulate_sample<TAPS>(make_float2(v.z, v.w), zb, __fmul_rn(cx.step, nf + 1.0f), aux2, lut, acc);
                     za = cmulf(za, D);
@@ -103,7 +103,7 @@ __device__ __forceinline__ void correlate_range(const ItemCtx& cx, const float (
             for (int r = tid; r < count; r += THREADS)
                 {
                     const int n = (r < head) ? 0 : n_main_end + (r - head);
-                    const float2 x = ldg_stream8(cx.base + ((cx.s0 + static_cast<unsigned long long>(n)) & cx.mask));
+                    const float2 x = ldg_stream_one<FMT>(sample_ptr<FMT>(cx.base, (cx.s0 + static_cast<unsigned long long>(n)) & cx.mask));
                     const float2 z = phasor_from_turns(cx.T0 + cx.DT * static_cast<unsigned long long>(n));
                     const float wr = fmaf(x.x, z.x, -x.y * z.y);
                     const float wi = fmaf(x.x, z.y, x.y * z.x);
@@ -122,7 +122,7 @@ __device__ __forceinline__ void correlate_range(const ItemCtx& cx, const float (
 // ---- main tiles, FAST path: arithmetic on sample pairs, no modulo, no F2I -----------------------------
 // Lane .x of every float2 value belongs to sample n0, lane .y to sample n0+1 (one LDG.128).  The chip lookup is pair_taps'
 // floor trick (exact for |index| < 2^22, guaranteed by the caller's range check); tbl_off = table_offset().
-template <int TAPS, bool WRAPS, int THREADS = kTrkThreads>
+template <int TAPS, bool WRAPS, int THREADS = kTrkThreads, int FMT = kCf32>
 __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const float (&shifts)[TAPS], unsigned int tbl_off,
     int tile_begin, int tile_end, int head, float2 (&acc)[TAPS])
 {
@@ -154,7 +154,7 @@ __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const fl
         zi2 = make_float2(za.y, zb.y);
     }
     float nfa = static_cast<float>(n0), nfb = static_cast<float>(n0 + 1);
-    const float2* ptr = cx.base + ((cx.s0 + static_cast<unsigned long long>(n0)) & cx.mask);
+    const char* ptr = sample_ptr<FMT>(cx.base, (cx.s0 + static_cast<unsigned long long>(n0)) & cx.mask);
 
     for (int tg = tile_begin; tg < tile_end; tg += kTrkReseed)
         {
@@ -165,9 +165,9 @@ __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const fl
                 {
                     float4 v;
                     if (WRAPS)
-                        v = ldg_stream16(cx.base + ((cx.s0 + static_cast<unsigned long long>(n0)) & cx.mask));
+                        v = ldg_stream_pair<FMT>(sample_ptr<FMT>(cx.base, (cx.s0 + static_cast<unsigned long long>(n0)) & cx.mask));
                     else
-                        v = ldg_stream16(ptr);
+                        v = ldg_stream_pair<FMT>(ptr);
                     // w = x * z, scalar: the LDG.128 delivers (re,im,re,im), so packed operands would
                     // need 8 register moves per tile; scalar results land directly in register pairs
                     float2 wr2, wi2;
@@ -181,7 +181,7 @@ __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const fl
                     nfa += static_cast<float>(kTile);
                     nfb += static_cast<float>(kTile);
                     n0 += kTile;
-                    ptr += kTile;
+                    ptr += kTile * 2 * FMT;
                 }
             // group seed advances by the rounded G, not re-seeded from the 64-bit phase: its error grows by about 1e-7
             // per group (8192 samples); see the measured bound in trk_kernels.cu
@@ -199,7 +199,7 @@ __device__ __forceinline__ void correlate_tiles_fast(const ItemCtx& cx, const fl
 // integer-sample shifts of tap 0's resampled sequence; carrier has a phase-rate term that lags
 // one sample (..._high_dynamic_rotator_dot_prod_32fc_xn.h:92-103).  Not the throughput path:
 // one sample per thread per step, exact phasor per sample.
-template <int TAPS, class Lookup, int THREADS = kTrkThreads>
+template <int TAPS, class Lookup, int THREADS = kTrkThreads, int FMT = kCf32>
 __device__ __forceinline__ void correlate_range_hd(const ItemCtx& cx, float rate, unsigned long long RT,
     const float (&shifts)[TAPS], const Lookup& lut, int n_begin, int n_end, float2 (&acc)[TAPS])
 {
@@ -215,7 +215,7 @@ __device__ __forceinline__ void correlate_range_hd(const ItemCtx& cx, float rate
         }
     for (int n = n_begin + threadIdx.x; n < n_end; n += THREADS)
         {
-            const float2 x = ldg_stream8(cx.base + ((cx.s0 + static_cast<unsigned long long>(n)) & cx.mask));
+            const float2 x = ldg_stream_one<FMT>(sample_ptr<FMT>(cx.base, (cx.s0 + static_cast<unsigned long long>(n)) & cx.mask));
             // rate exponent: (n-1)^2 for n>=1 with the reference's uint32 wrap of k*k, as float
             unsigned long long T = cx.T0 + cx.DT * static_cast<unsigned long long>(n);
             if (n >= 1)
@@ -246,7 +246,9 @@ __device__ __forceinline__ void correlate_range_hd(const ItemCtx& cx, float rate
 
 // REUSE (persistent tracker: one CTA keeps serving the same channel): tbl_cache[0..1] = [begin, end) of the chip-index
 // window already staged in smem_tbl; an epoch whose window lies inside it skips the staging pass.
-template <int TAPS, bool REUSE = false, int THREADS = kTrkThreads>
+// FMT: the SampleFormat of bd (the caller's to check); every path widens each sample to float right after its load and then
+// runs the same arithmetic, so a narrow band gives exactly the taps of a float band holding the same integers.
+template <int TAPS, bool REUSE = false, int THREADS = kTrkThreads, int FMT = kCf32>
 __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const BandDesc& bd, float* smem_tbl,
     int tbl_cap, float2* smem_red, int slice, int slices, float2 (&result)[TAPS], int* tbl_cache = nullptr)
 {
@@ -286,7 +288,7 @@ __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const 
             const unsigned long long RT = turns_from_rad(-static_cast<double>(it.phase_rate_step_rad));
             const int per = (cx.N + slices - 1) / slices;
             const int nb = min(cx.N, slice * per), ne = min(cx.N, nb + per);
-            correlate_range_hd<TAPS, LookupMod, THREADS>(cx, it.code_phase_rate_step_chips, RT, shifts, lut, nb, ne, acc);
+            correlate_range_hd<TAPS, LookupMod, THREADS, FMT>(cx, it.code_phase_rate_step_chips, RT, shifts, lut, nb, ne, acc);
         }
     else
         {
@@ -351,15 +353,15 @@ __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const 
                             // ring wrap inside the epoch? (uniform per item)
                             const bool wraps = ((cx.s0 & cx.mask) + static_cast<unsigned long long>(cx.N)) > cx.mask;
                             if (wraps)
-                                correlate_tiles_fast<TAPS, true, THREADS>(cx, shifts, tbl_off, tb, te, head, acc);
+                                correlate_tiles_fast<TAPS, true, THREADS, FMT>(cx, shifts, tbl_off, tb, te, head, acc);
                             else
-                                correlate_tiles_fast<TAPS, false, THREADS>(cx, shifts, tbl_off, tb, te, head, acc);
+                                correlate_tiles_fast<TAPS, false, THREADS, FMT>(cx, shifts, tbl_off, tb, te, head, acc);
                             // remainder samples only (no main tiles) through the scalar path
-                            correlate_range<TAPS, LookupExt, THREADS>(cx, shifts, lut, 0, 0, head, rem_here, n_main_end, acc);
+                            correlate_range<TAPS, LookupExt, THREADS, FMT>(cx, shifts, lut, 0, 0, head, rem_here, n_main_end, acc);
                         }
                     else
                         {
-                            correlate_range<TAPS, LookupExt, THREADS>(cx, shifts, lut, tb, te, head, rem_here, n_main_end, acc);
+                            correlate_range<TAPS, LookupExt, THREADS, FMT>(cx, shifts, lut, tb, te, head, rem_here, n_main_end, acc);
                         }
                 }
             else
@@ -372,7 +374,7 @@ __device__ void process_item(const b200_trk_item& it, const ChanDesc& ch, const 
                         }
                     __syncthreads();
                     LookupMod lut{in_smem ? smem_tbl : ch.code, L};
-                    correlate_range<TAPS, LookupMod, THREADS>(cx, shifts, lut, tb, te, head, rem_here, n_main_end, acc);
+                    correlate_range<TAPS, LookupMod, THREADS, FMT>(cx, shifts, lut, tb, te, head, rem_here, n_main_end, acc);
                 }
         }
 

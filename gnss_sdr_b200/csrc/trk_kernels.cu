@@ -11,7 +11,7 @@
 //   a3  src/algorithms/tracking/libs/cpu_multicorrelator_real_codes.cc:103-127 (phase set-up).
 //
 // Data movement: each sample is read exactly once per channel with coalesced 16-byte loads
-// (LDG.128 = 2 samples per lane); the code table is staged once per CTA in shared memory as an
+// (LDG.128 = 2 samples per lane; 8 or 4 bytes for the same 2 samples of an int16 or int8 band); the code table is staged once per CTA in shared memory as an
 // "extended" table that already contains the wrap-around, so the inner loop has no modulo.
 // Reductions: registers -> warp shuffles -> shared memory -> (optionally) a deterministic
 // cross-CTA combine when an epoch is split into slices for latency.
@@ -32,13 +32,13 @@ namespace b200
 {
 namespace
 {
-template <int TAPS>
+template <int TAPS, int FMT>
 __device__ __forceinline__ void run_item(const b200_trk_item& it, const ChanDesc& ch, const BandDesc& bd,
     float* smem_tbl, int tbl_cap, float2* smem_red, int* smem_flag, int item_id, int slice, int slices,
     float2* out, int out_stride, float2* partial, unsigned int* counters)
 {
     float2 result[TAPS];
-    process_item<TAPS>(it, ch, bd, smem_tbl, tbl_cap, smem_red, slice, slices, result);
+    process_item<TAPS, false, kTrkThreads, FMT>(it, ch, bd, smem_tbl, tbl_cap, smem_red, slice, slices, result);
     const int tid = threadIdx.x;
     if (slices == 1)
         {
@@ -82,7 +82,9 @@ __device__ __forceinline__ void run_item(const b200_trk_item& it, const ChanDesc
 // of 3 blocks slower on all four legs.
 // Other tap counts keep the register budget of two CTAs per SM (128) that the kernel which read the tap count per item had:
 // left to ptxas, <4>, <6> and <7> settle at 64-80 registers and spill.
-template <int TAPS>
+// One instantiation per SampleFormat FMT of the band as well: each reads only the items whose band has its format (a float
+// read of a narrow ring would run past its end) and leaves the others to the launch of theirs.
+template <int TAPS, int FMT>
 __global__ void __launch_bounds__(kTrkThreads, (TAPS == 1 || TAPS == 3 || TAPS == 5) ? 0 : 2)
     trk_correlate_kernel(const b200_trk_item* __restrict__ items, int n_items, const ChanDesc* __restrict__ chans, const BandDesc* __restrict__ bands, float2* __restrict__ out, int out_stride,
     int slices, float2* partial, unsigned int* counters, int tbl_cap, unsigned int only_mask)
@@ -102,17 +104,18 @@ __global__ void __launch_bounds__(kTrkThreads, (TAPS == 1 || TAPS == 3 || TAPS =
             const ChanDesc& ch = chans[it.channel];
             if (only_mask != 0u && ((1u << ch.taps) & only_mask) == 0u) continue;   // uniform per CTA iteration
             const BandDesc bd = bands[ch.band];
+            if (bd.fmt != FMT) continue;   // uniform per CTA iteration
             if (w != static_cast<int>(blockIdx.x)) __syncthreads();  // smem reuse across items
             if (it.n <= 0)
                 {
                     if (slice == 0 && threadIdx.x < ch.taps) out[static_cast<size_t>(item_id) * out_stride + threadIdx.x] = make_float2(0.f, 0.f);
                     continue;
                 }
-            run_item<TAPS>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters);
+            run_item<TAPS, FMT>(it, ch, bd, smem_tbl, tbl_cap, smem_red, smem_flag, item_id, slice, slices, out, out_stride, partial, counters);
         }
 }
 
-template <int T>
+template <int T, int FMT>
 int launch_one(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands, float2* out,
     int out_stride, int slices, float2* partial, unsigned int* counters, int tbl_cap, size_t smem_bytes, cudaStream_t stream, unsigned int only_mask)
 {
@@ -120,13 +123,13 @@ int launch_one(const b200_trk_item* items, int n_items, const ChanDesc* chans, c
     const int once_dev = once.begin();
     if (once_dev >= 0)
         {
-            B200_CUDA_TRY(cudaFuncSetAttribute(trk_correlate_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrkSmemMax));
+            B200_CUDA_TRY(cudaFuncSetAttribute(trk_correlate_kernel<T, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrkSmemMax));
             once.done(once_dev);
         }
     const long long work = static_cast<long long>(n_items) * slices;
     // plain grid for moderate sizes, grid-stride beyond (keeps blockIdx math in int)
     const int grid = static_cast<int>(work < (1LL << 20) ? work : (1LL << 20));
-    trk_correlate_kernel<T><<<grid, kTrkThreads, smem_bytes, stream>>>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap,
+    trk_correlate_kernel<T, FMT><<<grid, kTrkThreads, smem_bytes, stream>>>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap,
         only_mask);
     B200_CUDA_TRY(cudaGetLastError());
     return B200_OK;
@@ -140,10 +143,10 @@ size_t trk_partial_elems(int n_items, int slices)
 
 int launch_trk_batch(const b200_trk_item* items, int n_items, const ChanDesc* chans, const BandDesc* bands,
     float2* out, int out_stride, int slices, float2* partial, unsigned int* counters,
-    int max_code_len, unsigned int taps_mask, cudaStream_t stream, uint64_t& launched)
+    int max_code_len, unsigned int taps_mask, unsigned int fmt_mask, cudaStream_t stream, uint64_t& launched)
 {
     if (n_items <= 0) return B200_OK;
-    if (taps_mask == 0u)
+    if (taps_mask == 0u || fmt_mask == 0u)
         {
             set_error("tracking batch: no channel has a code table");
             return B200_ERR_STATE;
@@ -152,17 +155,25 @@ int launch_trk_batch(const b200_trk_item* items, int n_items, const ChanDesc* ch
     const int tbl_cap = trk_table_cap(max_code_len, 1, 1024);
     const size_t smem_bytes = static_cast<size_t>(tbl_cap) * 4 + (kTrkThreads / 32) * B200_MAX_TAPS * sizeof(float2) + 16;
     // Several tap counts in one batch (a tracked pilot's 5 + 1 taps, a multi-signal receiver): one launch per tap count, each
-    // serving its own items.  A kernel that read the tap count per item needed 128 registers and halved the occupancy.
+    // serving its own items.  A kernel that read the tap count per item needed 128 registers and halved the occupancy.  Bands
+    // of several sample formats: one launch per format as well.
     const bool mixed = (taps_mask & (taps_mask - 1u)) != 0u;
     for (int taps = 1; taps <= B200_MAX_TAPS; taps++)
         {
             if (!(taps_mask & (1u << taps))) continue;
             const unsigned int only_mask = mixed ? 1u << taps : 0u;
-            const int rc = with_taps<1, 2, 3, 4, 5, 6, 7, 8>(taps, [&](auto tc) {
-                return launch_one<decltype(tc)::value>(items, n_items, chans, bands, out, out_stride, slices, partial, counters, tbl_cap, smem_bytes, stream, only_mask);
-            });
-            if (rc) return rc;
-            launched++;
+            for (const int fmt : {kCf32, kI16, kI8})
+                {
+                    if (!(fmt_mask & (1u << fmt))) continue;
+                    const int rc = with_taps<1, 2, 3, 4, 5, 6, 7, 8>(taps, [&](auto tc) {
+                        return with_format(fmt, [&](auto fc) {
+                            return launch_one<decltype(tc)::value, decltype(fc)::value>(items, n_items, chans, bands, out, out_stride, slices,
+                                partial, counters, tbl_cap, smem_bytes, stream, only_mask);
+                        });
+                    });
+                    if (rc) return rc;
+                    launched++;
+                }
         }
     return B200_OK;
 }

@@ -131,7 +131,7 @@ __device__ void warp_correlate_general(const b200_trk_item& it, const ChanDesc& 
     const unsigned long long s0 = it.sample_index - bd.first_index;
     for (int n = lane; n < it.n; n += 32)
         {
-            const float2 x = ldg_stream8(bd.base + ((s0 + static_cast<unsigned long long>(n)) & bd.mask));
+            const float2 x = ldg_stream8(static_cast<const float2*>(bd.base) + ((s0 + static_cast<unsigned long long>(n)) & bd.mask));
             const float2 z = phasor_from_turns(T0 + DT * static_cast<unsigned long long>(n));
             const float wr = fmaf(x.x, z.x, -x.y * z.y);
             const float wi = fmaf(x.x, z.y, x.y * z.x);
@@ -390,12 +390,12 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
                                     // a run that straddles the end of the ring is split in two copies
                                     const unsigned long long p = (src + c0) & pb.mask;
                                     const unsigned int n1 = static_cast<unsigned int>(min(static_cast<unsigned long long>(kShRun), cap - p));
-                                    bulk_g2s(dst, pb.base + p, n1 * 8u, &sm.full[s]);
-                                    if (n1 < kShRun) bulk_g2s(dst + n1, pb.base, (kShRun - n1) * 8u, &sm.full[s]);
+                                    bulk_g2s(dst, static_cast<const float2*>(pb.base) + p, n1 * 8u, &sm.full[s]);
+                                    if (n1 < kShRun) bulk_g2s(dst + n1, static_cast<const float2*>(pb.base), (kShRun - n1) * 8u, &sm.full[s]);
                                 }
                             else if (lane < kShTile / kShRun && valid > c0)
                                 {
-                                    bulk_g2s(dst, pb.base + src + c0, min(valid - c0, static_cast<unsigned int>(kShRun)) * 8u, &sm.full[s]);
+                                    bulk_g2s(dst, static_cast<const float2*>(pb.base) + src + c0, min(valid - c0, static_cast<unsigned int>(kShRun)) * 8u, &sm.full[s]);
                                 }
                         }
                 }
@@ -652,7 +652,7 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
                     // no shared window for this group: stream this item's own tiles from the band store
                     for (int t = t_first; t < t_last; t++)
                         {
-                            const GlobalTileLoader ld{bd.base, bd.mask, my_hull + static_cast<unsigned long long>(t) * kShTile + 2ULL * lane, bd.limit};
+                            const GlobalTileLoader ld{static_cast<const float2*>(bd.base), bd.mask, my_hull + static_cast<unsigned long long>(t) * kShTile + 2ULL * lane, bd.limit};
                             process_tile(t, ld);
                         }
                 }
@@ -674,7 +674,7 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
                     if (n < it.n)
                         {
                             const unsigned long long s0 = it.sample_index - bd.first_index;
-                            const float2 x = ldg_stream8(bd.base + ((s0 + static_cast<unsigned long long>(n)) & bd.mask));
+                            const float2 x = ldg_stream8(static_cast<const float2*>(bd.base) + ((s0 + static_cast<unsigned long long>(n)) & bd.mask));
                             const float2 z = phasor_from_turns(T0 + DT * static_cast<unsigned long long>(n));
                             const float wr = fmaf(x.x, z.x, -x.y * z.y);
                             const float wi = fmaf(x.x, z.y, x.y * z.x);

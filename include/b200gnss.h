@@ -73,6 +73,19 @@ extern "C"
      * (== the reference's sample counter, Gnss_Synchro::Acq_samplestamp_samples).
      * capacity_samples is rounded up to a power of two; the store is a ring. */
     int b200_iq_create(b200_engine* e, int band, uint64_t capacity_samples);
+    /* b200_iq_create with the band's sample type, item_type as b200_iq_push_file and the reference's
+     * SignalSource.item_type: "gr_complex" (8 B per sample, what b200_iq_create makes), "ishort" (interleaved int16 I,Q
+     * = lv_16sc_t, 4 B) or "ibyte" (interleaved int8 I,Q, 2 B); anything else is B200_ERR_ARG.  A narrow band holds its
+     * samples at their own width: 2x (ishort) or 4x (ibyte) the samples of a gr_complex band in the same memory.  It takes
+     * only pushes of its own type - b200_iq_push_i16 (ishort) or b200_iq_push_i8 (ibyte), and b200_iq_push_file with its
+     * item type - which copy the integers into the ring as they are, with no conversion launch; every other push
+     * (b200_iq_push, b200_iq_push_at, b200_iq_refill, the other integer width, a file of another type) is B200_ERR_STATE
+     * and writes nothing.  The per-item tracking correlator and the band searches (b200_acq_search_band and its
+     * variants) read a narrow band in place and widen each sample to float on load; int -> float is exact, so their
+     * results equal those on a gr_complex band holding the same integers.  The shared-window correlator never runs a
+     * batch while a channel with a code table sits on a narrow band (b200_trk_kernel_choice), and the device loops
+     * refuse narrow bands (b200_trk_loop_create).  Re-creating a band with another type is allowed. */
+    int b200_iq_create_typed(b200_engine* e, int band, uint64_t capacity_samples, const char* item_type);
     /* Append n host samples (async H2D on the copy stream, ordered before later launches).
      * *first_index receives the absolute index of host[0]. */
     int b200_iq_push(b200_engine* e, int band, const b200_cf32* host, uint64_t n, uint64_t* first_index);
@@ -95,7 +108,8 @@ extern "C"
      * the raw integers cross PCIe and are converted to float on the device, replacing the CPU
      * adapters src/algorithms/data_type_adapter/gnuradio_blocks/cshort_to_gr_complex.cc:48
      * (volk_gnsssdr_16ic_convert_32fc) and adapters/ibyte_to_complex.cc.  n counts complex samples;
-     * host_iq holds 2*n integers.  Conversion is exact (int -> float). */
+     * host_iq holds 2*n integers.  Conversion is exact (int -> float).  Into a band of the push's own narrow type
+     * (b200_iq_create_typed) the integers are copied as they are. */
     int b200_iq_push_i16(b200_engine* e, int band, const int16_t* host_iq, uint64_t n, uint64_t* first_index);
     int b200_iq_push_i8(b200_engine* e, int band, const int8_t* host_iq, uint64_t n, uint64_t* first_index);
     /* Stream a sample file into the band the way File_Signal_Source feeds the flowgraph
@@ -103,11 +117,12 @@ extern "C"
      * :385-414): item_type "gr_complex", "ishort" or "ibyte" (interleaved I,Q); header_bytes and skip_samples are
      * skipped; at most max_samples complex samples (0 = to the end of the file) are pushed in blocks of chunk_samples
      * (0 = 2^20) through two pinned staging buffers, so the disk read of one block overlaps the PCIe copy of the
-     * previous one.  Integer types are converted on the device (b200_iq_push_i16 / _i8). */
+     * previous one.  Integer types are converted on the device (b200_iq_push_i16 / _i8), or copied as they are into a
+     * band of the same type. */
     int b200_iq_push_file(b200_engine* e, int band, const char* path, const char* item_type, uint64_t header_bytes,
         uint64_t skip_samples, uint64_t max_samples, uint64_t chunk_samples, uint64_t* first_index, uint64_t* samples_pushed);
     /* Use caller-owned device memory as the band (no copy): dev[0] is absolute index
-     * first_index; n_samples need not be a power of two (no wrap). */
+     * first_index; n_samples need not be a power of two (no wrap).  The band's type becomes gr_complex. */
     int b200_iq_attach_dev(b200_engine* e, int band, const b200_cf32* dev, uint64_t n_samples, uint64_t first_index);
 
     /* Refill an attached band from host memory: host[0..n) becomes samples first_index .. first_index + n of the band
@@ -297,7 +312,8 @@ extern "C"
     /* Create a loop over tracking channel `channel` (b200_trk_channel_create + b200_trk_channel_set_code
      * with the E,P,L / VE,E,P,L,VL shifts of start_tracking :1041-1054).  Filter coefficients are derived
      * here as Tracking_loop_filter::update_coefficients (tracking_loop_filter.cc:86-186) and
-     * Tracking_FLL_PLL_filter::set_params (tracking_FLL_PLL_filter.cc:23-54) do. */
+     * Tracking_FLL_PLL_filter::set_params (tracking_FLL_PLL_filter.cc:23-54) do.  The loops read gr_complex bands
+     * only: a channel on an ishort or ibyte band (b200_iq_create_typed) is B200_ERR_STATE. */
     int b200_trk_loop_create(b200_engine* e, int channel, const b200_trk_loop_conf* conf, int* loop_id);
     /* start_tracking() (:791-1078): take the acquisition result; nitems_read = absolute index of the
      * first sample the tracking block would see next (state 1 then skips to the PRN start). */
@@ -305,7 +321,8 @@ extern "C"
         uint64_t acq_samplestamp_samples, uint64_t nitems_read);
     /* Attach a data channel to a loop that tracks a pilot (track_pilot = true, :637-668, :820-903): every epoch
      * then also correlates data_channel - one correlator, at the pilot prompt's shift, on the loop's band, not
-     * high-dynamics; anything else is refused with B200_ERR_ARG - on the loop's item.  The records' prompt_I /
+     * high-dynamics; anything else is refused with B200_ERR_ARG, and a channel on a narrow band with B200_ERR_STATE -
+     * on the loop's item.  The records' prompt_I /
      * prompt_Q become the data prompt, as log_data writes it (:1614-1617); every other field and the whole loop
      * update keep using the pilot taps.  Accepted before b200_trk_loop_run or between runs; a second call
      * replaces the data channel.  Set cloop as a pilot loop needs it (b200_trk_loop_conf). */
@@ -315,7 +332,9 @@ extern "C"
      * samples are not all inside its band's [valid_from, write_index) (the window b200_iq_window reports) stalls:
      * samples not pushed yet, overwritten, or left behind by a gap, a restart or b200_iq_forget are never correlated.
      * records_host: n_loops x max_epochs records (loop-major); n_records_host[loop] = cycles logged.
-     * Either output may be NULL.  Same as b200_trk_loop_run_prompts with pilot_prompts_host = NULL. */
+     * Either output may be NULL.  Same as b200_trk_loop_run_prompts with pilot_prompts_host = NULL.
+     * B200_ERR_STATE, with nothing launched, while a started loop's channel or data channel sits on a narrow band (its
+     * band was re-created with b200_iq_create_typed after the loop was made). */
     int b200_trk_loop_run(b200_engine* e, int max_epochs, b200_trk_dump_record* records_host, int* n_records_host);
     /* b200_trk_loop_run plus the complex pilot prompt of every logged record: pilot_prompts_host (NULL: not
      * returned) is n_loops x max_epochs, loop-major like the records.  With a data channel the record carries the
