@@ -4,6 +4,12 @@ import pytest
 
 
 @pytest.fixture(scope="module")
+def torch():
+    import torch as t
+    return t
+
+
+@pytest.fixture(scope="module")
 def capi():
     import gnss_sdr_b200.capi as c
     return c

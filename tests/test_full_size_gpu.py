@@ -9,6 +9,7 @@ import pytest
 
 from gnss_synth import make_iq, trk_params_for
 from gpu_fixtures import capi  # noqa: F401
+import trk_rig as tr
 
 pytestmark = pytest.mark.gpu
 
@@ -24,31 +25,19 @@ def c2(capi, oracle):
     x1 = (rng.integers(-6, 7, n_iq) + 1j * rng.integers(-6, 7, n_iq)).astype(np.complex64)
     x2 = (rng.integers(-6, 7, n_iq) + 1j * rng.integers(-6, 7, n_iq)).astype(np.complex64)
     eng = capi.Engine(0)
-    bands = {}
-    for b, x in enumerate((x1, x2, 3 * x1 - 2 * x2)):
-        eng.iq_create(b, n_iq)
-        bands[b] = eng.iq_push(b, x)
+    bands = {b: tr.ring(eng, b, x) for b, x in enumerate((x1, x2, 3 * x1 - 2 * x2))}
     codes = [oracle.port.gps_ca_code(p) for p in range(1, NCH + 1)]
     shifts = [-0.5, 0.0, 0.5]
     items = {}
     steps = 1.023e6 * (1 + rng.uniform(-4000, 4000, NCH) / 1575.42e6) / FS
     phase0 = rng.uniform(0, 1023, NCH)
+    k = np.arange(NEP)
+    rems = [-np.mod(phase0[c] + steps[c] * k * N, 1023.0) for c in range(NCH)]
     for b in bands:
-        arr = np.zeros(NCH * NEP, capi.TRK_ITEM_DTYPE)
-        cids = []
-        for c in range(NCH):
-            cid = eng.channel_create(b, 3)
-            eng.channel_set_code(cid, codes[c], shifts)
-            cids.append(cid)
-        k = np.arange(NEP)
-        for c in range(NCH):
-            sl = arr[c::NCH]                       # epoch-major: the channels of one epoch are neighbours
-            sl["channel"] = cids[c]
-            sl["n"] = N
-            sl["sample_index"] = bands[b] + k * N + (c % 7)      # staggered epoch starts, as real channels have
-            sl["rem_code_phase_chips"] = -np.mod(phase0[c] + steps[c] * k * N, 1023.0)
-            sl["code_phase_step_chips"] = steps[c]
-        items[b] = arr
+        cids = [tr.channel(eng, b, codes[c], shifts) for c in range(NCH)]
+        # epoch-major: the channels of one epoch are neighbours; staggered epoch starts, as real channels have
+        items[b] = tr.items((cids[c], N, bands[b] + j * N + (c % 7), 0.0, 0.0, 0.0, rems[c][j], steps[c])
+                            for j in range(NEP) for c in range(NCH))
     yield eng, items, (x1, x2), codes, shifts
     eng.close()
 
@@ -102,22 +91,13 @@ def test_c2_full_size_signal_prompt_dominates(capi, oracle):
     n_ep = 200                                       # 0.2 s of the stream is enough for this property (5 M samples)
     iq = make_iq(codes, FS, N * n_ep + 64, svs, seed=6)
     eng = capi.Engine(0)
-    eng.iq_create(0, len(iq))
-    first = eng.iq_push(0, iq)
-    arr = np.zeros(NCH * n_ep, capi.TRK_ITEM_DTYPE)
+    first = tr.ring(eng, 0, iq)
+    rows = [None] * (NCH * n_ep)
     for c, sv in enumerate(svs):
-        cid = eng.channel_create(0, 3)
-        eng.channel_set_code(cid, codes[sv["prn"]], [-0.5, 0.0, 0.5])
+        cid = tr.channel(eng, 0, codes[sv["prn"]], [-0.5, 0.0, 0.5])
         s, rc, dp, rcode, st = trk_params_for(sv, FS, N, n_ep)
-        sl = arr[c::NCH]
-        sl["channel"] = cid
-        sl["n"] = N
-        sl["sample_index"] = first + s
-        sl["rem_carrier_phase_rad"] = rc
-        sl["phase_step_rad"] = dp
-        sl["rem_code_phase_chips"] = rcode
-        sl["code_phase_step_chips"] = st
-    taps = eng.trk_batch(arr, 3)
+        rows[c::NCH] = [(cid, N, first + int(s[k]), rc[k], dp[k], 0.0, rcode[k], st[k]) for k in range(n_ep)]
+    taps = eng.trk_batch(tr.items(rows), 3)
     eng.close()
     full = N * ca_amplitude(45.0, FS)
     for c in range(NCH):

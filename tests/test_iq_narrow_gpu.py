@@ -9,19 +9,14 @@ narrow band, and the device loops refuse narrow bands.
 import numpy as np
 import pytest
 
-from gpu_fixtures import capi, engine  # noqa: F401
-from trk_ref import int_code, int_oracle
+from gpu_fixtures import capi, engine, torch  # noqa: F401
+import trk_rig as tr
+from trk_ref import exact_taps, int_code
 
 pytestmark = pytest.mark.gpu
 
 ERR_ARG, ERR_STATE = -1, -4
 WIDTHS = {"ishort": np.int16, "ibyte": np.int8}
-
-
-@pytest.fixture(scope="module")
-def torch():
-    import torch as t
-    return t
 
 
 def _ints(rng, n, item_type):
@@ -47,43 +42,18 @@ class Pair:
             self.e.iq_push_int(b, iq)
         assert self.e.iq_window(0) == self.e.iq_window(1)
 
-    def channel(self, taps, code, shifts, hd=False):
+    def channel(self, code, shifts, hd=False):
         for b in (0, 1):
-            c = self.e.channel_create(b, taps)
-            self.e.channel_set_code(c, code, shifts, hd)
-            self.ch[b].append(c)
+            self.ch[b].append(tr.channel(self.e, b, code, shifts, hd))
         return len(self.ch[0]) - 1
 
     def items(self, specs):
         """specs: (channel index, start, n, rem_carr, dphi, rem_code, step[, rate]) -> (items on band 0, items on band 1)"""
-        out = []
-        for b in (0, 1):
-            it = np.zeros(len(specs), capi_dtype())
-            for k, s in enumerate(specs):
-                c, s0, n, rc, dp, rem, step = s[:7]
-                it[k] = (self.ch[b][c], n, s0, rc, dp, 0.0, rem, step, s[7] if len(s) > 7 else 0.0)
-            out.append(it)
-        return out
+        return [tr.items((self.ch[b][c], n, s0, rc, dp, 0.0, rem, step, *rate) for c, s0, n, rc, dp, rem, step, *rate in specs)
+                for b in (0, 1)]
 
     def close(self):
         self.e.close()
-
-
-def capi_dtype():
-    import gnss_sdr_b200.capi as c
-    return c.TRK_ITEM_DTYPE
-
-
-def _run_dev(torch, e, items, stride, slices):
-    items_t = torch.from_numpy(np.ascontiguousarray(items).view(np.uint8)).cuda()
-    out_t = torch.zeros((len(items), stride, 2), dtype=torch.float32, device="cuda")
-    e.trk_batch_dev(items_t.data_ptr(), len(items), out_t.data_ptr(), stride, slices)
-    e.sync()
-    return out_t.cpu().numpy()
-
-
-def _shifts(taps):
-    return [0.0] if taps == 1 else [float(s) for s in np.linspace(-0.5, 0.5, taps).astype(np.float32)]
 
 
 def _item_specs(rng, lo, hi, cap, chans, count):
@@ -118,9 +88,9 @@ def test_taps_equal_the_float_band(capi, torch, item_type, taps):
     lo, hi = p.e.iq_window(0)
     assert hi > 1 << 24
     code = np.sign(rng.standard_normal(1023)).astype(np.float32)
-    c_fast = p.channel(taps, code, _shifts(taps))
-    c_mod = p.channel(taps, code, [float(s) for s in np.linspace(-700.25, 1500.5, taps)] if taps > 1 else [900.5])
-    c_hd = p.channel(taps, code, _shifts(taps), hd=True)
+    c_fast = p.channel(code, tr.shifts(taps))
+    c_mod = p.channel(code, [float(s) for s in np.linspace(-700.25, 1500.5, taps)] if taps > 1 else [900.5])
+    c_hd = p.channel(code, tr.shifts(taps), hd=True)
     specs = _item_specs(rng, lo, hi, cap, [c_fast, c_mod], 24)
     specs += [(c_hd, s0, n, rc, dp, rem, step, 1e-7) for (_, s0, n, rc, dp, rem, step) in specs[:6]]
     a, b = p.items(specs)
@@ -128,7 +98,7 @@ def test_taps_equal_the_float_band(capi, torch, item_type, taps):
     many_a, many_b = np.tile(a, 50), np.tile(b, 50)         # > 1024 items: the copy-stream submit path
     assert p.e.trk_batch(many_b, 8).tobytes() == p.e.trk_batch(many_a, 8).tobytes()
     for slices in (1, 2, 7, 64):
-        assert _run_dev(torch, p.e, b, 8, slices).tobytes() == _run_dev(torch, p.e, a, 8, slices).tobytes(), slices
+        assert tr.run_dev(torch, p.e, b, 8, slices).tobytes() == tr.run_dev(torch, p.e, a, 8, slices).tobytes(), slices
     p.close()
 
 
@@ -142,16 +112,12 @@ def test_integer_exact_against_the_oracle(capi, oracle, item_type):
     iq = rng.integers(-100, 101, 2 * (1 << 14)).astype(WIDTHS[item_type])
     e.iq_push_int(0, iq)
     code_int = int_code(L, nonzero=True)
-    c = e.channel_create(0, len(shifts))
-    e.channel_set_code(c, code_int.astype(np.float32), shifts)
-    _, idx = oracle.port.resampler(1, code_int.astype(np.float32), rem, step, shifts, n, return_idx=True)
+    c = tr.channel(e, 0, code_int, shifts)
     for s0 in (0, 1, 9000):
         x = iq[2 * s0:2 * (s0 + n)].astype(np.int64)
-        it = np.zeros(1, capi.TRK_ITEM_DTYPE)
-        it[0] = (c, n, s0, 0.0, 0.0, 0.0, rem, step, 0.0)
-        got = e.trk_batch(it, len(shifts))[0]
-        assert np.array_equal(got.real.astype(np.int64), int_oracle(x[0::2], code_int, idx)), s0
-        assert np.array_equal(got.imag.astype(np.int64), int_oracle(x[1::2], code_int, idx)), s0
+        got = e.trk_batch(tr.items([(c, n, s0, 0.0, 0.0, 0.0, rem, step)]), len(shifts))[0]
+        assert np.array_equal(got.real.astype(np.int64), exact_taps(oracle, x[0::2], code_int, rem, step, shifts, n)), s0
+        assert np.array_equal(got.imag.astype(np.int64), exact_taps(oracle, x[1::2], code_int, rem, step, shifts, n)), s0
     e.close()
 
 
@@ -171,21 +137,15 @@ def test_mixed_band_types_and_tap_counts_in_one_batch(capi, torch):
         e.iq_push_int(2, iq8)
     lo, hi = e.iq_window(0)
     code = np.sign(rng.standard_normal(1023)).astype(np.float32)
-    chans = {}
-    for b in range(3):
-        for taps in (5, 1, 3):
-            chans[(b, taps)] = e.channel_create(b, taps)
-            e.channel_set_code(chans[(b, taps)], code, _shifts(taps))
+    chans = {(b, taps): tr.channel(e, b, code, tr.shifts(taps)) for b in range(3) for taps in (5, 1, 3)}
     base = _item_specs(rng, lo, hi, cap, [5, 1, 3], 18)
-    items = np.zeros((3, len(base)), capi.TRK_ITEM_DTYPE)
-    for b in range(3):
-        for k, (taps, s0, n, rc, dp, rem, step) in enumerate(base):
-            items[b, k] = (chans[(b, taps)], n, s0, rc, dp, 0.0, rem, step, 0.0)
+    items = np.stack([tr.items((chans[(b, taps)], n, s0, rc, dp, 0.0, rem, step) for taps, s0, n, rc, dp, rem, step in base)
+                      for b in range(3)])
     order = rng.permutation(3 * len(base))
     flat = items.reshape(-1)[order]
     k0 = e.launch_count()
     for slices in (1, 4):
-        out = _run_dev(torch, e, flat, 8, slices)
+        out = tr.run_dev(torch, e, flat, 8, slices)
         back = np.empty_like(out)
         back[order] = out
         back = back.reshape(3, len(base), 8, 2)
@@ -205,7 +165,7 @@ def test_shared_kernel_never_reads_a_narrow_band(capi, mode):
     p = Pair(capi, "ishort", 1 << 20, kernel=0)
     p.push(_ints(rng, 1 << 19, "ishort"))
     code = np.sign(rng.standard_normal(1023)).astype(np.float32)
-    chans = [p.channel(3, code, [-0.5, 0.0, 0.5]) for _ in range(8)]
+    chans = [p.channel(code, [-0.5, 0.0, 0.5]) for _ in range(8)]
     specs = [(chans[k % 8], 1000 + 4000 * (k // 8) + 37 * (k % 8), 4000, 0.5, 0.01 * (k % 8), 0.25, 0.25575)
              for k in range(1024)]
     a, b = p.items(specs)
@@ -244,14 +204,8 @@ def test_narrow_pushes_launch_nothing_and_files_match_arrays(capi, tmp_path, ite
     assert e.launch_count() == k0
     assert e.iq_window(0) == e.iq_window(1) == (n - 4096, n)
     code = np.sign(rng.standard_normal(1023)).astype(np.float32)
-    ch = []
-    for b in (0, 1):
-        ch.append(e.channel_create(b, 3))
-        e.channel_set_code(ch[b], code, [-0.5, 0.0, 0.5])
-    items = np.zeros(2, capi.TRK_ITEM_DTYPE)
-    for b in (0, 1):
-        items[b] = (ch[b], 3000, n - 3500, 0.3, 0.02, 0.0, 0.1, 0.3, 0.0)
-    out = e.trk_batch(items, 3)
+    ch = [tr.channel(e, b, code, [-0.5, 0.0, 0.5]) for b in (0, 1)]
+    out = e.trk_batch(tr.items((c, 3000, n - 3500, 0.3, 0.02, 0.0, 0.1, 0.3) for c in ch), 3)
     assert out[0].tobytes() == out[1].tobytes()
     e.close()
 
@@ -347,15 +301,12 @@ def test_retyped_band_takes_the_narrow_path(capi, item_type):
     e.iq_create(0, cap)
     e.iq_create(1, cap)
     code = np.sign(rng.standard_normal(1023)).astype(np.float32)
-    ch = [e.channel_create(b, 3) for b in (0, 1)]
-    for c in ch:
-        e.channel_set_code(c, code, [-0.5, 0.0, 0.5])
+    ch = [tr.channel(e, b, code, [-0.5, 0.0, 0.5]) for b in (0, 1)]
     iq = _ints(rng, 3 * cap // 2, item_type)
-    items = np.zeros(2, capi.TRK_ITEM_DTYPE)
     for b in (0, 1):
         for half in (iq[:cap], iq[cap:]):
             e.iq_push_int(b, half)
-        items[b] = (ch[b], 4000, 3 * cap // 2 - 4100, 0.4, 0.03, 0.0, 0.2, 0.25, 0.0)
+    items = tr.items((c, 4000, 3 * cap // 2 - 4100, 0.4, 0.03, 0.0, 0.2, 0.25) for c in ch)
     first = e.trk_batch(items, 3)
     assert first[0].tobytes() == first[1].tobytes()
     e.iq_create(1, cap, item_type)

@@ -13,8 +13,9 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from gnss_synth import make_iq, trk_params_for  # noqa: E402
-from gpu_fixtures import capi, engine  # noqa: E402,F401
-from trk_ref import int_code, int_oracle, ref_or_port_avx  # noqa: E402
+from gpu_fixtures import capi, engine, torch  # noqa: E402,F401
+import trk_rig as tr  # noqa: E402
+from trk_ref import exact_taps, int_code, ref_or_port_avx  # noqa: E402
 
 
 SHAPES = [
@@ -47,8 +48,7 @@ def test_single_correlator_integer_exact(capi, engine, oracle, n, L, shifts, rem
     x_int = rng.integers(-7, 8, n)
     x_int[x_int == 0] = 1
     code_int = int_code(L, nonzero=True)
-    _, idx = oracle.port.resampler(1, code_int.astype(np.float32), rem, step, shifts, n, return_idx=True)
-    want = int_oracle(x_int, code_int, idx)
+    want = exact_taps(oracle, x_int, code_int, rem, step, shifts, n)
     mc = capi.Multicorrelator(engine, n, len(shifts))
     mc.set_high_dynamics_resampler(False)
     mc.set_local_code_and_taps(code_int.astype(np.float32), shifts)
@@ -69,30 +69,12 @@ def test_batch_sample_offsets_integer_exact(capi, engine, oracle, first, offset)
     x_int = rng.integers(-7, 8, total)
     code_int = int_code(L)
     e = engine
-    band = 3
-    e.iq_create(band, total)
-    # advance the ring so absolute indices are large and the data wraps around the ring end
-    pad = np.zeros(total, np.complex64)
-    done = 0
-    while done < first:
-        k = min(total, first - done)
-        e.iq_push(band, pad[:k])
-        done += k
-    f0 = e.iq_push(band, x_int.astype(np.complex64))
+    # a lead-in of `first` zeros makes absolute indices large and wraps the data around the ring end
+    f0 = tr.ring(e, 3, x_int.astype(np.complex64), total, np.zeros(first, np.complex64))
     assert f0 == first
-    cid = e.channel_create(band, 3)
-    e.channel_set_code(cid, code_int.astype(np.float32), shifts)
-    s_idx = first + offset
-    items = np.zeros(1, capi.TRK_ITEM_DTYPE)
-    items["channel"] = cid
-    items["n"] = n
-    items["sample_index"] = s_idx
-    items["rem_code_phase_chips"] = rem
-    items["code_phase_step_chips"] = step
-    got = e.trk_batch(items, 3)[0]
-    xs = x_int[offset: offset + n]
-    _, idx = oracle.port.resampler(1, code_int.astype(np.float32), rem, step, shifts, n, return_idx=True)
-    want = int_oracle(xs, code_int, idx)
+    cid = tr.channel(e, 3, code_int, shifts)
+    got = e.trk_batch(tr.items([(cid, n, first + offset, 0.0, 0.0, 0.0, rem, step)]), 3)[0]
+    want = exact_taps(oracle, x_int[offset: offset + n], code_int, rem, step, shifts, n)
     assert np.array_equal(got.real.astype(np.int64), want)
     assert np.all(got.imag == 0)
 
@@ -156,28 +138,15 @@ def test_batch_c2_slice_of_baseline_config(capi, engine, oracle):
                 cn0=45.0, phase0=float(rng.uniform(0, 6.28))) for p in range(1, nch + 1)]
     iq = make_iq(codes, fs, n * nep + 64, svs, seed=2)
     e = engine
-    band = 1
-    e.iq_create(band, len(iq))
-    first = e.iq_push(band, iq)
+    first = tr.ring(e, 1, iq)
     shifts = [-0.5, 0.0, 0.5]
-    items = np.zeros(nch * nep, capi.TRK_ITEM_DTYPE)
-    cids = []
-    for sv in svs:
-        cid = e.channel_create(band, 3)
-        e.channel_set_code(cid, codes[sv["prn"]], shifts)
-        cids.append(cid)
-    params = []
+    cids = [tr.channel(e, 1, codes[sv["prn"]], shifts) for sv in svs]
+    rows = [None] * (nch * nep)
     for c, sv in enumerate(svs):
         s, rc, dp, rcode, st = trk_params_for(sv, fs, n, nep)
-        for k in range(nep):
-            it = items[k * nch + c]   # epoch-major order: channels of one epoch are neighbours
-            it["channel"] = cids[c]
-            it["n"] = n
-            it["sample_index"] = first + int(s[k])
-            it["rem_carrier_phase_rad"] = rc[k]
-            it["phase_step_rad"] = dp[k]
-            it["rem_code_phase_chips"] = rcode[k]
-            it["code_phase_step_chips"] = st[k]
+        for k in range(nep):   # epoch-major order: channels of one epoch are neighbours
+            rows[k * nch + c] = (cids[c], n, first + int(s[k]), rc[k], dp[k], 0.0, rcode[k], st[k])
+    items = tr.items(rows)
     got = e.trk_batch(items, 3)
     # oracle on a subset of items (every 7th) to keep the CPU side quick
     worst_ref, worst_truth = 0.0, 0.0
@@ -196,10 +165,9 @@ def test_batch_c2_slice_of_baseline_config(capi, engine, oracle):
     assert worst_truth < 1e-5
 
 
-def test_batch_slices_agree_and_are_deterministic(capi, engine, oracle):
+def test_batch_slices_agree_and_are_deterministic(capi, engine, torch, oracle):
     """Splitting an epoch over 1..64 CTAs changes only the float summation order (tiny) and
     repeated launches are bitwise identical (deterministic cross-CTA combine)."""
-    import torch
     n, L = 25000, 1023
     rng = np.random.default_rng(5)
     iq = (rng.standard_normal(n + 8) + 1j * rng.standard_normal(n + 8)).astype(np.complex64)
@@ -208,25 +176,11 @@ def test_batch_slices_agree_and_are_deterministic(capi, engine, oracle):
     band = 2
     iq_t = torch.from_numpy(iq.view(np.float32)).cuda()
     e.iq_attach_dev(band, iq_t.data_ptr(), n + 8, 0)
-    cid = e.channel_create(band, 3)
-    e.channel_set_code(cid, code, [-0.5, 0.0, 0.5])
-    items = np.zeros(1, capi.TRK_ITEM_DTYPE)
-    items["channel"] = cid
-    items["n"] = n
-    items["sample_index"] = 3
-    items["rem_carrier_phase_rad"] = 0.3
-    items["phase_step_rad"] = 1e-3
-    items["rem_code_phase_chips"] = 0.2
-    items["code_phase_step_chips"] = 0.04092
-    items_t = torch.from_numpy(items.view(np.uint8)).cuda()
+    cid = tr.channel(e, band, code, [-0.5, 0.0, 0.5])
+    items = tr.items([(cid, n, 3, 0.3, 1e-3, 0.0, 0.2, 0.04092)])
     outs = {}
     for slices in (1, 2, 7, 16, 64):
-        reps = []
-        for _ in range(3):
-            out_t = torch.zeros(8, 2, dtype=torch.float32, device="cuda")
-            e.trk_batch_dev(items_t.data_ptr(), 1, out_t.data_ptr(), 8, slices)
-            e.sync()
-            reps.append(out_t.cpu().numpy().copy())
+        reps = [tr.run_dev(torch, e, items, 8, slices)[0] for _ in range(3)]
         assert np.array_equal(reps[0], reps[1]) and np.array_equal(reps[0], reps[2])
         outs[slices] = reps[0][:3, 0] + 1j * reps[0][:3, 1]
     for s, v in outs.items():
@@ -242,25 +196,13 @@ def test_mixed_tap_counts_in_one_batch(capi, engine, oracle):
     code_a = int_code(L)
     code_b = ((np.arange(L) * 104729) % 29) - 14
     e = engine
-    band = 4
-    e.iq_create(band, 8192)
-    first = e.iq_push(band, x_int.astype(np.complex64))
+    first = tr.ring(e, 4, x_int.astype(np.complex64), 8192)
     sh5 = [-1.2, -0.3, 0.0, 0.3, 1.2]
-    ca = e.channel_create(band, 5)
-    cb = e.channel_create(band, 1)
-    e.channel_set_code(ca, code_a.astype(np.float32), sh5)
-    e.channel_set_code(cb, code_b.astype(np.float32), [0.0])
-    items = np.zeros(2, capi.TRK_ITEM_DTYPE)
-    items["channel"] = [ca, cb]
-    items["n"] = n
-    items["sample_index"] = first
-    items["rem_code_phase_chips"] = 0.41
-    items["code_phase_step_chips"] = 0.3411
-    got = e.trk_batch(items, 5)
-    _, ia = oracle.port.resampler(1, code_a.astype(np.float32), 0.41, 0.3411, sh5, n, return_idx=True)
-    _, ib = oracle.port.resampler(1, code_b.astype(np.float32), 0.41, 0.3411, [0.0], n, return_idx=True)
-    assert np.array_equal(got[0].real.astype(np.int64), int_oracle(x_int, code_a, ia))
-    assert np.array_equal(got[1, :1].real.astype(np.int64), int_oracle(x_int, code_b, ib))
+    ca = tr.channel(e, 4, code_a, sh5)
+    cb = tr.channel(e, 4, code_b, [0.0])
+    got = e.trk_batch(tr.items((c, n, first, 0.0, 0.0, 0.0, 0.41, 0.3411) for c in (ca, cb)), 5)
+    assert np.array_equal(got[0].real.astype(np.int64), exact_taps(oracle, x_int, code_a, 0.41, 0.3411, sh5, n))
+    assert np.array_equal(got[1, :1].real.astype(np.int64), exact_taps(oracle, x_int, code_b, 0.41, 0.3411, [0.0], n))
 
 
 def test_error_paths(capi, engine):
@@ -346,19 +288,9 @@ def test_submit_wait_overlapped_batches(capi, engine, oracle):
     rng = np.random.default_rng(21)
     iq = (rng.standard_normal(n * 6 + 8) + 1j * rng.standard_normal(n * 6 + 8)).astype(np.complex64)
     e = engine
-    band = 5
-    e.iq_create(band, len(iq))
-    first = e.iq_push(band, iq)
-    cid = e.channel_create(band, 3)
-    e.channel_set_code(cid, oracle.port.gps_ca_code(4), [-0.5, 0.0, 0.5])
-    items = np.zeros(6, capi.TRK_ITEM_DTYPE)
-    items["channel"] = cid
-    items["n"] = n
-    items["sample_index"] = first + np.arange(6) * n + 1
-    items["rem_carrier_phase_rad"] = 0.2
-    items["phase_step_rad"] = 2e-3
-    items["rem_code_phase_chips"] = 0.1
-    items["code_phase_step_chips"] = 0.25575
+    first = tr.ring(e, 5, iq)
+    cid = tr.channel(e, 5, oracle.port.gps_ca_code(4), [-0.5, 0.0, 0.5])
+    items = tr.items((cid, n, first + k * n + 1, 0.2, 2e-3, 0.0, 0.1, 0.25575) for k in range(6))
     want = e.trk_batch(items, 3)
     t = [e.trk_submit(items[k:k + 2], 3) for k in (0, 2, 4)]
     got = {k: e.trk_wait(t[k]) for k in (2, 0, 1)}
@@ -379,22 +311,12 @@ def test_integer_sample_ingestion_bitexact(capi, engine, oracle, dtype):
     as_c64 = (raw[0::2].astype(np.float32) + 1j * raw[1::2].astype(np.float32)).astype(np.complex64)
     e = engine
     res = {}
-    for name, band in (("float", 6), ("int", 7)):
-        e.iq_create(band, 32768)
-        # misalign the write position so that the data wraps around the ring end
-        e.iq_push(band, np.zeros(20001, np.complex64))
-        first = e.iq_push(band, as_c64) if name == "float" else e.iq_push_int(band, raw)
+    for name, band, data in (("float", 6, as_c64), ("int", 7, raw)):
+        # a lead-in misaligns the write position so that the data wraps around the ring end
+        first = tr.ring(e, band, data, 32768, np.zeros(20001, np.complex64))
         assert first == 20001
-        cid = e.channel_create(band, 3)
-        e.channel_set_code(cid, oracle.port.gps_ca_code(6), [-0.5, 0.0, 0.5])
-        items = np.zeros(5, capi.TRK_ITEM_DTYPE)
-        items["channel"] = cid
-        items["n"] = n
-        items["sample_index"] = first + np.arange(5) * n + 3
-        items["rem_carrier_phase_rad"] = 0.2
-        items["phase_step_rad"] = 2e-3
-        items["rem_code_phase_chips"] = 0.1
-        items["code_phase_step_chips"] = 0.25575
+        cid = tr.channel(e, band, oracle.port.gps_ca_code(6), [-0.5, 0.0, 0.5])
+        items = tr.items((cid, n, first + k * n + 3, 0.2, 2e-3, 0.0, 0.1, 0.25575) for k in range(5))
         res[name] = e.trk_batch(items, 3)
     assert np.array_equal(res["float"], res["int"])
     assert np.all(np.abs(res["int"]) > 0)
@@ -406,7 +328,7 @@ def test_integer_sample_ingestion_bitexact(capi, engine, oracle, dtype):
     (10230, [-0.5, 0.0, 0.5], 0.2046, 12000),                   # L5-sized table
     (1023, [0.0], 0.2557, 4001),                                # 1 tap, ragged length
 ])
-def test_shared_window_groups_staggered_integer_exact(capi, oracle, L, taps_shifts, step, n):
+def test_shared_window_groups_staggered_integer_exact(capi, torch, oracle, L, taps_shifts, step, n):
     """The shared-window kernel (groups of 8 items served from one TMA-staged copy of the samples):
     epochs of different channels start at different, odd/even sample offsets (as in a real receiver,
     where every channel is aligned to its own code period), item count not a multiple of 8, different
@@ -421,39 +343,19 @@ def test_shared_window_groups_staggered_integer_exact(capi, oracle, L, taps_shif
     rems = rng.uniform(-3, 3, n_ch).astype(np.float32)
     want = {}
     for c in range(n_ch):
-        _, idx = oracle.port.resampler(1, codes[c].astype(np.float32), float(rems[c]), step, taps_shifts, n, return_idx=True)
         for k in range(n_ep):
             s0 = int(starts[c]) + k * n
-            want[(k, c)] = int_oracle(x_int[s0:s0 + n], codes[c], idx)
+            want[(k, c)] = exact_taps(oracle, x_int[s0:s0 + n], codes[c], float(rems[c]), step, taps_shifts, n)
+    order = [(k, c) for k in range(n_ep) for c in range(n_ch)]
     results = {}
     for mode in ("1", "0"):
         e = capi.Engine(0)
         e.trk_kernel_choice(int(mode))
-        e.iq_create(0, total)
-        first = e.iq_push(0, x_int.astype(np.complex64))
-        cids = []
-        for c in range(n_ch):
-            cid = e.channel_create(0, len(taps_shifts))
-            e.channel_set_code(cid, codes[c].astype(np.float32), taps_shifts)
-            cids.append(cid)
-        items = np.zeros(n_ch * n_ep, capi.TRK_ITEM_DTYPE)
-        order = []
-        for k in range(n_ep):
-            for c in range(n_ch):
-                it = items[len(order)]
-                it["channel"] = cids[c]
-                it["n"] = n
-                it["sample_index"] = first + int(starts[c]) + k * n
-                it["rem_code_phase_chips"] = rems[c]
-                it["code_phase_step_chips"] = step
-                order.append((k, c))
+        first = tr.ring(e, 0, x_int.astype(np.complex64))
+        cids = [tr.channel(e, 0, codes[c], taps_shifts) for c in range(n_ch)]
+        items = tr.items((cids[c], n, first + int(starts[c]) + k * n, 0.0, 0.0, 0.0, rems[c], step) for k, c in order)
         # device-pointer entry point with slices = 1 is where the engine picks the shared kernel
-        import torch
-        items_t = torch.from_numpy(items.view(np.uint8)).cuda()
-        out_t = torch.zeros(len(order), len(taps_shifts), 2, dtype=torch.float32, device="cuda")
-        e.trk_batch_dev(items_t.data_ptr(), len(order), out_t.data_ptr(), len(taps_shifts), 1)
-        e.sync()
-        got = out_t.cpu().numpy()
+        got = tr.run_dev(torch, e, items, len(taps_shifts))
         results[mode] = got
         for i, key in enumerate(order):
             assert np.array_equal(got[i, :, 0].astype(np.int64), want[key]), (mode, key)
@@ -462,11 +364,10 @@ def test_shared_window_groups_staggered_integer_exact(capi, oracle, L, taps_shif
     assert np.array_equal(results["0"], results["1"])
 
 
-def test_shared_kernel_groups_that_cannot_share(capi, oracle):
+def test_shared_kernel_groups_that_cannot_share(capi, torch, oracle):
     """Groups of 8 items whose sample ranges are far apart (channel-major order: 8 consecutive epochs of one
     channel) or that sit on different bands cannot share a window; each warp then streams its own samples
     with the same arithmetic.  Integer-exact."""
-    import torch
     n, L, shifts, step = 6000, 1023, [-0.5, 0.0, 0.5], 0.1705
     rng = np.random.default_rng(4242)
     n_ch, n_ep = 4, 9
@@ -475,79 +376,39 @@ def test_shared_kernel_groups_that_cannot_share(capi, oracle):
     codes = [int_code(L, c) for c in range(n_ch)]
     e = capi.Engine(0)
     e.trk_kernel_choice(1)
-    firsts = []
-    for b in range(2):
-        e.iq_create(b, total)
-        firsts.append(e.iq_push(b, xs[b].astype(np.complex64)))
-    cids = []
-    for c in range(n_ch):
-        cid = e.channel_create(c % 2, 3)                          # channels alternate between the bands
-        e.channel_set_code(cid, codes[c].astype(np.float32), shifts)
-        cids.append(cid)
-    items = np.zeros(n_ch * n_ep, capi.TRK_ITEM_DTYPE)
-    order = []
-    for c in range(n_ch):                                         # channel-major: consecutive epochs of one channel
-        for k in range(n_ep):
-            it = items[len(order)]
-            it["channel"] = cids[c]
-            it["n"] = n
-            it["sample_index"] = firsts[c % 2] + 37 * c + k * n + (k % 2)
-            it["rem_code_phase_chips"] = 0.3 + c
-            it["code_phase_step_chips"] = step
-            order.append((c, k))
-    items_t = torch.from_numpy(items.view(np.uint8)).cuda()
-    out_t = torch.zeros(len(order), 3, 2, dtype=torch.float32, device="cuda")
-    e.trk_batch_dev(items_t.data_ptr(), len(order), out_t.data_ptr(), 3, 1)
-    e.sync()
-    got = out_t.cpu().numpy()
+    firsts = [tr.ring(e, b, xs[b].astype(np.complex64)) for b in range(2)]
+    cids = [tr.channel(e, c % 2, codes[c], shifts) for c in range(n_ch)]    # channels alternate between the bands
+    order = [(c, k) for c in range(n_ch) for k in range(n_ep)]           # channel-major: consecutive epochs of one channel
+    items = tr.items((cids[c], n, firsts[c % 2] + 37 * c + k * n + (k % 2), 0.0, 0.0, 0.0, 0.3 + c, step) for c, k in order)
+    got = tr.run_dev(torch, e, items, 3)
     e.close()
     for i, (c, k) in enumerate(order):
-        _, idx = oracle.port.resampler(1, codes[c].astype(np.float32), 0.3 + c, step, shifts, n, return_idx=True)
         s0 = 37 * c + k * n + (k % 2)
-        want = int_oracle(xs[c % 2][s0:s0 + n], codes[c], idx)
+        want = exact_taps(oracle, xs[c % 2][s0:s0 + n], codes[c], 0.3 + c, step, shifts, n)
         assert np.array_equal(got[i, :, 0].astype(np.int64), want), (c, k)
         assert np.all(got[i, :, 1] == 0)
 
 
-def test_kernel_choice_only_through_the_api(capi, oracle, monkeypatch):
+def test_kernel_choice_only_through_the_api(capi, torch, oracle, monkeypatch):
     """The engine picks the correlator kernel from b200_trk_kernel_choice alone; B200_TRK_SHARED in the environment
     changes nothing.  1024 overlapping C/A-like float items at 25 Msps on the device entry point: by default they take the
     shared-window kernel, byte for byte what forcing it (1) gives, and -1 means the default.  These items take its chunk
     path, whose float sums differ from the per-item kernel's in the last bits, so the per-item result (0) must differ."""
-    import torch
     monkeypatch.setenv("B200_TRK_SHARED", "0")
     fs, n, n_ch, n_ep = 25e6, 25000, 32, 32
     rng = np.random.default_rng(1024)
     total = n * (n_ep + 1)
     e = capi.Engine(0)
-    e.iq_create(0, 1 << 20)
-    first = e.iq_push(0, (rng.normal(size=total) + 1j * rng.normal(size=total)).astype(np.complex64))
-    cids = []
-    for c in range(n_ch):
-        cid = e.channel_create(0, 3)
-        e.channel_set_code(cid, oracle.port.gps_ca_code(c + 1), [-0.5, 0.0, 0.5])
-        cids.append(cid)
+    first = tr.ring(e, 0, (rng.normal(size=total) + 1j * rng.normal(size=total)).astype(np.complex64), 1 << 20)
+    cids = [tr.channel(e, 0, oracle.port.gps_ca_code(c + 1), [-0.5, 0.0, 0.5]) for c in range(n_ch)]
     starts = np.sort(rng.integers(0, n, n_ch))
     dopplers = rng.uniform(-4000.0, 4000.0, n_ch)
-    items = np.zeros(n_ch * n_ep, capi.TRK_ITEM_DTYPE)
-    for k in range(n_ep):                                          # epoch-major: a group's 8 items overlap in the band
-        for c in range(n_ch):
-            it = items[k * n_ch + c]
-            it["channel"] = cids[c]
-            it["n"] = n
-            it["sample_index"] = first + int(starts[c]) + k * n
-            it["rem_carrier_phase_rad"] = 0.1 * c
-            it["phase_step_rad"] = 2 * np.pi * dopplers[c] / fs
-            it["rem_code_phase_chips"] = 0.01 * c
-            it["code_phase_step_chips"] = 1.023e6 * (1 + dopplers[c] / 1575.42e6) / fs
-    items_t = torch.from_numpy(items.view(np.uint8)).cuda()
-    out_t = torch.zeros(len(items), 3, 2, dtype=torch.float32, device="cuda")
+    items = tr.items((cids[c], n, first + int(starts[c]) + k * n, 0.1 * c, 2 * np.pi * dopplers[c] / fs, 0.0, 0.01 * c,
+                      1.023e6 * (1 + dopplers[c] / 1575.42e6) / fs)
+                     for k in range(n_ep) for c in range(n_ch))    # epoch-major: a group's 8 items overlap in the band
 
     def run():
-        out_t.zero_()
-        e.trk_batch_dev(items_t.data_ptr(), len(items), out_t.data_ptr(), 3, 1)
-        e.sync()
-        return out_t.cpu().numpy().tobytes()
+        return tr.run_dev(torch, e, items, 3).tobytes()
 
     default = run()
     e.trk_kernel_choice(1)
@@ -575,23 +436,10 @@ def test_kernel_choice_by_layout_is_integer_exact(capi, oracle, layout):
     x = rng.integers(-9, 10, total)
     codes = [np.where(rng.integers(0, 2, L) > 0, 1, -1) for _ in range(n_ch)]
     e = capi.Engine(0)
-    e.iq_create(0, total)
-    first = e.iq_push(0, x.astype(np.complex64))
-    items = np.zeros(n_ch * n_ep, capi.TRK_ITEM_DTYPE)
-    where = []
-    for k in range(n_ep):
-        for c in range(n_ch):
-            if k == 0:
-                cid = e.channel_create(0, 3)
-                e.channel_set_code(cid, codes[c].astype(np.float32), shifts)
-            it = items[len(where)]
-            it["channel"] = c
-            it["n"] = n
-            s0 = k * n + (c % 5) + (c * span if layout == "distinct" else 0)
-            it["sample_index"] = first + s0
-            it["rem_code_phase_chips"] = 0.25 + c
-            it["code_phase_step_chips"] = step
-            where.append((c, s0))
+    first = tr.ring(e, 0, x.astype(np.complex64))
+    cids = [tr.channel(e, 0, codes[c], shifts) for c in range(n_ch)]
+    where = [(c, k * n + (c % 5) + (c * span if layout == "distinct" else 0)) for k in range(n_ep) for c in range(n_ch)]
+    items = tr.items((cids[c], n, first + s0, 0.0, 0.0, 0.0, 0.25 + c, step) for c, s0 in where)
     results = {}
     for mode in (2, 0, 1):
         e.trk_kernel_choice(mode)
@@ -601,8 +449,7 @@ def test_kernel_choice_by_layout_is_integer_exact(capi, oracle, layout):
     got = results[2]
     for i in range(0, len(where), 7):
         c, s0 = where[i]
-        _, idx = oracle.port.resampler(1, codes[c].astype(np.float32), 0.25 + c, step, shifts, n, return_idx=True)
-        want = int_oracle(x[s0:s0 + n], codes[c], idx)
+        want = exact_taps(oracle, x[s0:s0 + n], codes[c], 0.25 + c, step, shifts, n)
         assert np.array_equal(got[i].real.astype(np.int64), want), (c, s0)
         assert np.all(got[i].imag == 0)
 
@@ -642,17 +489,11 @@ def test_file_source_push_matches_array_push(oracle, tmp_path, item_type):
     assert pushed == total - skip and first_a == first_b == 0
     first_c, pushed_c = e.iq_push_file(1, path, item_type, header_bytes=header, skip_samples=0, max_samples=5000, chunk_samples=1024)
     assert pushed_c == 5000 and first_c == total - skip
-    items = np.zeros(8, capi.TRK_ITEM_DTYPE)
     _, rc, dp, rcode, st = gs.trk_params_for(sv, fs, n, 8)
     out = []
     for b in (0, 1):
-        ch = e.channel_create(b, 3)
-        e.channel_set_code(ch, code, [-0.5, 0.0, 0.5])
-        items["channel"], items["n"] = ch, n
-        items["sample_index"] = np.arange(8) * n
-        items["rem_carrier_phase_rad"], items["phase_step_rad"] = rc, dp
-        items["rem_code_phase_chips"], items["code_phase_step_chips"] = rcode, st
-        out.append(e.trk_batch(items, 3))
+        ch = tr.channel(e, b, code, [-0.5, 0.0, 0.5])
+        out.append(e.trk_batch(tr.items((ch, n, k * n, rc[k], dp[k], 0.0, rcode[k], st[k]) for k in range(8)), 3))
     assert out[0].tobytes() == out[1].tobytes()
     assert np.abs(out[0][:, 1]).min() > 0
     with pytest.raises(capi.B200Error):
@@ -679,19 +520,14 @@ def test_push_at_is_idempotent_and_handles_gaps(capi, oracle):
     assert eng.iq_window(2) == (base, base + 16000)
     code = np.where(rng.integers(0, 2, 1023) > 0, 1.0, -1.0).astype(np.float32)
     shifts = [-0.5, 0.0, 0.5]
-    ch = eng.channel_create(2, 3)
-    eng.channel_set_code(ch, code, shifts)
-    items = np.zeros(1, capi.TRK_ITEM_DTYPE)
-    items[0] = (ch, 4000, base + 8000, 0.2, 0.01, 0.0, 0.3, 0.2557, 0.0)
-    got = eng.trk_batch(items, 3)[0]
+    row = (tr.channel(eng, 2, code, shifts), 4000, base + 8000, 0.2, 0.01, 0.0, 0.3, 0.2557)
+    got = eng.trk_batch(tr.items([row]), 3)[0]
     want = oracle.port.multicorrelator(1, iq[8000:12000], code, shifts, 0.2, 0.01, 0.3, 0.2557)
     assert np.max(np.abs(got - want)) <= 1e-3 * np.abs(want[1])
-    items[0]["sample_index"] = base + 14000  # runs past the write index
     with pytest.raises(capi.B200Error):
-        eng.trk_batch(items, 3)
-    items[0]["sample_index"] = base - 100    # before the gap
+        eng.trk_batch(tr.items([row], sample_index=base + 14000), 3)    # runs past the write index
     with pytest.raises(capi.B200Error):
-        eng.trk_batch(items, 3)
+        eng.trk_batch(tr.items([row], sample_index=base - 100), 3)      # before the gap
     eng.close()
 
 
@@ -703,14 +539,10 @@ def test_channel_set_taps_takes_effect_in_stream_order(capi, oracle):
     n = 4000
     iq = (rng.standard_normal(8 * n) + 1j * rng.standard_normal(8 * n)).astype(np.complex64)
     code = np.where(rng.integers(0, 2, 1023) > 0, 1.0, -1.0).astype(np.float32)
-    eng.iq_create(0, 1 << 16)
-    eng.iq_push(0, iq)
-    ch = eng.channel_create(0, 3)
+    tr.ring(eng, 0, iq, 1 << 16)
     wide, narrow = [-0.5, 0.0, 0.5], [-0.15, 0.0, 0.15]
-    eng.channel_set_code(ch, code, wide)
-    items = np.zeros(2, capi.TRK_ITEM_DTYPE)
-    for k in range(2):
-        items[k] = (ch, n, k * n, 0.1, 0.02, 0.0, 0.4, 0.2557, 0.0)
+    ch = tr.channel(eng, 0, code, wide)
+    items = tr.items((ch, n, k * n, 0.1, 0.02, 0.0, 0.4, 0.2557) for k in range(2))
     a = eng.trk_batch(items, 3)
     eng.channel_set_taps(ch, narrow)
     b = eng.trk_batch(items, 3)
@@ -801,11 +633,8 @@ def test_push_at_restarts_when_the_stream_starts_over(capi, oracle):
     assert eng.iq_window(1) == (2000, 6000)
     assert eng.iq_push_at(1, 0, iq[:10000]) == 10000                   # and back (older index: restart)
     code = np.where(rng.integers(0, 2, 1023) > 0, 1.0, -1.0).astype(np.float32)
-    ch = eng.channel_create(1, 3)
-    eng.channel_set_code(ch, code, [-0.5, 0.0, 0.5])
-    items = np.zeros(1, capi.TRK_ITEM_DTYPE)
-    items[0] = (ch, 4000, 5000, 0.0, 0.0, 0.0, 0.3, 0.2557, 0.0)
-    got = eng.trk_batch(items, 3)[0]
+    ch = tr.channel(eng, 1, code, [-0.5, 0.0, 0.5])
+    got = eng.trk_batch(tr.items([(ch, 4000, 5000, 0.0, 0.0, 0.0, 0.3, 0.2557)]), 3)[0]
     want = oracle.port.multicorrelator(1, iq[5000:9000], code, [-0.5, 0.0, 0.5], 0.0, 0.0, 0.3, 0.2557)
     assert np.array_equal(got, want)
     eng.close()

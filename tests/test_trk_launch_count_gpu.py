@@ -8,8 +8,9 @@ count: a loop with a data channel has 3- or 5-tap pilot items and 1-tap data ite
 import numpy as np
 import pytest
 
-from gpu_fixtures import capi  # noqa: F401
+from gpu_fixtures import capi, torch  # noqa: F401
 import loop_rig as tl
+import trk_rig as tr
 
 pytestmark = pytest.mark.gpu
 
@@ -20,14 +21,9 @@ def batch_engine(capi, taps_list):
     """one band of random samples, one channel per entry of taps_list, one 4000-sample item per channel"""
     rng = np.random.default_rng(len(taps_list))
     e = capi.Engine(0)
-    e.iq_create(0, 1 << 16)
-    e.iq_push(0, (rng.normal(size=1 << 15) + 1j * rng.normal(size=1 << 15)).astype(np.complex64))
-    items = np.zeros(len(taps_list), capi.TRK_ITEM_DTYPE)
-    for i, taps in enumerate(taps_list):
-        ch = e.channel_create(0, taps)
-        e.channel_set_code(ch, rng.choice([-1.0, 1.0], 1023).astype(np.float32), list(np.linspace(-0.5, 0.5, taps)))
-        items[i] = (ch, N, 100 * i, 0.3, 0.01, 0.0, 0.2, 1.023e6 / 4e6, 0.0)
-    return e, items
+    tr.ring(e, 0, (rng.normal(size=1 << 15) + 1j * rng.normal(size=1 << 15)).astype(np.complex64), 1 << 16)
+    chans = [tr.channel(e, 0, rng.choice([-1.0, 1.0], 1023), list(np.linspace(-0.5, 0.5, taps))) for taps in taps_list]
+    return e, tr.items((ch, N, 100 * i, 0.3, 0.01, 0.0, 0.2, 1.023e6 / 4e6) for i, ch in enumerate(chans))
 
 
 @pytest.mark.parametrize("taps_list,launches", [
@@ -45,16 +41,11 @@ def test_per_item_batch_counts_one_launch_per_tap_count(capi, taps_list, launche
     e.close()
 
 
-def test_shared_window_batch_counts_one_launch(capi):
-    import torch
+def test_shared_window_batch_counts_one_launch(capi, torch):
     e, items = batch_engine(capi, [3] * 16)
     e.trk_kernel_choice(1)
-    items_dev = torch.from_numpy(items.view(np.uint8).copy()).cuda()
-    out_dev = torch.zeros(len(items) * 8, dtype=torch.complex64, device="cuda")
-    torch.cuda.synchronize()
     k0 = e.launch_count()
-    e.trk_batch_dev(items_dev.data_ptr(), len(items), out_dev.data_ptr(), 8, 1)
-    e.sync()
+    tr.run_dev(torch, e, items, 8)
     assert e.launch_count() - k0 == 1
     e.close()
 

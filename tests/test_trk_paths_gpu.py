@@ -28,13 +28,13 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from gnss_synth import make_iq, trk_params_for  # noqa: E402
-from gpu_fixtures import capi  # noqa: E402,F401
-from trk_ref import int_code, int_oracle  # noqa: E402
+from gpu_fixtures import capi, torch  # noqa: E402,F401
+import trk_rig as tr  # noqa: E402
+from trk_ref import exact_taps, int_code  # noqa: E402
 
 RING = 1 << 18          # ring bands of the per-item tests: 262 144 samples ...
 WRAP_AT = 60000         # ... whose end falls between data samples WRAP_AT - 1 and WRAP_AT
 N_DATA = RING - 4096
-SENTINEL = -12345.0     # outputs a launch must not touch keep this value
 ST25 = 1.023e6 * (1 + 3000 / 1575.42e6) / 25e6   # C/A chips per sample at 25 Msps, +3 kHz
 EDGE_NS = [0, 1, 7, 8, 9, 511, 512, 513, 1023, 1024, 1025, 8192 + 9, 16384 + 8]
 SLICES = [1, 2, 3, 7, 64]
@@ -54,16 +54,6 @@ def _report_worst():
     print()
 
 
-@pytest.fixture(scope="module")
-def torch():
-    import torch as t
-    return t
-
-
-def _shifts(taps, spread):
-    return [0.0] if taps == 1 else [float(s) for s in np.linspace(-spread, spread, taps).astype(np.float32)]
-
-
 def _hd_phase(n, rem_carr, dphi, drate):
     """the reference's high-dynamics carrier phase in float64: the rate term lags one sample and its exponent is
     float32((n-1)^2 mod 2^32) (the rotator squares an unsigned int)"""
@@ -74,65 +64,48 @@ def _hd_phase(n, rem_carr, dphi, drate):
     return -(float(np.float32(rem_carr)) + k.astype(np.float64) * float(np.float32(dphi)) + e * float(np.float32(drate)))
 
 
-def _run(torch, e, items, stride, slices=1):
-    """one b200_trk_batch_dev launch -> float32 (items, stride, 2); columns the launch leaves alone read SENTINEL"""
-    items_t = torch.from_numpy(np.ascontiguousarray(items).view(np.uint8)).cuda()
-    out_t = torch.full((len(items), stride, 2), SENTINEL, dtype=torch.float32, device="cuda")
-    e.trk_batch_dev(items_t.data_ptr(), len(items), out_t.data_ptr(), stride, slices)
-    e.sync()
-    return out_t.cpu().numpy()
-
-
 class Rig:
     """One engine with two ring bands: band 0 holds small-integer samples, band 1 complex Gaussian noise.  Each case
     gets a channel on each band; its integer item has a zero carrier, its float item a rotating one."""
 
     def __init__(self, capi, oracle, seed):
-        self.capi, self.oracle = capi, oracle
+        self.oracle = oracle
         self.e = capi.Engine(0)
         self.e.trk_kernel_choice(0)           # the per-item kernel
         rng = np.random.default_rng(seed)
         self.xi = rng.integers(-7, 8, N_DATA)
         self.xi[self.xi == 0] = 1
         self.xf = (rng.standard_normal(N_DATA) + 1j * rng.standard_normal(N_DATA)).astype(np.complex64)
-        self.first = []
-        for band, data in ((0, self.xi.astype(np.complex64)), (1, self.xf)):
-            self.e.iq_create(band, RING)
-            self.e.iq_push(band, np.zeros(RING - WRAP_AT, np.complex64))
-            self.first.append(self.e.iq_push(band, data))
-        self.items = []
+        lead = np.zeros(RING - WRAP_AT, np.complex64)
+        self.first = [tr.ring(self.e, band, data, RING, lead) for band, data in ((0, self.xi.astype(np.complex64)),
+                                                                                  (1, self.xf))]
+        self.rows = []
         self.cases = []
 
     def add(self, group, code, shifts, n, start, rem, step, hd=False, rate=0.0, carrier=(1.1, 0.21, 0.0)):
         """start: index of the epoch's first sample in the data (the ring's end lies before data sample WRAP_AT)"""
         assert start + n <= N_DATA
         for band in (0, 1):
-            cid = self.e.channel_create(band, len(shifts))
-            self.e.channel_set_code(cid, code.astype(np.float32), shifts, high_dyn=hd)
-            it = np.zeros(1, self.capi.TRK_ITEM_DTYPE)[0]
-            it["channel"], it["n"], it["sample_index"] = cid, n, self.first[band] + start
-            it["rem_code_phase_chips"], it["code_phase_step_chips"] = rem, step
-            if hd:
-                it["code_phase_rate_step_chips"] = rate
-            if band == 1:
-                it["rem_carrier_phase_rad"], it["phase_step_rad"], it["phase_rate_step_rad"] = carrier
-            self.items.append(it)
-            self.cases.append((group, band, code, shifts, n, start, rem, step, hd, rate, carrier if band == 1 else (0, 0, 0)))
+            cid = tr.channel(self.e, band, code, shifts, hd)
+            rc, dp, dr = carrier if band == 1 else (0, 0, 0)
+            self.rows.append((cid, n, self.first[band] + start, rc, dp, dr, rem, step, rate))
+            self.cases.append((group, band, code, shifts, n, start, rem, step, hd, rate, (rc, dp, dr)))
 
-    def item_array(self):
-        return np.array(self.items, dtype=self.capi.TRK_ITEM_DTYPE)
+    def items(self):
+        return tr.items(self.rows)
 
     def expected(self, k):
         """integer item: exact taps (int64); float item: (float64 truth, sigma per tap)"""
         group, band, code, shifts, n, start, rem, step, hd, rate, (rc, dp, dr) = self.cases[k]
         port = self.oracle.port
+        if band == 0 and not hd:
+            return exact_taps(self.oracle, self.xi[start:start + n], code, rem, step, shifts, n)
         if hd:
             codes = port.hd_resampler_avx(code.astype(np.float32), rem, step, rate, shifts, n).astype(np.float64)
         else:
-            codes, idx = port.resampler(1, code.astype(np.float32), rem, step, shifts, n, return_idx=True)
+            codes = port.resampler(1, code.astype(np.float32), rem, step, shifts, n)
         if band == 0:
-            x = self.xi[start:start + n]
-            return (codes.astype(np.int64) * x[None, :]).sum(axis=1) if hd else int_oracle(x, code, idx)
+            return (codes.astype(np.int64) * self.xi[start:start + n][None, :]).sum(axis=1)
         x = self.xf[start:start + n]
         if hd:
             xr = x.astype(np.complex128) * np.exp(1j * _hd_phase(n, rc, dp, dr))
@@ -146,7 +119,7 @@ class Rig:
         group, band, _, shifts, n = self.cases[k][:5]
         taps = len(shifts)
         got = out[k]
-        assert np.all(got[taps:] == SENTINEL), (label, group, "wrote past its taps")
+        assert np.all(got[taps:] == tr.SENTINEL), (label, group, "wrote past its taps")
         want = self.expected(k)
         if band == 0:
             assert np.array_equal(got[:taps, 0].astype(np.int64), want), (label, group, got[:taps, 0], want)
@@ -171,7 +144,7 @@ def test_every_per_item_path_at_every_tap_count(capi, torch, oracle, taps):
     """One engine per table size, so that the shared-memory table capacity (the longest code + 64) selects the path:
     with 1023-entry tables, every case but the modulo ones fits the extended table; with a 60 000-entry table (longer
     than the 50 944 entries shared memory holds) an epoch spanning 70 000 chips reads the table from global memory."""
-    near = _shifts(taps, 0.6)
+    near = tr.shifts(taps, 0.6)
     carrier = (1.1, 0.2 + 0.013 * taps, 0.0)
     small = Rig(capi, oracle, 100 + taps)
     code = int_code(1023, taps, nonzero=True)
@@ -184,16 +157,16 @@ def test_every_per_item_path_at_every_tap_count(capi, torch, oracle, taps):
     if taps > 1:
         far = [float(s) for s in np.linspace(-700.25, 500.5, taps).astype(np.float32)]
         small.add("modulo, smem, far taps", code, far, 6000, 7001, 3.3, 0.7, carrier=carrier)
-    small.add("high dynamics, smem", code, _shifts(taps, 0.5), 100000, 9000, 0.37, 0.04092, hd=True, rate=3e-12,
+    small.add("high dynamics, smem", code, tr.shifts(taps), 100000, 9000, 0.37, 0.04092, hd=True, rate=3e-12,
               carrier=(0.7, 1.1e-3, 2e-9))
     big = Rig(capi, oracle, 200 + taps)
     code_b = int_code(60000, taps, nonzero=True)
     big.add("modulo, gmem", code_b, near, 100000, 1000, 0.37, 0.7, carrier=carrier)
-    big.add("high dynamics, gmem", code_b, _shifts(taps, 0.5), 70001, 2001, 0.37, 0.7, hd=True, rate=1e-11,
+    big.add("high dynamics, gmem", code_b, tr.shifts(taps), 70001, 2001, 0.37, 0.7, hd=True, rate=1e-11,
             carrier=(0.7, -1.3e-3, -3e-9))
     for rig in (small, big):
-        out = _run(torch, rig.e, rig.item_array(), 8)
-        for k in range(len(rig.items)):
+        out = tr.run_dev(torch, rig.e, rig.items(), 8)
+        for k in range(len(rig.cases)):
             rig.check(out, k, "per-item paths")
         rig.close()
 
@@ -209,7 +182,6 @@ def test_single_correlator_six_and_seven_taps_integer_exact(capi, oracle, n, L, 
     x_int = rng.integers(-7, 8, n)
     x_int[x_int == 0] = 1
     code_int = int_code(L, 0, nonzero=True)
-    _, idx = oracle.port.resampler(1, code_int.astype(np.float32), rem, step, shifts, n, return_idx=True)
     e = capi.Engine(0)
     mc = capi.Multicorrelator(e, n, len(shifts))
     mc.set_high_dynamics_resampler(False)
@@ -217,7 +189,7 @@ def test_single_correlator_six_and_seven_taps_integer_exact(capi, oracle, n, L, 
     got = mc.Carrier_wipeoff_multicorrelator_resampler(x_int.astype(np.complex64), 0.0, 0.0, 0.0, rem, step, 0.0)
     mc.free()
     e.close()
-    assert np.array_equal(got.real.astype(np.int64), int_oracle(x_int, code_int, idx))
+    assert np.array_equal(got.real.astype(np.int64), exact_taps(oracle, x_int, code_int, rem, step, shifts, n))
     assert np.all(got.imag == 0)
 
 
@@ -228,13 +200,13 @@ def test_edge_lengths_at_every_tap_count(capi, torch, oracle, taps):
     16-tile re-seed groups, at both sample parities; an empty epoch gives zeros."""
     rig = Rig(capi, oracle, 300 + taps)
     code = int_code(1023, taps + 8, nonzero=True)
-    shifts = _shifts(taps, 0.5)
+    shifts = tr.shifts(taps)
     for n in EDGE_NS:
         for parity in (0, 1):
             rig.add(f"n={n} parity={parity}", code, shifts, n, 20000 + parity, 0.41 - 0.1 * parity, ST25 * 1.5,
                     carrier=(2.3, -0.31, 0.0))
-    out = _run(torch, rig.e, rig.item_array(), 8)
-    for k in range(len(rig.items)):
+    out = tr.run_dev(torch, rig.e, rig.items(), 8)
+    for k in range(len(rig.cases)):
         rig.check(out, k, "edge lengths")
     rig.close()
 
@@ -247,17 +219,17 @@ def test_slices_at_every_tap_count(capi, torch, oracle, taps):
     2e-5 of the one-slice result and of the truth, and three launches give the same bits."""
     rig = Rig(capi, oracle, 400 + taps)
     code = int_code(1023, taps + 16, nonzero=True)
-    shifts = _shifts(taps, 0.5)
+    shifts = tr.shifts(taps)
     rig.add("48 tiles", code, shifts, 25000, 1000, 0.2, ST25)
     rig.add("7 tiles", code, shifts, 7 * 512 + 5, 30000, 0.7, ST25 * 2)
     rig.add("odd start", code, shifts, 25001, 40001, -0.3, ST25)
     rig.add("ring wrap", code, shifts, 20000, WRAP_AT - 7001, 0.9, ST25)
     rig.add("modulo", code, shifts, 100000, 70000, 0.37, 0.0409)
     rig.add("high dynamics", code, shifts, 30001, 180000, 0.37, 0.04092, hd=True, rate=2e-12, carrier=(0.4, 2e-3, 1e-9))
-    items = rig.item_array()
+    items = rig.items()
     outs = {}
     for slices in SLICES:
-        reps = [_run(torch, rig.e, items, 8, slices) for _ in range(3)]
+        reps = [tr.run_dev(torch, rig.e, items, 8, slices) for _ in range(3)]
         assert np.array_equal(reps[0], reps[1]) and np.array_equal(reps[0], reps[2]), slices
         outs[slices] = reps[0]
         for k in range(len(items)):
@@ -281,18 +253,18 @@ def test_mixed_tap_counts_with_slices(capi, torch, oracle, slices):
     rig = Rig(capi, oracle, 500 + slices)
     for taps in (1, 2, 5, 8):
         code = int_code(1023 if taps != 5 else 2046, taps + 24, nonzero=True)
-        shifts = _shifts(taps, 0.6)
+        shifts = tr.shifts(taps, 0.6)
         rig.add(f"{taps} taps", code, shifts, 25000 + taps, 1000 * taps, 0.3, ST25)
         rig.add(f"{taps} taps, ring wrap", code, shifts, 9000 + taps, WRAP_AT - 3001, -1.3, ST25)
         rig.add(f"{taps} taps, empty", code, shifts, 0, 0, 0.0, ST25)
         rig.add(f"{taps} taps, high dynamics", code, shifts, 8111, 100000 + 9000 * taps, 0.37, 0.04092, hd=True,
                 rate=1e-10, carrier=(0.2, 1e-3, 1e-8))
     launches = rig.e.launch_count()
-    out = _run(torch, rig.e, rig.item_array(), 8, slices)
+    out = tr.run_dev(torch, rig.e, rig.items(), 8, slices)
     assert rig.e.launch_count() - launches == 4
-    out2 = _run(torch, rig.e, rig.item_array(), 8, slices)
+    out2 = tr.run_dev(torch, rig.e, rig.items(), 8, slices)
     assert np.array_equal(out, out2)
-    for k in range(len(rig.items)):
+    for k in range(len(rig.cases)):
         rig.check(out, k, "mixed tap counts")
     rig.close()
 
@@ -344,17 +316,15 @@ def test_long_epochs_against_float64(capi, torch, oracle, fs, taps):
             assert ratio <= 1e-4, (path, label, ratio)
 
     e = capi.Engine(0)
-    e.iq_create(0, n * len(cases))
-    first = e.iq_push(0, np.concatenate(segs))
-    items = np.zeros(len(cases), capi.TRK_ITEM_DTYPE)
+    first = tr.ring(e, 0, np.concatenate(segs))
+    rows = []
     for k in range(len(cases)):
-        cid = e.channel_create(0, taps)
-        e.channel_set_code(cid, code, shifts)
         rc, dphi, rcode, st = params[k]
-        items[k] = (cid, n, first + k * n, rc, dphi, 0.0, rcode, st, 0.0)
+        rows.append((tr.channel(e, 0, code, shifts), n, first + k * n, rc, dphi, 0.0, rcode, st))
+    items = tr.items(rows)
     for mode, path in ((0, "per-item kernel"), (1, "shared kernel")):
         e.trk_kernel_choice(mode)
-        out = _run(torch, e, items, 8)
+        out = tr.run_dev(torch, e, items, 8)
         for k in range(len(cases)):
             check(out[k, :taps, 0] + 1j * out[k, :taps, 1].astype(np.float64), k, path)
     mc = capi.Multicorrelator(e, n, taps)
@@ -375,7 +345,7 @@ def test_shared_kernel_paths_integer_exact(capi, torch, oracle, taps):
     the whole-epoch table through warp_tile (C/A at 4 Msps), the sliding code window (8184-entry table), groups whose
     epochs lie too far apart to share (each warp streams its own tiles) and the off-table fallback (rem = 2e6)."""
     rng = np.random.default_rng(600 + taps)
-    shifts = _shifts(taps, 0.6)
+    shifts = tr.shifts(taps, 0.6)
     blocks = [   # (path, L, n, step, rem base, spacing of the 8 starts)
         ("chunk", 1023, 25000, ST25, 0.0, 37),
         ("chunk", 1023, 25001, ST25, 0.0, 53),
@@ -388,24 +358,20 @@ def test_shared_kernel_paths_integer_exact(capi, torch, oracle, taps):
     x = rng.integers(-7, 8, total)
     e = capi.Engine(0)
     e.trk_kernel_choice(1)
-    e.iq_create(0, total)
-    first = e.iq_push(0, x.astype(np.complex64))
-    items, want = [], []
+    first = tr.ring(e, 0, x.astype(np.complex64))
+    rows, want = [], []
     pos = 1
     for b, (path, L, n, step, rem0, sp) in enumerate(blocks):
         for j in range(8):
             code = int_code(L, 8 * b + j, nonzero=True)
-            cid = e.channel_create(0, taps)
-            e.channel_set_code(cid, code.astype(np.float32), shifts)
+            cid = tr.channel(e, 0, code, shifts)
             s0 = pos + j * sp
             rem = float(np.float32(rem0 + float(rng.uniform(-3, 3)) if rem0 == 0.0 else rem0 + 0.25 * j))
-            items.append((cid, n, first + s0, 0.0, 0.0, 0.0, rem, step, 0.0))
-            _, idx = oracle.port.resampler(1, code.astype(np.float32), rem, step, shifts, n, return_idx=True)
-            want.append((path, int_oracle(x[s0:s0 + n], code, idx)))
+            rows.append((cid, n, first + s0, 0.0, 0.0, 0.0, rem, step))
+            want.append((path, exact_taps(oracle, x[s0:s0 + n], code, rem, step, shifts, n)))
         pos += 7 * sp + n + 2
-    items = np.array(items, dtype=capi.TRK_ITEM_DTYPE)
     launches = e.launch_count()
-    out = _run(torch, e, items, taps)
+    out = tr.run_dev(torch, e, tr.items(rows), taps)
     assert e.launch_count() - launches == 1
     e.close()
     for i, (path, w) in enumerate(want):
@@ -433,20 +399,17 @@ def test_shared_kernel_linear_band_to_its_last_sample(capi, torch, oracle, total
         ("whole table", 0.25575, [4001, 4000] * 4, 17),
         ("no share", 0.1705, [4003, 4096] * 4, 7001),
     ]
-    items, want = [], []
+    rows, want = [], []
     for g, (path, step, ns, gap) in enumerate(groups):
         for j in range(8):
             n = ns[j]
             s0 = total - n - gap * max(6 - j, 0)   # items 6 and 7 end at the band's last sample
             code = int_code(1023, 8 * g + j, nonzero=True)
-            cid = e.channel_create(0, 3)
-            e.channel_set_code(cid, code.astype(np.float32), shifts)
+            cid = tr.channel(e, 0, code, shifts)
             rem = float(np.float32(rng.uniform(-3, 3)))
-            items.append((cid, n, s0, 0.0, 0.0, 0.0, rem, step, 0.0))
-            _, idx = oracle.port.resampler(1, code.astype(np.float32), rem, step, shifts, n, return_idx=True)
-            want.append((path, n, int_oracle(x[s0:s0 + n], code, idx)))
-    items = np.array(items, dtype=capi.TRK_ITEM_DTYPE)
-    out = _run(torch, e, items, 3)
+            rows.append((cid, n, s0, 0.0, 0.0, 0.0, rem, step))
+            want.append((path, n, exact_taps(oracle, x[s0:s0 + n], code, rem, step, shifts, n)))
+    out = tr.run_dev(torch, e, tr.items(rows), 3)
     e.close()
     for i, (path, n, w) in enumerate(want):
         assert np.array_equal(out[i, :, 0].astype(np.int64), w), (path, n, i)

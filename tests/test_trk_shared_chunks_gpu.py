@@ -11,7 +11,8 @@ from gnss_sdr_b200.build import LIB, build_variant  # noqa: E402
 from gnss_synth import make_iq, trk_params_for  # noqa: E402
 from gpu_fixtures import capi  # noqa: E402,F401
 from ring_worker import run_worker  # noqa: E402
-from trk_ref import int_oracle, ref_or_port_avx  # noqa: E402
+import trk_rig as tr  # noqa: E402
+from trk_ref import chip_indices, exact_taps, ref_or_port_avx  # noqa: E402
 
 SHIFTS = [-0.5, 0.0, 0.5]
 CA_16368 = 1023.0 / 16368
@@ -26,21 +27,14 @@ def run_shared(capi, x_int, chans, epochs, filler=0, capacity=None):
     e = capi.Engine(0)
     try:
         e.trk_kernel_choice(1)
-        e.iq_create(0, capacity or len(x_int))
-        if filler:
-            e.iq_push(0, np.ones(filler, np.complex64))
-        first = e.iq_push(0, x_int.astype(np.complex64))
-        cids = []
-        for code, *_ in chans:
-            cid = e.channel_create(0, len(SHIFTS))
-            e.channel_set_code(cid, code.astype(np.float32), SHIFTS)
-            cids.append(cid)
+        first = tr.ring(e, 0, x_int.astype(np.complex64), capacity, np.ones(filler, np.complex64) if filler else None)
+        cids = [tr.channel(e, 0, code, SHIFTS) for code, *_ in chans]
         keys, rows = [], []
         for c, (code, rem, step, n, start) in enumerate(chans):
             for k in range(epochs):
                 keys.append((c, k))
-                rows.append((cids[c], n, first + start + k * n, 0.0, 0.0, 0.0, rem, step, 0.0))
-        items = np.array(rows, dtype=capi.TRK_ITEM_DTYPE)
+                rows.append((cids[c], n, first + start + k * n, 0.0, 0.0, 0.0, rem, step))
+        items = tr.items(rows)
         order = np.argsort(items["sample_index"], kind="stable")
         got = e.trk_batch(items[order], len(SHIFTS))
     finally:
@@ -50,15 +44,15 @@ def run_shared(capi, x_int, chans, epochs, filler=0, capacity=None):
 
 def check_exact(oracle, x_int, chans, epochs, got):
     for c, (code, rem, step, n, start) in enumerate(chans):
-        _, idx = oracle.port.resampler(1, code.astype(np.float32), float(np.float32(rem)), step, SHIFTS, n, return_idx=True)
         for k in range(epochs):
             s0 = start + k * n
-            want = int_oracle(x_int[s0:s0 + n], code, idx)
+            want = exact_taps(oracle, x_int[s0:s0 + n], code, float(np.float32(rem)), step, SHIFTS, n)
             assert np.array_equal(got[(c, k)].real.astype(np.int64), want), (c, k, step, n, rem)
             assert np.all(got[(c, k)].imag == 0), (c, k)
 
 
-def int_code(rng, L=1023):
+def random_code(rng, L=1023):
+    """a table of L integers drawn uniformly from [-15, 15]"""
     return rng.integers(-15, 16, L)
 
 
@@ -68,12 +62,11 @@ def test_chip_boundary_at_every_chunk_position(capi, oracle):
     rng = np.random.default_rng(11)
     n, step, epochs = 25000, CA_25, 2
     x = rng.integers(-7, 8, n * epochs + 1024)
-    chans = [(int_code(rng), float(np.float32(-(j + 0.5) * step)), step, n, 0) for j in range(16)]
+    chans = [(random_code(rng), float(np.float32(-(j + 0.5) * step)), step, n, 0) for j in range(16)]
     # the rises of the prompt tap inside 16-sample chunks cover every position
     pos = set()
     for code, rem, *_ in chans:
-        _, idx = oracle.port.resampler(1, code.astype(np.float32), rem, step, SHIFTS, n, return_idx=True)
-        d = np.flatnonzero(np.diff(idx[1])) + 1
+        d = np.flatnonzero(np.diff(chip_indices(oracle, code, rem, step, SHIFTS, n)[1])) + 1
         pos |= set((d % 16).tolist())
     assert pos == set(range(16))
     check_exact(oracle, x, chans, epochs, run_shared(capi, x, chans, epochs))
@@ -96,7 +89,7 @@ def test_staggered_groups_integer_exact(capi, oracle, step, n):
     starts = np.sort(rng.integers(0, n, n_ch))
     starts[1] |= 1
     x = rng.integers(-7, 8, n * (epochs + 1) + 1024)
-    chans = [(int_code(rng), float(rng.uniform(-3, 3)), step, n, int(starts[c])) for c in range(n_ch)]
+    chans = [(random_code(rng), float(rng.uniform(-3, 3)), step, n, int(starts[c])) for c in range(n_ch)]
     check_exact(oracle, x, chans, epochs, run_shared(capi, x, chans, epochs))
 
 
@@ -107,7 +100,7 @@ def test_one_cta_holds_items_on_both_paths(capi, oracle):
     n, epochs, n_ch = 6000, 3, 12
     starts = np.sort(rng.integers(0, 700, n_ch))
     x = rng.integers(-7, 8, n * (epochs + 1) + 1024)
-    chans = [(int_code(rng), float(rng.uniform(-2, 2)), CA_25 if c % 2 else 0.1705, n, int(starts[c])) for c in range(n_ch)]
+    chans = [(random_code(rng), float(rng.uniform(-2, 2)), CA_25 if c % 2 else 0.1705, n, int(starts[c])) for c in range(n_ch)]
     check_exact(oracle, x, chans, epochs, run_shared(capi, x, chans, epochs))
 
 
@@ -120,7 +113,7 @@ def test_ring_band_wraps_inside_a_tile(capi, oracle):
     x = rng.integers(-7, 8, n * epochs + 3000)
     starts = np.sort(rng.integers(0, 2000, n_ch))
     assert (cap - filler - (int(starts[0]) & ~1)) % 16 != 0     # not on a chunk boundary of the first group's tiles
-    chans = [(int_code(rng), float(rng.uniform(-2, 2)), CA_25, n, int(starts[c])) for c in range(n_ch)]
+    chans = [(random_code(rng), float(rng.uniform(-2, 2)), CA_25, n, int(starts[c])) for c in range(n_ch)]
     check_exact(oracle, x, chans, epochs, run_shared(capi, x, chans, epochs, filler=filler, capacity=cap))
 
 
@@ -135,22 +128,14 @@ def test_float_signal_full_epochs_within_bounds(capi, oracle):
     iq = make_iq(codes, fs, n * nep + 64, svs, seed=21)
     e = capi.Engine(0)
     e.trk_kernel_choice(1)
-    e.iq_create(0, len(iq))
-    first = e.iq_push(0, iq)
-    items = np.zeros(nch * nep, capi.TRK_ITEM_DTYPE)
+    first = tr.ring(e, 0, iq)
+    rows = [None] * (nch * nep)
     for c, sv in enumerate(svs):
-        cid = e.channel_create(0, 3)
-        e.channel_set_code(cid, codes[sv["prn"]], SHIFTS)
+        cid = tr.channel(e, 0, codes[sv["prn"]], SHIFTS)
         s, rc, dp, rcode, st = trk_params_for(sv, fs, n, nep)
         for k in range(nep):
-            it = items[k * nch + c]
-            it["channel"] = cid
-            it["n"] = n
-            it["sample_index"] = first + int(s[k])
-            it["rem_carrier_phase_rad"] = rc[k]
-            it["phase_step_rad"] = dp[k]
-            it["rem_code_phase_chips"] = rcode[k]
-            it["code_phase_step_chips"] = st[k]
+            rows[k * nch + c] = (cid, n, first + int(s[k]), rc[k], dp[k], 0.0, rcode[k], st[k])
+    items = tr.items(rows)
     order = np.argsort(items["sample_index"], kind="stable")
     got = np.empty((len(items), 3), np.complex64)
     got[order] = e.trk_batch(items[order], 3)

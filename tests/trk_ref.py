@@ -9,6 +9,16 @@ def int_oracle(x_int, code_int, idx):
     return np.array([np.sum(x_int * code_int[idx[t]]) for t in range(idx.shape[0])], dtype=np.int64)
 
 
+def chip_indices(oracle, code, rem, step, shifts, n):
+    """the reference's chip index of every tap and sample (taps x n): its resampler with the a_avx association"""
+    return oracle.port.resampler(1, np.asarray(code, np.float32), rem, step, shifts, n, return_idx=True)[1]
+
+
+def exact_taps(oracle, x_int, code_int, rem, step, shifts, n):
+    """exact integer taps of the n samples x_int against the small-integer table code_int, at the reference's indices"""
+    return int_oracle(x_int, code_int, chip_indices(oracle, code_int, rem, step, shifts, n))
+
+
 def int_code(L, salt=0, nonzero=False):
     """((k * (7919 + 2 salt)) mod 31) - 15 for k < L, values in [-15, 15]; nonzero: its zeros replaced by 16"""
     c = ((np.arange(L) * (7919 + 2 * salt)) % 31) - 15
