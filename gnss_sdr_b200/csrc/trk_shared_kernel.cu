@@ -58,6 +58,8 @@ constexpr int kShTblCap = 1152;  // floats of warp-private code storage: whole-e
 constexpr int kShWin = 256;      // ... else two 256-entry windows (double-buffered, refilled per tile with cp.async)
 constexpr int kShThreads = (kShK + 1) * 32;
 constexpr int kShReseed = 64;    // 64-sample steps between exact phasor re-seeds (4096 samples)
+constexpr int kShReseedTiles = kShReseed / (kShTile / 64);  // ... that is, tiles
+static_assert((kShReseedTiles & (kShReseedTiles - 1)) == 0, "the chunk path tests the re-seed tile with a mask");
 // Tiles sit in shared memory as 8 runs of 64 samples (4 chunks of 16), each run followed by 16 bytes of padding: 528-byte
 // run stride, one bulk copy per run.  On the chunk path lane l owns chunk 4 (l % 8) + l / 8, so the 8 lanes of a quarter
 // warp read 8 different runs, whose starts fall on 8 distinct 16-byte bank groups: LDS.128 without conflicts.
@@ -113,6 +115,22 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned int 
         "r"(parity), "r"(0x989680u)  // suspend-time hint: the warp sleeps in hardware instead of spinning
         : "memory");
 }
+// Where tile t sits in the ring: slot t % kShStages, whose barriers are in phase (t / kShStages) & 1.  The chunk path
+// carries it from tile to tile (next) instead of recomputing it.
+struct RingPos
+{
+    int s;
+    unsigned int par;
+    static __device__ __forceinline__ RingPos of(int t) { return {t % kShStages, static_cast<unsigned int>((t / kShStages) & 1)}; }
+    __device__ __forceinline__ void next()
+    {
+        if (++s == kShStages)
+            {
+                s = 0;
+                par ^= 1u;
+            }
+    }
+};
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, unsigned int bytes, unsigned long long* bar)
 {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
@@ -225,14 +243,22 @@ __device__ __forceinline__ float2 select16(const float2 (&R)[kShChunk], int m)
 // m comes from an estimate that the exact index formula a(n) = fl(fl(step n) + aux), i(n) = floor(a(n)), then decides
 // (item set-up: the bound there keeps the estimate within one sample).  From the chunk's first valid sample lo, the
 // index rises at b = lo + j, j >= 1 the first with a(b) >= i0 + 1; with e = (i0 + 1) - a(lo) in (0, 1] that is near
-// lo + e / step, and c = fl(fl(e) inv_step + 1/2) puts b in {lo + k, lo + k + 1}, k = floor(c) (c clamped to 16.5: m is
-// 15 for any b >= lo + 16).  One evaluation of i(lo + k) picks the one: m = b - 1.  The formula is non-decreasing in n
-// for step > 0, and it alone decides, so no sample's index is estimated.
+// lo + e / step, and c = fl(fl(e) inv_step + 1/2) puts b in {lo + k, lo + k + 1}, k = floor(c).  One evaluation of
+// i(lo + k) picks the one: m = b - 1.  c is clamped to 15.5: for b >= lo + 16 that gives k = 15 and i(lo + 15) = i0, so
+// m = 15; for b <= lo + 15, c < 16 and k keeps its value.  So k <= 15, and m = k - [i(lo + k) > i0] lies in [0, 15]
+// (k = 0 only when b = lo + 1).  The formula is non-decreasing in n for step > 0, and it alone decides, so no sample's
+// index is estimated.
 // MASKED as in warp_tile: lo is the first sample of the chunk inside the epoch; masked samples add zero to R, so every m
 // past the epoch's last sample selects the same sum.  Accumulates into acc_re / acc_im.
+// unpaired = 0 (warp-uniform, the item set-up) when the first and the last of three taps are a whole number of chips
+// apart, so that in almost every chunk both rise at the same sample; 1 otherwise.  When every lane of the warp finds the
+// same m for the two, the last tap takes the first tap's R_m instead of running its own select tree: the same value, so
+// nothing in the arithmetic changes.  Each tap still decides its own m and reads its own c[i0], c[i0 + 1] at its own i0
+// (fl(y + 1) and fl(y) + 1 may floor differently).
 template <int TAPS, bool MASKED>
 __device__ __forceinline__ void warp_tile_chunks(const float4* x4, const float4* rot4, float n0f, float vlo, float vhi,
-    float step, float inv_step, const float2 (&aux2)[TAPS], unsigned int tbl_off, float2 z0, float2 (&acc_re)[TAPS], float2 (&acc_im)[TAPS])
+    float step, float inv_step, const float2 (&aux2)[TAPS], unsigned int tbl_off, int unpaired, float2 z0, float2 (&acc_re)[TAPS],
+    float2 (&acc_im)[TAPS])
 {
     float2 R[kShChunk];
     float2 r = make_float2(0.f, 0.f);
@@ -268,23 +294,32 @@ __device__ __forceinline__ void warp_tile_chunks(const float4* x4, const float4*
             const float g = __fadd_rn(__fmul_rn(step, lo), a);
             t0[t] = __fadd_rd(g, kFloorMagic);                                      // kFloorMagic + i0
             const float e = __fsub_rn(__fsub_rn(t0[t], kFloorMagic - 1.0f), g);    // (i0 + 1) - a(lo)
-            const float c = fminf(__fmaf_rn(e, inv_step, 0.5f), 16.5f);
+            const float c = fminf(__fmaf_rn(e, inv_step, 0.5f), 15.5f);
             const float tk = __fadd_rd(c, kFloorMagic);                             // kFloorMagic + k
             const float tb = __fadd_rd(__fadd_rn(__fmul_rn(step, __fadd_rn(tk, lo_m)), a), kFloorMagic);
             const int k = __float_as_int(tk) - __float_as_int(kFloorMagic);
             const int mt = lo_off + k - (tb != t0[t] ? 1 : 0);
-            m[t] = MASKED ? min(max(mt, 0), kShChunk - 1) : min(mt, kShChunk - 1);
+            m[t] = MASKED ? min(max(mt, 0), kShChunk - 1) : mt;
         }
+    // tap t's share of the chunk, P = R_m
+    auto add_tap = [&](int t, float2 P) {
+        const unsigned int addr = (__float_as_uint(t0[t]) << 2) + tbl_off;
+        const float c0 = lds_f32(addr), c1 = lds_f32(addr + 4u);
+        const float dc = c0 - c1;
+        const float vr = fmaf(dc, P.x, c1 * r.x), vi = fmaf(dc, P.y, c1 * r.y);
+        acc_re[t].x = fmaf(z0.x, vr, fmaf(-z0.y, vi, acc_re[t].x));
+        acc_im[t].x = fmaf(z0.x, vi, fmaf(z0.y, vr, acc_im[t].x));
+    };
+    const float2 P0 = select16(R, m[0]);
+    add_tap(0, P0);
 #pragma unroll
-    for (int t = 0; t < TAPS; t++)
+    for (int t = 1; t < (TAPS == 3 ? TAPS - 1 : TAPS); t++) add_tap(t, select16(R, m[t]));
+    if (TAPS == 3)
         {
-            const float2 P = select16(R, m[t]);
-            const unsigned int addr = (__float_as_uint(t0[t]) << 2) + tbl_off;
-            const float c0 = lds_f32(addr), c1 = lds_f32(addr + 4u);
-            const float dc = c0 - c1;
-            const float vr = fmaf(dc, P.x, c1 * r.x), vi = fmaf(dc, P.y, c1 * r.y);
-            acc_re[t].x = fmaf(z0.x, vr, fmaf(-z0.y, vi, acc_re[t].x));
-            acc_im[t].x = fmaf(z0.x, vi, fmaf(z0.y, vr, acc_im[t].x));
+            if (__all_sync(0xffffffffu, ((m[TAPS - 1] ^ m[0]) | unpaired) == 0))
+                add_tap(TAPS - 1, P0);
+            else
+                add_tap(TAPS - 1, select16(R, m[TAPS - 1]));
         }
 }
 
@@ -314,7 +349,7 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
             for (int s = 0; s < kShStages; s++)
                 {
                     mbar_init(&sm.full[s], 1);
-                    mbar_init(&sm.empty[s], kShK);
+                    mbar_init(&sm.empty[s], kShK * 32);  // every consumer lane releases the slot
                 }
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         }
@@ -408,6 +443,7 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
     for (int t = 0; t < TAPS; t++) acc[t] = make_float2(0.f, 0.f);
 
     bool table_path = false, whole_table = false, chunked = false;
+    int unpaired = 1;
     float2 z0 = make_float2(0.f, 0.f), E = z0;  // chunk path: phasor of the lane's chunk start, its advance per tile
     unsigned long long my_hull = 0;
     int body = 0, a_i = 0, t_first = 0, t_last = 0;
@@ -442,6 +478,9 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
                     smin = fminf(smin, sh);
                     smax = fmaxf(smax, sh);
                 }
+            // chunk path, three taps: the first and the last may share their running-sum pick (warp_tile_chunks)
+            const float spread = ch->shifts[TAPS - 1] - ch->shifts[0];
+            unpaired = (spread != 0.f && spread == rintf(spread)) ? 0 : 1;
             // The code replica is staged per TILE: a tile spans 512*step chips (+ the tap spread), so a
             // 256-entry window per warp serves any code length (1023-chip C/A, 8184-value E1, 10230-chip L5).
             const float span_bound = ceilf(fabsf(step) * static_cast<float>(kShTile)) + ceilf(smax - smin) + 6.0f;
@@ -577,7 +616,7 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
             warp_tile<TAPS, false>(load, vlo, vhi, step, aux2, tbl_off, Dr2, Di2, fa, fb, zr, zi, are, aim);
         else
             warp_tile<TAPS, true>(load, vlo, vhi, step, aux2, tbl_off, Dr2, Di2, fa, fb, zr, zi, are, aim);
-        if (++tiles_in_group == kShReseed / 8)
+        if (++tiles_in_group == kShReseedTiles)
             {
                 // re-seed: the group seed advances by the rounded G = exp(j DT 64*kShReseed) and replaces the
                 // running phasor (bounds the drift of the 64 recurrence steps in between; the seed itself is not
@@ -593,7 +632,21 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
 
     // Walks the group's tiles through the ring, calling work(t, slot) on the tiles of this warp's epoch.  Every consumer
     // waits for every tile, also the ones it skips: a warp that ran ahead could otherwise arrive twice on empty[s] within
-    // one phase and let the producer overwrite a slot that a slower warp is still reading.
+    // one phase and let the producer overwrite a slot that a slower warp is still reading.  Every lane arrives on empty[s]
+    // when it is done with the slot, so no lane has to wait for the others before the slot is released.
+    auto ring_wait = [&](int t, const RingPos& rp) {
+        mbar_wait(&sm.full[rp.s], rp.par);
+#if SH_STRESS
+        stress_delay(static_cast<unsigned int>(t) * 17u + static_cast<unsigned int>(warp) * 101u + blockIdx.x * 13u);
+#endif
+    };
+    auto ring_release = [&](int t, const RingPos& rp) {
+#if SH_STRESS
+        stress_delay(static_cast<unsigned int>(t) * 29u + static_cast<unsigned int>(warp) * 53u + blockIdx.x * 5u + 1u);
+        __syncwarp();
+#endif
+        mbar_arrive(&sm.empty[rp.s]);
+    };
     auto for_each_ring_tile = [&](const auto& work) {
         for (int t = 0; t < n_tiles; t++)
             {
@@ -608,35 +661,86 @@ __global__ void __launch_bounds__(kShThreads, kShMinBlocks) trk_shared_kernel(co
                 stress_delay(static_cast<unsigned int>(t) * 29u + static_cast<unsigned int>(warp) * 53u + blockIdx.x * 5u + 1u);
                 __syncwarp();
 #endif
-                if (lane == 0) mbar_arrive(&sm.empty[s]);
+                mbar_arrive(&sm.empty[s]);
             }
     };
     // The two paths walk the ring in separate loops, so that none of warp_tile's lane state is live on the chunk path.
     if (chunked)
         {
             const float inv_step = __frcp_rn(step);  // for the boundary estimate (bound at the chunked test)
-            for_each_ring_tile([&](int t, int s) {
-                const int n_tile0 = t * kShTile - a_i;
-                const float n0f = static_cast<float>(n_tile0 + kShChunk * lane_chunk(lane));
-                const float vlo = static_cast<float>(max(n_tile0, 0)), vhi = static_cast<float>(min(n_tile0 + kShTile, body) - 1);
-                const float4* x4 = reinterpret_cast<const float4*>(&sm.tiles[s][(lane & 7) * kShRunStride + (lane >> 3) * kShChunk]);
-                const float4* rot4 = reinterpret_cast<const float4*>(&sm.rot[warp][0]);
-                if (n_tile0 >= 0 && n_tile0 + kShTile <= body)
-                    warp_tile_chunks<TAPS, false>(x4, rot4, n0f, vlo, vhi, step, inv_step, aux2, tbl_off, z0, are, aim);
+            const float4* rot4 = reinterpret_cast<const float4*>(&sm.rot[warp][0]);
+            // the lane's chunk in ring slot 0; slot s lies s * kShTileSlot samples further
+            const float4* x4_0 = reinterpret_cast<const float4*>(&sm.tiles[0][(lane & 7) * kShRunStride + (lane >> 3) * kShChunk]);
+            // one tile of the epoch in ring slot s: its first sample is epoch index n_tile0, the lane's chunk n0f; interior =
+            // the whole tile lies in the epoch; reseed = z0 is re-seeded after it (every kShReseedTiles-th tile of the epoch)
+            auto chunk_tile = [&](const float4* x4, int n_tile0, float n0f, bool interior, bool reseed) {
+                if (interior)
+                    {
+                        warp_tile_chunks<TAPS, false>(x4, rot4, n0f, 0.f, 0.f, step, inv_step, aux2, tbl_off, unpaired, z0, are, aim);
+                    }
                 else
-                    warp_tile_chunks<TAPS, true>(x4, rot4, n0f, vlo, vhi, step, inv_step, aux2, tbl_off, z0, are, aim);
-                if ((t - t_first + 1) % (kShReseed / 8) == 0)
+                    {
+                        const float vlo = static_cast<float>(max(n_tile0, 0)), vhi = static_cast<float>(min(n_tile0 + kShTile, body) - 1);
+                        warp_tile_chunks<TAPS, true>(x4, rot4, n0f, vlo, vhi, step, inv_step, aux2, tbl_off, unpaired, z0, are, aim);
+                    }
+                if (reseed)
                     {
                         // exact re-seed from the 64-bit phase of the lane's next chunk start, every 4096 samples
-                        const long long n_next = static_cast<long long>(t + 1) * kShTile + kShChunk * lane_chunk(lane) - a_i;
+                        const long long n_next = n_tile0 + kShTile + kShChunk * lane_chunk(lane);
                         z0 = phasor_from_turns(sm.item_turns[warp][0] + sm.item_turns[warp][1] * static_cast<unsigned long long>(n_next));
                     }
                 else
                     {
                         z0 = cmulf(z0, E);
                     }
-                __syncwarp();
-            });
+            };
+            if constexpr (TAPS == 5)
+                {
+                    // Five taps walk the ring as the other paths do, deriving everything from t: with the carried walk
+                    // below, ptxas spilled more in <5>'s set-up and epilogue (38 / 116 B against 22 / 76 B).
+                    for_each_ring_tile([&](int t, int s) {
+                        const int n_tile0 = t * kShTile - a_i;
+                        chunk_tile(x4_0 + s * (kShTileSlot / 2), n_tile0, static_cast<float>(n_tile0 + kShChunk * lane_chunk(lane)), n_tile0 >= 0 && n_tile0 + kShTile <= body,
+                            (t - t_first + 1) % kShReseedTiles == 0);
+                    });
+                }
+            else
+                {
+                    // Tile t of the epoch, t_first <= t < t_last, starts at epoch index n_tile0 = t kShTile - a_i (the last
+                    // one holds sample body - 1).  The loop runs on n_tile0 and carries n0f (exact in float: the chunked
+                    // test keeps body below 2^22) and the ring position.
+                    const int n_first = t_first * kShTile - a_i;
+                    float n0f = static_cast<float>(n_first + kShChunk * lane_chunk(lane));
+                    // the whole tile lies in the epoch when 0 <= n_tile0 <= body - kShTile
+                    const unsigned int n_interior = static_cast<unsigned int>(max(body - kShTile + 1, 0));
+                    // n_tile0 - n_first is a multiple of kShTile, so the bits of n_tile0 just above kShTile's say when to
+                    // re-seed
+                    const int reseed_at = n_first + (kShReseedTiles - 1) * kShTile;
+                    // (chunked implies a shared window, so t_last <= n_tiles)
+#pragma unroll 1
+                    for (int t = 0; t < t_first; t++)
+                        {
+                            ring_wait(t, RingPos::of(t));
+                            ring_release(t, RingPos::of(t));
+                        }
+                    RingPos ring = RingPos::of(t_first);
+                    for (int n_tile0 = n_first; n_tile0 < body; n_tile0 += kShTile)
+                        {
+                            const int t = (n_tile0 + a_i) / kShTile;  // the stress builds' delays only
+                            ring_wait(t, ring);
+                            chunk_tile(x4_0 + ring.s * (kShTileSlot / 2), n_tile0, n0f, static_cast<unsigned int>(n_tile0) < n_interior,
+                                ((n_tile0 ^ reseed_at) & ((kShReseedTiles - 1) * kShTile)) == 0);
+                            ring_release(t, ring);
+                            ring.next();
+                            n0f += static_cast<float>(kShTile);
+                        }
+#pragma unroll 1
+                    for (int t = t_last; t < n_tiles; t++)
+                        {
+                            ring_wait(t, RingPos::of(t));
+                            ring_release(t, RingPos::of(t));
+                        }
+                }
         }
     else
         {
