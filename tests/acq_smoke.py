@@ -1,29 +1,22 @@
 """One small acquisition on cuda:0 checked against the numpy oracle (used by __graft_entry__.smoke)."""
-import numpy as np
 
 
 def run(eng):
     import gnss_sdr_b200.capi as capi
     import oracle
-    from oracle.acq_np import AcqConf, PcpsAcquisitionOracle
+    import acq_rig as ar
     from gnss_synth import make_iq
     fs, prn = 4e6, 1
     code = oracle.port.gps_ca_code(prn)
     sv = dict(prn=prn, doppler=1680.0, code_phase_chips=(-524 / (fs / 1.023e6)) % 1023, cn0=47.0, phase0=0.4)
     iq = make_iq({prn: code}, fs, 4000, [sv], seed=1)
-    conf = AcqConf(fs_in=int(fs), samples_per_ms=4000.0, samples_per_code=4000.0, samples_per_chip=3, doppler_max=5000,
-                   doppler_step=250, pfa=0.001)
-    o = PcpsAcquisitionOracle(conf)
-    sampled = oracle.port.gps_ca_code_complex_sampled(prn, int(fs))
-    o.set_local_code(sampled)
-    want = o.acquisition_core(iq)
-    acq = capi.PcpsAcquisition(eng, fs_in=int(fs), samples_per_ms=4000.0, samples_per_chip=3, doppler_max=5000,
-                               doppler_step=250)
+    p = ar.params(fs, doppler_max=5000, doppler_step=250)
+    sampled = ar.ca_code(oracle.port, prn, fs)
+    want = ar.oracle(p, sampled, pfa=0.001).acquisition_core(iq)
+    acq = capi.PcpsAcquisition(eng, **p)
     acq.set_local_code(0, sampled)
     got = acq.search(iq, [0])[0]
     acq.close()
-    assert (int(got["index_time"]), int(got["index_doppler"])) == (want["index_time"], want["index_doppler"]), (got, want)
-    rel = abs(got["test_statistics"] - want["test_statistics"]) / want["test_statistics"]
-    assert rel < 1e-4, rel
+    ar.check(got, want, ("test_statistics",))
     print(f"smoke: acq PRN {prn}: delay {got['index_time']} samples, doppler {got['doppler']} Hz, "
           f"stat {got['test_statistics']:.2f} (oracle {want['test_statistics']:.2f})")

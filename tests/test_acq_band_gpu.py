@@ -14,41 +14,11 @@ import pytest
 
 import gnss_synth as gs
 from gpu_fixtures import capi, engine  # noqa: F401
+import acq_rig as ar
 
 pytestmark = pytest.mark.gpu
 
-ERR_ARG, ERR_STATE, ERR_RANGE = -1, -4, -5
-
-
-def _pow2(n):
-    return 1 << (int(n) - 1).bit_length()
-
-
-def _make(capi, engine, spms, *, cfar=True, keep_grid=False, dwells=1, bits=False, ms_per_code=1, sampled_ms=1, slots=2):
-    fs = int(round(spms * 1000))
-    return capi.PcpsAcquisition(engine, fs_in=fs, samples_per_ms=float(spms), samples_per_chip=max(1, int(fs / 1.023e6)),
-                                doppler_max=1000, doppler_step=500, use_CFAR_algorithm_flag=cfar, keep_grid=keep_grid,
-                                max_dwells=dwells, n_code_slots=slots, bit_transition_flag=bits, sampled_ms=sampled_ms,
-                                ms_per_code=ms_per_code)
-
-
-def _pair(capi, engine, rng, spms, **kw):
-    """two acquisition objects with the same configuration and codes: one searched from the host, one from the band"""
-    host, band = _make(capi, engine, spms, **kw), _make(capi, engine, spms, **kw)
-    c = host.conf
-    need = c.fft_size // 2 if c.code_layout == 1 else c.consumed_samples
-    codes = [rng.choice([-1.0, 1.0], need).astype(np.complex64) for _ in range(c.n_code_slots)]
-    for a in (host, band):
-        for s, code in enumerate(codes):
-            a.set_local_code(s, code)
-    return host, band, codes
-
-
-def _stream(rng, n, code, fs):
-    """noise with one code-modulated carrier in it (a clear peak for the statistics)"""
-    t = np.arange(n)
-    x = np.resize(np.roll(code, int(rng.integers(0, code.size))), n) * np.exp(2j * np.pi * rng.uniform(-900, 900) / fs * t)
-    return (0.5 * x + rng.normal(0, 1.0, n) + 1j * rng.normal(0, 1.0, n)).astype(np.complex64)
+PEAKS, BITS = dict(use_CFAR_algorithm_flag=False), dict(bit_transition_flag=True)
 
 
 def _push_chunks(engine, band, x, chunk):
@@ -56,32 +26,25 @@ def _push_chunks(engine, band, x, chunk):
         engine.iq_push(band, x[k:k + chunk])
 
 
-def _grids(acq):
-    c = acq.conf
-    if not (c.keep_grid or c.max_dwells > 1):
-        return b""
-    return b"".join(acq.read_grid(s).tobytes() for s in range(c.n_code_slots))
-
-
 # (id, samples per ms, options): every plan family, with the search options each supports
 CASES = [
     ("single4000_cfar", 4000, dict()),
-    ("single4000_peaks", 4000, dict(cfar=False)),
-    ("single4000_grid_dwells", 4000, dict(keep_grid=True, dwells=2)),
-    ("single4000_bits", 4000, dict(bits=True)),
+    ("single4000_peaks", 4000, PEAKS),
+    ("single4000_grid_dwells", 4000, dict(keep_grid=True, max_dwells=2)),
+    ("single4000_bits", 4000, BITS),
     ("single4000_zero_padded", 4000, dict(ms_per_code=2)),
     ("single25000_cfar", 25000, dict()),
-    ("single25000_peaks_grid", 25000, dict(cfar=False, keep_grid=True)),
-    ("two50000_cfar_dwells", 50000, dict(dwells=2)),
-    ("two50000_peaks", 50000, dict(cfar=False)),
-    ("two50000_bits", 25000, dict(bits=True, cfar=False)),
+    ("single25000_peaks_grid", 25000, dict(PEAKS, keep_grid=True)),
+    ("two50000_cfar_dwells", 50000, dict(max_dwells=2)),
+    ("two50000_peaks", 50000, PEAKS),
+    ("two50000_bits", 25000, dict(BITS, **PEAKS)),
     ("two50000_zero_padded", 25000, dict(ms_per_code=2)),
     ("two200000_cfar", 50000, dict(sampled_ms=4, ms_per_code=4)),
-    ("two200000_peaks_grid", 50000, dict(sampled_ms=4, ms_per_code=4, cfar=False, keep_grid=True)),
-    ("chirpz16368_cfar_dwells", 16368, dict(dwells=2)),
+    ("two200000_peaks_grid", 50000, dict(PEAKS, sampled_ms=4, ms_per_code=4, keep_grid=True)),
+    ("chirpz16368_cfar_dwells", 16368, dict(max_dwells=2)),
     ("chirpz16368_zero_padded", 16368, dict(ms_per_code=2)),
     ("chirpz5456_grid", 5456, dict(keep_grid=True)),
-    ("chirpz5456_bits", 5456, dict(bits=True)),
+    ("chirpz5456_bits", 5456, BITS),
 ]
 
 
@@ -89,12 +52,12 @@ CASES = [
 def test_band_search_is_byte_identical_to_host_search(capi, engine, spms, opts):
     """The window straddles the end of an owned ring; every dwell takes the next window."""
     rng = np.random.default_rng(spms + len(opts))
-    host, acq, codes = _pair(capi, engine, rng, spms, **opts)
+    host, acq, codes = ar.pair(capi, engine, rng, 1000 * spms, **opts)
     c = host.conf
     n, fs, dwells = c.consumed_samples, c.fs_in, c.max_dwells
-    cap = _pow2(3 * n)
+    cap = ar.pow2(3 * n)
     total = 2 * cap + 2 * n
-    x = _stream(rng, total, np.resize(codes[1], n), fs)
+    x = ar.stream(rng, total, np.resize(codes[1], n), fs)
     engine.iq_create(4, cap)
     _push_chunks(engine, 4, x, cap // 3 + 7)
     idx = 2 * cap - n // 3                     # crosses ring offset 0
@@ -105,7 +68,7 @@ def test_band_search_is_byte_identical_to_host_search(capi, engine, spms, opts):
         want = host.search(x[s0:s0 + n], [1, 0], dwell_counter=d)
         got = acq.search_band(4, s0, [1, 0], dwell_counter=d)
         assert got.tobytes() == want.tobytes(), (d, got, want)
-    assert _grids(acq) == _grids(host)
+    assert ar.grids(acq) == ar.grids(host)
     host.close()
     acq.close()
 
@@ -114,10 +77,10 @@ def test_windows_at_the_band_edges(capi, engine):
     """A window that ends exactly at write_index, one that starts exactly at the oldest sample still held, one that starts
     exactly at valid_from after a gap push; one sample further is refused."""
     rng = np.random.default_rng(7)
-    host, acq, codes = _pair(capi, engine, rng, 4000)
+    host, acq, codes = ar.pair(capi, engine, rng, 4e6)
     n = host.conf.consumed_samples
     cap = 16384
-    x = _stream(rng, 3 * cap + 1000, np.resize(codes[0], n), 4e6)
+    x = ar.stream(rng, 3 * cap + 1000, np.resize(codes[0], n), 4e6)
     engine.iq_create(5, cap)
     _push_chunks(engine, 5, x, 5000)
     lo, hi = engine.iq_window(5)
@@ -127,9 +90,9 @@ def test_windows_at_the_band_edges(capi, engine):
     for s0 in (hi - n + 1, lo - 1):
         with pytest.raises(capi.B200Error) as ei:
             acq.search_band(5, s0, [0, 1])
-        assert ei.value.code == ERR_RANGE
+        assert ei.value.code == ar.ERR_RANGE
     gap = hi + 12345
-    y = _stream(rng, 2 * n, np.resize(codes[1], n), 4e6)
+    y = ar.stream(rng, 2 * n, np.resize(codes[1], n), 4e6)
     engine.iq_push_at(5, gap, y)
     assert engine.iq_window(5) == (gap, gap + y.size)
     assert acq.search_band(5, gap, [0, 1]).tobytes() == host.search(y[:n], [0, 1]).tobytes()
@@ -141,11 +104,11 @@ def test_windows_at_the_band_edges(capi, engine):
 def test_step_two_from_the_band(capi, engine, spms):
     """Step two on the window after step one's equals b200_acq_search_step_two on a host copy of it."""
     rng = np.random.default_rng(spms)
-    host, acq, codes = _pair(capi, engine, rng, spms, slots=1)
+    host, acq, codes = ar.pair(capi, engine, rng, 1000 * spms, n_code_slots=1)
     c = host.conf
     n, fs = c.consumed_samples, c.fs_in
-    cap = _pow2(3 * n)
-    x = _stream(rng, cap + n, np.resize(codes[0], n), fs)
+    cap = ar.pow2(3 * n)
+    x = ar.stream(rng, cap + n, np.resize(codes[0], n), fs)
     engine.iq_create(6, cap)
     _push_chunks(engine, 6, x, n // 2 + 3)
     idx = cap - n // 2 - n                     # step one before the ring end, step two across it
@@ -165,21 +128,21 @@ def test_search_is_ordered_after_pushes_without_host_synchronisation(capi, engin
     """The ring holds PRN A's signal; PRN B's is pushed over the same ring slots (16-bit, 8-bit and float pushes) and searched
     right away, with no sync() in between: the result is B's, byte-equal to the host search of the converted samples."""
     rng = np.random.default_rng(11)
-    host, acq, codes = _pair(capi, engine, rng, 25000)
+    host, acq, codes = ar.pair(capi, engine, rng, 25e6)
     n, fs = host.conf.consumed_samples, host.conf.fs_in
-    cap = _pow2(2 * n)
+    cap = ar.pow2(2 * n)
     engine.iq_create(7, cap)
     for rep in range(3):
         for kind in ("i16", "i8", "f32"):
-            engine.iq_push(7, 20.0 * _stream(rng, cap, np.resize(codes[0], n), fs))   # the ring is A's everywhere
-            b = 20.0 * _stream(rng, n, codes[1], fs)
+            engine.iq_push(7, 20.0 * ar.stream(rng, cap, np.resize(codes[0], n), fs))   # the ring is A's everywhere
+            b = 20.0 * ar.stream(rng, n, codes[1], fs)
             if kind == "f32":
                 conv = b.astype(np.complex64)
                 first = engine.iq_push(7, conv)
             else:
                 dt, lim = (np.int16, 32767) if kind == "i16" else (np.int8, 127)
-                raw = np.clip(np.round(np.stack([b.real, b.imag], 1).ravel()), -lim, lim).astype(dt)
-                conv = (raw[0::2].astype(np.float32) + 1j * raw[1::2].astype(np.float32)).astype(np.complex64)
+                raw = ar.to_int(b, dt, clip=(-lim, lim))
+                conv = ar.from_int(raw)
                 first = engine.iq_push_int(7, raw)
             got = acq.search_band(7, first, [0, 1])
             assert got[1]["test_statistics"] > 3 * got[0]["test_statistics"], (rep, kind, got)   # found B, not A
@@ -192,10 +155,10 @@ def test_attached_band_then_refill(capi, engine):
     """A caller-owned device buffer attached with a non-zero first_index, then refilled from the host at another index."""
     import torch
     rng = np.random.default_rng(13)
-    host, acq, codes = _pair(capi, engine, rng, 4000)
+    host, acq, codes = ar.pair(capi, engine, rng, 4e6)
     n = host.conf.consumed_samples
     m, first_index = 5 * n + 17, 10_000_000
-    x = _stream(rng, m, np.resize(codes[0], n), 4e6)
+    x = ar.stream(rng, m, np.resize(codes[0], n), 4e6)
     xt = torch.from_numpy(x.view(np.float32)).cuda()
     torch.cuda.synchronize()
     engine.iq_attach_dev(8, xt.data_ptr(), m, first_index)
@@ -204,8 +167,8 @@ def test_attached_band_then_refill(capi, engine):
         assert got.tobytes() == host.search(x[off:off + n], [0, 1]).tobytes(), off
     with pytest.raises(capi.B200Error) as ei:
         acq.search_band(8, first_index + m - n + 1, [0, 1])
-    assert ei.value.code == ERR_RANGE
-    y = _stream(rng, 3 * n, np.resize(codes[1], n), 4e6)
+    assert ei.value.code == ar.ERR_RANGE
+    y = ar.stream(rng, 3 * n, np.resize(codes[1], n), 4e6)
     engine.iq_refill_ptr(8, y.ctypes.data, y.size, 77_000)
     assert engine.iq_window(8) == (77_000, 77_000 + y.size)
     for off in (0, 2 * n):
@@ -219,20 +182,20 @@ def test_attached_band_then_refill(capi, engine):
 
 def test_refusals_launch_nothing(capi, engine):
     rng = np.random.default_rng(17)
-    acq = _pair(capi, engine, rng, 4000)[1]
+    acq = ar.pair(capi, engine, rng, 4e6)[1]
     n = acq.conf.consumed_samples
     cap = 16384
     engine.iq_create(9, cap)
-    _push_chunks(engine, 9, _stream(rng, 2 * cap, np.zeros(n, np.complex64), 4e6), cap // 2)
+    _push_chunks(engine, 9, ar.stream(rng, 2 * cap, np.zeros(n, np.complex64), 4e6), cap // 2)
     lo, hi = engine.iq_window(9)
 
-    def refused(band, s0, code=ERR_RANGE):
+    def refused(band, s0, code=ar.ERR_RANGE):
         k0 = engine.launch_count()
         with pytest.raises(capi.B200Error) as ei:
             acq.search_band(band, s0, [0, 1])
         assert ei.value.code == code, str(ei.value)
         assert engine.launch_count() == k0
-        if code == ERR_RANGE:
+        if code == ar.ERR_RANGE:
             assert f"[{s0}, {(s0 + n) % 2**64})" in str(ei.value) and f"band {band}" in str(ei.value), str(ei.value)
         return str(ei.value)
 
@@ -249,33 +212,33 @@ def test_refusals_launch_nothing(capi, engine):
     engine.iq_push_at(9, w + 50_000, np.zeros(2 * n, np.complex64))
     refused(9, w + 50_000 - 1)                                     # before valid_from after a gap
     acq.search_band(9, w + 50_000, [0, 1])
-    refused(15, 0, ERR_STATE)                                      # a band nobody created
-    refused(16, 0, ERR_ARG)                                        # no such band
+    refused(15, 0, ar.ERR_STATE)                                   # a band nobody created
+    refused(16, 0, ar.ERR_ARG)                                     # no such band
     # one search in flight per object
     acq.search_band_submit(9, w + 50_000, [0, 1])
     with pytest.raises(capi.B200Error) as ei:
         acq.search_band_submit(9, w + 50_000, [0, 1])
-    assert ei.value.code == ERR_STATE
+    assert ei.value.code == ar.ERR_STATE
     with pytest.raises(capi.B200Error) as ei:
         acq.search_step_two_band(9, w + 50_000, 0, 1.0)
-    assert ei.value.code == ERR_STATE
+    assert ei.value.code == ar.ERR_STATE
     res = acq.search_wait()
     assert res.tobytes() == acq.search_band(9, w + 50_000, [0, 1]).tobytes()
     acq.close()
 
 
 @pytest.mark.parametrize("spms,opts", [
-    (4000, dict()), (4000, dict(cfar=False)),
-    (50000, dict()), (50000, dict(cfar=False)), (50000, dict(cfar=False, keep_grid=True)),
+    (4000, dict()), (4000, PEAKS),
+    (50000, dict()), (50000, PEAKS), (50000, dict(PEAKS, keep_grid=True)),
     (16368, dict()),
 ], ids=["single_cfar", "single_peaks", "two_level_cfar", "two_level_peaks", "two_level_peaks_grid", "chirp_z_cfar"])
 def test_band_search_launches_what_search_dev_launches(capi, engine, spms, opts):
     import torch
     rng = np.random.default_rng(19)
-    acq = _pair(capi, engine, rng, spms, **opts)[1]
+    acq = ar.pair(capi, engine, rng, 1000 * spms, **opts)[1]
     n = acq.conf.consumed_samples
-    x = _stream(rng, n, np.zeros(n, np.complex64), acq.conf.fs_in)
-    engine.iq_create(10, _pow2(n))
+    x = ar.stream(rng, n, np.zeros(n, np.complex64), acq.conf.fs_in)
+    engine.iq_create(10, ar.pow2(n))
     engine.iq_push(10, x)
     xt = torch.from_numpy(x.view(np.float32)).cuda()
     res = torch.zeros(2 * capi.ACQ_RESULT_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
@@ -310,7 +273,7 @@ def test_cold_start_from_a_pushed_file_into_device_loops(capi, tmp_path):
     codes = {sv["prn"]: gs.gps_ca_code(sv["prn"]) for sv in svs}
     iq = gs.make_iq(codes, fs, total, [dict(prn=sv["prn"], doppler=sv["doppler"], cn0=sv["cn0"],
                                             code_phase_chips=(-sv["delay"] * 1.023e6 / fs) % 1023) for sv in svs], seed=29)
-    raw = np.clip(np.round(np.stack([iq.real, iq.imag], 1).ravel() * scale), -32767, 32767).astype(np.int16)
+    raw = ar.to_int(iq, np.int16, scale, clip=(-32767, 32767))
     path = tmp_path / "gps_l1_4msps.ishort"
     raw.tofile(path)
     del iq, raw
@@ -319,10 +282,8 @@ def test_cold_start_from_a_pushed_file_into_device_loops(capi, tmp_path):
     e.iq_create(0, total)
     first, pushed = e.iq_push_file(0, str(path), "ishort")
     assert (first, pushed) == (0, total)
-    acq = capi.PcpsAcquisition(e, fs_in=int(fs), samples_per_ms=float(spms), samples_per_chip=int(fs / 1.023e6), doppler_max=5000,
-                               doppler_step=100, n_code_slots=32)
-    for p in range(1, 33):
-        acq.set_local_code(p - 1, gs.gps_ca_code_complex_sampled(p, int(fs)))
+    acq = ar.make(capi, e, fs, doppler_max=5000, doppler_step=100, n_code_slots=32)
+    ar.load_codes(acq, [ar.ca_code(gs, p, fs) for p in range(1, 33)])
     res = acq.search_band(0, abs_index, np.arange(32))
     c = acq.conf
     th = 2.0 * gammaincinv(2.0, (1.0 - pfa) ** (1.0 / (c.effective_fft_size * c.num_doppler_bins)))

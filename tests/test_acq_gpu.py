@@ -16,6 +16,7 @@ pytestmark = pytest.mark.gpu
 
 from gnss_synth import make_iq  # noqa: E402
 from gpu_fixtures import capi, engine  # noqa: E402,F401
+import acq_rig as ar  # noqa: E402
 
 
 def _bits(a):
@@ -30,26 +31,11 @@ def _signal(oracle, prns_present, fs, n, seed, cn0=45.0):
     return make_iq(codes, fs, n, svs, seed=seed), svs
 
 
-def _oracle_acq(oracle, fs, spms, spchip, dmax, dstep, prn, iq, cfar=True, dwells=1, center=0, **kw):
-    from oracle.acq_np import AcqConf, PcpsAcquisitionOracle
-    conf = AcqConf(fs_in=int(fs), samples_per_ms=spms, samples_per_code=spms, samples_per_chip=spchip, doppler_max=dmax,
-                   doppler_step=dstep, pfa=0.001 if cfar else 0.0, threshold=0.0, use_CFAR_algorithm_flag=cfar,
-                   max_dwells=dwells, **kw)
-    o = PcpsAcquisitionOracle(conf)
-    if center:
-        o.set_doppler_center(center)
-    o.set_local_code(oracle.port.gps_ca_code_complex_sampled(prn, int(fs)) if kw.get("sampled_ms", 1) == 1 else
-                     np.tile(oracle.port.gps_ca_code_complex_sampled(prn, int(fs)), kw["sampled_ms"]))
-    return o
-
-
 @pytest.mark.parametrize("fs,dmax,dstep,center", [(4e6, 5000, 250, 0), (4e6, 5000, 100, 0), (25e6, 10125, 250, 0),
                                                    (4e6, 5000, 250, 1375), (2.048e6, 5000, 500, 0)])
 def test_wipeoff_grid_bitexact(capi, engine, oracle, fs, dmax, dstep, center):
     import ctypes as C
-    spms = fs / 1000.0
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=spms, samples_per_chip=int(fs / 1.023e6),
-                               doppler_max=dmax, doppler_step=dstep)
+    acq = ar.make(capi, engine, fs, doppler_max=dmax, doppler_step=dstep)
     if center:
         acq.set_doppler_center(center, 0)
     got = acq.read_wipeoffs()
@@ -75,33 +61,21 @@ def test_wipeoff_grid_bitexact(capi, engine, oracle, fs, dmax, dstep, center):
                                                  (25e6, 5000, 250, False), (8e6, 5000, 500, True), (2.048e6, 5000, 250, True),
                                                  (12.5e6, 5000, 250, True), (5e6, 5000, 250, False)])
 def test_single_prn_acquisition_parity(capi, engine, oracle, fs, dmax, dstep, cfar):
-    spms = fs / 1000.0
-    n = int(spms)
-    spchip = int(fs / 1.023e6)
+    p = ar.params(fs, doppler_max=dmax, doppler_step=dstep, use_CFAR_algorithm_flag=cfar, keep_grid=True)
     prn = 7
-    iq, svs = _signal(oracle, [7, 12, 20], fs, n, seed=int(fs / 1e3) + dstep)
-    o = _oracle_acq(oracle, fs, spms, spchip, dmax, dstep, prn, iq, cfar=cfar)
+    iq, svs = _signal(oracle, [7, 12, 20], fs, int(p["samples_per_ms"]), seed=int(fs / 1e3) + dstep)
+    code = ar.ca_code(oracle.port, prn, fs)
+    o = ar.oracle(p, code, pfa=0.001 if cfar else 0.0)
     want = o.acquisition_core(iq)
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=spms, samples_per_chip=spchip, doppler_max=dmax,
-                               doppler_step=dstep, use_CFAR_algorithm_flag=cfar, keep_grid=True)
-    acq.set_local_code(0, oracle.port.gps_ca_code_complex_sampled(prn, int(fs)))
+    acq = capi.PcpsAcquisition(engine, **p)
+    acq.set_local_code(0, code)
     got = acq.search(iq, [0])[0]
-    assert int(got["index_time"]) == want["index_time"]
-    assert int(got["index_doppler"]) == want["index_doppler"]
-    assert int(got["doppler"]) == want["doppler"]
-    assert abs(got["grid_maximum"] - want["grid_maximum"]) / want["grid_maximum"] < 1e-4
-    assert abs(got["test_statistics"] - want["test_statistics"]) / want["test_statistics"] < 1e-4
-    if cfar:
-        assert abs(got["input_power"] - want["input_power"]) / want["input_power"] < 1e-4
-    else:
-        assert abs(got["second_peak"] - want["second_peak"]) / want["second_peak"] < 1e-4
+    ar.check(got, want, ar.CFAR_STATS if cfar else ar.PEAK_STATS)
     # the satellite is really there: Doppler within a bin, code phase within half a chip
     sv = svs[0]
     assert abs(want["doppler"] - sv["doppler"]) <= 666   # the reference test's own Doppler tolerance (1 ms main lobe)
     # whole magnitude grid
-    g = acq.read_grid(0)
-    ref_g = o.magnitude_grid[:, :acq.conf.effective_fft_size]
-    assert np.max(np.abs(g - ref_g)) / ref_g.max() < 2e-5
+    ar.check_grid(acq.read_grid(0), o.magnitude_grid, cols=acq.conf.effective_fft_size)
     acq.close()
 
 
@@ -110,10 +84,9 @@ def test_multi_prn_sweep_shares_forward_ffts(capi, engine, oracle):
     fs, dmax, dstep = 4e6, 5000, 250
     present = [3, 9, 17, 22, 31]
     iq, _ = _signal(oracle, present, fs, 4000, seed=44, cn0=46.0)
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=4000.0, samples_per_chip=3, doppler_max=dmax,
-                               doppler_step=dstep, n_code_slots=32)
-    for p in range(1, 33):
-        acq.set_local_code(p - 1, oracle.port.gps_ca_code_complex_sampled(p, int(fs)))
+    p = ar.params(fs, doppler_max=dmax, doppler_step=dstep, n_code_slots=32)
+    acq = capi.PcpsAcquisition(engine, **p)
+    ar.load_codes(acq, [ar.ca_code(oracle.port, prn, fs) for prn in range(1, 33)])
     res = acq.search(iq, np.arange(32))
     # arbitrary slot subsets / orders give the same per-PRN answers
     sub = [30, 2, 16, 8]
@@ -122,14 +95,11 @@ def test_multi_prn_sweep_shares_forward_ffts(capi, engine, oracle):
         assert res2[k] == res[s]
     from oracle.acq_np import compute_threshold
     th = compute_threshold(0.001, 4000, acq.conf.num_doppler_bins, 1)
-    detected = {p for p in range(1, 33) if res[p - 1]["test_statistics"] > th}
+    detected = {prn for prn in range(1, 33) if res[prn - 1]["test_statistics"] > th}
     assert detected == set(present)
-    for p in (3, 17, 5, 28):
-        o = _oracle_acq(oracle, fs, 4000.0, 3, dmax, dstep, p, iq)
-        want = o.acquisition_core(iq)
-        got = res[p - 1]
-        assert (int(got["index_time"]), int(got["index_doppler"])) == (want["index_time"], want["index_doppler"])
-        assert abs(got["test_statistics"] - want["test_statistics"]) / want["test_statistics"] < 1e-4
+    for prn in (3, 17, 5, 28):
+        want = ar.oracle(p, ar.ca_code(oracle.port, prn, fs), pfa=0.001).acquisition_core(iq)
+        ar.check(res[prn - 1], want, ("test_statistics",))
     acq.close()
 
 
@@ -138,23 +108,21 @@ def test_noncoherent_dwells_accumulate(capi, engine, oracle):
     CFAR input power is divided by the dwell counter (:431)."""
     fs, dmax, dstep, prn = 4e6, 5000, 250, 11
     iq, _ = _signal(oracle, [prn], fs, 12000, seed=77, cn0=38.0)
-    o = _oracle_acq(oracle, fs, 4000.0, 3, dmax, dstep, prn, iq, dwells=3)
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=4000.0, samples_per_chip=3, doppler_max=dmax,
-                               doppler_step=dstep, max_dwells=3)
-    acq.set_local_code(0, oracle.port.gps_ca_code_complex_sampled(prn, int(fs)))
+    p = ar.params(fs, doppler_max=dmax, doppler_step=dstep, max_dwells=3)
+    code = ar.ca_code(oracle.port, prn, fs)
+    o = ar.oracle(p, code, pfa=0.001)
+    acq = capi.PcpsAcquisition(engine, **p)
+    acq.set_local_code(0, code)
     for k in range(3):
         seg = iq[4000 * k: 4000 * (k + 1)]
-        want = o.acquisition_core(seg) if k == 0 else None
         if k > 0:
             # keep accumulating regardless of the threshold decision, like a block below threshold would
             o.num_noncoherent_integrations_counter = k
-            want = o.acquisition_core(seg)
+        want = o.acquisition_core(seg)
         got = acq.search(seg, [0], dwell_counter=k + 1)[0]
-        assert (int(got["index_time"]), int(got["index_doppler"])) == (want["index_time"], want["index_doppler"])
-        assert abs(got["test_statistics"] - want["test_statistics"]) / want["test_statistics"] < 1e-4
+        ar.check(got, want, ("test_statistics",))
         o.num_noncoherent_integrations_counter = k + 1
-    g = acq.read_grid(0)
-    assert np.max(np.abs(g - o.magnitude_grid[:, :4000])) / o.magnitude_grid.max() < 2e-5
+    ar.check_grid(acq.read_grid(0), o.magnitude_grid, cols=4000)
     acq.close()
 
 
@@ -164,35 +132,21 @@ def test_bit_transition_and_padded_layouts(capi, engine, oracle):
     fs, dmax, dstep, prn = 4e6, 5000, 250, 5
     # (a) bit transition
     iq, _ = _signal(oracle, [prn], fs, 8000, seed=5, cn0=47.0)
-    from oracle.acq_np import AcqConf, PcpsAcquisitionOracle
-    conf = AcqConf(fs_in=int(fs), samples_per_ms=4000.0, samples_per_code=4000.0, samples_per_chip=3, doppler_max=dmax,
-                   doppler_step=dstep, pfa=0.001, bit_transition_flag=True)
-    o = PcpsAcquisitionOracle(conf)
-    code = oracle.port.gps_ca_code_complex_sampled(prn, int(fs))
-    code2 = np.tile(code, 2)
-    o.set_local_code(code2)
-    want = o.acquisition_core(iq)
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=4000.0, samples_per_chip=3, doppler_max=dmax,
-                               doppler_step=dstep, bit_transition_flag=True)
+    code2 = ar.ca_code(oracle.port, prn, fs, 2)
+    p = ar.params(fs, doppler_max=dmax, doppler_step=dstep, bit_transition_flag=True)
+    want = ar.oracle(p, code2, pfa=0.001).acquisition_core(iq)
+    acq = capi.PcpsAcquisition(engine, **p)
     assert (acq.conf.fft_size, acq.conf.effective_fft_size, acq.conf.consumed_samples) == (8000, 4000, 8000)
     acq.set_local_code(0, code2)
-    got = acq.search(iq, [0])[0]
-    assert (int(got["index_time"]), int(got["index_doppler"])) == (want["index_time"], want["index_doppler"])
-    assert abs(got["test_statistics"] - want["test_statistics"]) / want["test_statistics"] < 1e-4
+    ar.check(acq.search(iq, [0])[0], want, ("test_statistics",))
     acq.close()
     # (b) sampled_ms = 2 with ms_per_code = 1 ... equal -> plain; use ms_per_code=4 analogue: sampled 1, code 4
-    conf = AcqConf(fs_in=int(fs), samples_per_ms=4000.0, samples_per_code=4000.0, samples_per_chip=3, doppler_max=dmax,
-                   doppler_step=dstep, pfa=0.001, sampled_ms=2, ms_per_code=4)
-    o = PcpsAcquisitionOracle(conf)
-    o.set_local_code(code2)
-    want = o.acquisition_core(iq)
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=4000.0, samples_per_chip=3, doppler_max=dmax,
-                               doppler_step=dstep, sampled_ms=2, ms_per_code=4)
+    p = ar.params(fs, doppler_max=dmax, doppler_step=dstep, sampled_ms=2, ms_per_code=4)
+    want = ar.oracle(p, code2, pfa=0.001).acquisition_core(iq)
+    acq = capi.PcpsAcquisition(engine, **p)
     assert (acq.conf.fft_size, acq.conf.consumed_samples, acq.conf.code_layout) == (16000, 8000, 2)
     acq.set_local_code(0, code2)
-    got = acq.search(iq, [0])[0]
-    assert (int(got["index_time"]), int(got["index_doppler"])) == (want["index_time"], want["index_doppler"])
-    assert abs(got["test_statistics"] - want["test_statistics"]) / want["test_statistics"] < 1e-4
+    ar.check(acq.search(iq, [0])[0], want, ("test_statistics",))
     acq.close()
 
 
@@ -200,15 +154,13 @@ def test_doppler_center_assisted(capi, engine, oracle):
     fs, prn = 4e6, 14
     iq, svs = _signal(oracle, [prn], fs, 4000, seed=14)
     center = int(round(svs[0]["doppler"] / 250.0)) * 250
-    o = _oracle_acq(oracle, fs, 4000.0, 3, 1000, 125, prn, iq, center=center)
-    want = o.acquisition_core(iq)
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=4000.0, samples_per_chip=3, doppler_max=1000,
-                               doppler_step=125)
+    p = ar.params(fs, doppler_max=1000, doppler_step=125)
+    code = ar.ca_code(oracle.port, prn, fs)
+    want = ar.oracle(p, code, pfa=0.001, center=center).acquisition_core(iq)
+    acq = capi.PcpsAcquisition(engine, **p)
     acq.set_doppler_center(center, 0)
-    acq.set_local_code(0, oracle.port.gps_ca_code_complex_sampled(prn, int(fs)))
-    got = acq.search(iq, [0])[0]
-    assert int(got["doppler"]) == want["doppler"]
-    assert int(got["index_time"]) == want["index_time"]
+    acq.set_local_code(0, code)
+    ar.check(acq.search(iq, [0])[0], want, stats=())
     assert abs(want["doppler"] - svs[0]["doppler"]) <= 666
     acq.close()
 
@@ -219,9 +171,7 @@ def test_fft_round_trip_property_all_supported_radices(capi, engine, oracle):
     for sizes exercising radices 2,3,4,5,7,8."""
     rng = np.random.default_rng(9)
     for n in (4096, 6000, 8400, 16000, 25000, 27000, 27648, 2 * 3 * 5 * 7, 4802):
-        fs = n * 1000
-        acq = capi.PcpsAcquisition(engine, fs_in=fs, samples_per_ms=float(n), samples_per_chip=max(1, n // 1023),
-                                   doppler_max=1000, doppler_step=500)
+        acq = ar.make(capi, engine, n * 1000, doppler_max=1000, doppler_step=500)
         code = rng.choice([-1.0, 1.0], n).astype(np.float32).astype(np.complex64) * 1j
         acq.set_local_code(0, code)
         k = int(rng.integers(0, n))
@@ -235,11 +185,10 @@ def test_fft_round_trip_property_all_supported_radices(capi, engine, oracle):
 
 def test_acq_error_paths(capi, engine):
     with pytest.raises(capi.B200Error):   # 16368 = 2^4*3*11*31 goes through chirp-z, which has the CFAR statistic only
-        capi.PcpsAcquisition(engine, fs_in=16368000, samples_per_ms=16368.0, samples_per_chip=16, doppler_max=5000, doppler_step=250,
-                             use_CFAR_algorithm_flag=False)
+        ar.make(capi, engine, 16368000, doppler_max=5000, doppler_step=250, use_CFAR_algorithm_flag=False)
     with pytest.raises(capi.B200Error):   # beyond 8 x 27648 points
-        capi.PcpsAcquisition(engine, fs_in=300000000, samples_per_ms=300000.0, samples_per_chip=290, doppler_max=1000, doppler_step=500)
-    acq = capi.PcpsAcquisition(engine, fs_in=4000000, samples_per_ms=4000.0, samples_per_chip=3, doppler_max=5000, doppler_step=250)
+        ar.make(capi, engine, 300000000, samples_per_chip=290, doppler_max=1000, doppler_step=500)
+    acq = ar.make(capi, engine, 4000000, doppler_max=5000, doppler_step=250)
     with pytest.raises(capi.B200Error):   # search before set_local_code
         acq.search(np.zeros(4000, np.complex64), [0])
     acq.set_local_code(0, np.ones(4000, np.complex64))
@@ -252,26 +201,22 @@ def test_two_step_acquisition(capi, engine, oracle):
     """make_2_steps (pcps_acquisition.cc:294-301,:605-626): the second step searches 4 bins of 125 Hz
     around the first step's Doppler on the next buffer, keeps the first step's input power, and uses the
     float Doppler formula."""
-    from oracle.acq_np import AcqConf, PcpsAcquisitionOracle
     fs, prn = 4e6, 8
     iq, svs = _signal(oracle, [prn], fs, 8000, seed=88, cn0=47.0)
-    conf = AcqConf(fs_in=int(fs), samples_per_ms=4000.0, samples_per_code=4000.0, samples_per_chip=3, doppler_max=5000,
-                   doppler_step=500, pfa=0.001, pfa2=0.001, make_2_steps=True, doppler_step2=125.0, num_doppler_bins_step2=4)
-    o = PcpsAcquisitionOracle(conf)
-    code = oracle.port.gps_ca_code_complex_sampled(prn, int(fs))
-    o.set_local_code(code)
+    p = ar.params(fs, doppler_max=5000, doppler_step=500)
+    code = ar.ca_code(oracle.port, prn, fs)
+    o = ar.oracle(p, code, pfa=0.001, pfa2=0.001, make_2_steps=True, doppler_step2=125.0, num_doppler_bins_step2=4)
     w1 = o.acquisition_core(iq[:4000])
     assert not w1["positive"] and o.step_two          # first step passed the threshold, second pending
     w2 = o.acquisition_core(iq[4000:8000])
     assert w2["positive"] and w2["step_two"]
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=4000.0, samples_per_chip=3, doppler_max=5000, doppler_step=500)
+    acq = capi.PcpsAcquisition(engine, **p)
     acq.set_local_code(0, code)
     g1 = acq.search(iq[:4000], [0])[0]
-    assert (int(g1["index_time"]), int(g1["doppler"])) == (w1["index_time"], w1["doppler"])
+    ar.check(g1, w1, stats=())
     acq.set_step_two(float(g1["doppler"]), 125.0, 4)
     g2 = acq.search_step_two(iq[4000:8000], 0, float(g1["input_power"]))
-    assert (int(g2["index_time"]), int(g2["index_doppler"]), int(g2["doppler"])) == (w2["index_time"], w2["index_doppler"], w2["doppler"])
-    assert abs(g2["test_statistics"] - w2["test_statistics"]) / w2["test_statistics"] < 1e-4
+    ar.check(g2, w2, ("test_statistics",))
     assert abs(w2["doppler"] - svs[0]["doppler"]) < abs(w1["doppler"] - svs[0]["doppler"]) + 63   # refined (within half a fine bin)
     acq.close()
 
@@ -286,32 +231,27 @@ def test_two_step_acquisition(capi, engine, oracle):
 def test_two_level_fft_sizes(capi, engine, oracle, fs, sampled_ms, dmax, dstep, cfar):
     """fft_size above the single-CTA limit: one radix-n1 stage through global memory + in-shared-memory
     blocks.  Same contract as the small sizes: exact indices, statistics within 1e-4, grid within 2e-5."""
-    spms = fs / 1000.0
-    n = int(spms) * sampled_ms
-    spchip = int(fs / 1.023e6)
+    p = ar.params(fs, doppler_max=dmax, doppler_step=dstep, use_CFAR_algorithm_flag=cfar, sampled_ms=sampled_ms,
+                  ms_per_code=sampled_ms, keep_grid=True)
+    spms = int(p["samples_per_ms"])
+    n = spms * sampled_ms
     prn = 7
-    codes = {p: oracle.port.gps_ca_code(p) for p in (7, 21)}
+    codes = {q: oracle.port.gps_ca_code(q) for q in (7, 21)}
     svs = [dict(prn=7, doppler=dstep * round(0.6 * dmax / dstep) + 10.0, code_phase_chips=321.4, cn0=42.0, phase0=1.0),
            dict(prn=21, doppler=-0.3 * dmax, code_phase_chips=77.7, cn0=42.0, phase0=2.0)]
     iq = make_iq(codes, fs, n, svs, seed=int(fs / 1e3) + sampled_ms)
-    o = _oracle_acq(oracle, fs, spms, spchip, dmax, dstep, prn, iq, cfar=cfar, sampled_ms=sampled_ms, ms_per_code=sampled_ms)
+    local = ar.ca_code(oracle.port, prn, fs, sampled_ms)
+    o = ar.oracle(p, local, pfa=0.001 if cfar else 0.0)
     want = o.acquisition_core(iq)
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=spms, samples_per_chip=spchip, doppler_max=dmax,
-                               doppler_step=dstep, use_CFAR_algorithm_flag=cfar, sampled_ms=sampled_ms, ms_per_code=sampled_ms,
-                               keep_grid=True)
+    acq = capi.PcpsAcquisition(engine, **p)
     assert acq.conf.fft_size == n
-    acq.set_local_code(0, np.tile(oracle.port.gps_ca_code_complex_sampled(prn, int(fs)), sampled_ms))
+    acq.set_local_code(0, local)
     got = acq.search(iq, [0])[0]
     # with sampled_ms code periods in the buffer the correlation has sampled_ms mathematically equal peaks one
     # code period apart; which one wins is rounding noise, and update_synchro folds it away
     # (Acq_delay_samples = fmod(index_time, samples_per_code), pcps_acquisition.cc:582)
-    assert int(got["index_time"]) % int(spms) == want["index_time"] % int(spms)
-    assert int(got["index_doppler"]) == want["index_doppler"]
-    assert abs(got["grid_maximum"] - want["grid_maximum"]) / want["grid_maximum"] < 1e-4
-    assert abs(got["test_statistics"] - want["test_statistics"]) / want["test_statistics"] < 1e-4
-    g = acq.read_grid(0)
-    ref_g = o.magnitude_grid[:, :acq.conf.effective_fft_size]
-    assert np.max(np.abs(g - ref_g)) / ref_g.max() < 2e-5
+    ar.check(got, want, ("grid_maximum", "test_statistics"), period=spms)
+    ar.check_grid(acq.read_grid(0), o.magnitude_grid, cols=acq.conf.effective_fft_size)
     assert abs(want["doppler"] - svs[0]["doppler"]) <= max(dstep, 666 / sampled_ms)
     acq.close()
 
@@ -326,49 +266,38 @@ def test_chirp_z_sizes_with_large_prime_factors(capi, engine, oracle, fs, sample
     """fft_size with prime factors above 7: every N-point transform becomes a circular convolution with a chirp, done with
     M-point transforms (M >= 2N - 1).  Same contract as the other sizes (exact indices, statistics 1e-4, grid 2e-5 of the
     peak), plus two dwells and a Doppler-centre change through the same path."""
-    spms = fs / 1000.0
-    n = int(spms) * sampled_ms
-    spchip = int(fs / 1.023e6)
+    kw = dict(sampled_ms=sampled_ms, ms_per_code=sampled_ms) if sampled_ms > 1 else {}
+    p = ar.params(fs, doppler_max=dmax, doppler_step=dstep, use_CFAR_algorithm_flag=True, keep_grid=True, max_dwells=2,
+                  n_code_slots=2, **kw)
+    spms = int(p["samples_per_ms"])
+    n = spms * sampled_ms
     prn = 7
-    codes = {p: oracle.port.gps_ca_code(p) for p in (7, 21)}
+    codes = {q: oracle.port.gps_ca_code(q) for q in (7, 21)}
     svs = [dict(prn=7, doppler=dstep * round(0.6 * dmax / dstep) + 10.0, code_phase_chips=321.4, cn0=47.0, phase0=1.0),
            dict(prn=21, doppler=-dstep * round(0.3 * dmax / dstep) + 20.0, code_phase_chips=77.7, cn0=47.0, phase0=2.0)]
     iq = make_iq(codes, fs, 2 * n, svs, seed=int(fs / 1e3) + sampled_ms)
-    kw = dict(sampled_ms=sampled_ms, ms_per_code=sampled_ms) if sampled_ms > 1 else {}
-    o = _oracle_acq(oracle, fs, spms, spchip, dmax, dstep, prn, iq, cfar=True, dwells=2, **kw)
+    local = ar.ca_code(oracle.port, prn, fs, sampled_ms)
+    o = ar.oracle(p, local, pfa=0.001)
     want = o.acquisition_core(iq[:n])
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=spms, samples_per_chip=spchip, doppler_max=dmax,
-                               doppler_step=dstep, use_CFAR_algorithm_flag=True, keep_grid=True, max_dwells=2, n_code_slots=2, **kw)
+    acq = capi.PcpsAcquisition(engine, **p)
     assert acq.conf.fft_size == n
-    local = oracle.port.gps_ca_code_complex_sampled(prn, int(fs))
-    acq.set_local_code(1, np.tile(local, sampled_ms))
-    acq.set_local_code(0, np.tile(oracle.port.gps_ca_code_complex_sampled(21, int(fs)), sampled_ms))
+    acq.set_local_code(1, local)
+    acq.set_local_code(0, ar.ca_code(oracle.port, 21, fs, sampled_ms))
     both = acq.search(iq[:n], [0, 1])
-    got = both[1]
-    assert int(got["index_time"]) % int(spms) == want["index_time"] % int(spms)
-    assert int(got["index_doppler"]) == want["index_doppler"]
-    assert int(got["doppler"]) == want["doppler"]
-    assert abs(got["grid_maximum"] - want["grid_maximum"]) / want["grid_maximum"] < 1e-4
-    assert abs(got["test_statistics"] - want["test_statistics"]) / want["test_statistics"] < 1e-4
-    assert abs(got["input_power"] - want["input_power"]) / want["input_power"] < 1e-4
-    g = acq.read_grid(1)
-    ref_g = o.magnitude_grid[:, :acq.conf.effective_fft_size]
-    assert np.max(np.abs(g - ref_g)) / ref_g.max() < 2e-5
+    ar.check(both[1], want, period=spms)
+    ar.check_grid(acq.read_grid(1), o.magnitude_grid, cols=acq.conf.effective_fft_size)
     assert abs(want["doppler"] - svs[0]["doppler"]) <= max(dstep, 666 / sampled_ms)
     assert abs(int(both[0]["doppler"]) - svs[1]["doppler"]) <= max(dstep, 666 / sampled_ms)
     # second dwell accumulates on the grid
     o.num_noncoherent_integrations_counter = 1   # keep accumulating whatever the threshold decided
     want2 = o.acquisition_core(iq[n:])
     got2 = acq.search(iq[n:], [1], dwell_counter=2)[0]
-    assert int(got2["index_doppler"]) == want2["index_doppler"]
-    assert abs(got2["test_statistics"] - want2["test_statistics"]) / want2["test_statistics"] < 1e-4
+    ar.check(got2, want2, ("test_statistics",), period=spms)
     # assisted acquisition: moving the Doppler centre rebuilds the chirped wipe-off rows
-    o3 = _oracle_acq(oracle, fs, spms, spchip, dmax, dstep, prn, iq, cfar=True, center=875, **kw)
-    want3 = o3.acquisition_core(iq[:n])
+    want3 = ar.oracle(p, local, pfa=0.001, max_dwells=1, center=875).acquisition_core(iq[:n])
     acq.set_doppler_center(875)
     got3 = acq.search(iq[:n], [1])[0]
-    assert int(got3["doppler"]) == want3["doppler"]
-    assert abs(got3["test_statistics"] - want3["test_statistics"]) / want3["test_statistics"] < 1e-4
+    ar.check(got3, want3, ("test_statistics",), period=spms)
     acq.close()
 
 
@@ -381,17 +310,15 @@ def test_async_search_matches_synchronous_and_guards_misuse(oracle):
     code = gs.gps_ca_code(3)
     iq = gs.make_iq({3: code}, fs, n, [dict(prn=3, doppler=2100.0, code_phase_chips=400.0, cn0=48.0)], seed=8)
     e = capi.Engine()
-    a = capi.PcpsAcquisition(e, fs_in=int(fs), samples_per_ms=float(n), samples_per_chip=4, doppler_max=5000, doppler_step=250, n_code_slots=2)
-    b = capi.PcpsAcquisition(e, fs_in=int(fs), samples_per_ms=float(n), samples_per_chip=4, doppler_max=5000, doppler_step=250, n_code_slots=2)
+    a, b = (ar.make(capi, e, fs, samples_per_chip=4, doppler_max=5000, doppler_step=250, n_code_slots=2) for _ in range(2))
     for o in (a, b):
-        o.set_local_code(0, gs.gps_ca_code_complex_sampled(3, int(fs)))
-        o.set_local_code(1, gs.gps_ca_code_complex_sampled(4, int(fs)))
+        ar.load_codes(o, [ar.ca_code(gs, prn, fs) for prn in (3, 4)])
     want = a.search(iq, [0, 1])
     a.search_submit(iq, [0, 1])
     b.search_submit(iq, [1, 0])
     with pytest.raises(capi.B200Error) as ei:
         a.search_submit(iq, [0])
-    assert ei.value.code == -4
+    assert ei.value.code == ar.ERR_STATE
     ra, rb = a.search_wait(), b.search_wait()
     assert ra.tobytes() == want.tobytes()
     assert rb[::-1].tobytes() == want.tobytes()
@@ -408,32 +335,23 @@ def test_async_search_matches_synchronous_and_guards_misuse(oracle):
 def test_host_searches_refused_while_a_sweep_is_in_flight(entry):
     """Every search that returns results to the host is B200_ERR_STATE while a submitted sweep is in flight, and the
     sweep's results are still the synchronous search's."""
-    import ctypes as C
     from gnss_sdr_b200 import capi
     import gnss_synth as gs
     fs, n, band = 4e6, 4000, 0
     iq = gs.make_iq({3: gs.gps_ca_code(3)}, fs, n, [dict(prn=3, doppler=2100.0, code_phase_chips=400.0, cn0=48.0)], seed=8)
-    raw = np.round(iq.view(np.float32) * 100).astype(np.int16)
+    raw = ar.to_int(iq, np.int16, 100)
     e = capi.Engine()
     e.iq_create(band, 8192)
     e.iq_push(band, iq)
-    a = capi.PcpsAcquisition(e, fs_in=int(fs), samples_per_ms=float(n), samples_per_chip=4, doppler_max=5000, doppler_step=250, n_code_slots=2)
-    a.set_local_code(0, gs.gps_ca_code_complex_sampled(3, int(fs)))
-    a.set_local_code(1, gs.gps_ca_code_complex_sampled(4, int(fs)))
+    a = ar.make(capi, e, fs, samples_per_chip=4, doppler_max=5000, doppler_step=250, n_code_slots=2)
+    ar.load_codes(a, [ar.ca_code(gs, prn, fs) for prn in (3, 4)])
     a.set_step_two(2100.0, 125.0, 4)   # so that a step-two call is otherwise legal
     want = a.search(iq, [0, 1])
-    res, slot = np.zeros(1, capi.ACQ_RESULT_DTYPE), np.zeros(1, np.uint32)
-
-    def i16(name, *args):
-        rc = getattr(capi.lib, name)(a.h, raw.ctypes.data, *args, res.ctypes.data)
-        if rc:
-            raise capi.B200Error(rc, name)
-
     calls = {
         "search": lambda: a.search(iq, [0]),
-        "search_i16": lambda: i16("b200_acq_search_i16", slot.ctypes.data, 1, 1),
+        "search_i16": lambda: ar.search_i16(a, raw, [0]),
         "search_step_two": lambda: a.search_step_two(iq, 0, 1.0),
-        "search_step_two_i16": lambda: i16("b200_acq_search_step_two_i16", 0, 1, C.c_float(1.0)),
+        "search_step_two_i16": lambda: ar.search_step_two_i16(a, raw, 0, 1.0),
         "search_submit": lambda: a.search_submit(iq, [0]),
         "search_band": lambda: a.search_band(band, 0, [0]),
         "search_band_submit": lambda: a.search_band_submit(band, 0, [0]),
@@ -442,7 +360,7 @@ def test_host_searches_refused_while_a_sweep_is_in_flight(entry):
     a.search_submit(iq, [0, 1])
     with pytest.raises(capi.B200Error) as ei:
         calls[entry]()
-    assert ei.value.code == -4
+    assert ei.value.code == ar.ERR_STATE
     assert a.search_wait().tobytes() == want.tobytes()
     a.close()
     e.close()

@@ -10,6 +10,7 @@ checked in test_acq_chirpz_modes_gpu.py.
 import numpy as np
 import pytest
 
+import acq_rig as ar
 from gpu_fixtures import capi, engine  # noqa: F401
 
 pytestmark = pytest.mark.gpu
@@ -24,12 +25,10 @@ pytestmark = pytest.mark.gpu
     (50e6, 1, False, False, 10),   # N = 50000, no grid: the second-peak row is recomputed
 ])
 def test_search_counts_the_kernels_it_issues(capi, engine, fs, sampled_ms, cfar, keep_grid, launches):
-    spms = fs / 1000.0
-    acq = capi.PcpsAcquisition(engine, fs_in=int(fs), samples_per_ms=spms, samples_per_chip=int(fs / 1.023e6), doppler_max=1000,
-                               doppler_step=500, use_CFAR_algorithm_flag=cfar, sampled_ms=sampled_ms, ms_per_code=sampled_ms,
-                               keep_grid=keep_grid)
+    acq = ar.make(capi, engine, fs, doppler_max=1000, doppler_step=500, use_CFAR_algorithm_flag=cfar, sampled_ms=sampled_ms,
+                  ms_per_code=sampled_ms, keep_grid=keep_grid)
     n = acq.conf.fft_size
-    assert n == int(spms) * sampled_ms
+    assert n == int(fs / 1000.0) * sampled_ms
     rng = np.random.default_rng(n)
     acq.set_local_code(0, rng.choice([-1.0, 1.0], n).astype(np.complex64))
     iq = (rng.normal(size=n) + 1j * rng.normal(size=n)).astype(np.complex64)

@@ -15,31 +15,17 @@ import numpy as np
 import pytest
 
 from gpu_fixtures import capi, engine  # noqa: F401
+import acq_rig as ar
 
 pytestmark = pytest.mark.gpu
 
-GRID_TOL = 2e-5
-STAT_TOL = 1e-4
 MARGIN = 1e-3
+BINS4 = dict(doppler_max=1000, doppler_step=500)   # 4 Doppler bins: -1000, -500, 0, +500 Hz
 
 
-def _params(n, *, spc=None, cfar=True, keep_grid=False, slots=3, **kw):
-    """PcpsAcquisition keywords for a 1 ms code of n samples (fs = n kHz) and 4 Doppler bins (-1000 .. +500 Hz)."""
-    fs = kw.pop("fs_in", n * 1000)
-    spc = max(1, int(fs / 1.023e6)) if spc is None else spc
-    return dict(fs_in=fs, samples_per_ms=float(kw.pop("samples_per_ms", n)), samples_per_chip=spc, doppler_max=1000,
-                doppler_step=500, use_CFAR_algorithm_flag=cfar, keep_grid=keep_grid, n_code_slots=slots, **kw)
-
-
-def _oracle(p, **extra):
-    """PcpsAcquisitionOracle with the same configuration; only its statistics rules are used."""
-    from oracle.acq_np import AcqConf, PcpsAcquisitionOracle
-    conf = AcqConf(fs_in=p["fs_in"], samples_per_ms=p["samples_per_ms"], samples_per_code=p["samples_per_ms"],
-                   samples_per_chip=p["samples_per_chip"], sampled_ms=p.get("sampled_ms", 1), ms_per_code=p.get("ms_per_code", 1),
-                   doppler_max=p["doppler_max"], doppler_step=p["doppler_step"], max_dwells=p.get("max_dwells", 1),
-                   bit_transition_flag=p.get("bit_transition_flag", False), use_CFAR_algorithm_flag=p["use_CFAR_algorithm_flag"],
-                   **extra)
-    return PcpsAcquisitionOracle(conf)
+def _params(n, **kw):
+    """PcpsAcquisition keywords for a 1 ms code of n samples (fs = n kHz) and 4 Doppler bins."""
+    return ar.params(n * 1000, **BINS4, **kw)
 
 
 def _codes(rng, slots, n):
@@ -86,27 +72,16 @@ def _assert_unique_peak(grid):
     assert top[1] >= (1.0 + MARGIN) * top[0], f"input has no unique arg-max: {top[1]:.6g} vs runner-up {top[0]:.6g}"
 
 
-def _check(got, want, cfar, what=""):
-    assert (int(got["index_time"]), int(got["index_doppler"]), int(got["doppler"])) == \
-        (want["index_time"], want["index_doppler"], want["doppler"]), (what, got, want)
-    for k in ("grid_maximum", "test_statistics", "input_power" if cfar else "second_peak"):
-        assert abs(float(got[k]) - want[k]) <= STAT_TOL * abs(want[k]), (what, k, float(got[k]), want[k])
-
-
-def _grid_err(acq, slot, ref):
-    return float(np.max(np.abs(acq.read_grid(slot) - ref)) / ref.max())
-
-
 def _search_all_slots(capi, engine, p, codes, iq, dwell_inputs=()):
     """Search every other slot in descending order ([2, 0] of three), then all of them in order (and again on each further
     dwell input); check every slot's record against the float64 reference, and that both searches give it the same bytes.
     Returns (acq, records of the last search, reference grids)."""
     acq = capi.PcpsAcquisition(engine, **p)
-    conf, cfar = acq.conf, bool(p["use_CFAR_algorithm_flag"])
-    for s, code in enumerate(codes):
-        acq.set_local_code(s, code)
+    conf = acq.conf
+    ar.load_codes(acq, codes)
     wipe = acq.read_wipeoffs()
-    o = _oracle(p)
+    o = ar.oracle(p)
+    stats = ar.CFAR_STATS if o.c.use_CFAR_algorithm_flag else ar.PEAK_STATS
     assert (o.c.fft_size, o.c.effective_fft_size, o.c.num_doppler_bins) == (conf.fft_size, conf.effective_fft_size, conf.num_doppler_bins)
     refs = [_ref_grid(conf, wipe, iq, c) for c in codes]
     every = list(range(len(codes)))
@@ -120,15 +95,15 @@ def _search_all_slots(capi, engine, p, codes, iq, dwell_inputs=()):
         res = acq.search(x, every, dwell_counter=d)
     for s, g in enumerate(refs):
         _assert_unique_peak(g)
-        _check(res[s], _ref_stats(o, g, 1 + len(dwell_inputs)), cfar, f"slot {s}")
+        ar.check(res[s], _ref_stats(o, g, 1 + len(dwell_inputs)), stats, f"slot {s}")
     return acq, res, refs
 
 
 def _plan_case(capi, engine, n, cfar, keep_grid, seed, slots=3, **kw):
-    p = _params(n, cfar=cfar, keep_grid=keep_grid, slots=slots, **kw)
+    p = _params(n, use_CFAR_algorithm_flag=cfar, keep_grid=keep_grid, n_code_slots=slots, **kw)
     rng = np.random.default_rng(seed)
-    probe = _oracle(p).c
-    need = probe.fft_size // 2 if probe.bit_transition_flag else probe.consumed_samples
+    probe = ar.oracle(p).c
+    need = ar.code_len(probe)
     codes = _codes(rng, slots, need)
     # slot s: amplitude 1 - 0.2 s, its own delay and Doppler bin (bins are -1000, -500, 0, +500 Hz)
     # zero-padded layout: a delay k splits the correlation into peaks of k and consumed - k samples; keep them far apart
@@ -136,12 +111,11 @@ def _plan_case(capi, engine, n, cfar, keep_grid, seed, slots=3, **kw):
     placements = [(s, 1.0 - 0.2 * s, int(rng.integers(0, kmax)), (500.0, -1000.0, -500.0)[s]) for s in range(slots)]
     iq = _signal(rng, codes, probe, p["fs_in"], placements)
     acq, res, refs = _search_all_slots(capi, engine, p, codes, iq)
-    errs = [_grid_err(acq, s, refs[s]) for s in range(slots)] if keep_grid else []
+    errs = [ar.check_grid(acq.read_grid(s), refs[s]) for s in range(slots)] if keep_grid else []
     fft_size, layout = acq.conf.fft_size, acq.conf.code_layout
     acq.close()
     if errs:
         print(f"grid error vs float64, fft_size {fft_size}, code layout {layout}: {max(errs):.3e} of the peak")
-        assert max(errs) < GRID_TOL, errs
 
 
 # two-level sizes: expected plan n1 x [in-shared-memory radices] in the comment.  (56 000 points in test_acq_gpu.py plans as
@@ -177,15 +151,14 @@ def test_single_cta_plans_against_float64(capi, engine, n):
 def test_fft_plan_only_from_the_size(capi, engine, monkeypatch):
     """B200_ACQ_RADIX25 in the environment selects nothing: with B200_ACQ_RADIX25=0 a 25 000-point search still plans
     [8, 25, 25, 5], so its records and grids, which [8, 5, 5, 5, 5, 5] would sum in another order, are the same bytes."""
-    p = _params(25000, keep_grid=True)
+    p = _params(25000, keep_grid=True, n_code_slots=3)
     rng = np.random.default_rng(25)
     codes = _codes(rng, 3, 25000)
-    iq = _signal(rng, codes, _oracle(p).c, p["fs_in"], [(0, 1.0, 777, 500.0), (1, 0.8, 12345, -1000.0)])
+    iq = _signal(rng, codes, ar.oracle(p).c, p["fs_in"], [(0, 1.0, 777, 500.0), (1, 0.8, 12345, -1000.0)])
 
     def search():
         acq = capi.PcpsAcquisition(engine, **p)
-        for s, code in enumerate(codes):
-            acq.set_local_code(s, code)
+        ar.load_codes(acq, codes)
         out = acq.search(iq, [0, 1, 2]).tobytes() + b"".join(acq.read_grid(s).tobytes() for s in range(3))
         acq.close()
         return out
@@ -198,37 +171,36 @@ def test_fft_plan_only_from_the_size(capi, engine, monkeypatch):
 @pytest.mark.parametrize("n", [7, 8, 25])   # one stage of 7, one of 8, two of 5
 def test_smallest_sizes_search_right_or_refuse(capi, engine, n):
     try:
-        capi.PcpsAcquisition(engine, **_params(n, slots=1)).close()
+        capi.PcpsAcquisition(engine, **_params(n)).close()
     except capi.B200Error:
         return   # refusing a size is allowed; a wrong answer is not
     rng = np.random.default_rng(n)
     for cfar, keep_grid in ((True, True), (False, False)):
-        p = _params(n, cfar=cfar, keep_grid=keep_grid, slots=1)
+        p = _params(n, use_CFAR_algorithm_flag=cfar, keep_grid=keep_grid)
         code = _codes(rng, 1, n)
         iq = np.roll(code[0], 3).astype(np.complex64)   # zero Doppler: exact wipe-off row, no noise
         acq = capi.PcpsAcquisition(engine, **p)
         acq.set_local_code(0, code[0])
         ref = _ref_grid(acq.conf, acq.read_wipeoffs(), iq, code[0])
         _assert_unique_peak(ref)
-        _check(acq.search(iq, [0])[0], _ref_stats(_oracle(p), ref), cfar, f"N = {n}")
+        ar.check(acq.search(iq, [0])[0], _ref_stats(ar.oracle(p), ref), ar.CFAR_STATS if cfar else ar.PEAK_STATS, f"N = {n}")
         if keep_grid:
-            assert _grid_err(acq, 0, ref) < GRID_TOL
+            ar.check_grid(acq.read_grid(0), ref)
         acq.close()
 
 
 def test_two_level_dwells_accumulate_against_float64(capi, engine):
     """max_dwells = 2 at 125 000 points (5 x [8, 5, 5, 5, 5, 5]): the grid and the CFAR input power (divided by the dwell
     counter) of two accumulated dwells."""
-    p = _params(125000, max_dwells=2)
+    p = _params(125000, max_dwells=2, n_code_slots=3)
     rng = np.random.default_rng(2)
     codes = _codes(rng, 3, 125000)
     placements = [(0, 1.0, 4321, 500.0), (1, 0.8, 99999, -1000.0), (2, 0.6, 7, -500.0)]
-    conf = _oracle(p).c
+    conf = ar.oracle(p).c
     iq1, iq2 = (_signal(rng, codes, conf, p["fs_in"], placements, noise=2.0) for _ in range(2))
     acq, _, refs = _search_all_slots(capi, engine, p, codes, iq1, dwell_inputs=[iq2])
-    errs = [_grid_err(acq, s, refs[s]) for s in range(3)]
+    errs = [ar.check_grid(acq.read_grid(s), refs[s]) for s in range(3)]
     print(f"grid error vs float64, N = 125000, two dwells: {max(errs):.3e} of the peak")
-    assert max(errs) < GRID_TOL
     acq.close()
 
 
@@ -249,14 +221,14 @@ def test_two_level_zero_padded_layout(capi, engine, cfar, keep_grid):
 def test_two_level_step_two_against_float64(capi, engine):
     """Step two at 175 000 points (7 x [8, 5, 5, 5, 5, 5]): 4 bins of 125 Hz around the step-one Doppler, the wipe-off rows
     of update_grid_doppler_wipeoffs_step2, the float Doppler formula and the step-one input power."""
-    p = _params(175000, keep_grid=True, slots=1)
+    p = _params(175000, keep_grid=True)
     rng = np.random.default_rng(175)
     code = _codes(rng, 1, 175000)
-    conf = _oracle(p).c
+    conf = ar.oracle(p).c
     iq1 = _signal(rng, code, conf, p["fs_in"], [(0, 1.0, 123456, 500.0)])
     acq, res, _ = _search_all_slots(capi, engine, p, code, iq1)
     first = res[0]
-    o = _oracle(p, num_doppler_bins_step2=4, doppler_step2=125.0)
+    o = ar.oracle(p, num_doppler_bins_step2=4, doppler_step2=125.0)
     o.doppler_center_step_two = np.float32(first["doppler"])
     o.update_grid_doppler_wipeoffs_step2()
     iq2 = _signal(rng, code, conf, p["fs_in"], [(0, 1.0, 123456, float(first["doppler"]) - 125.0)])
@@ -266,9 +238,9 @@ def test_two_level_step_two_against_float64(capi, engine):
     _assert_unique_peak(ref)
     o.step_two = True
     o.input_power = np.float32(first["input_power"])
-    _check(got, _ref_stats(o, ref), True, "step two")
+    ar.check(got, _ref_stats(o, ref), what="step two")
     assert int(got["doppler"]) == int(first["doppler"]) - 125
-    assert _grid_err(acq, 0, ref) < GRID_TOL   # as many step-two bins as step-one bins: the whole grid of the slot
+    ar.check_grid(acq.read_grid(0), ref)   # as many step-two bins as step-one bins: the whole grid of the slot
     acq.close()
 
 
@@ -287,13 +259,13 @@ def test_second_peak_exclusion_window(capi, engine, window_refs, n, spc, keep_gr
     (pcps_acquisition.cc:485-509), before its second arg-max.  Input: the code rolled by k plus half of it rolled by
     k + lag.  lag = -spc and spc - 1 fall inside the window, -spc - 1 and spc do not, so an off-by-one at either end moves
     second_peak from a sidelobe to a quarter of the peak or back."""
-    p = _params(n, spc=spc, cfar=False, keep_grid=keep_grid, slots=1)
+    p = _params(n, samples_per_chip=spc, use_CFAR_algorithm_flag=False, keep_grid=keep_grid)
     rng = np.random.default_rng(n + spc)
     code = _codes(rng, 1, n)[0]
     acq = capi.PcpsAcquisition(engine, **p)
     acq.set_local_code(0, code)
     wipe = acq.read_wipeoffs()
-    o = _oracle(p)
+    o = ar.oracle(p)
     for k in (0, 1, spc - 1, spc, n - spc - 1, n - spc, n - 1):
         for lag in (-spc - 1, -spc, spc - 1, spc):
             key = (n, spc, k, lag)
@@ -308,9 +280,9 @@ def test_second_peak_exclusion_window(capi, engine, window_refs, n, spc, keep_gr
             ratio = want["second_peak"] / want["grid_maximum"]
             assert (ratio < 0.01) if inside else (0.15 < ratio < 0.4), (k, lag, ratio)
             got = acq.search(iq, [0])[0]
-            _check(got, want, False, f"k = {k}, lag = {lag}")
+            ar.check(got, want, ar.PEAK_STATS, f"k = {k}, lag = {lag}")
             if keep_grid:
-                assert _grid_err(acq, 0, ref) < GRID_TOL
+                ar.check_grid(acq.read_grid(0), ref)
     acq.close()
 
 
@@ -323,7 +295,7 @@ def test_second_peak_exclusion_window(capi, engine, window_refs, n, spc, keep_gr
     122760,   # M = 245 760 = 10 x [8, 8, 8, 8, 2, 3]
 ])
 def test_chirp_z_selftest_dft_against_float64(capi, engine, n):
-    acq = capi.PcpsAcquisition(engine, **_params(n, slots=1))
+    acq = capi.PcpsAcquisition(engine, **_params(n))
     rng = np.random.default_rng(n)
     x = (rng.normal(size=n) + 1j * rng.normal(size=n)).astype(np.complex64)
     want = np.fft.fft(x.astype(np.complex128))
@@ -344,12 +316,11 @@ def test_chirp_z_largest_radix_search_against_float64(capi, engine, keep_grid):
 @pytest.mark.parametrize("n", [4000, 75000, 16368])   # single CTA, 3 x [8, 5, 5, 5, 5, 5], chirp-z
 def test_search_dev_leaves_what_search_returns(capi, engine, n):
     import torch
-    p = _params(n)
+    p = _params(n, n_code_slots=3)
     acq = capi.PcpsAcquisition(engine, **p)
     rng = np.random.default_rng(n)
     codes = _codes(rng, 3, n)
-    for s, c in enumerate(codes):
-        acq.set_local_code(s, c)
+    ar.load_codes(acq, codes)
     iq = _signal(rng, codes, acq.conf, p["fs_in"], [(1, 1.0, 77, 500.0), (0, 0.7, n // 3, 0.0)])
     want = acq.search(iq, [1, 2, 0])
     x = torch.from_numpy(iq.view(np.float32)).cuda()
@@ -363,19 +334,14 @@ def test_search_dev_leaves_what_search_returns(capi, engine, n):
 
 @pytest.mark.parametrize("n", [4000, 75000])   # single CTA, 3 x [8, 5, 5, 5, 5, 5]
 def test_search_i16_equals_search_on_widened_samples(capi, engine, n):
-    p = _params(n, slots=2)
+    p = _params(n, n_code_slots=2)
     acq = capi.PcpsAcquisition(engine, **p)
     rng = np.random.default_rng(n + 16)
     codes = _codes(rng, 2, n)
-    for s, c in enumerate(codes):
-        acq.set_local_code(s, c)
-    iq = _signal(rng, codes, acq.conf, p["fs_in"], [(0, 1.0, 1234, -500.0)], noise=1.0) * 300
-    raw = np.round(np.stack([iq.real, iq.imag], axis=1)).astype(np.int16).reshape(-1)
-    slots = np.array([1, 0], np.uint32)
-    got = np.zeros(2, capi.ACQ_RESULT_DTYPE)
-    assert capi.lib.b200_acq_search_i16(acq.h, raw.ctypes.data, slots.ctypes.data, 2, 1, got.ctypes.data) == 0
-    want = acq.search(raw[0::2].astype(np.float32) + 1j * raw[1::2].astype(np.float32), slots)
-    assert got.tobytes() == want.tobytes()
+    ar.load_codes(acq, codes)
+    raw = ar.to_int(_signal(rng, codes, acq.conf, p["fs_in"], [(0, 1.0, 1234, -500.0)], noise=1.0), np.int16, 300)
+    got = ar.search_i16(acq, raw, [1, 0])
+    assert got.tobytes() == acq.search(ar.from_int(raw), [1, 0]).tobytes()
     acq.close()
 
 
@@ -386,7 +352,7 @@ def test_sweep_best_dev_breaks_ties_like_best_peak(capi, engine, n, prns):
     the lowest PRN, then the lowest Doppler bin, then the lowest code phase, whatever order the results come in."""
     import torch
     from gnss_sdr_b200 import dist as bd
-    acq = capi.PcpsAcquisition(engine, **_params(4000, slots=1))
+    acq = capi.PcpsAcquisition(engine, **_params(4000))
     rng = np.random.default_rng(1000 * n + len(prns))
     res = np.zeros(max(n, 1), capi.ACQ_RESULT_DTYPE)
     res["test_statistics"] = rng.choice(np.float32([0.0, 2.5, 7.25]), res.size)

@@ -7,6 +7,7 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 
+import acq_rig as ar  # noqa: E402
 from gnss_synth import GPS_L1_FREQ, make_iq  # noqa: E402
 from trk_loop import run_tracking  # noqa: E402
 
@@ -22,8 +23,8 @@ def test_acquisition_to_tracking_chain(oracle):
 
     eng = capi.Engine(0)
     # ---- acquisition (the reference test's configuration: doppler_max 5000, step 100 would be 100 bins; 250 here)
-    acq = capi.PcpsAcquisition(eng, fs_in=int(fs), samples_per_ms=4000.0, samples_per_chip=3, doppler_max=5000, doppler_step=250)
-    acq.set_local_code(0, oracle.port.gps_ca_code_complex_sampled(prn, int(fs)))
+    acq = ar.make(capi, eng, fs, doppler_max=5000, doppler_step=250)
+    acq.set_local_code(0, ar.ca_code(oracle.port, prn, fs))
     r = acq.search(iq[:4000], [0])[0]
     acq.close()
     acq_delay = float(np.fmod(np.float32(r["index_time"]), np.float32(4000.0)))

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from gnss_synth import make_iq, trk_params_for
+import acq_rig as ar
 from gpu_fixtures import capi  # noqa: F401
 import trk_rig as tr
 
@@ -114,10 +115,8 @@ ACQ_FS, ACQ_N, DMAX, DSTEP = 25_000_000, 25000, 10000, 250     # C4's grid moved
 @pytest.fixture(scope="module")
 def c4(capi, oracle):
     eng = capi.Engine(0)
-    acq = capi.PcpsAcquisition(eng, fs_in=ACQ_FS, samples_per_ms=float(ACQ_N), samples_per_chip=24, doppler_max=DMAX, doppler_step=DSTEP,
-                               n_code_slots=32)
-    for p in range(1, 33):
-        acq.set_local_code(p - 1, oracle.port.gps_ca_code_complex_sampled(p, ACQ_FS))
+    acq = ar.make(capi, eng, ACQ_FS, doppler_max=DMAX, doppler_step=DSTEP, n_code_slots=32)
+    ar.load_codes(acq, [ar.ca_code(oracle.port, p, ACQ_FS) for p in range(1, 33)])
     present = [2, 5, 9, 13, 17, 21, 26, 30]
     rng = np.random.default_rng(8)
     codes = {p: oracle.port.gps_ca_code(p) for p in present}

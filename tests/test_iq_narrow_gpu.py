@@ -9,13 +9,14 @@ narrow band, and the device loops refuse narrow bands.
 import numpy as np
 import pytest
 
+from acq_rig import ERR_ARG, ERR_STATE
+import acq_rig as ar
 from gpu_fixtures import capi, engine, torch  # noqa: F401
 import trk_rig as tr
 from trk_ref import exact_taps, int_code
 
 pytestmark = pytest.mark.gpu
 
-ERR_ARG, ERR_STATE = -1, -4
 WIDTHS = {"ishort": np.int16, "ibyte": np.int8}
 
 
@@ -320,38 +321,12 @@ def test_retyped_band_takes_the_narrow_path(capi, item_type):
 
 
 # ---- acquisition band search --------------------------------------------------------------------------------------------
-def _acq(capi, engine, spms, *, cfar=True, keep_grid=False, dwells=1, bits=False, slots=2):
-    fs = int(round(spms * 1000))
-    return capi.PcpsAcquisition(engine, fs_in=fs, samples_per_ms=float(spms), samples_per_chip=max(1, int(fs / 1.023e6)),
-                                doppler_max=1000, doppler_step=500, use_CFAR_algorithm_flag=cfar, keep_grid=keep_grid,
-                                max_dwells=dwells, n_code_slots=slots, bit_transition_flag=bits)
-
-
-def _acq_stream(rng, n, code, fs, item_type):
-    t = np.arange(n)
-    x = np.resize(np.roll(code, int(rng.integers(0, code.size))), n) * np.exp(2j * np.pi * rng.uniform(-900, 900) / fs * t)
-    x = 0.5 * x + rng.normal(0, 1.0, n) + 1j * rng.normal(0, 1.0, n)
-    info = np.iinfo(WIDTHS[item_type])
-    scale = 3000.0 if item_type == "ishort" else 30.0
-    iq = np.empty(2 * n, WIDTHS[item_type])
-    iq[0::2] = np.clip(np.round(scale * x.real), info.min, info.max)
-    iq[1::2] = np.clip(np.round(scale * x.imag), info.min, info.max)
-    return iq
-
-
-def _grids(acq):
-    c = acq.conf
-    if not (c.keep_grid or c.max_dwells > 1):
-        return b""
-    return b"".join(acq.read_grid(s).tobytes() for s in range(c.n_code_slots))
-
-
 ACQ_CASES = [
     ("single4000_cfar", 4000, dict()),
-    ("single25000_peaks", 25000, dict(cfar=False)),
-    ("two50000_cfar_dwells", 50000, dict(dwells=2)),
-    ("chirpz16368_cfar_dwells", 16368, dict(dwells=2)),
-    ("chirpz5456_bits_grid", 5456, dict(bits=True, keep_grid=True)),
+    ("single25000_peaks", 25000, dict(use_CFAR_algorithm_flag=False)),
+    ("two50000_cfar_dwells", 50000, dict(max_dwells=2)),
+    ("chirpz16368_cfar_dwells", 16368, dict(max_dwells=2)),
+    ("chirpz5456_bits_grid", 5456, dict(bit_transition_flag=True, keep_grid=True)),
 ]
 
 
@@ -361,16 +336,13 @@ def test_band_search_equals_the_float_band(capi, engine, item_type, spms, opts):
     """The window straddles the ring's end and every dwell takes the next window; then b200_acq_search_band_submit and
     b200_acq_search_step_two_band on the same windows."""
     rng = np.random.default_rng(spms + len(opts) + len(item_type))
-    acqs = [_acq(capi, engine, spms, **opts) for _ in range(2)]
+    *acqs, codes = ar.pair(capi, engine, rng, 1000 * spms, **opts)
     c = acqs[0].conf
-    need = c.fft_size // 2 if c.code_layout == 1 else c.consumed_samples
-    codes = [rng.choice([-1.0, 1.0], need).astype(np.complex64) for _ in range(c.n_code_slots)]
-    for a in acqs:
-        for s, code in enumerate(codes):
-            a.set_local_code(s, code)
     n, dwells = c.consumed_samples, c.max_dwells
-    cap = 1 << (int(3 * n) - 1).bit_length()
-    iq = _acq_stream(rng, 2 * cap + 2 * n, np.resize(codes[1], n), c.fs_in, item_type)
+    cap = ar.pow2(3 * n)
+    info = np.iinfo(WIDTHS[item_type])
+    x = ar.stream(rng, 2 * cap + 2 * n, np.resize(codes[1], n), c.fs_in, np.complex128)
+    iq = ar.to_int(x, WIDTHS[item_type], 3000.0 if item_type == "ishort" else 30.0, clip=(info.min, info.max))
     engine.iq_create(6, cap)
     engine.iq_create(7, cap, item_type)
     for k in range(0, iq.size, 2 * (cap // 3 + 7)):
@@ -382,12 +354,12 @@ def test_band_search_equals_the_float_band(capi, engine, item_type, spms, opts):
         want = acqs[0].search_band(6, s0, [1, 0], dwell_counter=d)
         got = acqs[1].search_band(7, s0, [1, 0], dwell_counter=d)
         assert got.tobytes() == want.tobytes(), (d, got, want)
-    assert _grids(acqs[1]) == _grids(acqs[0])
+    assert ar.grids(acqs[1]) == ar.grids(acqs[0])
     acqs[0].search_band_submit(6, idx, [0, 1])
     want = acqs[0].search_wait()
     acqs[1].search_band_submit(7, idx, [0, 1])
     assert acqs[1].search_wait().tobytes() == want.tobytes()
-    if not opts.get("bits"):
+    if not opts.get("bit_transition_flag"):
         for a in acqs:
             a.set_step_two(100.0, 125.0, 4)
         want = acqs[0].search_step_two_band(6, idx, 1, 1.0)
