@@ -21,6 +21,7 @@ if not os.path.exists(LIB_PATH):
 lib = C.CDLL(LIB_PATH)
 
 B200_MAX_TAPS = 8
+B200_ACQ_MAX_RESAMPLER_TAPS = 1024
 ERRORS = {0: "OK", -1: "ERR_ARG", -2: "ERR_CUDA", -3: "ERR_NOMEM", -4: "ERR_STATE", -5: "ERR_RANGE", -6: "ERR_NODEV"}
 
 
@@ -88,6 +89,8 @@ _SIGS = {
     "b200_acq_search_band": ([_vp, C.c_int, C.c_uint64, _vp, C.c_uint32, C.c_uint32, _vp], C.c_int),
     "b200_acq_search_band_submit": ([_vp, C.c_int, C.c_uint64, _vp, C.c_uint32, C.c_uint32], C.c_int),
     "b200_acq_search_step_two_band": ([_vp, C.c_int, C.c_uint64, C.c_uint32, C.c_uint32, C.c_float, _vp], C.c_int),
+    "b200_acq_resampler_design": ([C.c_int64, C.c_int64, C.c_uint32, C.POINTER(C.c_uint32), _vp, C.POINTER(C.c_uint32)], C.c_int),
+    "b200_acq_set_band_resampler": ([_vp, C.c_uint32, _vp, C.c_uint32], C.c_int),
     "b200_acq_read_grid": ([_vp, C.c_uint32, _vp], C.c_int),
     "b200_acq_selftest_dft": ([_vp, _vp, _vp], C.c_int),
     "b200_acq_read_wipeoffs": ([_vp, _vp], C.c_int),
@@ -470,9 +473,21 @@ class PcpsAcquisition:
         _chk(lib.b200_acq_search_dev(self.h, in_dev_ptr, slots.ctypes.data, slots.size, dwell_counter, results_dev_ptr),
              "b200_acq_search_dev")
 
+    def set_band_resampler(self, decimation: int, taps):
+        """decimate the band searches' input by `decimation` through the FIR `taps` (acq_resampler_design); decimation 1
+        turns the resampler off.  The object works at the decimated rate, its bands hold the full rate."""
+        taps = np.ascontiguousarray(taps, np.float32)
+        _chk(lib.b200_acq_set_band_resampler(self.h, int(decimation), taps.ctypes.data if taps.size else None, taps.size),
+             "b200_acq_set_band_resampler")
+
     def search_band(self, band: int, abs_index: int, slots, dwell_counter: int = 1) -> np.ndarray:
         """search samples [abs_index, abs_index + consumed_samples) of one of the engine's bands; the result's sample stamp
-        for loop_start is abs_index + consumed_samples"""
+        for loop_start is abs_index + consumed_samples.  Dwell k takes the window k * consumed_samples further on.
+
+        With a band resampler of decimation D and T taps, the search reads [abs_index - (T - 1), abs_index + (consumed - 1) D
+        + 1) and searches y[j] = sum_k taps[k] x[abs_index + j D - k]; dwell k takes abs_index + k consumed D.  Mapped to the
+        full rate as the reference does (pcps_acquisition.cc:583-597): the sample stamp is abs_index + consumed D and the
+        delay fmod(index_time, samples_per_code) D - (T - 1) / 2."""
         slots = np.ascontiguousarray(slots, np.uint32)
         res = np.zeros(slots.size, ACQ_RESULT_DTYPE)
         _chk(lib.b200_acq_search_band(self.h, band, int(abs_index), slots.ctypes.data, slots.size, dwell_counter, res.ctypes.data),
@@ -480,7 +495,7 @@ class PcpsAcquisition:
         return res
 
     def search_band_submit(self, band: int, abs_index: int, slots, dwell_counter: int = 1):
-        """queue search_band's sweep; search_wait() collects its results"""
+        """queue search_band's sweep (the same window, resampler and stamp rules); search_wait() collects its results"""
         slots = np.ascontiguousarray(slots, np.uint32)
         _chk(lib.b200_acq_search_band_submit(self.h, band, int(abs_index), slots.ctypes.data, slots.size, dwell_counter),
              "b200_acq_search_band_submit")
@@ -543,6 +558,21 @@ def acq_dump_write(filename: str, grid: np.ndarray, *, doppler_max: int, doppler
     d.acq_doppler_hz, d.acq_delay_samples, d.test_statistic, d.threshold = acq_doppler_hz, acq_delay_samples, test_statistic, threshold
     d.input_power, d.doppler_step_narrow, d.doppler_grid_narrow_min, d.sample_counter = input_power, doppler_step_narrow, doppler_grid_narrow_min, sample_counter
     _chk(lib.b200_acq_dump_write(filename.encode(), C.byref(d)), "b200_acq_dump_write")
+
+
+def acq_resampler_design(fs_in: int, opt_acq_fs: int) -> tuple:
+    """-> (decimation, float32 taps): the acquisition resampler the reference inserts for a stream at fs_in and a signal
+    acquired at opt_acq_fs (gnss_flowgraph.cc:1117-1212); (1, no taps) where it inserts none"""
+    d, n = C.c_uint32(0), C.c_uint32(0)
+    rc = lib.b200_acq_resampler_design(int(fs_in), int(opt_acq_fs), 0, C.byref(d), None, C.byref(n))
+    if rc == 0:
+        return d.value, np.zeros(0, np.float32)
+    if rc != -5:
+        _chk(rc, "b200_acq_resampler_design")
+    taps = np.zeros(n.value, np.float32)
+    _chk(lib.b200_acq_resampler_design(int(fs_in), int(opt_acq_fs), taps.size, C.byref(d), taps.ctypes.data, C.byref(n)),
+         "b200_acq_resampler_design")
+    return d.value, taps
 
 
 def acq_dump_filename(base: str, system: str, signal: str, channel: int, dump_number: int, prn: int) -> str:

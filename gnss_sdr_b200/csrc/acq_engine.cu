@@ -48,6 +48,10 @@ struct b200_acq
     uint32_t pending_slots{0};
     bool pending{false};
     std::vector<int> slots_on_device;  // slot list last uploaded (sweeps usually repeat it)
+    // band-search resampler (b200_acq_set_band_resampler): band searches read a full-rate span and decimate it into in_dev
+    uint32_t decimation{1};            // 1: off
+    uint32_t n_taps{0};
+    DevBuf<float> resampler_taps;      // B200_ACQ_MAX_RESAMPLER_TAPS
     // Bluestein (chirp-z) path for transform sizes the mixed-radix planner cannot factor (e.g. 16 368 = 2^4 * 3 * 11 * 31):
     // every N-point DFT is a circular convolution with a chirp, done with M-point transforms (M >= 2N-1, two-level plan).
     struct Bluestein
@@ -297,6 +301,7 @@ int search_impl(b200_acq* a, AcqInput in, const uint32_t* slots, uint32_t n_slot
 
 // The samples of one search that returns its records to the host: consumed_samples complex values in the caller's memory,
 // as b200_cf32 or as I,Q-interleaved int16, or samples [abs_index, abs_index + consumed_samples) of one of the engine's bands
+// (with a band resampler set, the span decimate_band reads)
 struct SearchSource
 {
     enum Kind { kHostF32, kHostI16, kBand } kind;
@@ -473,16 +478,15 @@ extern "C"
         return rc;
     }
 
-    // The view of samples [abs_index, abs_index + consumed_samples) of one of the engine's bands, with a->stream made to wait
-    // for every write to the band queued so far.  The window check and the waits share one critical section of e->mu, so no
+    // The view of samples [abs_index, abs_index + n) of one of the engine's bands, with a->stream made to wait for every
+    // write to the band queued so far.  The window check and the waits share one critical section of e->mu, so no
     // push can be queued between them.  Float pushes and refills are copies on the copy stream (copy_done marks the latest);
     // integer pushes are converted on the compute stream, and raw_free[raw_last] follows the band's latest conversion.  The
     // search waits for those two events only, not for the whole compute stream, so it never queues behind tracking batches.
-    static int band_input(b200_acq* a, int band, uint64_t abs_index, AcqInput* in)
+    static int band_input(b200_acq* a, int band, unsigned long long abs_index, unsigned long long n, AcqInput* in)
     {
         if (band < 0 || band >= kMaxBands) return B200_ERR_ARG;
         b200_engine* e = a->e;
-        const unsigned long long n = a->c.consumed_samples;
         std::lock_guard<std::mutex> lk(e->mu);
         const Band& b = e->bands[band];
         if (!b.in_use)
@@ -506,6 +510,35 @@ extern "C"
         return B200_OK;
     }
 
+    // A band search through the resampler: the span [abs_index - (T - 1), abs_index + (consumed - 1) D + 1) of the band,
+    // filtered and decimated into in_dev, in_dev[j] = sum_k h[k] x[abs_index + j D - k]; one launch more than a plain band
+    // search, and a refused span launches nothing.
+    static int decimate_band(b200_acq* a, int band, uint64_t abs_index)
+    {
+        const uint64_t history = a->n_taps - 1, n_out = a->c.consumed_samples;
+        const uint64_t count = history + (n_out - 1) * a->decimation + 1;
+        if (abs_index < history)
+            {
+                set_error("band %d: the resampler's span of sample %llu starts %llu samples before index 0 (start at index >= %llu)", band,
+                    (unsigned long long)abs_index, (unsigned long long)(history - abs_index), (unsigned long long)history);
+                return B200_ERR_RANGE;
+            }
+        if (count > 0x7fffffffULL)
+            {
+                set_error("band %d: the resampler's span of %llu samples exceeds 2^31 - 1", band, (unsigned long long)count);
+                return B200_ERR_RANGE;
+            }
+        AcqInput span{};
+        int rc = band_input(a, band, abs_index - history, count, &span);
+        if (rc) return rc;
+        uint64_t launched = 0;
+        rc = acq_launch_decimate(span, a->resampler_taps, static_cast<int>(a->n_taps), static_cast<int>(a->decimation), static_cast<int>(n_out),
+            a->in_dev, launched, a->stream);
+        if (rc) return rc;
+        a->e->launches += launched;
+        return B200_OK;
+    }
+
     // Every search that returns its records to the host goes through here: refused while a sweep is in flight, it stages
     // the input, queues the search on a->stream and its n_slots records into results_pin, and records `done` for
     // b200_acq_search_wait.
@@ -516,7 +549,9 @@ extern "C"
         if (const int rc = check_no_search_in_flight(a)) return rc;
         B200_ENTER_DEVICE(a->e->device);
         AcqInput in = AcqInput::linear(a->in_dev);
-        int rc = src.kind == SearchSource::kBand ? band_input(a, src.band, src.abs_index, &in) : stage_host(a, src);
+        int rc = src.kind != SearchSource::kBand ? stage_host(a, src)
+                 : a->decimation > 1              ? decimate_band(a, src.band, src.abs_index)
+                                                  : band_input(a, src.band, src.abs_index, a->c.consumed_samples, &in);
         if (rc) return rc;
         rc = search_impl(a, in, slots, n_slots, dwell_counter, a->results_dev, step_two, prev_input_power);
         if (rc) return rc;
@@ -638,6 +673,37 @@ extern "C"
     {
         return search_and_wait(a, SearchSource{SearchSource::kBand, nullptr, band, abs_index}, &slot, 1, dwell_counter, 1, prev_input_power,
             result_host);
+    }
+
+    int b200_acq_set_band_resampler(b200_acq* a, uint32_t decimation, const float* taps, uint32_t n_taps)
+    {
+        if (!a) return B200_ERR_ARG;
+        if (const int rc = check_no_search_in_flight(a)) return rc;
+        if (decimation == 1)
+            {
+                a->decimation = 1;
+                a->n_taps = 0;
+                return B200_OK;
+            }
+        if (decimation == 0 || n_taps == 0 || !taps)
+            {
+                set_error("b200_acq_set_band_resampler: decimation %u with %u taps at %p", decimation, n_taps, static_cast<const void*>(taps));
+                return B200_ERR_ARG;
+            }
+        if (n_taps > B200_ACQ_MAX_RESAMPLER_TAPS)
+            {
+                set_error("b200_acq_set_band_resampler: %u taps, at most %d", n_taps, B200_ACQ_MAX_RESAMPLER_TAPS);
+                return B200_ERR_RANGE;
+            }
+        B200_ENTER_DEVICE(a->e->device);
+        if (!a->resampler_taps) B200_CUDA_TRY(a->resampler_taps.alloc(B200_ACQ_MAX_RESAMPLER_TAPS));
+        // synchronised: the caller's taps are free again on return, and no earlier search on the stream still reads the old ones
+        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
+        B200_CUDA_TRY(cudaMemcpyAsync(a->resampler_taps, taps, sizeof(float) * n_taps, cudaMemcpyHostToDevice, a->stream));
+        B200_CUDA_TRY(cudaStreamSynchronize(a->stream));
+        a->decimation = decimation;
+        a->n_taps = n_taps;
+        return B200_OK;
     }
 
     int b200_acq_sweep_best_dev(b200_acq* a, const b200_acq_result* results_dev, const uint32_t* prn_of_result_dev, uint32_t n_results,

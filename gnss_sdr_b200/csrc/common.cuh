@@ -308,4 +308,8 @@ int acq_launch_rows_times_vector(const float2* a, size_t a_stride, const float2*
     cudaStream_t st);
 int acq_launch_sweep_best(const b200_acq_result* results, const unsigned int* prn_of_result, int n, b200_acq_peak* out, uint64_t& launched,
     cudaStream_t st);
+// acquisition resampler (acq_resampler.cu): out[j] = sum_{k < n_taps} taps[k] * x(j * decimation + n_taps - 1 - k), j < n_out, for
+// the span x = in; every product and sum rounded on its own, k ascending.  n_taps <= B200_ACQ_MAX_RESAMPLER_TAPS.
+int acq_launch_decimate(AcqInput in, const float* taps, int n_taps, int decimation, int n_out, float2* out, uint64_t& launched,
+    cudaStream_t st);
 }  // namespace b200

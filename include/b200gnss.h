@@ -460,13 +460,52 @@ extern "C"
      *    b200_acq_search_dev is for).
      * b200_acq_search_band replaces b200_acq_search (synchronous); b200_acq_search_band_submit replaces
      * b200_acq_search_submit (results through b200_acq_search_wait, one search in flight per object);
-     * b200_acq_search_step_two_band replaces b200_acq_search_step_two. */
+     * b200_acq_search_step_two_band replaces b200_acq_search_step_two.
+     * With a band resampler set (b200_acq_set_band_resampler below), the window, the dwells and the sample stamp are
+     * those given there. */
     int b200_acq_search_band(b200_acq* a, int band, uint64_t abs_index, const uint32_t* slots, uint32_t n_slots,
         uint32_t dwell_counter, b200_acq_result* results_host);
     int b200_acq_search_band_submit(b200_acq* a, int band, uint64_t abs_index, const uint32_t* slots, uint32_t n_slots,
         uint32_t dwell_counter);
     int b200_acq_search_step_two_band(b200_acq* a, int band, uint64_t abs_index, uint32_t slot, uint32_t dwell_counter,
         float prev_input_power, b200_acq_result* result_host);
+    /* The acquisition resampler of GNSS-SDR.use_acquisition_resampler = true (gnss_flowgraph.cc:1117-1212): the reference
+     * acquires a signal from a full-rate stream at its optimal acquisition rate (2 Msps for GPS L1 C/A, Galileo E1 and L2C,
+     * 10 Msps for L5, E5a and E5b) through a decimating low-pass FIR, while tracking stays at the full rate.
+     *
+     * b200_acq_resampler_design: that filter for a stream at fs_in and a signal whose optimal rate is opt_acq_fs.  Host-only.
+     *  - *decimation = floor(fs_in / opt_acq_fs), lowered until it divides fs_in (:1164-1170).  When opt_acq_fs >= fs_in or
+     *    the decimation comes out as 1 the reference inserts nothing: *decimation = 1, *n_taps = 0, B200_OK.
+     *  - Otherwise the taps of gr::filter::firdes::low_pass(1.0, fs_in, fs_d / 2.1, fs_d / 2) with fs_d = fs_in / decimation:
+     *    Hamming window, ntaps = int(53 fs_in / (22 transition)) made odd, windowed sinc scaled to unit DC gain.  Computed
+     *    in double, returned as float.  The taps are symmetric; the filter's latency is (n_taps - 1) / 2 full-rate samples.
+     *  - More taps than max_taps is B200_ERR_RANGE with the count needed in b200_last_error() and in *n_taps (*decimation
+     *    is set too); taps may be NULL when max_taps is 0.
+     * The acquisition object for that signal is created at fs_in / decimation, with the sizes Acq_Conf::SetDerivedParams
+     * derives from that rate (acq_conf.cc:98-124). */
+#define B200_ACQ_MAX_RESAMPLER_TAPS 1024
+    int b200_acq_resampler_design(int64_t fs_in, int64_t opt_acq_fs, uint32_t max_taps, uint32_t* decimation, float* taps,
+        uint32_t* n_taps);
+    /* b200_acq_set_band_resampler: put the decimating filter taps[0..n_taps) in front of this object's band searches
+     * (b200_acq_search_band, _band_submit, _step_two_band).  The object works at the decimated rate; its bands hold the full
+     * rate.  Input sample j < consumed_samples of a band search becomes y[j] = sum_{k < n_taps} taps[k] x[abs_index + j D - k]
+     * (x: the band, D: decimation; k ascending from 0, every product and sum rounded to float on its own), so the search
+     * computes bit for bit what b200_acq_search computes on that float32 vector.  The filter runs once per search ahead of
+     * the forward stage: a decimated band search issues the kernels of b200_acq_search_dev plus one.
+     *  - The span read is [abs_index - (n_taps - 1), abs_index + (consumed_samples - 1) D + 1).  It must lie inside the
+     *    band's [valid_from, write_index), or the search is B200_ERR_RANGE with the span and the window in
+     *    b200_last_error() and nothing launched.  Samples before a band's first index are not zeros: start at
+     *    abs_index >= n_taps - 1.  Every band type works, and a span may wrap around the ring's end.
+     *  - Dwell k and step two take abs_index + k consumed_samples D.
+     *  - Mapping the result to the full rate is the host's (pcps_acquisition.cc:583-597): the sample stamp for
+     *    b200_trk_loop_start is abs_index + consumed_samples D, and the full-rate delay is
+     *    fmod(index_time, samples_per_code) D - (n_taps - 1) / 2.
+     *  - The host-input searches (b200_acq_search, _i16, _submit, _step_two*) and b200_acq_search_dev ignore the resampler:
+     *    their input is already at the object's rate.
+     * decimation == 1 turns the resampler off (taps and n_taps are then not read).  decimation == 0, n_taps == 0 or NULL
+     * taps is B200_ERR_ARG; n_taps > B200_ACQ_MAX_RESAMPLER_TAPS is B200_ERR_RANGE; a call while a sweep is in flight is
+     * B200_ERR_STATE.  The taps are copied to the device before the call returns. */
+    int b200_acq_set_band_resampler(b200_acq* a, uint32_t decimation, const float* taps, uint32_t n_taps);
     /* Multi-GPU cold start (SURVEY 8e): the PRN x Doppler grid is sharded by PRN; each rank reduces its sweep to ONE
      * 16-byte record on the device and the ranks exchange the records (an all-gather of N x 16 bytes over NVLink; the
      * host or a peer then takes the best, ties to the lowest PRN / bin / code phase as the reference's strict '>' scans).
