@@ -22,6 +22,8 @@ lib = C.CDLL(LIB_PATH)
 
 B200_MAX_TAPS = 8
 B200_ACQ_MAX_RESAMPLER_TAPS = 1024
+B200_IQ_MAX_CONDITIONER_TAPS = 4096
+B200_IQ_MAX_CONDITIONER_DECIMATION = 4096
 ERRORS = {0: "OK", -1: "ERR_ARG", -2: "ERR_CUDA", -3: "ERR_NOMEM", -4: "ERR_STATE", -5: "ERR_RANGE", -6: "ERR_NODEV"}
 
 
@@ -52,6 +54,9 @@ _SIGS = {
     "b200_iq_forget": ([_vp, C.c_int], C.c_int),
     "b200_trk_kernel_choice": ([_vp, C.c_int], C.c_int),
     "b200_iq_refill": ([_vp, C.c_int, _vp, C.c_uint64, C.c_uint64], C.c_int),
+    "b200_iq_read": ([_vp, C.c_int, C.c_uint64, C.c_uint64, _vp], C.c_int),
+    "b200_iq_set_conditioner": ([_vp, C.c_int, C.c_int, C.c_uint32, _vp, C.c_uint32, C.c_double, C.c_double], C.c_int),
+    "b200_iq_conditioner_lowpass": ([C.c_double, C.c_uint32, C.c_double, C.c_double, C.c_uint32, _vp, C.POINTER(C.c_uint32)], C.c_int),
     "b200_trk_set_taps": ([_vp, _vp], C.c_int),
     "b200_trk_set_local_code_and_taps_cplx": ([_vp, C.c_int, _vp, _vp], C.c_int),
     "b200_trk_correlate_cplx": ([_vp, _vp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, _vp], C.c_int),
@@ -143,6 +148,7 @@ class Engine:
         _chk(lib.b200_engine_create(C.byref(h), device, _vp(stream) if stream else None), "b200_engine_create")
         self.h = h
         self.device = device
+        self._band_types = {}   # item type of each band made by iq_create (iq_read's output format)
 
     def close(self):
         if self.h:
@@ -176,6 +182,7 @@ class Engine:
         """item_type: "gr_complex" (float samples), "ishort" or "ibyte" (interleaved int16 / int8 I,Q kept at their own
         width; such a band takes only iq_push_int / iq_push_file pushes of its own type)"""
         _chk(lib.b200_iq_create_typed(self.h, band, capacity, item_type.encode()), "b200_iq_create_typed")
+        self._band_types[band] = item_type
 
     def iq_push(self, band: int, iq: np.ndarray) -> int:
         iq = np.ascontiguousarray(iq, np.complex64)
@@ -232,7 +239,27 @@ class Engine:
         return first.value, n.value
 
     def iq_attach_dev(self, band: int, dev_ptr: int, n_samples: int, first_index: int = 0):
+        self._band_types[band] = "gr_complex"
         _chk(lib.b200_iq_attach_dev(self.h, band, dev_ptr, n_samples, first_index), "b200_iq_attach_dev")
+
+    def iq_read(self, band: int, abs_index: int, n: int) -> np.ndarray:
+        """samples [abs_index, abs_index + n) of the band's window in its own format: complex64 for a gr_complex band,
+        interleaved (I, Q) int16 / int8 (2 n values) for an ishort / ibyte band"""
+        fmt = self._band_types.get(band, "gr_complex")
+        out = np.zeros(n, np.complex64) if fmt == "gr_complex" else np.zeros(2 * n, np.int16 if fmt == "ishort" else np.int8)
+        _chk(lib.b200_iq_read(self.h, band, int(abs_index), int(n), out.ctypes.data if n else None), "b200_iq_read")
+        return out
+
+    def iq_set_conditioner(self, dst_band: int, src_band: int, decimation: int, taps, intermediate_freq_hz: float,
+                           sampling_freq_hz: float):
+        """fill dst_band with the frequency-translating decimating FIR of every push into src_band
+        (freq_xlating_fir_filter_ccf(decimation, taps, IF, fs)); empty taps remove dst_band's conditioner"""
+        taps = np.ascontiguousarray(taps, np.float32)
+        _chk(lib.b200_iq_set_conditioner(self.h, dst_band, src_band, int(decimation), taps.ctypes.data if taps.size else None,
+                                         taps.size, float(intermediate_freq_hz), float(sampling_freq_hz)), "b200_iq_set_conditioner")
+
+    def iq_remove_conditioner(self, dst_band: int):
+        _chk(lib.b200_iq_set_conditioner(self.h, dst_band, 0, 1, None, 0, 0.0, 1.0), "b200_iq_set_conditioner")
 
     # channels
     def channel_create(self, band: int, taps: int) -> int:
@@ -573,6 +600,19 @@ def acq_resampler_design(fs_in: int, opt_acq_fs: int) -> tuple:
     _chk(lib.b200_acq_resampler_design(int(fs_in), int(opt_acq_fs), taps.size, C.byref(d), taps.ctypes.data, C.byref(n)),
          "b200_acq_resampler_design")
     return d.value, taps
+
+
+def iq_conditioner_lowpass(sampling_freq_hz: float, decimation: int, bw_hz: float = 0.0, tw_hz: float = 0.0) -> np.ndarray:
+    """float32 taps of the input filter's filter_type = lowpass design (freq_xlating_fir_filter.cc:103-110): firdes::low_pass(1,
+    fs, bw, tw), bw = (fs / decimation) / 2 and tw = bw / 10 where not given (<= 0)"""
+    n = C.c_uint32(0)
+    rc = lib.b200_iq_conditioner_lowpass(float(sampling_freq_hz), int(decimation), float(bw_hz), float(tw_hz), 0, None, C.byref(n))
+    if rc != -5:
+        _chk(rc, "b200_iq_conditioner_lowpass")
+    taps = np.zeros(n.value, np.float32)
+    _chk(lib.b200_iq_conditioner_lowpass(float(sampling_freq_hz), int(decimation), float(bw_hz), float(tw_hz), taps.size,
+                                         taps.ctypes.data, C.byref(n)), "b200_iq_conditioner_lowpass")
+    return taps
 
 
 def acq_dump_filename(base: str, system: str, signal: str, channel: int, dump_number: int, prn: int) -> str:

@@ -481,8 +481,9 @@ extern "C"
     // The view of samples [abs_index, abs_index + n) of one of the engine's bands, with a->stream made to wait for every
     // write to the band queued so far.  The window check and the waits share one critical section of e->mu, so no
     // push can be queued between them.  Float pushes and refills are copies on the copy stream (copy_done marks the latest);
-    // integer pushes are converted on the compute stream, and raw_free[raw_last] follows the band's latest conversion.  The
-    // search waits for those two events only, not for the whole compute stream, so it never queues behind tracking batches.
+    // integer pushes are converted on the compute stream, and raw_free[raw_last] follows the band's latest conversion; a band
+    // a conditioner fills is written on the compute stream too, and cond_done follows its latest launch.  The search waits
+    // for those events only, not for the whole compute stream, so it never queues behind tracking batches.
     static int band_input(b200_acq* a, int band, unsigned long long abs_index, unsigned long long n, AcqInput* in)
     {
         if (band < 0 || band >= kMaxBands) return B200_ERR_ARG;
@@ -502,6 +503,7 @@ extern "C"
             }
         B200_CUDA_TRY(cudaStreamWaitEvent(a->stream, e->copy_done, 0));
         if (b.raw_last >= 0) B200_CUDA_TRY(cudaStreamWaitEvent(a->stream, b.raw_free[b.raw_last], 0));
+        if (b.cond_recorded) B200_CUDA_TRY(cudaStreamWaitEvent(a->stream, b.cond_done, 0));
         // a ring window may wrap around the ring's end; an attached buffer is linear from first_index (mask ~0), and the
         // window check keeps the window inside it.  A narrow band is read at its own width (AcqInput::at widens on load).
         const unsigned long long off = (abs_index - b.first_index) & b.mask;

@@ -1,9 +1,10 @@
 // The acquisition resampler of GNSS-SDR.use_acquisition_resampler (src/core/receiver/gnss_flowgraph.cc:1117-1212): a
 // decimating low-pass FIR between the signal conditioner and a signal's acquisition blocks, so acquisition runs at the
 // signal's optimal acquisition rate while tracking keeps the full rate.  b200_acq_resampler_design restates the filter
-// design (host only); acq_launch_decimate is the filter itself, run once per band search ahead of its forward stage.
+// design (host only) through firdes_low_pass, which b200_iq_conditioner_lowpass shares; acq_launch_decimate is the filter itself, run once per band search ahead of its forward stage.
 #include "common.cuh"
 
+#include <climits>
 #include <cmath>
 
 using namespace b200;
@@ -40,6 +41,28 @@ __global__ void __launch_bounds__(256) acq_decimate_kernel(AcqInput in, const fl
 
 namespace b200
 {
+long long firdes_low_pass(double fs, double cutoff, double transition, long long max_taps, float* taps)
+{
+    const double count = kHammingAttenuationDb * fs / (22.0 * transition);
+    if (!(count < 0x1p62)) return LLONG_MAX;  // no buffer holds that many
+    long long nt = static_cast<long long>(count);
+    if ((nt & 1) == 0) nt++;
+    if (nt > max_taps) return nt;
+    const long long m = (nt - 1) / 2;
+    const double pi = 3.14159265358979323846;
+    const double fwT0 = 2.0 * pi * cutoff / fs;
+    // taps[M + n] = w[M + n] sin(n fwT0) / (n pi), taps[M] = w[M] fwT0 / pi; Hamming w[i] = 0.54 - 0.46 cos(2 pi i / (ntaps - 1))
+    const auto windowed_sinc = [&](long long n) {
+        const double w = 0.54 - 0.46 * std::cos(2.0 * pi * static_cast<double>(n + m) / static_cast<double>(nt - 1));
+        return w * (n == 0 ? fwT0 / pi : std::sin(static_cast<double>(n) * fwT0) / (static_cast<double>(n) * pi));
+    };
+    double dc_gain = 0.0;
+    for (long long n = -m; n <= m; n++) dc_gain += windowed_sinc(n);
+    // scaled to unit DC gain in double, each tap rounded once to float
+    for (long long n = -m; n <= m; n++) taps[n + m] = static_cast<float>(windowed_sinc(n) / dc_gain);
+    return nt;
+}
+
 int acq_launch_decimate(AcqInput in, const float* taps, int n_taps, int decimation, int n_out, float2* out, uint64_t& launched,
     cudaStream_t st)
 {
@@ -72,9 +95,7 @@ extern "C"
         // firdes::low_pass(1.0, fs, acq_fs_dec / 2.1, acq_fs_dec / 2) with the Hamming window, in double
         const double fs = static_cast<double>(fs_in);
         const double acq_fs_dec = fs / static_cast<double>(d);
-        const double cutoff = acq_fs_dec / 2.1, transition = acq_fs_dec / 2.0;
-        int64_t nt = static_cast<int64_t>(kHammingAttenuationDb * fs / (22.0 * transition));
-        if ((nt & 1) == 0) nt++;
+        const int64_t nt = firdes_low_pass(fs, acq_fs_dec / 2.1, acq_fs_dec / 2.0, max_taps, taps);
         if (d > UINT32_MAX || nt > UINT32_MAX)
             {
                 set_error("b200_acq_resampler_design: decimation %lld with %lld taps is out of range", (long long)d, (long long)nt);
@@ -87,18 +108,6 @@ extern "C"
                 set_error("b200_acq_resampler_design: %lld taps needed (decimation %lld), max_taps is %u", (long long)nt, (long long)d, max_taps);
                 return B200_ERR_RANGE;
             }
-        const int64_t m = (nt - 1) / 2;
-        const double pi = 3.14159265358979323846;
-        const double fwT0 = 2.0 * pi * cutoff / fs;
-        // taps[M + n] = w[M + n] sin(n fwT0) / (n pi), taps[M] = w[M] fwT0 / pi; Hamming w[i] = 0.54 - 0.46 cos(2 pi i / (ntaps - 1))
-        const auto windowed_sinc = [&](int64_t n) {
-            const double w = 0.54 - 0.46 * std::cos(2.0 * pi * static_cast<double>(n + m) / static_cast<double>(nt - 1));
-            return w * (n == 0 ? fwT0 / pi : std::sin(static_cast<double>(n) * fwT0) / (static_cast<double>(n) * pi));
-        };
-        double dc_gain = 0.0;
-        for (int64_t n = -m; n <= m; n++) dc_gain += windowed_sinc(n);
-        // scaled to unit DC gain in double, each tap rounded once to float
-        for (int64_t n = -m; n <= m; n++) taps[n + m] = static_cast<float>(windowed_sinc(n) / dc_gain);
         return B200_OK;
     }
 }

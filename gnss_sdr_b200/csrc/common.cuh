@@ -202,6 +202,21 @@ namespace b200
 // sample-type adapters (ingest_kernels.cu)
 int launch_convert_i16(const short* raw, float2* ring, unsigned long long mask, unsigned long long dst_off, unsigned long long n, cudaStream_t st);
 int launch_convert_i8(const signed char* raw, float2* ring, unsigned long long mask, unsigned long long dst_off, unsigned long long n, cudaStream_t st);
+
+// signal conditioner (iq_conditioner.cu): outputs [j0, j0 + n_out) of b200_iq_set_conditioner's filter from the ring src (slot
+// mask src_mask, SampleFormat src_fmt) into the float ring dst.  taps: the n_taps composite taps c[k]; real_taps: IF = 0 (c[k]
+// real, no rotator); (rot_hi, rot_lo): cond_rotator_step's phase step per output.  n_out == 0 launches nothing.
+int launch_iq_condition(const void* src, int src_fmt, unsigned long long src_mask, const float2* taps, int n_taps, int decimation,
+    unsigned long long j0, unsigned long long n_out, int real_taps, unsigned long long rot_hi, unsigned long long rot_lo, float2* dst,
+    unsigned long long dst_mask, cudaStream_t st);
+// decimation * intermediate_freq_hz / sampling_freq_hz mod 1 (cycles per output) as a 128-bit binary fraction, computed exactly
+// from the two doubles; sampling_freq_hz > 0
+void cond_rotator_step(double intermediate_freq_hz, double sampling_freq_hz, unsigned decimation, unsigned long long* hi,
+    unsigned long long* lo);
+// gr::filter::firdes::low_pass(1.0, fs, cutoff, transition) with the Hamming window, in double (acq_resampler.cu): returns the
+// tap count int(53 fs / (22 transition)) made odd, and writes the taps, each rounded once to float, only when that count is
+// <= max_taps
+long long firdes_low_pass(double fs, double cutoff, double transition, long long max_taps, float* taps);
 }  // namespace b200
 
 // ---- acquisition launchers (acq_kernels.cu) ----------------------------------------------------------

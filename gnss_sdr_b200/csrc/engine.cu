@@ -6,6 +6,7 @@
 #include "common.cuh"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -229,6 +230,90 @@ extern "C"
         return B200_OK;
     }
 
+    // ---- signal conditioners (b200_iq_set_conditioner) ------------------------------------------------------------
+    static unsigned long long ceil_div(unsigned long long a, unsigned long long d) { return a / d + (a % d != 0); }
+
+    // the largest tap count among the conditioners that read `band` (0: none feeds from it)
+    static unsigned conditioner_taps(const b200_engine* e, int band)
+    {
+        unsigned t = 0;
+        for (const Band& d : e->bands)
+            if (d.cond.src == band) t = std::max(t, d.cond.n_taps);
+        return t;
+    }
+
+    // caller holds e->mu: the window of a conditioned band follows its source's: write_index = ceil(src write_index / D),
+    // valid_from = 0 at stream start, else ceil((src valid_from + T - 1) / D), never below cond.floor nor above write_index
+    static void conditioned_window(b200_engine* e, Band& d)
+    {
+        const Band& s = e->bands[d.cond.src];
+        const unsigned long long dec = d.cond.decimation;
+        d.write_index = ceil_div(s.write_index, dec);
+        const unsigned long long rule = s.valid_from == 0 ? 0 : ceil_div(s.valid_from + d.cond.n_taps - 1, dec);
+        d.valid_from = std::min(std::max(rule, d.cond.floor), d.write_index);
+    }
+
+    // caller holds e->mu: the source `band` moved its valid_from (a push_at gap or restart, b200_iq_forget): its
+    // destinations' windows follow, and a restarted stream is valid again from its own start
+    static void source_restarted(b200_engine* e, int band)
+    {
+        for (Band& d : e->bands)
+            if (d.cond.src == band)
+                {
+                    d.cond.floor = 0;
+                    conditioned_window(e, d);
+                }
+    }
+
+    // caller holds e->mu: `band` (re-created or attached) is neither end of a conditioner any more
+    static void drop_conditioners(b200_engine* e, int band)
+    {
+        e->bands[band].cond.src = -1;
+        for (Band& d : e->bands)
+            if (d.cond.src == band) d.cond.src = -1;
+    }
+
+    static int record_cond_done(Band& b, cudaStream_t st)
+    {
+        if (!b.cond_done) B200_CUDA_TRY(b.cond_done.create(cudaEventDisableTiming));
+        B200_CUDA_TRY(cudaEventRecord(b.cond_done, st));
+        b.cond_recorded = true;
+        return B200_OK;
+    }
+
+    // caller holds e->mu: `band` has been written up to its write_index from old_write.  Each conditioner that reads it
+    // launches once for its newly complete outputs [ceil(old_write / D), ceil(write_index / D)) on the compute stream, and
+    // cond_done marks that launch on its destination and the last one on the source.  No conditioner: nothing is issued.
+    static int run_conditioners(b200_engine* e, int band, unsigned long long old_write)
+    {
+        Band& s = e->bands[band];
+        bool launched = false;
+        for (Band& d : e->bands)
+            {
+                if (d.cond.src != band) continue;
+                const unsigned long long dec = d.cond.decimation, j0 = ceil_div(old_write, dec), j1 = ceil_div(s.write_index, dec);
+                if (j1 > j0)
+                    {
+                        const int rc = launch_iq_condition(s.dev, s.fmt, s.mask, d.cond.taps, static_cast<int>(d.cond.n_taps), static_cast<int>(dec), j0,
+                            j1 - j0, d.cond.real_taps, d.cond.rot_hi, d.cond.rot_lo, reinterpret_cast<float2*>(d.dev.get()), d.mask, e->stream);
+                        if (rc) return rc;
+                        e->launches++;
+                        if (const int rc2 = record_cond_done(d, e->stream)) return rc2;
+                        launched = true;
+                    }
+                conditioned_window(e, d);
+            }
+        return launched ? record_cond_done(s, e->stream) : B200_OK;
+    }
+
+    // B200_OK, or B200_ERR_STATE with the error text when a conditioner fills `band`
+    static int check_not_conditioned(const Band& b, int band)
+    {
+        if (b.cond.src < 0) return B200_OK;
+        set_error("band %d is filled by its conditioner from band %d: it takes no pushes of its own", band, b.cond.src);
+        return B200_ERR_STATE;
+    }
+
     // ---- bands -----------------------------------------------------------------------------
     // caller holds e->mu; before the band is re-created or attached: queued launches may still read its owned ring
     static int release_owned_ring(b200_engine* e, Band& b)
@@ -254,6 +339,7 @@ extern "C"
         B200_ENTER_DEVICE(e->device);
         Band& b = e->bands[band];
         if (const int rc = release_owned_ring(e, b)) return rc;
+        drop_conditioners(e, band);
         const unsigned long long cap = next_pow2(capacity_samples);
         cudaError_t err = b.dev.alloc(cap * 2ULL * fmt);
         if (err != cudaSuccess)
@@ -303,16 +389,27 @@ extern "C"
         Band& b = e->bands[band];
         if (const int rc = b.check_owned_ring(band)) return rc;
         if (const int rc = check_push_format(b, band, fmt)) return rc;
+        if (const int rc = check_not_conditioned(b, band)) return rc;
         if (n > b.capacity)
             {
                 set_error("push of %llu samples exceeds ring capacity %llu", (unsigned long long)n, b.capacity);
                 return B200_ERR_RANGE;
             }
+        if (const unsigned taps = conditioner_taps(e, band))
+            if (n > b.capacity - (taps - 1))
+                {
+                    set_error("push of %llu samples into band %d: its conditioners' %u-tap history must stay in the ring, at most %llu per push",
+                        (unsigned long long)n, band, taps, b.capacity - (taps - 1));
+                    return B200_ERR_RANGE;
+                }
         B200_ENTER_DEVICE(e->device);
         if (first_index) *first_index = b.write_index;
         if (n == 0) return B200_OK;
+        const unsigned long long old_write = b.write_index;
         if (fmt == b.fmt)
             {
+                // slots that a conditioner launch queued by an earlier push still reads are overwritten only after it
+                if (b.cond_recorded) B200_CUDA_TRY(cudaStreamWaitEvent(e->copy_stream, b.cond_done, 0));
                 const int rc = copy_in(e, b.dev, b.capacity, b.write_index & b.mask, host, n, 2 * static_cast<size_t>(fmt));
                 if (rc) return rc;
             }
@@ -344,7 +441,7 @@ extern "C"
                 b.raw_last = k;
             }
         b.write_index += n;
-        return B200_OK;
+        return run_conditioners(e, band, old_write);
     }
 
     int b200_iq_push(b200_engine* e, int band, const b200_cf32* host, uint64_t n, uint64_t* first_index)
@@ -375,6 +472,7 @@ extern "C"
             Band& b = e->bands[band];
             if (const int rc = b.check_owned_ring(band)) return rc;
             if (const int rc = check_push_format(b, band, kCf32)) return rc;
+            if (const int rc = check_not_conditioned(b, band)) return rc;
             // what the ring holds right now
             const unsigned long long lo = b.window_lo();
             if (abs_index >= lo && abs_index + n <= b.write_index) return B200_OK;  // every sample of this block is already in the band
@@ -384,6 +482,7 @@ extern "C"
                     // index (a new capture, a test): what the ring held is history, the band restarts at abs_index
                     b.valid_from = abs_index;
                     b.write_index = abs_index;
+                    source_restarted(e, band);
                 }
             skip = b.write_index - abs_index;
         }
@@ -400,6 +499,8 @@ extern "C"
         Band& b = e->bands[band];
         if (!b.in_use || b.attached) return B200_ERR_STATE;
         b.valid_from = b.write_index;
+        if (b.cond.src >= 0) b.cond.floor = b.write_index;
+        source_restarted(e, band);
         return B200_OK;
     }
 
@@ -421,15 +522,18 @@ extern "C"
         SampleFormat fmt;
         if (const int rc = parse_item_type(item_type, "iq_push_file", &fmt)) return rc;
         unsigned long long capacity;
+        unsigned history;
         {
             std::lock_guard<std::mutex> lk(e->mu);
             const Band& b = e->bands[band];
             if (const int rc = b.check_owned_ring(band)) return rc;
             if (const int rc = check_push_format(b, band, fmt)) return rc;
             capacity = b.capacity;
+            history = conditioner_taps(e, band);
         }
         if (chunk_samples == 0) chunk_samples = 1ULL << 20;
         if (chunk_samples > capacity / 2) chunk_samples = capacity / 2 ? capacity / 2 : 1;
+        if (history > 1 && chunk_samples > capacity - (history - 1)) chunk_samples = capacity - (history - 1);
         B200_ENTER_DEVICE(e->device);
         FILE* f = std::fopen(path, "rb");
         if (!f)
@@ -499,6 +603,7 @@ extern "C"
         std::lock_guard<std::mutex> lk(e->mu);
         Band& b = e->bands[band];
         if (const int rc = release_owned_ring(e, b)) return rc;
+        drop_conditioners(e, band);
         b.base = dev;
         b.fmt = kCf32;
         b.capacity = n_samples;
@@ -540,6 +645,105 @@ extern "C"
             }
         b.valid_from = first_index;
         b.write_index = first_index + n;
+        return B200_OK;
+    }
+
+    int b200_iq_read(b200_engine* e, int band, uint64_t abs_index, uint64_t n, void* host)
+    {
+        if (!e || band < 0 || band >= kMaxBands || (!host && n)) return B200_ERR_ARG;
+        std::lock_guard<std::mutex> lk(e->mu);
+        const Band& b = e->bands[band];
+        if (!b.in_use)
+            {
+                set_error("band %d holds no samples (call b200_iq_create or b200_iq_attach_dev)", band);
+                return B200_ERR_STATE;
+            }
+        if (!b.holds(abs_index, n))
+            {
+                set_error("band %d: samples [%llu, %llu) are outside the band's window [%llu, %llu)", band, (unsigned long long)abs_index,
+                    (unsigned long long)(abs_index + n), b.window_lo(), b.write_index);
+                return B200_ERR_RANGE;
+            }
+        if (n == 0) return B200_OK;
+        B200_ENTER_DEVICE(e->device);
+        // every write into a band is ordered before later work on the compute stream (copy_in, conversions, conditioners)
+        const size_t item = 2 * static_cast<size_t>(b.fmt);
+        const unsigned long long off = (abs_index - b.first_index) & b.mask;
+        const unsigned long long first = std::min<unsigned long long>(n, b.capacity - off);
+        B200_CUDA_TRY(cudaMemcpyAsync(host, static_cast<const char*>(b.base) + off * item, first * item, cudaMemcpyDeviceToHost, e->stream));
+        if (n > first)
+            B200_CUDA_TRY(cudaMemcpyAsync(static_cast<char*>(host) + first * item, b.base, (n - first) * item, cudaMemcpyDeviceToHost, e->stream));
+        B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
+        return B200_OK;
+    }
+
+    int b200_iq_set_conditioner(b200_engine* e, int dst_band, int src_band, uint32_t decimation, const float* taps, uint32_t n_taps,
+        double intermediate_freq_hz, double sampling_freq_hz)
+    {
+        if (!e || dst_band < 0 || dst_band >= kMaxBands) return B200_ERR_ARG;
+        if (n_taps == 0)
+            {
+                std::lock_guard<std::mutex> lk(e->mu);
+                e->bands[dst_band].cond.src = -1;
+                return B200_OK;
+            }
+        if (src_band < 0 || src_band >= kMaxBands || !taps || decimation < 1 || !(sampling_freq_hz > 0.0) || !std::isfinite(sampling_freq_hz) ||
+            !std::isfinite(intermediate_freq_hz))
+            {
+                set_error("iq_set_conditioner: band %d, decimation %u, taps %s, fs %g Hz, IF %g Hz: bad argument", src_band, decimation,
+                    taps ? "set" : "NULL", sampling_freq_hz, intermediate_freq_hz);
+                return B200_ERR_ARG;
+            }
+        if (dst_band == src_band)
+            {
+                set_error("iq_set_conditioner: band %d cannot condition into itself", dst_band);
+                return B200_ERR_ARG;
+            }
+        if (n_taps > B200_IQ_MAX_CONDITIONER_TAPS || decimation > B200_IQ_MAX_CONDITIONER_DECIMATION)
+            {
+                set_error("iq_set_conditioner: %u taps, decimation %u: at most %d taps and decimation %d", n_taps, decimation,
+                    B200_IQ_MAX_CONDITIONER_TAPS, B200_IQ_MAX_CONDITIONER_DECIMATION);
+                return B200_ERR_RANGE;
+            }
+        std::lock_guard<std::mutex> lk(e->mu);
+        Band& d = e->bands[dst_band];
+        const Band& s = e->bands[src_band];
+        if (const int rc = s.check_owned_ring(src_band)) return rc;
+        if (const int rc = d.check_owned_ring(dst_band)) return rc;
+        if (d.fmt != kCf32)
+            {
+                set_error("iq_set_conditioner: band %d holds %s samples: a conditioner writes gr_complex", dst_band, item_type_name(d.fmt));
+                return B200_ERR_STATE;
+            }
+        if (conditioner_taps(e, dst_band) > 0 || s.cond.src >= 0)
+            {
+                set_error("iq_set_conditioner: band %d -> band %d would chain conditioners", src_band, dst_band);
+                return B200_ERR_STATE;
+            }
+        if (d.capacity * decimation < s.capacity || s.capacity < n_taps)
+            {
+                set_error("iq_set_conditioner: band %d (%llu samples) must hold band %d's %llu samples decimated by %u, and band %d at least %u taps",
+                    dst_band, d.capacity, src_band, s.capacity, decimation, src_band, n_taps);
+                return B200_ERR_RANGE;
+            }
+        B200_ENTER_DEVICE(e->device);
+        // c[k] = h[k] e^{+i k w}, w = 2 pi IF / fs, in double, each component rounded once to float
+        const double pi = 3.14159265358979323846;
+        const double w = 2.0 * pi * intermediate_freq_hz / sampling_freq_hz;
+        std::vector<float2> c(n_taps);
+        for (uint32_t k = 0; k < n_taps; k++)
+            c[k] = make_float2(static_cast<float>(taps[k] * std::cos(k * w)), static_cast<float>(taps[k] * std::sin(k * w)));
+        B200_CUDA_TRY(cudaStreamSynchronize(e->stream));  // launches already queued may still read the old taps
+        if (!d.cond.taps.fits(n_taps)) B200_CUDA_TRY(d.cond.taps.alloc(n_taps));
+        B200_CUDA_TRY(cudaMemcpyAsync(d.cond.taps, c.data(), sizeof(float2) * n_taps, cudaMemcpyHostToDevice, e->stream));
+        B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
+        d.cond.src = src_band;
+        d.cond.decimation = decimation;
+        d.cond.n_taps = n_taps;
+        d.cond.real_taps = intermediate_freq_hz == 0.0;
+        cond_rotator_step(intermediate_freq_hz, sampling_freq_hz, decimation, &d.cond.rot_hi, &d.cond.rot_lo);
+        d.cond.floor = ceil_div(s.write_index, decimation);  // set mid-stream: the destination starts empty there
+        conditioned_window(e, d);
         return B200_OK;
     }
 

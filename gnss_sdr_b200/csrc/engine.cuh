@@ -32,6 +32,19 @@ struct Band
     CudaEvent raw_free[2];  // conversion that read the buffer has finished
     int raw_next{0};
     int raw_last{-1};       // raw_free[raw_last] is recorded right after the band's latest conversion (-1: none yet)
+    // the signal conditioner that fills this band from another (b200_iq_set_conditioner); src < 0: none
+    struct Conditioner
+    {
+        int src{-1};
+        unsigned decimation{1};
+        unsigned n_taps{0};
+        bool real_taps{true};                // IF = 0: real taps, no rotator
+        unsigned long long rot_hi{0}, rot_lo{0};  // cond_rotator_step
+        unsigned long long floor{0};         // no output below this is valid: where the conditioner was set or the band forgotten
+        DevBuf<float2> taps;                 // composite taps c[k]
+    } cond;
+    CudaEvent cond_done;        // recorded on the compute stream after the latest conditioner launch that read or wrote the band
+    bool cond_recorded{false};  // cond_done has been recorded
 
     // B200_OK, or B200_ERR_STATE with the error text when this is not a ring made by b200_iq_create
     int check_owned_ring(int band) const

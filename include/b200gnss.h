@@ -131,6 +131,65 @@ extern "C"
      * and NCCL broadcasts that buffer to the peers over NVLink (bench.py, SURVEY 8e). */
     int b200_iq_refill(b200_engine* e, int band, const b200_cf32* host, uint64_t n, uint64_t first_index);
 
+    /* Copy samples [abs_index, abs_index + n) of a band to host memory in the band's own item format (8 B per gr_complex
+     * sample, 4 B per ishort, 2 B per ibyte sample), after every write to the band queued so far; synchronous.  What the
+     * reference's input filter writes to its dump file (freq_xlating_fir_filter.cc:171-176, 192-194), read back from a conditioned
+     * band.  The samples must lie inside b200_iq_window, else B200_ERR_RANGE; an unused band is B200_ERR_STATE. */
+    int b200_iq_read(b200_engine* e, int band, uint64_t abs_index, uint64_t n, void* host);
+
+    /* ---- signal conditioner: frequency-translating decimating FIR on the device ------------------------------------
+     * InputFilter.implementation = Freq_Xlating_Fir_Filter (src/algorithms/input_filter/adapters/freq_xlating_fir_filter.cc
+     * :56-119), which instantiates gr::filter::freq_xlating_fir_filter_ccf(D, h, IF, fs) (:119): a receiver with a wideband
+     * or IF front end moves the signal to baseband, low-pass filters and decimates it, and tracks at the filtered rate.
+     *
+     * b200_iq_set_conditioner links src_band to dst_band: every write into the source (b200_iq_push, _push_i16, _push_i8,
+     * _push_at, _push_file) also fills the destination with, in absolute stream indices,
+     *     y[j] = r(j) sum_{k=0}^{T-1} c[k] x[j D - k],   x[m < 0] = 0,
+     *     c[k] = h[k] e^{+i k w},   r(j) = e^{-i w D j},   w = 2 pi IF / fs,
+     * T = n_taps, D = decimation, h = taps.  The zero history below index 0 is the block's own at stream start, so
+     * destination index j is the reference conditioner's j-th output and sample stamps line up with a reference flowgraph.
+     *  - The composite taps c[k] are computed on the host in double and rounded once to float.  The sum runs k ascending
+     *    from zero, every float product and sum rounded on its own: at IF = 0 (c = h, r = 1) the output is bit for bit that
+     *    float32 loop.  Otherwise the sum is complex, (c.re x.re - c.im x.im) and (c.re x.im + c.im x.re) per tap, and y is
+     *    the sum times r(j) in double, rounded once to float.
+     *  - r(j) is computed per output from its absolute index j: D IF / fs mod 1 is taken exactly from the two doubles as a
+     *    128-bit binary fraction q, phi(j) = j q mod 1 (top 64 bits, exact for every j < 2^64), r(j) = cos(2 pi phi) -
+     *    i sin(2 pi phi) in double.  GNU Radio instead advances a float rotator output by output (gr::blocks::rotator),
+     *    whose phase error grows with the stream; this one does not, so outputs past 2^32 are as accurate as the first.
+     *  - The source may be a gr_complex, ishort or ibyte owned ring (integers are widened exactly at load); the
+     *    destination must be a gr_complex owned ring whose capacity times D is at least the source's capacity.  One source
+     *    may feed several destinations (GPS L1 and Galileo E1 at different IFs); a destination cannot also be a source,
+     *    nor a source a destination.  Attached bands (b200_iq_attach_dev) are refused at either end.
+     *  - After a push, each conditioner of the source launches once, on the engine's compute stream, for the outputs that
+     *    became complete, [ceil(old_write / D), ceil(new_write / D)); a band search, batch or loop run issued after the
+     *    push reads them, with no host synchronisation.  The next push's copy into the source waits for that launch.
+     *  - The destination's window: write_index = ceil(src write_index / D); valid_from = 0 while the source's valid_from
+     *    is 0 (stream start), else ceil((src valid_from + T - 1) / D), and never below where the conditioner was set or the
+     *    destination was last b200_iq_forget-ed (an empty window while fewer outputs exist).  So a b200_iq_push_at gap or
+     *    a b200_iq_forget on the source opens a gap in the destination, and the loops stall there as on any band.  Set on
+     *    a source that already holds samples, the destination starts empty at ceil(src write_index / D).
+     *  - While a conditioner is set, a direct push or push_at into its destination is B200_ERR_STATE, and a push into its
+     *    source of more than capacity - (T - 1) samples is B200_ERR_RANGE (the filter's history must still be in the ring).
+     *  - n_taps == 0 removes the destination's conditioner (src_band, taps and the rest are then not read); so does
+     *    re-creating or attaching either band.  Setting a conditioner on a destination that has one replaces it.
+     *  - Refused, with nothing launched and both windows unchanged: decimation < 1 or NULL taps (B200_ERR_ARG),
+     *    decimation > B200_IQ_MAX_CONDITIONER_DECIMATION or n_taps > B200_IQ_MAX_CONDITIONER_TAPS (B200_ERR_RANGE),
+     *    sampling_freq_hz <= 0 or a frequency that is not finite (B200_ERR_ARG), dst_band == src_band (B200_ERR_ARG),
+     *    a band that is not an owned ring, a narrow destination, or a chain (B200_ERR_STATE), a destination too small
+     *    (B200_ERR_RANGE).
+     * The pm_remez band-pass design of the adapter's default filter_type is not restated: pass its taps. */
+#define B200_IQ_MAX_CONDITIONER_TAPS 4096
+#define B200_IQ_MAX_CONDITIONER_DECIMATION 4096
+    int b200_iq_set_conditioner(b200_engine* e, int dst_band, int src_band, uint32_t decimation, const float* taps, uint32_t n_taps,
+        double intermediate_freq_hz, double sampling_freq_hz);
+    /* The adapter's filter_type = lowpass branch (freq_xlating_fir_filter.cc:103-110): gr::filter::firdes::low_pass(1, fs, bw,
+     * tw) with the Hamming window, bw_hz <= 0 meaning the default (fs / decimation) / 2 and tw_hz <= 0 the default bw / 10.
+     * The same design b200_acq_resampler_design computes: ntaps = int(53 fs / (22 tw)) made odd, windowed sinc scaled to unit
+     * DC gain in double, each tap rounded once to float.  More taps than max_taps is B200_ERR_RANGE with the count needed in
+     * *n_taps and b200_last_error(); taps may be NULL when max_taps is 0.  Host-only. */
+    int b200_iq_conditioner_lowpass(double sampling_freq_hz, uint32_t decimation, double bw_hz, double tw_hz, uint32_t max_taps,
+        float* taps, uint32_t* n_taps);
+
     /* ---- tracking: single correlator, 1:1 with Cpu_Multicorrelator_Real_Codes ----------- */
     /* src/algorithms/tracking/libs/cpu_multicorrelator_real_codes.h:37-61 */
     /* init(max_signal_length_samples, n_correlators)                       (.cc:35-50) */
