@@ -59,6 +59,14 @@ class TrkLoopStatus(C.Structure):
     ]
 
 
+class PulseBlankingStatus(C.Structure):
+    """b200_pulse_blanking_status"""
+    _fields_ = [
+        ("origin", C.c_uint64), ("segments", C.c_uint64), ("blanked", C.c_uint64), ("n", C.c_int64),
+        ("noise_power", C.c_float), ("threshold", C.c_float), ("last_filtered", C.c_int32), ("length", C.c_int32),
+    ]
+
+
 class TrkDumpRecord(C.Structure):
     """b200_trk_dump_record: one epoch of the reference's tracking dump file, unpadded as the header packs it (the u64 at
     offset 28 and the double sit on 4-byte boundaries)."""

@@ -7,7 +7,7 @@ import os
 import numpy as np
 
 from .abi import (ACQ_RESULT_DTYPE, TRK_DUMP_RECORD_DTYPE, TRK_ITEM_DTYPE, AcqConf, AcqDump, AcqResult,  # noqa: F401
-                  TrkDumpRecord, TrkItem, TrkLoopConf, TrkLoopStatus)
+                  PulseBlankingStatus, TrkDumpRecord, TrkItem, TrkLoopConf, TrkLoopStatus)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200_LIB selects an alternative build of the SAME library (A/B kernel experiments); default = in-tree build
@@ -24,6 +24,7 @@ B200_MAX_TAPS = 8
 B200_ACQ_MAX_RESAMPLER_TAPS = 1024
 B200_IQ_MAX_CONDITIONER_TAPS = 4096
 B200_IQ_MAX_CONDITIONER_DECIMATION = 4096
+B200_IQ_MAX_BLANKING_LENGTH = 4096
 ERRORS = {0: "OK", -1: "ERR_ARG", -2: "ERR_CUDA", -3: "ERR_NOMEM", -4: "ERR_STATE", -5: "ERR_RANGE", -6: "ERR_NODEV"}
 
 
@@ -57,6 +58,9 @@ _SIGS = {
     "b200_iq_read": ([_vp, C.c_int, C.c_uint64, C.c_uint64, _vp], C.c_int),
     "b200_iq_set_conditioner": ([_vp, C.c_int, C.c_int, C.c_uint32, _vp, C.c_uint32, C.c_double, C.c_double], C.c_int),
     "b200_iq_conditioner_lowpass": ([C.c_double, C.c_uint32, C.c_double, C.c_double, C.c_uint32, _vp, C.POINTER(C.c_uint32)], C.c_int),
+    "b200_iq_set_pulse_blanking": ([_vp, C.c_int, C.c_int, C.c_float, C.c_int32, C.c_int32, C.c_int32], C.c_int),
+    "b200_iq_pulse_blanking_threshold": ([C.c_float, C.c_int32, C.POINTER(C.c_float)], C.c_int),
+    "b200_iq_pulse_blanking_status": ([_vp, C.c_int, C.POINTER(PulseBlankingStatus)], C.c_int),
     "b200_trk_set_taps": ([_vp, _vp], C.c_int),
     "b200_trk_set_local_code_and_taps_cplx": ([_vp, C.c_int, _vp, _vp], C.c_int),
     "b200_trk_correlate_cplx": ([_vp, _vp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, _vp], C.c_int),
@@ -260,6 +264,23 @@ class Engine:
 
     def iq_remove_conditioner(self, dst_band: int):
         _chk(lib.b200_iq_set_conditioner(self.h, dst_band, 0, 1, None, 0, 0.0, 1.0), "b200_iq_set_conditioner")
+
+    def iq_set_pulse_blanking(self, dst_band: int, src_band: int, pfa: float = 0.04, length: int = 32, segments_est: int = 12500,
+                              segments_reset: int = 5000000):
+        """fill dst_band with the pulse-blanking input filter of every push into src_band (pulse_blanking_cc(pfa, length,
+        segments_est, segments_reset); the defaults are the adapter's)"""
+        _chk(lib.b200_iq_set_pulse_blanking(self.h, dst_band, src_band, float(pfa), int(length), int(segments_est), int(segments_reset)),
+             "b200_iq_set_pulse_blanking")
+
+    def iq_remove_pulse_blanking(self, dst_band: int):
+        _chk(lib.b200_iq_set_pulse_blanking(self.h, dst_band, 0, 0.04, 0, 0, 0), "b200_iq_set_pulse_blanking")
+
+    def iq_pulse_blanking_status(self, dst_band: int) -> dict:
+        """origin, segments (processed), blanked, n, noise_power (est), threshold, last_filtered and length of dst_band's
+        blanker, after every push queued so far"""
+        st = PulseBlankingStatus()
+        _chk(lib.b200_iq_pulse_blanking_status(self.h, dst_band, C.byref(st)), "b200_iq_pulse_blanking_status")
+        return {name: getattr(st, name) for name, _ in PulseBlankingStatus._fields_}
 
     # channels
     def channel_create(self, band: int, taps: int) -> int:
@@ -613,6 +634,14 @@ def iq_conditioner_lowpass(sampling_freq_hz: float, decimation: int, bw_hz: floa
     _chk(lib.b200_iq_conditioner_lowpass(float(sampling_freq_hz), int(decimation), float(bw_hz), float(tw_hz), taps.size,
                                          taps.ctypes.data, C.byref(n)), "b200_iq_conditioner_lowpass")
     return taps
+
+
+def pulse_blanking_threshold(pfa: float, length: int) -> float:
+    """the blanker's float threshold (pulse_blanking_cc.cc:57-58): the chi-squared upper quantile with 2 length degrees of
+    freedom at the float pfa"""
+    t = C.c_float(0.0)
+    _chk(lib.b200_iq_pulse_blanking_threshold(float(pfa), int(length), C.byref(t)), "b200_iq_pulse_blanking_threshold")
+    return t.value
 
 
 def acq_dump_filename(base: str, system: str, signal: str, channel: int, dump_number: int, prn: int) -> str:

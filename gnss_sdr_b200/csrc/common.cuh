@@ -217,6 +217,26 @@ void cond_rotator_step(double intermediate_freq_hz, double sampling_freq_hz, uns
 // tap count int(53 fs / (22 transition)) made odd, and writes the taps, each rounded once to float, only when that count is
 // <= max_taps
 long long firdes_low_pass(double fs, double cutoff, double transition, long long max_taps, float* taps);
+
+// pulse blanker (iq_blanker.cu).  The state pulse_blanking_cc carries from one segment to the next (n_segments_,
+// noise_power_estimation_, last_filtered_), kept in device memory, and the segments it has zeroed.
+struct BlankState
+{
+    long long n;
+    float est;
+    int last_filtered;
+    unsigned long long blanked;
+};
+// energies[k] of the n_seg segments of L samples from absolute index s0 of the ring src (slot mask src_mask, SampleFormat src_fmt)
+int launch_blank_energy(const void* src, int src_fmt, unsigned long long src_mask, unsigned long long s0, int L, int n_seg, float* energy,
+    cudaStream_t st);
+// the block's state machine over those energies: flags[k] = 1 where segment k is zeroed; *state carried (fresh: initial state)
+int launch_blank_scan(const float* energy, int n_seg, int fresh, int L, long long n_est, long long n_reset, float thres, BlankState* state,
+    unsigned char* flags, cudaStream_t st);
+// the n_seg L samples from s0: copied from src (widened) or zeroed by flags, into the float ring dst.  Each launcher issues one
+// kernel, none for n_seg == 0.
+int launch_blank_apply(const void* src, int src_fmt, unsigned long long src_mask, unsigned long long s0, int L, int n_seg,
+    const unsigned char* flags, float2* dst, unsigned long long dst_mask, cudaStream_t st);
 }  // namespace b200
 
 // ---- acquisition launchers (acq_kernels.cu) ----------------------------------------------------------

@@ -253,8 +253,54 @@ extern "C"
         d.valid_from = std::min(std::max(rule, d.cond.floor), d.write_index);
     }
 
+    // ---- pulse blankers (b200_iq_set_pulse_blanking) ---------------------------------------------------------------
+    // the longest segment among the blankers that read `band` (0: none feeds from it)
+    static int blanker_length(const b200_engine* e, int band)
+    {
+        int L = 0;
+        for (const Band& d : e->bands)
+            if (d.blank.src == band) L = std::max(L, d.blank.length);
+        return L;
+    }
+
+    // caller holds e->mu: the most samples one push into `band` may carry so that no blanker reading it, or reading a
+    // conditioner it feeds, loses a pending sample (at most L - 1 wait for their segment): capacity - (L - 1) for the
+    // band's own blankers, D (capacity - (L - 1)) of the conditioner's destination for chained ones; ~0: no blanker
+    static unsigned long long blanker_push_limit(const b200_engine* e, int band)
+    {
+        unsigned long long lim = ~0ULL;
+        if (const int L = blanker_length(e, band)) lim = e->bands[band].capacity - (L - 1);
+        for (int m = 0; m < kMaxBands; m++)
+            if (e->bands[m].cond.src == band)
+                if (const int L = blanker_length(e, m)) lim = std::min(lim, e->bands[m].cond.decimation * (e->bands[m].capacity - (L - 1)));
+        return lim;
+    }
+
+    // caller holds e->mu: the blanker of `d` starts over at its source's valid_from with the block's initial state
+    static void restart_blanker(b200_engine* e, Band& d)
+    {
+        Band::Blanker& k = d.blank;
+        const Band& s = e->bands[k.src];
+        k.origin = k.seen_valid_from = s.valid_from;
+        k.segments = 0;
+        k.floor = 0;
+        k.fresh = true;
+    }
+
+    // caller holds e->mu: the window of a blanked band follows its source's.  A source valid_from that has moved (chained:
+    // the conditioner's window after a gap) restarts the blanker there; write_index = origin + segments L (whole segments
+    // only), valid_from = origin, never below blank.floor nor above write_index
+    static void blanked_window(b200_engine* e, Band& d)
+    {
+        Band::Blanker& k = d.blank;
+        if (e->bands[k.src].valid_from != k.seen_valid_from) restart_blanker(e, d);
+        d.write_index = k.origin + k.segments * static_cast<unsigned long long>(k.length);
+        d.valid_from = std::min(std::max(k.origin, k.floor), d.write_index);
+    }
+
     // caller holds e->mu: the source `band` moved its valid_from (a push_at gap or restart, b200_iq_forget): its
-    // destinations' windows follow, and a restarted stream is valid again from its own start
+    // destinations' windows follow, and a restarted stream is valid again from its own start.  Blankers that read it, or
+    // read a conditioner it feeds, start over.
     static void source_restarted(b200_engine* e, int band)
     {
         for (Band& d : e->bands)
@@ -263,14 +309,24 @@ extern "C"
                     d.cond.floor = 0;
                     conditioned_window(e, d);
                 }
+        for (Band& d : e->bands)
+            if (d.blank.src >= 0 && (d.blank.src == band || e->bands[d.blank.src].cond.src == band))
+                {
+                    restart_blanker(e, d);
+                    blanked_window(e, d);
+                }
     }
 
-    // caller holds e->mu: `band` (re-created or attached) is neither end of a conditioner any more
-    static void drop_conditioners(b200_engine* e, int band)
+    // caller holds e->mu: `band` (re-created or attached) is neither end of a conditioner or blanker any more
+    static void drop_stages(b200_engine* e, int band)
     {
         e->bands[band].cond.src = -1;
+        e->bands[band].blank.src = -1;
         for (Band& d : e->bands)
-            if (d.cond.src == band) d.cond.src = -1;
+            {
+                if (d.cond.src == band) d.cond.src = -1;
+                if (d.blank.src == band) d.blank.src = -1;
+            }
     }
 
     static int record_cond_done(Band& b, cudaStream_t st)
@@ -306,12 +362,72 @@ extern "C"
         return launched ? record_cond_done(s, e->stream) : B200_OK;
     }
 
-    // B200_OK, or B200_ERR_STATE with the error text when a conditioner fills `band`
+    // caller holds e->mu: `band` has been written up to its write_index.  Each blanker that reads it launches its three
+    // kernels for the segments that became complete, on the compute stream, and cond_done marks them on its destination and
+    // the last ones on the source.  No complete segment: nothing is issued.
+    static int run_blankers(b200_engine* e, int band)
+    {
+        Band& s = e->bands[band];
+        bool launched = false;
+        for (Band& d : e->bands)
+            {
+                if (d.blank.src != band) continue;
+                Band::Blanker& k = d.blank;
+                blanked_window(e, d);
+                const unsigned long long L = static_cast<unsigned long long>(k.length), done = (s.write_index - k.origin) / L;
+                const unsigned long long n_seg = done - k.segments;
+                if (n_seg > 0)
+                    {
+                        if (n_seg > k.energy.capacity())
+                            {
+                                set_error("pulse blanker of band %d: %llu segments in one push, room for %zu", band, n_seg, k.energy.capacity());
+                                return B200_ERR_STATE;
+                            }
+                        const unsigned long long s0 = k.origin + k.segments * L;
+                        const int ns = static_cast<int>(n_seg);
+                        int rc = launch_blank_energy(s.dev, s.fmt, s.mask, s0, k.length, ns, k.energy, e->stream);
+                        if (!rc) rc = launch_blank_scan(k.energy, ns, k.fresh, k.length, k.n_est, k.n_reset, k.thres, k.state, k.flags, e->stream);
+                        if (!rc)
+                            rc = launch_blank_apply(s.dev, s.fmt, s.mask, s0, k.length, ns, k.flags, reinterpret_cast<float2*>(d.dev.get()), d.mask,
+                                e->stream);
+                        if (rc) return rc;
+                        e->launches += 3;
+                        k.fresh = false;
+                        k.segments = done;
+                        if (const int rc2 = record_cond_done(d, e->stream)) return rc2;
+                        launched = true;
+                    }
+                blanked_window(e, d);
+            }
+        return launched ? record_cond_done(s, e->stream) : B200_OK;
+    }
+
+    // caller holds e->mu: after a write into `band` from old_write, its conditioners launch, then the blankers that read it
+    // or read a destination those conditioners just filled
+    static int run_stages(b200_engine* e, int band, unsigned long long old_write)
+    {
+        if (const int rc = run_conditioners(e, band, old_write)) return rc;
+        if (const int rc = run_blankers(e, band)) return rc;
+        for (int m = 0; m < kMaxBands; m++)
+            if (e->bands[m].cond.src == band)
+                if (const int rc = run_blankers(e, m)) return rc;
+        return B200_OK;
+    }
+
+    // B200_OK, or B200_ERR_STATE with the error text when a conditioner or a blanker fills `band`
     static int check_not_conditioned(const Band& b, int band)
     {
-        if (b.cond.src < 0) return B200_OK;
-        set_error("band %d is filled by its conditioner from band %d: it takes no pushes of its own", band, b.cond.src);
-        return B200_ERR_STATE;
+        if (b.cond.src >= 0)
+            {
+                set_error("band %d is filled by its conditioner from band %d: it takes no pushes of its own", band, b.cond.src);
+                return B200_ERR_STATE;
+            }
+        if (b.blank.src >= 0)
+            {
+                set_error("band %d is filled by its pulse blanker from band %d: it takes no pushes of its own", band, b.blank.src);
+                return B200_ERR_STATE;
+            }
+        return B200_OK;
     }
 
     // ---- bands -----------------------------------------------------------------------------
@@ -339,7 +455,7 @@ extern "C"
         B200_ENTER_DEVICE(e->device);
         Band& b = e->bands[band];
         if (const int rc = release_owned_ring(e, b)) return rc;
-        drop_conditioners(e, band);
+        drop_stages(e, band);
         const unsigned long long cap = next_pow2(capacity_samples);
         cudaError_t err = b.dev.alloc(cap * 2ULL * fmt);
         if (err != cudaSuccess)
@@ -402,6 +518,12 @@ extern "C"
                         (unsigned long long)n, band, taps, b.capacity - (taps - 1));
                     return B200_ERR_RANGE;
                 }
+        if (n > blanker_push_limit(e, band))
+            {
+                set_error("push of %llu samples into band %d: the pending samples of its pulse blankers must stay in the ring, at most %llu per push",
+                    (unsigned long long)n, band, blanker_push_limit(e, band));
+                return B200_ERR_RANGE;
+            }
         B200_ENTER_DEVICE(e->device);
         if (first_index) *first_index = b.write_index;
         if (n == 0) return B200_OK;
@@ -441,7 +563,7 @@ extern "C"
                 b.raw_last = k;
             }
         b.write_index += n;
-        return run_conditioners(e, band, old_write);
+        return run_stages(e, band, old_write);
     }
 
     int b200_iq_push(b200_engine* e, int band, const b200_cf32* host, uint64_t n, uint64_t* first_index)
@@ -500,6 +622,7 @@ extern "C"
         if (!b.in_use || b.attached) return B200_ERR_STATE;
         b.valid_from = b.write_index;
         if (b.cond.src >= 0) b.cond.floor = b.write_index;
+        if (b.blank.src >= 0) b.blank.floor = b.write_index;
         source_restarted(e, band);
         return B200_OK;
     }
@@ -523,6 +646,7 @@ extern "C"
         if (const int rc = parse_item_type(item_type, "iq_push_file", &fmt)) return rc;
         unsigned long long capacity;
         unsigned history;
+        unsigned long long blank_limit;
         {
             std::lock_guard<std::mutex> lk(e->mu);
             const Band& b = e->bands[band];
@@ -530,10 +654,12 @@ extern "C"
             if (const int rc = check_push_format(b, band, fmt)) return rc;
             capacity = b.capacity;
             history = conditioner_taps(e, band);
+            blank_limit = blanker_push_limit(e, band);
         }
         if (chunk_samples == 0) chunk_samples = 1ULL << 20;
         if (chunk_samples > capacity / 2) chunk_samples = capacity / 2 ? capacity / 2 : 1;
         if (history > 1 && chunk_samples > capacity - (history - 1)) chunk_samples = capacity - (history - 1);
+        if (chunk_samples > blank_limit) chunk_samples = blank_limit;
         B200_ENTER_DEVICE(e->device);
         FILE* f = std::fopen(path, "rb");
         if (!f)
@@ -603,7 +729,7 @@ extern "C"
         std::lock_guard<std::mutex> lk(e->mu);
         Band& b = e->bands[band];
         if (const int rc = release_owned_ring(e, b)) return rc;
-        drop_conditioners(e, band);
+        drop_stages(e, band);
         b.base = dev;
         b.fmt = kCf32;
         b.capacity = n_samples;
@@ -720,6 +846,11 @@ extern "C"
                 set_error("iq_set_conditioner: band %d -> band %d would chain conditioners", src_band, dst_band);
                 return B200_ERR_STATE;
             }
+        if (d.blank.src >= 0 || s.blank.src >= 0)
+            {
+                set_error("iq_set_conditioner: band %d -> band %d: a pulse blanker fills band %d", src_band, dst_band, d.blank.src >= 0 ? dst_band : src_band);
+                return B200_ERR_STATE;
+            }
         if (d.capacity * decimation < s.capacity || s.capacity < n_taps)
             {
                 set_error("iq_set_conditioner: band %d (%llu samples) must hold band %d's %llu samples decimated by %u, and band %d at least %u taps",
@@ -744,6 +875,106 @@ extern "C"
         cond_rotator_step(intermediate_freq_hz, sampling_freq_hz, decimation, &d.cond.rot_hi, &d.cond.rot_lo);
         d.cond.floor = ceil_div(s.write_index, decimation);  // set mid-stream: the destination starts empty there
         conditioned_window(e, d);
+        return B200_OK;
+    }
+
+    int b200_iq_set_pulse_blanking(b200_engine* e, int dst_band, int src_band, float pfa, int32_t length, int32_t segments_est,
+        int32_t segments_reset)
+    {
+        if (!e || dst_band < 0 || dst_band >= kMaxBands) return B200_ERR_ARG;
+        if (length == 0)
+            {
+                std::lock_guard<std::mutex> lk(e->mu);
+                e->bands[dst_band].blank.src = -1;
+                return B200_OK;
+            }
+        if (src_band < 0 || src_band >= kMaxBands || length < 0 || segments_est < 0 || segments_reset < 0 || !(pfa > 0.f && pfa < 1.f))
+            {
+                set_error("iq_set_pulse_blanking: band %d, pfa %g, length %d, segments_est %d, segments_reset %d: bad argument", src_band,
+                    static_cast<double>(pfa), length, segments_est, segments_reset);
+                return B200_ERR_ARG;
+            }
+        if (dst_band == src_band)
+            {
+                set_error("iq_set_pulse_blanking: band %d cannot blank into itself", dst_band);
+                return B200_ERR_ARG;
+            }
+        if (length > B200_IQ_MAX_BLANKING_LENGTH)
+            {
+                set_error("iq_set_pulse_blanking: length %d: at most %d", length, B200_IQ_MAX_BLANKING_LENGTH);
+                return B200_ERR_RANGE;
+            }
+        float thres = 0.f;
+        if (const int rc = b200_iq_pulse_blanking_threshold(pfa, length, &thres)) return rc;
+        std::lock_guard<std::mutex> lk(e->mu);
+        Band& d = e->bands[dst_band];
+        const Band& s = e->bands[src_band];
+        if (const int rc = s.check_owned_ring(src_band)) return rc;
+        if (const int rc = d.check_owned_ring(dst_band)) return rc;
+        if (d.fmt != kCf32)
+            {
+                set_error("iq_set_pulse_blanking: band %d holds %s samples: a blanker writes gr_complex", dst_band, item_type_name(d.fmt));
+                return B200_ERR_STATE;
+            }
+        // the one chain allowed is conditioner -> blanker: the source may be a conditioner's destination, nothing else
+        if (d.cond.src >= 0 || conditioner_taps(e, dst_band) > 0 || blanker_length(e, dst_band) > 0 || s.blank.src >= 0)
+            {
+                set_error("iq_set_pulse_blanking: band %d -> band %d would chain a blanker with another stage", src_band, dst_band);
+                return B200_ERR_STATE;
+            }
+        if (d.capacity < s.capacity || s.capacity < static_cast<unsigned long long>(length))
+            {
+                set_error("iq_set_pulse_blanking: band %d (%llu samples) must hold band %d's %llu samples, and band %d at least %d", dst_band,
+                    d.capacity, src_band, s.capacity, src_band, length);
+                return B200_ERR_RANGE;
+            }
+        B200_ENTER_DEVICE(e->device);
+        Band::Blanker& k = d.blank;
+        const unsigned long long max_seg = s.capacity / static_cast<unsigned long long>(length) + 1;
+        B200_CUDA_TRY(cudaStreamSynchronize(e->stream));  // launches already queued may still use the old buffers
+        if (!k.state) B200_CUDA_TRY(k.state.alloc(1));
+        if (!k.energy.fits(max_seg)) B200_CUDA_TRY(k.energy.alloc(max_seg));
+        if (!k.flags.fits(max_seg)) B200_CUDA_TRY(k.flags.alloc(max_seg));
+        k.src = src_band;
+        k.length = length;
+        k.n_est = segments_est;
+        k.n_reset = segments_reset;
+        k.thres = thres;
+        k.origin = s.write_index;  // a fresh stream: 0; mid-stream: where the next sample lands
+        k.seen_valid_from = s.valid_from;
+        k.segments = 0;
+        k.floor = 0;
+        k.fresh = true;
+        blanked_window(e, d);
+        return B200_OK;
+    }
+
+    int b200_iq_pulse_blanking_status(b200_engine* e, int dst_band, b200_pulse_blanking_status* status)
+    {
+        if (!e || dst_band < 0 || dst_band >= kMaxBands || !status) return B200_ERR_ARG;
+        std::lock_guard<std::mutex> lk(e->mu);
+        const Band& d = e->bands[dst_band];
+        if (d.blank.src < 0)
+            {
+                set_error("band %d has no pulse blanker (call b200_iq_set_pulse_blanking)", dst_band);
+                return B200_ERR_STATE;
+            }
+        const Band::Blanker& k = d.blank;
+        BlankState st{};
+        if (!k.fresh)
+            {
+                B200_ENTER_DEVICE(e->device);
+                B200_CUDA_TRY(cudaMemcpyAsync(&st, k.state, sizeof(st), cudaMemcpyDeviceToHost, e->stream));
+                B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
+            }
+        status->origin = k.origin;
+        status->segments = k.segments;
+        status->blanked = st.blanked;
+        status->n = st.n;
+        status->noise_power = st.est;
+        status->threshold = k.thres;
+        status->last_filtered = st.last_filtered;
+        status->length = k.length;
         return B200_OK;
     }
 

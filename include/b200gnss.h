@@ -190,6 +190,80 @@ extern "C"
     int b200_iq_conditioner_lowpass(double sampling_freq_hz, uint32_t decimation, double bw_hz, double tw_hz, uint32_t max_taps,
         float* taps, uint32_t* n_taps);
 
+    /* ---- pulse blanking on the device ------------------------------------------------------------------------------
+     * InputFilter.implementation = Pulse_Blanking_Filter (src/algorithms/input_filter/adapters/pulse_blanking_filter.cc:43-84),
+     * which instantiates pulse_blanking_cc(pfa, length, segments_est, segments_reset)
+     * (gnuradio_blocks/pulse_blanking_cc.cc:33-98): pulsed interference (DME/TACAN, radar, switching front ends) is removed
+     * before acquisition and tracking see it.
+     *
+     * b200_iq_set_pulse_blanking links src_band to dst_band: every write into the source that completes segments fills the
+     * destination with the block's output in absolute stream indices, dst[j] = src[j] widened, or 0 where j's segment is
+     * blanked.  Segments are [o + k L, o + (k + 1) L), L = length, counted from the blanker's origin o.  For each, in order:
+     *     e = sum_{i < L} (re_i re_i + im_i im_i)        (each square and sum rounded on its own, i ascending from 0.0)
+     *     n < E and not last_filtered:  est = (float(n) est + e / float(2L)) / float(n + 1), copied        (estimation)
+     *     else if e / est > thres:      zeroed, last_filtered = true                                         (detection)
+     *     else:                         copied, last_filtered = false, and n = 0 if n > R
+     *     n++
+     * E = segments_est, R = segments_reset, thres = b200_iq_pulse_blanking_threshold(pfa, L); every float operation is
+     * rounded on its own and e / est follows IEEE (E = 0: est stays 0, e / 0 is +inf and blanks, 0 / 0 is NaN and copies).
+     *  - The energy sum is the generic VOLK order (volk_32f_accumulator_s32f_generic).  A VOLK dispatched to its AVX kernel
+     *    sums in another order and can differ from this in the last bit of a segment energy.
+     *  - The block keeps n in an int32; here it is 64-bit, which differs only after 2^31 segments without a reset (R near
+     *    INT32_MAX), where the block's counter overflows.
+     *  - The block processes a segment only once a sample past it has arrived (pulse_blanking_cc.cc:71); here every whole
+     *    segment is published at once.  That delays the block's output and changes no value.
+     *  - Origin and state: a blanker set on a fresh stream starts at index 0, one set on a source that already holds samples
+     *    at the source's write index, with the block's initial state (n = 0, est = 0, last_filtered = false).  When the
+     *    source's valid_from moves (a b200_iq_push_at gap or restart, b200_iq_forget on the source, or, chained, the
+     *    conditioner's window moving), the blanker restarts at the new valid_from with its initial state.  So the
+     *    destination always equals a reference block started on the stream at the origin.
+     *  - The destination's window: write_index = o + floor((src write_index - o) / L) L (whole segments only);
+     *    valid_from = o, never below where the destination was last b200_iq_forget-ed, nor above write_index.
+     *  - The source may be a gr_complex, ishort or ibyte owned ring (integers are widened exactly, as Ishort_To_Complex and
+     *    Ibyte_To_Complex do); the destination a gr_complex owned ring at least as large.  One source may feed several
+     *    blankers.  The one chain allowed is a conditioner followed by a blanker: the source may be a conditioner's
+     *    destination, which is the adapter's IF > 1 arm (pulse_blanking_filter.cc:73-84, freq_xlating_fir_filter_ccf(1,
+     *    firdes::low_pass(1, fs, bw, tw), IF, fs) before the blanker): b200_iq_conditioner_lowpass, b200_iq_set_conditioner
+     *    with decimation 1, then this.  A blanker or conditioner fed from a blanker's destination is refused.
+     *  - After a push, the source's conditioners launch first, as before; then each blanker that reads the band or a
+     *    destination just filled launches three kernels (segment energies, the state machine, copy or zero) on the compute
+     *    stream when the write completed at least one segment, and none otherwise.  The state lives in device memory; a
+     *    band search, batch or loop run issued after the push reads the blanked samples with no host synchronisation.  The
+     *    next copy into a ring a blanker reads waits for its launches.
+     *  - At most L - 1 source samples wait for their segment to complete, and they must stay in the ring: a push of more
+     *    than capacity - (L - 1) samples into a blanker's source, or, chained, of more than D (capacity - (L - 1)) samples
+     *    into the conditioner's source (capacity of the conditioner's destination, D its decimation), is B200_ERR_RANGE,
+     *    refused before any byte is written; b200_iq_push_file cuts its blocks to fit.
+     *  - While a blanker is set, a direct push or push_at into its destination is B200_ERR_STATE.  length == 0 removes the
+     *    destination's blanker (the other arguments are then not read); so does re-creating or attaching either band.
+     *    Setting a blanker on a destination that has one replaces it, restarting at the rule above.
+     *  - Refused, with nothing launched and both windows unchanged: dst_band == src_band, length < 0, segments_est < 0,
+     *    segments_reset < 0, or pfa outside (0, 1) (B200_ERR_ARG); length > B200_IQ_MAX_BLANKING_LENGTH or a destination
+     *    smaller than the source or a source smaller than L (B200_ERR_RANGE); a band that is not an owned ring, a narrow
+     *    destination, a destination that a conditioner fills or that feeds a stage, or a source that a blanker fills
+     *    (B200_ERR_STATE). */
+#define B200_IQ_MAX_BLANKING_LENGTH 4096
+    int b200_iq_set_pulse_blanking(b200_engine* e, int dst_band, int src_band, float pfa, int32_t length, int32_t segments_est,
+        int32_t segments_reset);
+    /* thres of pulse_blanking_cc.cc:57-58, quantile(complement(chi_squared(2 length), pfa)): the x at which the chi-squared
+     * upper tail with 2L degrees of freedom, e^{-x/2} sum_{k < L} (x/2)^k / k!, equals pfa, found in double and rounded once
+     * to float.  pfa outside (0, 1) or length outside [1, B200_IQ_MAX_BLANKING_LENGTH] is B200_ERR_ARG.  Host-only. */
+    int b200_iq_pulse_blanking_threshold(float pfa, int32_t length, float* thres);
+    typedef struct
+    {
+        uint64_t origin;       /* absolute index of segment 0 */
+        uint64_t segments;     /* segments processed since the origin */
+        uint64_t blanked;      /* of them, zeroed */
+        int64_t n;             /* the block's n_segments_ */
+        float noise_power;     /* noise_power_estimation_ (est) */
+        float threshold;       /* thres_ */
+        int32_t last_filtered; /* last_filtered_ */
+        int32_t length;        /* L */
+    } b200_pulse_blanking_status;
+    /* The state of dst_band's blanker after every push queued so far (synchronous): how much it blanks, and the state
+     * machine it carries.  A band with no blanker is B200_ERR_STATE. */
+    int b200_iq_pulse_blanking_status(b200_engine* e, int dst_band, b200_pulse_blanking_status* status);
+
     /* ---- tracking: single correlator, 1:1 with Cpu_Multicorrelator_Real_Codes ----------- */
     /* src/algorithms/tracking/libs/cpu_multicorrelator_real_codes.h:37-61 */
     /* init(max_signal_length_samples, n_correlators)                       (.cc:35-50) */
