@@ -67,6 +67,16 @@ class PulseBlankingStatus(C.Structure):
     ]
 
 
+class NotchStatus(C.Structure):
+    """b200_notch_status"""
+    _fields_ = [
+        ("origin", C.c_uint64), ("segments", C.c_uint64), ("filtered", C.c_uint64), ("n", C.c_int64),
+        ("noise_power", C.c_float), ("threshold", C.c_float), ("z0_re", C.c_float), ("z0_im", C.c_float),
+        ("last_out_re", C.c_float), ("last_out_im", C.c_float), ("filter_state", C.c_int32), ("n_coeff", C.c_int32),
+        ("length", C.c_int32), ("variant", C.c_int32),
+    ]
+
+
 class TrkDumpRecord(C.Structure):
     """b200_trk_dump_record: one epoch of the reference's tracking dump file, unpadded as the header packs it (the u64 at
     offset 28 and the double sit on 4-byte boundaries)."""

@@ -7,7 +7,7 @@ import os
 import numpy as np
 
 from .abi import (ACQ_RESULT_DTYPE, TRK_DUMP_RECORD_DTYPE, TRK_ITEM_DTYPE, AcqConf, AcqDump, AcqResult,  # noqa: F401
-                  PulseBlankingStatus, TrkDumpRecord, TrkItem, TrkLoopConf, TrkLoopStatus)
+                  NotchStatus, PulseBlankingStatus, TrkDumpRecord, TrkItem, TrkLoopConf, TrkLoopStatus)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200_LIB selects an alternative build of the SAME library (A/B kernel experiments); default = in-tree build
@@ -25,6 +25,9 @@ B200_ACQ_MAX_RESAMPLER_TAPS = 1024
 B200_IQ_MAX_CONDITIONER_TAPS = 4096
 B200_IQ_MAX_CONDITIONER_DECIMATION = 4096
 B200_IQ_MAX_BLANKING_LENGTH = 4096
+B200_NOTCH = 0
+B200_NOTCH_LITE = 1
+B200_IQ_MAX_NOTCH_LENGTH = 1024
 ERRORS = {0: "OK", -1: "ERR_ARG", -2: "ERR_CUDA", -3: "ERR_NOMEM", -4: "ERR_STATE", -5: "ERR_RANGE", -6: "ERR_NODEV"}
 
 
@@ -61,6 +64,8 @@ _SIGS = {
     "b200_iq_set_pulse_blanking": ([_vp, C.c_int, C.c_int, C.c_float, C.c_int32, C.c_int32, C.c_int32], C.c_int),
     "b200_iq_pulse_blanking_threshold": ([C.c_float, C.c_int32, C.POINTER(C.c_float)], C.c_int),
     "b200_iq_pulse_blanking_status": ([_vp, C.c_int, C.POINTER(PulseBlankingStatus)], C.c_int),
+    "b200_iq_set_notch": ([_vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int32, C.c_int32, C.c_int32, C.c_int32], C.c_int),
+    "b200_iq_notch_status": ([_vp, C.c_int, C.POINTER(NotchStatus)], C.c_int),
     "b200_trk_set_taps": ([_vp, _vp], C.c_int),
     "b200_trk_set_local_code_and_taps_cplx": ([_vp, C.c_int, _vp, _vp], C.c_int),
     "b200_trk_correlate_cplx": ([_vp, _vp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, _vp], C.c_int),
@@ -281,6 +286,27 @@ class Engine:
         st = PulseBlankingStatus()
         _chk(lib.b200_iq_pulse_blanking_status(self.h, dst_band, C.byref(st)), "b200_iq_pulse_blanking_status")
         return {name: getattr(st, name) for name, _ in PulseBlankingStatus._fields_}
+
+    def iq_set_notch(self, dst_band: int, src_band: int, variant: int = B200_NOTCH_LITE, pfa: float = 0.001, p_c_factor: float = 0.9,
+                     length: int = 32, segments_est: int = 12500, segments_reset: int = 5000000, segments_coeff: int = 1):
+        """fill dst_band with the notch input filter of every push into src_band: variant B200_NOTCH (Notch(pfa, p_c_factor,
+        length, segments_est, segments_reset)) or B200_NOTCH_LITE (NotchLite(p_c_factor, pfa, length, segments_est,
+        segments_reset, segments_coeff)); the defaults are the adapters'"""
+        _chk(lib.b200_iq_set_notch(self.h, dst_band, src_band, int(variant), float(pfa), float(p_c_factor), int(length), int(segments_est),
+                                   int(segments_reset), int(segments_coeff)), "b200_iq_set_notch")
+
+    def iq_remove_notch(self, dst_band: int):
+        _chk(lib.b200_iq_set_notch(self.h, dst_band, 0, B200_NOTCH_LITE, 0.001, 0.9, 0, 0, 0, 1), "b200_iq_set_notch")
+
+    def iq_notch_status(self, dst_band: int) -> dict:
+        """origin, segments, filtered, n, noise_power (est), threshold, z0, last_out (complex), filter_state, n_coeff,
+        length and variant of dst_band's notch, after every push queued so far"""
+        st = NotchStatus()
+        _chk(lib.b200_iq_notch_status(self.h, dst_band, C.byref(st)), "b200_iq_notch_status")
+        d = {name: getattr(st, name) for name, _ in NotchStatus._fields_}
+        d["z0"] = complex(d.pop("z0_re"), d.pop("z0_im"))
+        d["last_out"] = complex(d.pop("last_out_re"), d.pop("last_out_im"))
+        return d
 
     # channels
     def channel_create(self, band: int, taps: int) -> int:

@@ -237,6 +237,50 @@ int launch_blank_scan(const float* energy, int n_seg, int fresh, int L, long lon
 // kernel, none for n_seg == 0.
 int launch_blank_apply(const void* src, int src_fmt, unsigned long long src_mask, unsigned long long s0, int L, int n_seg,
     const unsigned char* flags, float2* dst, unsigned long long dst_mask, cudaStream_t st);
+
+// notch filters (iq_notch.cu).  The state Notch / NotchLite carry from one segment to the next, kept in device memory, with
+// the IIR's double carry on the absolute grid of kNotchGrid output samples counted from the origin.
+constexpr int kNotchGrid = 1024;
+struct NotchState
+{
+    long long n;                    // n_segments_
+    float est;                      // noise_pow_est_
+    int filter_state;               // filter_state_
+    int n_coeff;                    // n_segments_coeff_ (Lite)
+    int last_seg;                   // the last filtered segment of the latest push (-1: none)
+    float2 z0;                      // z_0_
+    float2 last_out, last_in;       // last_out_ after the latest push; and before it (read by the apply pass)
+    double2 y_grid;                 // y entering the grid block in progress
+    double2 pa, pb;                 // that block's map y -> pa y + pb over its samples so far
+    unsigned long long filtered;    // segments filtered
+};
+// the resources of one notch: flags[k] bit 0 filtered, bit 1 a run starts; zsrc[k] the segment (push index) whose z0
+// segment k uses (Lite; < 0: the carried one); zseg[k] that z0; zs[i] the per-sample z0 of the push (Notch)
+struct NotchBufs
+{
+    NotchState* state;
+    const double2* twiddle;  // exp(-2 pi i m / L), m < L, made on the host
+    float* energy;
+    float* sig2lin;
+    unsigned char* flags;
+    int* zsrc;
+    float2* zseg;
+    float2* zs;
+    double2* block_ab;       // (A, B) of each grid block of the push
+    double2* y_grid;         // y entering each grid block of the push
+};
+struct NotchParams
+{
+    int variant;  // B200_NOTCH or B200_NOTCH_LITE
+    int L;
+    long long n_est, n_reset;
+    int n_coeff;
+    float thres, p;
+    unsigned long long origin;
+};
+// the six launches of a push that completes n_seg >= 1 segments, from segment seg0 (counted from the origin), on st
+int launch_notch(const void* src, int src_fmt, unsigned long long src_mask, const NotchParams& prm, unsigned long long seg0, int n_seg,
+    int fresh, const NotchBufs& b, float2* dst, unsigned long long dst_mask, cudaStream_t st);
 }  // namespace b200
 
 // ---- acquisition launchers (acq_kernels.cu) ----------------------------------------------------------

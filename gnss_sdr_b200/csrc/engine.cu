@@ -253,33 +253,54 @@ extern "C"
         d.valid_from = std::min(std::max(rule, d.cond.floor), d.write_index);
     }
 
-    // ---- pulse blankers (b200_iq_set_pulse_blanking) ---------------------------------------------------------------
-    // the longest segment among the blankers that read `band` (0: none feeds from it)
-    static int blanker_length(const b200_engine* e, int band)
+    // ---- segment stages: pulse blankers (b200_iq_set_pulse_blanking) and notches (b200_iq_set_notch) -------------------
+    // samples of the source beyond its published segments that a stage may still read: a blanker's L - 1 pending; a
+    // notch's L - 1 pending and one more (Lite: the one before the segment, and at L = 1 the one after it too; Notch: the one
+    // after it)
+    static unsigned long long stage_reach(const Band::SegStage& k)
     {
-        int L = 0;
-        for (const Band& d : e->bands)
-            if (d.blank.src == band) L = std::max(L, d.blank.length);
-        return L;
+        const unsigned long long L = static_cast<unsigned long long>(k.length);
+        if (k.kind == Band::kBlanker) return L - 1;
+        return L + (k.variant == B200_NOTCH_LITE && L == 1 ? 1 : 0);
     }
 
-    // caller holds e->mu: the most samples one push into `band` may carry so that no blanker reading it, or reading a
-    // conditioner it feeds, loses a pending sample (at most L - 1 wait for their segment): capacity - (L - 1) for the
-    // band's own blankers, D (capacity - (L - 1)) of the conditioner's destination for chained ones; ~0: no blanker
-    static unsigned long long blanker_push_limit(const b200_engine* e, int band)
+    // source samples past a segment's end that must exist before it is published (a Notch's look-ahead, Lite's at L = 1)
+    static unsigned long long stage_lead(const Band::SegStage& k)
     {
-        unsigned long long lim = ~0ULL;
-        if (const int L = blanker_length(e, band)) lim = e->bands[band].capacity - (L - 1);
+        return k.kind == Band::kNotch && (k.variant == B200_NOTCH || k.length == 1) ? 1 : 0;
+    }
+
+    // the widest reach among the stages that read `band` (0 and false: none feeds from it)
+    static bool stage_reach_of(const b200_engine* e, int band, unsigned long long* reach)
+    {
+        bool any = false;
+        *reach = 0;
+        for (const Band& d : e->bands)
+            if (d.stage.src == band)
+                {
+                    any = true;
+                    *reach = std::max(*reach, stage_reach(d.stage));
+                }
+        return any;
+    }
+
+    // caller holds e->mu: the most samples one push into `band` may carry so that no stage reading it, or reading a
+    // conditioner it feeds, loses a sample it still needs: capacity - reach for the band's own stages, D (capacity - reach)
+    // of the conditioner's destination for chained ones; ~0: no stage
+    static unsigned long long stage_push_limit(const b200_engine* e, int band)
+    {
+        unsigned long long lim = ~0ULL, r;
+        if (stage_reach_of(e, band, &r)) lim = e->bands[band].capacity - r;
         for (int m = 0; m < kMaxBands; m++)
             if (e->bands[m].cond.src == band)
-                if (const int L = blanker_length(e, m)) lim = std::min(lim, e->bands[m].cond.decimation * (e->bands[m].capacity - (L - 1)));
+                if (stage_reach_of(e, m, &r)) lim = std::min(lim, e->bands[m].cond.decimation * (e->bands[m].capacity - r));
         return lim;
     }
 
-    // caller holds e->mu: the blanker of `d` starts over at its source's valid_from with the block's initial state
-    static void restart_blanker(b200_engine* e, Band& d)
+    // caller holds e->mu: the stage of `d` starts over at its source's valid_from with the block's initial state
+    static void restart_stage(b200_engine* e, Band& d)
     {
-        Band::Blanker& k = d.blank;
+        Band::SegStage& k = d.stage;
         const Band& s = e->bands[k.src];
         k.origin = k.seen_valid_from = s.valid_from;
         k.segments = 0;
@@ -287,19 +308,19 @@ extern "C"
         k.fresh = true;
     }
 
-    // caller holds e->mu: the window of a blanked band follows its source's.  A source valid_from that has moved (chained:
-    // the conditioner's window after a gap) restarts the blanker there; write_index = origin + segments L (whole segments
-    // only), valid_from = origin, never below blank.floor nor above write_index
-    static void blanked_window(b200_engine* e, Band& d)
+    // caller holds e->mu: the window of a staged band follows its source's.  A source valid_from that has moved (chained:
+    // the conditioner's window after a gap) restarts the stage there; write_index = origin + segments L (whole segments
+    // only), valid_from = origin, never below stage.floor nor above write_index
+    static void staged_window(b200_engine* e, Band& d)
     {
-        Band::Blanker& k = d.blank;
-        if (e->bands[k.src].valid_from != k.seen_valid_from) restart_blanker(e, d);
+        Band::SegStage& k = d.stage;
+        if (e->bands[k.src].valid_from != k.seen_valid_from) restart_stage(e, d);
         d.write_index = k.origin + k.segments * static_cast<unsigned long long>(k.length);
         d.valid_from = std::min(std::max(k.origin, k.floor), d.write_index);
     }
 
     // caller holds e->mu: the source `band` moved its valid_from (a push_at gap or restart, b200_iq_forget): its
-    // destinations' windows follow, and a restarted stream is valid again from its own start.  Blankers that read it, or
+    // destinations' windows follow, and a restarted stream is valid again from its own start.  Stages that read it, or
     // read a conditioner it feeds, start over.
     static void source_restarted(b200_engine* e, int band)
     {
@@ -310,22 +331,22 @@ extern "C"
                     conditioned_window(e, d);
                 }
         for (Band& d : e->bands)
-            if (d.blank.src >= 0 && (d.blank.src == band || e->bands[d.blank.src].cond.src == band))
+            if (d.stage.src >= 0 && (d.stage.src == band || e->bands[d.stage.src].cond.src == band))
                 {
-                    restart_blanker(e, d);
-                    blanked_window(e, d);
+                    restart_stage(e, d);
+                    staged_window(e, d);
                 }
     }
 
-    // caller holds e->mu: `band` (re-created or attached) is neither end of a conditioner or blanker any more
+    // caller holds e->mu: `band` (re-created or attached) is neither end of a conditioner or segment stage any more
     static void drop_stages(b200_engine* e, int band)
     {
         e->bands[band].cond.src = -1;
-        e->bands[band].blank.src = -1;
+        e->bands[band].stage.src = -1;
         for (Band& d : e->bands)
             {
                 if (d.cond.src == band) d.cond.src = -1;
-                if (d.blank.src == band) d.blank.src = -1;
+                if (d.stage.src == band) d.stage.src = -1;
             }
     }
 
@@ -362,59 +383,72 @@ extern "C"
         return launched ? record_cond_done(s, e->stream) : B200_OK;
     }
 
-    // caller holds e->mu: `band` has been written up to its write_index.  Each blanker that reads it launches its three
-    // kernels for the segments that became complete, on the compute stream, and cond_done marks them on its destination and
-    // the last ones on the source.  No complete segment: nothing is issued.
-    static int run_blankers(b200_engine* e, int band)
+    // caller holds e->mu: `band` has been written up to its write_index.  Each segment stage that reads it launches its
+    // kernels (a blanker three, a notch six) for the segments that became complete, on the compute stream, and cond_done
+    // marks them on its destination and the last ones on the source.  No complete segment: nothing is issued.
+    static int run_seg_stages(b200_engine* e, int band)
     {
         Band& s = e->bands[band];
         bool launched = false;
         for (Band& d : e->bands)
             {
-                if (d.blank.src != band) continue;
-                Band::Blanker& k = d.blank;
-                blanked_window(e, d);
-                const unsigned long long L = static_cast<unsigned long long>(k.length), done = (s.write_index - k.origin) / L;
-                const unsigned long long n_seg = done - k.segments;
+                if (d.stage.src != band) continue;
+                Band::SegStage& k = d.stage;
+                staged_window(e, d);
+                const unsigned long long L = static_cast<unsigned long long>(k.length), lead = stage_lead(k);
+                const unsigned long long done = s.write_index >= k.origin + lead ? (s.write_index - k.origin - lead) / L : 0;
+                const unsigned long long n_seg = done > k.segments ? done - k.segments : 0;
                 if (n_seg > 0)
                     {
                         if (n_seg > k.energy.capacity())
                             {
-                                set_error("pulse blanker of band %d: %llu segments in one push, room for %zu", band, n_seg, k.energy.capacity());
+                                set_error("segment stage of band %d: %llu segments in one push, room for %zu", band, n_seg, k.energy.capacity());
                                 return B200_ERR_STATE;
                             }
-                        const unsigned long long s0 = k.origin + k.segments * L;
                         const int ns = static_cast<int>(n_seg);
-                        int rc = launch_blank_energy(s.dev, s.fmt, s.mask, s0, k.length, ns, k.energy, e->stream);
-                        if (!rc) rc = launch_blank_scan(k.energy, ns, k.fresh, k.length, k.n_est, k.n_reset, k.thres, k.state, k.flags, e->stream);
-                        if (!rc)
-                            rc = launch_blank_apply(s.dev, s.fmt, s.mask, s0, k.length, ns, k.flags, reinterpret_cast<float2*>(d.dev.get()), d.mask,
-                                e->stream);
+                        float2* const dst = reinterpret_cast<float2*>(d.dev.get());
+                        int rc;
+                        if (k.kind == Band::kBlanker)
+                            {
+                                const unsigned long long s0 = k.origin + k.segments * L;
+                                rc = launch_blank_energy(s.dev, s.fmt, s.mask, s0, k.length, ns, k.energy, e->stream);
+                                if (!rc) rc = launch_blank_scan(k.energy, ns, k.fresh, k.length, k.n_est, k.n_reset, k.thres, k.state, k.flags, e->stream);
+                                if (!rc) rc = launch_blank_apply(s.dev, s.fmt, s.mask, s0, k.length, ns, k.flags, dst, d.mask, e->stream);
+                                if (!rc) e->launches += 3;
+                            }
+                        else
+                            {
+                                const NotchParams prm{k.variant, k.length, k.n_est, k.n_reset, k.n_coeff, k.thres, k.p, k.origin};
+                                const NotchBufs bufs{k.notch_state, k.twiddle, k.energy, k.sig2lin, k.flags, k.zsrc, k.zseg, k.zs, k.block_ab, k.y_grid};
+                                rc = launch_notch(s.dev, s.fmt, s.mask, prm, k.segments, ns, k.fresh, bufs, dst, d.mask, e->stream);
+                                if (!rc) e->launches += 6;
+                            }
                         if (rc) return rc;
-                        e->launches += 3;
                         k.fresh = false;
                         k.segments = done;
                         if (const int rc2 = record_cond_done(d, e->stream)) return rc2;
                         launched = true;
                     }
-                blanked_window(e, d);
+                staged_window(e, d);
             }
         return launched ? record_cond_done(s, e->stream) : B200_OK;
     }
 
-    // caller holds e->mu: after a write into `band` from old_write, its conditioners launch, then the blankers that read it
-    // or read a destination those conditioners just filled
+    // caller holds e->mu: after a write into `band` from old_write, its conditioners launch, then the segment stages that
+    // read it or read a destination those conditioners just filled
     static int run_stages(b200_engine* e, int band, unsigned long long old_write)
     {
         if (const int rc = run_conditioners(e, band, old_write)) return rc;
-        if (const int rc = run_blankers(e, band)) return rc;
+        if (const int rc = run_seg_stages(e, band)) return rc;
         for (int m = 0; m < kMaxBands; m++)
             if (e->bands[m].cond.src == band)
-                if (const int rc = run_blankers(e, m)) return rc;
+                if (const int rc = run_seg_stages(e, m)) return rc;
         return B200_OK;
     }
 
-    // B200_OK, or B200_ERR_STATE with the error text when a conditioner or a blanker fills `band`
+    static const char* stage_name(const Band::SegStage& k) { return k.kind == Band::kBlanker ? "pulse blanker" : "notch"; }
+
+    // B200_OK, or B200_ERR_STATE with the error text when a conditioner or a segment stage fills `band`
     static int check_not_conditioned(const Band& b, int band)
     {
         if (b.cond.src >= 0)
@@ -422,9 +456,9 @@ extern "C"
                 set_error("band %d is filled by its conditioner from band %d: it takes no pushes of its own", band, b.cond.src);
                 return B200_ERR_STATE;
             }
-        if (b.blank.src >= 0)
+        if (b.stage.src >= 0)
             {
-                set_error("band %d is filled by its pulse blanker from band %d: it takes no pushes of its own", band, b.blank.src);
+                set_error("band %d is filled by its %s from band %d: it takes no pushes of its own", band, stage_name(b.stage), b.stage.src);
                 return B200_ERR_STATE;
             }
         return B200_OK;
@@ -518,10 +552,10 @@ extern "C"
                         (unsigned long long)n, band, taps, b.capacity - (taps - 1));
                     return B200_ERR_RANGE;
                 }
-        if (n > blanker_push_limit(e, band))
+        if (n > stage_push_limit(e, band))
             {
-                set_error("push of %llu samples into band %d: the pending samples of its pulse blankers must stay in the ring, at most %llu per push",
-                    (unsigned long long)n, band, blanker_push_limit(e, band));
+                set_error("push of %llu samples into band %d: the samples its segment stages still read must stay in the ring, at most %llu per push",
+                    (unsigned long long)n, band, stage_push_limit(e, band));
                 return B200_ERR_RANGE;
             }
         B200_ENTER_DEVICE(e->device);
@@ -622,7 +656,7 @@ extern "C"
         if (!b.in_use || b.attached) return B200_ERR_STATE;
         b.valid_from = b.write_index;
         if (b.cond.src >= 0) b.cond.floor = b.write_index;
-        if (b.blank.src >= 0) b.blank.floor = b.write_index;
+        if (b.stage.src >= 0) b.stage.floor = b.write_index;
         source_restarted(e, band);
         return B200_OK;
     }
@@ -654,7 +688,7 @@ extern "C"
             if (const int rc = check_push_format(b, band, fmt)) return rc;
             capacity = b.capacity;
             history = conditioner_taps(e, band);
-            blank_limit = blanker_push_limit(e, band);
+            blank_limit = stage_push_limit(e, band);
         }
         if (chunk_samples == 0) chunk_samples = 1ULL << 20;
         if (chunk_samples > capacity / 2) chunk_samples = capacity / 2 ? capacity / 2 : 1;
@@ -846,9 +880,10 @@ extern "C"
                 set_error("iq_set_conditioner: band %d -> band %d would chain conditioners", src_band, dst_band);
                 return B200_ERR_STATE;
             }
-        if (d.blank.src >= 0 || s.blank.src >= 0)
+        if (d.stage.src >= 0 || s.stage.src >= 0)
             {
-                set_error("iq_set_conditioner: band %d -> band %d: a pulse blanker fills band %d", src_band, dst_band, d.blank.src >= 0 ? dst_band : src_band);
+                set_error("iq_set_conditioner: band %d -> band %d: a %s fills band %d", src_band, dst_band, stage_name(d.stage.src >= 0 ? d.stage : s.stage),
+                    d.stage.src >= 0 ? dst_band : src_band);
                 return B200_ERR_STATE;
             }
         if (d.capacity * decimation < s.capacity || s.capacity < n_taps)
@@ -878,14 +913,66 @@ extern "C"
         return B200_OK;
     }
 
+    // caller holds e->mu: the band rules every segment stage shares, for `who` linking src_band to dst_band: both owned
+    // rings, a gr_complex destination at least as large as the source, a source of at least min_src samples, and no chain
+    // but conditioner -> stage (the destination neither filled by nor feeding any stage, the source not a stage's)
+    static int check_stage_bands(b200_engine* e, const char* who, int dst_band, int src_band, unsigned long long min_src)
+    {
+        const Band& d = e->bands[dst_band];
+        const Band& s = e->bands[src_band];
+        if (const int rc = s.check_owned_ring(src_band)) return rc;
+        if (const int rc = d.check_owned_ring(dst_band)) return rc;
+        if (d.fmt != kCf32)
+            {
+                set_error("%s: band %d holds %s samples: a segment stage writes gr_complex", who, dst_band, item_type_name(d.fmt));
+                return B200_ERR_STATE;
+            }
+        unsigned long long reach;
+        if (d.cond.src >= 0 || conditioner_taps(e, dst_band) > 0 || stage_reach_of(e, dst_band, &reach) || s.stage.src >= 0)
+            {
+                set_error("%s: band %d -> band %d would chain a segment stage with another stage", who, src_band, dst_band);
+                return B200_ERR_STATE;
+            }
+        if (d.capacity < s.capacity || s.capacity < min_src)
+            {
+                set_error("%s: band %d (%llu samples) must hold band %d's %llu samples, and band %d at least %llu", who, dst_band, d.capacity,
+                    src_band, s.capacity, src_band, min_src);
+                return B200_ERR_RANGE;
+            }
+        return B200_OK;
+    }
+
+    // caller holds e->mu: dst_band's stage, its parameters set, starts reading src_band at the source's write index (a
+    // fresh stream: 0; mid-stream: where the next sample lands) from the block's initial state
+    static void start_stage(b200_engine* e, int dst_band, int src_band)
+    {
+        Band& d = e->bands[dst_band];
+        const Band& s = e->bands[src_band];
+        Band::SegStage& k = d.stage;
+        k.src = src_band;
+        k.origin = s.write_index;
+        k.seen_valid_from = s.valid_from;
+        k.segments = 0;
+        k.floor = 0;
+        k.fresh = true;
+        staged_window(e, d);
+    }
+
+    // dst_band's segment stage, if it is of this kind, is removed; a stage of the other kind stays
+    static void remove_stage(b200_engine* e, int dst_band, Band::StageKind kind)
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        Band::SegStage& k = e->bands[dst_band].stage;
+        if (k.kind == kind) k.src = -1;
+    }
+
     int b200_iq_set_pulse_blanking(b200_engine* e, int dst_band, int src_band, float pfa, int32_t length, int32_t segments_est,
         int32_t segments_reset)
     {
         if (!e || dst_band < 0 || dst_band >= kMaxBands) return B200_ERR_ARG;
         if (length == 0)
             {
-                std::lock_guard<std::mutex> lk(e->mu);
-                e->bands[dst_band].blank.src = -1;
+                remove_stage(e, dst_band, Band::kBlanker);
                 return B200_OK;
             }
         if (src_band < 0 || src_band >= kMaxBands || length < 0 || segments_est < 0 || segments_reset < 0 || !(pfa > 0.f && pfa < 1.f))
@@ -907,45 +994,21 @@ extern "C"
         float thres = 0.f;
         if (const int rc = b200_iq_pulse_blanking_threshold(pfa, length, &thres)) return rc;
         std::lock_guard<std::mutex> lk(e->mu);
-        Band& d = e->bands[dst_band];
-        const Band& s = e->bands[src_band];
-        if (const int rc = s.check_owned_ring(src_band)) return rc;
-        if (const int rc = d.check_owned_ring(dst_band)) return rc;
-        if (d.fmt != kCf32)
-            {
-                set_error("iq_set_pulse_blanking: band %d holds %s samples: a blanker writes gr_complex", dst_band, item_type_name(d.fmt));
-                return B200_ERR_STATE;
-            }
-        // the one chain allowed is conditioner -> blanker: the source may be a conditioner's destination, nothing else
-        if (d.cond.src >= 0 || conditioner_taps(e, dst_band) > 0 || blanker_length(e, dst_band) > 0 || s.blank.src >= 0)
-            {
-                set_error("iq_set_pulse_blanking: band %d -> band %d would chain a blanker with another stage", src_band, dst_band);
-                return B200_ERR_STATE;
-            }
-        if (d.capacity < s.capacity || s.capacity < static_cast<unsigned long long>(length))
-            {
-                set_error("iq_set_pulse_blanking: band %d (%llu samples) must hold band %d's %llu samples, and band %d at least %d", dst_band,
-                    d.capacity, src_band, s.capacity, src_band, length);
-                return B200_ERR_RANGE;
-            }
+        if (const int rc = check_stage_bands(e, "iq_set_pulse_blanking", dst_band, src_band, static_cast<unsigned long long>(length))) return rc;
         B200_ENTER_DEVICE(e->device);
-        Band::Blanker& k = d.blank;
-        const unsigned long long max_seg = s.capacity / static_cast<unsigned long long>(length) + 1;
+        Band& d = e->bands[dst_band];
+        Band::SegStage& k = d.stage;
+        const unsigned long long max_seg = e->bands[src_band].capacity / static_cast<unsigned long long>(length) + 1;
         B200_CUDA_TRY(cudaStreamSynchronize(e->stream));  // launches already queued may still use the old buffers
         if (!k.state) B200_CUDA_TRY(k.state.alloc(1));
         if (!k.energy.fits(max_seg)) B200_CUDA_TRY(k.energy.alloc(max_seg));
         if (!k.flags.fits(max_seg)) B200_CUDA_TRY(k.flags.alloc(max_seg));
-        k.src = src_band;
+        k.kind = Band::kBlanker;
         k.length = length;
         k.n_est = segments_est;
         k.n_reset = segments_reset;
         k.thres = thres;
-        k.origin = s.write_index;  // a fresh stream: 0; mid-stream: where the next sample lands
-        k.seen_valid_from = s.valid_from;
-        k.segments = 0;
-        k.floor = 0;
-        k.fresh = true;
-        blanked_window(e, d);
+        start_stage(e, dst_band, src_band);
         return B200_OK;
     }
 
@@ -954,12 +1017,12 @@ extern "C"
         if (!e || dst_band < 0 || dst_band >= kMaxBands || !status) return B200_ERR_ARG;
         std::lock_guard<std::mutex> lk(e->mu);
         const Band& d = e->bands[dst_band];
-        if (d.blank.src < 0)
+        if (d.stage.src < 0 || d.stage.kind != Band::kBlanker)
             {
                 set_error("band %d has no pulse blanker (call b200_iq_set_pulse_blanking)", dst_band);
                 return B200_ERR_STATE;
             }
-        const Band::Blanker& k = d.blank;
+        const Band::SegStage& k = d.stage;
         BlankState st{};
         if (!k.fresh)
             {
@@ -975,6 +1038,109 @@ extern "C"
         status->threshold = k.thres;
         status->last_filtered = st.last_filtered;
         status->length = k.length;
+        return B200_OK;
+    }
+
+    int b200_iq_set_notch(b200_engine* e, int dst_band, int src_band, int variant, float pfa, float p_c_factor, int32_t length,
+        int32_t segments_est, int32_t segments_reset, int32_t segments_coeff)
+    {
+        if (!e || dst_band < 0 || dst_band >= kMaxBands) return B200_ERR_ARG;
+        if (length == 0)
+            {
+                remove_stage(e, dst_band, Band::kNotch);
+                return B200_OK;
+            }
+        const bool lite = variant == B200_NOTCH_LITE;
+        if (src_band < 0 || src_band >= kMaxBands || (variant != B200_NOTCH && !lite) || !(pfa > 0.f && pfa < 1.f) ||
+            !(std::fabs(p_c_factor) < 1.f) || length < 0 || segments_est < 0 || segments_reset < 0 || (lite && segments_coeff < 1))
+            {
+                set_error("iq_set_notch: band %d, variant %d, pfa %g, p_c_factor %g, length %d, segments_est %d, segments_reset %d, segments_coeff %d: "
+                          "bad argument", src_band, variant, static_cast<double>(pfa), static_cast<double>(p_c_factor), length, segments_est,
+                    segments_reset, segments_coeff);
+                return B200_ERR_ARG;
+            }
+        if (dst_band == src_band)
+            {
+                set_error("iq_set_notch: band %d cannot filter into itself", dst_band);
+                return B200_ERR_ARG;
+            }
+        if (length > B200_IQ_MAX_NOTCH_LENGTH)
+            {
+                set_error("iq_set_notch: length %d: at most %d", length, B200_IQ_MAX_NOTCH_LENGTH);
+                return B200_ERR_RANGE;
+            }
+        float thres = 0.f;
+        if (const int rc = b200_iq_pulse_blanking_threshold(pfa, length, &thres)) return rc;
+        std::lock_guard<std::mutex> lk(e->mu);
+        if (const int rc = check_stage_bands(e, "iq_set_notch", dst_band, src_band, static_cast<unsigned long long>(length) + (lite && length == 1 ? 2 : 1))) return rc;
+        B200_ENTER_DEVICE(e->device);
+        Band& d = e->bands[dst_band];
+        Band::SegStage& k = d.stage;
+        const unsigned long long cap = e->bands[src_band].capacity, max_seg = cap / static_cast<unsigned long long>(length) + 1;
+        const unsigned long long max_samples = max_seg * static_cast<unsigned long long>(length), max_blocks = max_samples / kNotchGrid + 2;
+        // W[m] = exp(-2 pi i m / L) in double: the forward FFT's twiddles
+        const double pi = 3.14159265358979323846;
+        std::vector<double2> w(static_cast<size_t>(length));
+        for (int m = 0; m < length; m++)
+            {
+                const double a = -2.0 * pi * m / length;
+                w[m] = make_double2(std::cos(a), std::sin(a));
+            }
+        B200_CUDA_TRY(cudaStreamSynchronize(e->stream));  // launches already queued may still use the old buffers
+        if (!k.notch_state) B200_CUDA_TRY(k.notch_state.alloc(1));
+        if (!k.energy.fits(max_seg)) B200_CUDA_TRY(k.energy.alloc(max_seg));
+        if (!k.sig2lin.fits(max_seg)) B200_CUDA_TRY(k.sig2lin.alloc(max_seg));
+        if (!k.flags.fits(max_seg)) B200_CUDA_TRY(k.flags.alloc(max_seg));
+        if (!k.zsrc.fits(max_seg)) B200_CUDA_TRY(k.zsrc.alloc(max_seg));
+        if (!k.zseg.fits(max_seg)) B200_CUDA_TRY(k.zseg.alloc(max_seg));
+        if (!lite && !k.zs.fits(max_samples)) B200_CUDA_TRY(k.zs.alloc(max_samples));
+        if (!k.block_ab.fits(2 * max_blocks)) B200_CUDA_TRY(k.block_ab.alloc(2 * max_blocks));
+        if (!k.y_grid.fits(max_blocks)) B200_CUDA_TRY(k.y_grid.alloc(max_blocks));
+        if (!k.twiddle.fits(w.size())) B200_CUDA_TRY(k.twiddle.alloc(w.size()));
+        B200_CUDA_TRY(cudaMemcpyAsync(k.twiddle, w.data(), sizeof(double2) * w.size(), cudaMemcpyHostToDevice, e->stream));
+        B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
+        k.kind = Band::kNotch;
+        k.variant = variant;
+        k.length = length;
+        k.n_est = segments_est;
+        k.n_reset = segments_reset;
+        k.n_coeff = lite ? segments_coeff : 1;
+        k.p = p_c_factor;
+        k.thres = thres;
+        start_stage(e, dst_band, src_band);
+        return B200_OK;
+    }
+
+    int b200_iq_notch_status(b200_engine* e, int dst_band, b200_notch_status* status)
+    {
+        if (!e || dst_band < 0 || dst_band >= kMaxBands || !status) return B200_ERR_ARG;
+        std::lock_guard<std::mutex> lk(e->mu);
+        const Band& d = e->bands[dst_band];
+        if (d.stage.src < 0 || d.stage.kind != Band::kNotch)
+            {
+                set_error("band %d has no notch (call b200_iq_set_notch)", dst_band);
+                return B200_ERR_STATE;
+            }
+        const Band::SegStage& k = d.stage;
+        NotchState st{};
+        if (!k.fresh)
+            {
+                B200_ENTER_DEVICE(e->device);
+                B200_CUDA_TRY(cudaMemcpyAsync(&st, k.notch_state, sizeof(st), cudaMemcpyDeviceToHost, e->stream));
+                B200_CUDA_TRY(cudaStreamSynchronize(e->stream));
+            }
+        status->origin = k.origin;
+        status->segments = k.segments;
+        status->filtered = st.filtered;
+        status->n = st.n;
+        status->noise_power = st.est;
+        status->threshold = k.thres;
+        status->z0 = b200_cf32{st.z0.x, st.z0.y};
+        status->last_out = b200_cf32{st.last_out.x, st.last_out.y};
+        status->filter_state = st.filter_state;
+        status->n_coeff = st.n_coeff;
+        status->length = k.length;
+        status->variant = k.variant;
         return B200_OK;
     }
 

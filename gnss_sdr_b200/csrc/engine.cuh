@@ -43,23 +43,39 @@ struct Band
         unsigned long long floor{0};         // no output below this is valid: where the conditioner was set or the band forgotten
         DevBuf<float2> taps;                 // composite taps c[k]
     } cond;
-    // the pulse blanker that fills this band from another (b200_iq_set_pulse_blanking); src < 0: none
-    struct Blanker
+    // the segment stage that fills this band from another: a pulse blanker (b200_iq_set_pulse_blanking) or a notch
+    // (b200_iq_set_notch); src < 0: none.  Both share the origin, restart, window, push-limit and chain rules.
+    enum StageKind
+    {
+        kBlanker,
+        kNotch,
+    };
+    struct SegStage
     {
         int src{-1};
+        StageKind kind{kBlanker};
         int length{0};                       // L
         long long n_est{0}, n_reset{0};      // E, R
         float thres{0.f};
         unsigned long long origin{0};        // absolute index of segment 0
         unsigned long long segments{0};      // processed since origin
-        unsigned long long seen_valid_from{0};  // the source's valid_from the origin follows: a move restarts the blanker
+        unsigned long long seen_valid_from{0};  // the source's valid_from the origin follows: a move restarts the stage
         unsigned long long floor{0};         // no output below this is valid: where the band was last forgotten
         bool fresh{true};                    // the next scan starts from the block's initial state
         DevBuf<BlankState> state;
         DevBuf<float> energy;                // one per segment of a push
         DevBuf<unsigned char> flags;
-    } blank;
-    CudaEvent cond_done;        // recorded on the compute stream after the latest conditioner or blanker launch that read or wrote the band
+        // notch only
+        int variant{0};
+        int n_coeff{1};
+        float p{0.f};
+        DevBuf<NotchState> notch_state;
+        DevBuf<double2> twiddle, block_ab, y_grid;
+        DevBuf<float> sig2lin;
+        DevBuf<int> zsrc;
+        DevBuf<float2> zseg, zs;
+    } stage;
+    CudaEvent cond_done;        // recorded on the compute stream after the latest conditioner or stage launch that read or wrote the band
     bool cond_recorded{false};  // cond_done has been recorded
 
     // B200_OK, or B200_ERR_STATE with the error text when this is not a ring made by b200_iq_create

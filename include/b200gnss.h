@@ -236,7 +236,7 @@ extern "C"
      *    refused before any byte is written; b200_iq_push_file cuts its blocks to fit.
      *  - While a blanker is set, a direct push or push_at into its destination is B200_ERR_STATE.  length == 0 removes the
      *    destination's blanker (the other arguments are then not read); so does re-creating or attaching either band.
-     *    Setting a blanker on a destination that has one replaces it, restarting at the rule above.
+     *    Setting a blanker on a destination that has one, or a notch, replaces it, restarting at the rule above.
      *  - Refused, with nothing launched and both windows unchanged: dst_band == src_band, length < 0, segments_est < 0,
      *    segments_reset < 0, or pfa outside (0, 1) (B200_ERR_ARG); length > B200_IQ_MAX_BLANKING_LENGTH or a destination
      *    smaller than the source or a source smaller than L (B200_ERR_RANGE); a band that is not an owned ring, a narrow
@@ -263,6 +263,94 @@ extern "C"
     /* The state of dst_band's blanker after every push queued so far (synchronous): how much it blanks, and the state
      * machine it carries.  A band with no blanker is B200_ERR_STATE. */
     int b200_iq_pulse_blanking_status(b200_engine* e, int dst_band, b200_pulse_blanking_status* status);
+
+    /* ---- notch filters on the device -------------------------------------------------------------------------------
+     * InputFilter.implementation = Notch_Filter and Notch_Filter_Lite (src/core/receiver/gnss_block_factory.cc:835-841;
+     * adapters/notch_filter.cc, adapters/notch_filter_lite.cc), which instantiate Notch(pfa, p_c_factor, length,
+     * segments_est, segments_reset) (gnuradio_blocks/notch_cc.cc:63-121) and NotchLite(p_c_factor, pfa, length,
+     * segments_est, segments_reset, segments_coeff) (notch_lite_cc.cc:71-138): continuous-wave and narrowband interference
+     * is removed before acquisition and tracking see it.
+     *
+     * b200_iq_set_notch links src_band to dst_band: every write into the source that completes segments fills the
+     * destination with the block's output in absolute stream indices.  Segment k is written to [o + k L, o + (k + 1) L),
+     * L = length, o the notch's origin, and reads in[i] = src[o + k L + s + i], s = 0 for B200_NOTCH_LITE (the block's
+     * set_history(2); in[-1] of the origin's segment is the zero history item, even when the ring holds a sample there) and
+     * s = 1 for B200_NOTCH (the block's in++ without history: output j comes from input j + 1, so segment k is published
+     * only once source index o + (k + 1) L exists).  For each segment, in order, every float operation rounded on its own:
+     *     n < E and the filter off (estimation):  X[q] = sum_m in[m] W[m q mod L], W[m] = exp(-2 pi i m / L), in double
+     *         (W made on the host in double, m ascending, each product and sum rounded); dB[q] = float(10 log10(|X[q]|^2 +
+     *         1e-20)) in double; floor = volk_32f_s32f_calc_spectral_noise_floor_32f(dB, 15) in float (mean = sum / L + 15,
+     *         then the mean of the dB[q] <= mean, or mean if none); sig2lin = float(10^(double(floor / 10))) / float(2L);
+     *         est = (float(n) est + sig2lin) / float(n + 1); the segment is copied.
+     *     else e = Re(volk_32fc_x2_conjugate_dot_prod_32fc(in, in, L)), in the generic order: even and odd samples into
+     *         two sums of re re + im im, added, then + |in[L-1]|^2 when L is odd;
+     *         e / est > thres (filtering): at the filter's switch-on last_out = 0 and (Lite) n_coeff = 0.
+     *             Lite: when n_coeff == 0, z0 = exp(i float((a1 + a2) / 2)), a1 = atan2 of in[1] conj(in[0]), a2 of
+     *             in[L-1] conj(in[L-2]); then n_coeff = (n_coeff + 1) mod segments_coeff.
+     *             Notch: per sample, z0 = exp(i atan2 of in[i] conj(in[i-1])).
+     *             out[i] = (in[i] - z0 in[i-1]) + (p z0) last_out, last_out = out[i]   (gr_complex products).
+     *         else: copied, the filter off, and n = 0 if n > R.
+     *     n++
+     * E = segments_est, R = segments_reset, p = p_c_factor, thres = b200_iq_pulse_blanking_threshold(pfa, L) (the same
+     * chi-squared quantile).  atan2, log10, pow, sin and cos are computed in double and rounded once to float.
+     *  - The IIR is split-invariant: output samples are cut into blocks of 1024 on an absolute grid counted from the origin.
+     *    Each block's affine map y -> A y + B is composed in double in sample order (a run start sets A = 0, B = b); y is
+     *    carried from grid point to grid point in double, y_{g+1} = A_g y_g + B_g, and kept in the notch's state across
+     *    pushes; inside a block the float recursion above runs serially from float(y_g).  So a filtered sample is within a
+     *    float rounding bound (scaled by 1 / (1 - |p|)^2) of a float64 recursion with the same z0 and inputs, and the
+     *    destination's bytes do not depend on how the source was pushed, which is why the device does not run the block's
+     *    one serial float recursion per run: that recursion is as accurate (its rounding errors are damped by |p z0| <= |p|
+     *    (1 + 2^-23), so they stay within the same 1 / (1 - |p|) form however long the run), but it cannot be split across
+     *    threads.  Everything else (energies, est and every sig2lin, decisions, resets, runs, z0, copied and estimation
+     *    samples) follows the statement above bit for bit.
+     *  - Against the block itself: its spectrum comes from a float FFT and its transcendentals from the float libm
+     *    functions, so est and z0 differ from the block's in the last few bits; a decision close to the threshold can
+     *    then differ.  The reference's estimator compares a time-domain energy with a mean of dB values, which sits about
+     *    2.5 dB under the mean power for noise, so the filter is on for much of a clean stream; this is reproduced.
+     *  - Origin, window, chains, removal and replacement follow the pulse blanker above: the origin is 0 on a fresh stream
+     *    and the source's write index when set mid-stream, the notch restarts with the block's initial state whenever the
+     *    source's valid_from moves, and the destination holds whole segments only.  The source may be a conditioner's
+     *    destination; nothing else chains (notch -> any stage, blanker -> notch and notch -> blanker are refused).
+     *  - A push that completes segments launches six kernels on the compute stream (energies; the noise floor, which
+     *    returns at once when no segment of the push can be in estimation; the state machine; the block maps; the carry;
+     *    the output); none otherwise.  The state lives in device memory; a band search, batch or loop run issued after the
+     *    push reads the notched samples with no host synchronisation.
+     *  - A segment needs one sample beyond the L - 1 pending (Lite: the one before it, and at L = 1 also the one after it;
+     *    Notch: the one after it): a push of more than capacity - L samples (Lite at L = 1: capacity - 2) into a notch's
+     *    source, or D times that of the conditioner's destination through a chained conditioner, is B200_ERR_RANGE, refused
+     *    before any byte is written; b200_iq_push_file cuts its blocks to fit.
+     *  - Departures from the block: |p_c_factor| >= 1 or a non-finite one is refused (the block would run an unstable
+     *    filter); n is 64-bit (the block's int32 overflows after 2^31 segments without a reset).
+     *  - length == 0 removes the destination's notch (the other arguments are then not read); a pulse blanker there stays,
+     *    and b200_iq_set_pulse_blanking with length 0 likewise leaves a notch in place.  Setting a notch on a destination
+     *    that a blanker or notch fills replaces it, restarting with the block's initial state.  Refused, with nothing launched and both
+     *    windows unchanged: an unknown variant, pfa outside (0, 1), a bad p_c_factor, length, segments_est or
+     *    segments_reset < 0, dst_band == src_band, or Lite with segments_coeff < 1 (B200_ERR_ARG; Notch does not read
+     *    segments_coeff); length > B200_IQ_MAX_NOTCH_LENGTH, a destination smaller than the source, or a source smaller than
+     *    L + 1 (Lite at L = 1: 3), which could take no push (B200_ERR_RANGE); a band that is not an owned ring, a narrow destination, a destination a stage fills or
+     *    that feeds one, or a forbidden chain (B200_ERR_STATE). */
+#define B200_NOTCH 0      /* Notch_Filter: z0 per sample, output j from input j + 1 */
+#define B200_NOTCH_LITE 1 /* Notch_Filter_Lite: z0 per coefficient period, output j from input j */
+#define B200_IQ_MAX_NOTCH_LENGTH 1024
+    int b200_iq_set_notch(b200_engine* e, int dst_band, int src_band, int variant, float pfa, float p_c_factor, int32_t length,
+        int32_t segments_est, int32_t segments_reset, int32_t segments_coeff);
+    typedef struct
+    {
+        uint64_t origin;       /* absolute index of segment 0 (destination indices) */
+        uint64_t segments;     /* segments processed since the origin */
+        uint64_t filtered;     /* of them, filtered */
+        int64_t n;             /* n_segments_ */
+        float noise_power;     /* noise_pow_est_ */
+        float threshold;       /* thres_ */
+        b200_cf32 z0;          /* z_0_ */
+        b200_cf32 last_out;    /* last_out_ (the split-invariant recursion's) */
+        int32_t filter_state;  /* filter_state_ */
+        int32_t n_coeff;       /* n_segments_coeff_ (Lite; 0 for Notch) */
+        int32_t length;        /* L */
+        int32_t variant;       /* B200_NOTCH or B200_NOTCH_LITE */
+    } b200_notch_status;
+    /* The state of dst_band's notch after every push queued so far (synchronous).  A band with no notch is B200_ERR_STATE. */
+    int b200_iq_notch_status(b200_engine* e, int dst_band, b200_notch_status* status);
 
     /* ---- tracking: single correlator, 1:1 with Cpu_Multicorrelator_Real_Codes ----------- */
     /* src/algorithms/tracking/libs/cpu_multicorrelator_real_codes.h:37-61 */
