@@ -64,15 +64,16 @@ def _check_status(e, band, res, k, origin, variant, length):
     assert _f32(st["last_out"].real) == _f32(want["last_out"][0]) and _f32(st["last_out"].imag) == _f32(want["last_out"][1])
 
 
-CASES = [(nn.NOTCH_LITE, 1, 1), (nn.NOTCH_LITE, 7, 3), (nn.NOTCH_LITE, 32, 1), (nn.NOTCH_LITE, 301, 3),
-         (nn.NOTCH, 7, 1), (nn.NOTCH, 32, 1), (nn.NOTCH, 301, 1)]
+CASES = [(nn.NOTCH_LITE, 1, 1), (nn.NOTCH_LITE, 2, 3), (nn.NOTCH_LITE, 7, 3), (nn.NOTCH_LITE, 32, 1), (nn.NOTCH_LITE, 301, 3),
+         (nn.NOTCH, 1, 1), (nn.NOTCH, 2, 1), (nn.NOTCH, 7, 1), (nn.NOTCH, 32, 1), (nn.NOTCH, 301, 1)]
 
 
 @pytest.mark.parametrize("variant,length,n_coeff", CASES)
 @pytest.mark.parametrize("item_type", ["gr_complex", "ishort", "ibyte"])
 def test_bit_exact_push_by_push(capi, engine, item_type, variant, length, n_coeff):
     """odd push sizes three times around a 4096-sample source ring with small E and R; the status after every push;
-    filtered samples within the stated bound of the float64 truth"""
+    filtered samples within the stated bound of the float64 truth.  L = 1 and 2 run the floor kernel on one warp, and
+    the full Notch at L = 1 reads one look-ahead sample per segment"""
     e = engine
     rng = np.random.default_rng(1000 * length + 10 * variant + len(item_type))
     cap = 1 << 12
